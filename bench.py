@@ -75,7 +75,9 @@ WORKLOADS = {
 def parse():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
-    ap.add_argument("--steps", type=int, default=3)
+    ap.add_argument("--steps", type=int, default=3,
+                    help="timed steps of the device-resident leg and of the end-to-end leg (each leg also runs untimed "
+                         "warm-up calls first: --warmup of them, and one for the end-to-end leg's pinned buffers)")
     ap.add_argument("--warmup", type=int, default=3)
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--workload", default="radon", choices=sorted(WORKLOADS))
@@ -84,9 +86,12 @@ def parse():
     ap.add_argument("--draws", type=int, default=-1)
     ap.add_argument("--cpu-chains", type=int, default=0, help="reference arm / cpu_baseline: chains per step (0 = host cores)")
     ap.add_argument("--precision", default="fp64", choices=["fp64", "tc_fp16x2"],
-                    help="logistic / mvgauss: fp64 DMMA (parity mode) or the tcgen05 split-fp16 tensor-core performance mode")
+                    help="logistic / mvgauss: fp64 DMMA (parity mode) or the wgmma split-fp16 tensor-core performance mode")
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-e2e", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write what the last timed step computed (draws, sampler stats, per-chain "
+                         "summaries of a fixed, seeded sample of chains, at most 64 MB) as DIR/<name>.npy")
     args = ap.parse_args()
     args.wl = WORKLOADS[args.workload]
     args.tune = args.wl["tune"] if args.tune < 0 else args.tune
@@ -286,8 +291,38 @@ def reference_arm(args):
     print(json.dumps(line))
 
 
+DUMP_BUDGET = 64_000_000  # bytes, .npy headers included
+
+
+def dump_outputs(out_dir, res):
+    """Writes the arrays the timed path returned in its last step as float64 .npy files: the draws [k, draws, n], every
+    sampler stat [k, draws] and every per-chain summary of k chains, plus their indices (chain_index).  k chains are a
+    fixed sample (seed 0) chosen so that the files stay within DUMP_BUDGET; all chains when they fit."""
+    import torch
+
+    os.makedirs(out_dir, exist_ok=True)
+    C = int(res.draws.shape[0])
+    parts = [res.draws] + list(res.stats.values()) + list(res.summary.values())
+    per_chain = 8 * sum(int(np.prod(tuple(a.shape[1:]))) for a in parts)
+    headers = 256 * (2 + len(res.stats) + len(res.summary))  # an .npy header is at most a few hundred bytes
+    k = min(C, max(1, (DUMP_BUDGET - 8 * C - headers) // per_chain))
+    idx = np.sort(np.random.default_rng(0).choice(C, k, replace=False))
+
+    def take(a):
+        if isinstance(a, torch.Tensor):
+            return a.index_select(0, torch.as_tensor(idx, device=a.device)).cpu().numpy()
+        return np.asarray(a)[idx]
+
+    arrays = {"chain_index": idx, "draws": res.draws}
+    arrays.update({f"stat_{name}": v for name, v in res.stats.items()})
+    arrays.update({f"summary_{name}": v for name, v in res.summary.items()})
+    for name, a in arrays.items():
+        a = idx if name == "chain_index" else take(a)
+        np.save(os.path.join(out_dir, name + ".npy"), np.asarray(a, dtype=np.float64))
+
+
 # ---------------------------------------------------------------------------------------------
-# clocks sampling during the timed region (B200_PROFILING.md recipe)
+# clocks sampling during the timed region
 # ---------------------------------------------------------------------------------------------
 class ClockSampler:
     Q = ("index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.active,clocks_event_reasons.hw_slowdown,"
@@ -340,55 +375,37 @@ def measured_peaks():
             return float(json.load(open(p))["hbm_gbs"]), "measured"
         except Exception:
             pass
-    return 6650.0, "fallback"
+    return 3350.0, "fallback: H100 SXM data sheet HBM3 bandwidth"
 
 
-def ncu_traffic(workload, evals_per_launch):
-    """(DRAM bytes per launch, source) from the committed ncu --set full capture of this workload's kernel
-    (profiles/traffic.json: dram__bytes_read.sum + dram__bytes_write.sum per grad-eval of the captured launch, scaled by
-    the grad-evals of this launch -- the capture is a shorter launch of the same kernel); None if nothing is committed."""
-    p = os.path.join(ROOT, "profiles", "traffic.json")
-    if os.path.isfile(p):
-        try:
-            e = json.load(open(p))[workload]
-            return float(e["dram_bytes_per_grad_eval"]) * evals_per_launch, e.get("source", "profiles/traffic.json")
-        except Exception:
-            return None
-    return None
-
-
-def make_roofline(workload, wl, per_launch, k_ms, fp64, dmma, peaks, traffic):
+def make_roofline(workload, wl, per_launch, k_ms, fp64, dmma, peaks):
     """The `roofline` object of the bench line.  per_launch: grad evaluations of one run (start states included);
-    k_ms: its CUDA-event duration; fp64 / dmma: TFLOP/s measured in this process (or None); peaks: (HBM GB/s, source);
-    traffic: (DRAM bytes per launch or None, how it was obtained).
+    k_ms: its CUDA-event duration; fp64 / dmma: TFLOP/s measured in this process (or None); peaks: (HBM GB/s, source).
 
     The top-level `bound`/`frac` is the BINDING resource.  The persistent kernels keep observed data and chain state on
     chip, so their DRAM traffic is orders of magnitude below the algorithmic bytes and the binding pipe is fp64: the
     HBM-by-algorithmic-bytes figure SURVEY 8(d) asks for is reported as the secondary `hbm_by_algorithmic_bytes` object
-    (it is NOT a utilisation of anything), next to the DRAM bytes ncu measured."""
-    t_bytes, t_how = traffic if traffic else (None, None)
+    (it is NOT a utilisation of anything)."""
     if wl["bound"] == "onchip":
         peak, how = peaks
         gbs = wl["per_eval"] * per_launch / (k_ms * 1e-3) / 1e9
         hbm = {"achieved": gbs, "peak": peak, "unit": "GB/s", "frac": gbs / peak, "peak_source": how,
-               "algorithmic_bytes_per_eval": wl["per_eval"], "dram_bytes_measured": t_bytes, "dram_bytes_source": t_how,
+               "algorithmic_bytes_per_eval": wl["per_eval"],
                "note": "algorithmic bytes / kernel time; not a DRAM utilisation (data and chain state are on chip)"}
-        fpeak = fp64 or 36.0
+        fpeak = fp64 or 34.0
         tf = wl["flops_per_eval"] * per_launch / (k_ms * 1e-3) / 1e12
         return {"bound": "fp64", "achieved": tf, "peak": fpeak, "unit": "TFLOP/s", "frac": tf / fpeak,
-                "traffic": t_bytes, "traffic_source": t_how,
                 "peak_source": "DFMA micro-benchmark in this run (b200_measure_fp64_tflops; MEASURED_PEAKS.json has only HBM "
-                               "and bf16)" if fp64 else "fallback 36.0 (DFMA peak measured on this pool, profiles/)",
+                               "and bf16)" if fp64 else "fallback 34.0 (H100 SXM data sheet fp64 non-tensor rate)",
                 "algorithmic_flops_per_eval": wl["flops_per_eval"], "kernel": wl["kernel"], "kernel_ms": k_ms,
                 "note": wl["note"], "hbm_by_algorithmic_bytes": hbm}
     # dense contraction on the fp64 tensor path: no fp64 entry in MEASURED_PEAKS.json (HBM + bf16 only), so the
     # denominator is the DMMA rate measured in this process by the library's own micro-benchmark
-    peak = dmma or 37.0
+    peak = dmma or 67.0
     achieved = wl["per_eval"] * per_launch / (k_ms * 1e-3) / 1e12
     return {"bound": "tensor", "achieved": achieved, "peak": peak, "unit": "TFLOP/s", "frac": achieved / peak,
-            "traffic": t_bytes, "traffic_source": t_how,
             "peak_source": "fp64 DMMA micro-benchmark in this run (MEASURED_PEAKS.json has no fp64 entry)"
-            if dmma else "fallback 37.0 (scripts/mb/dmma.cu measured on this pool)",
+            if dmma else "fallback 67.0 (H100 SXM data sheet fp64 tensor-core rate)",
             "kernel": wl["kernel"], "kernel_ms": k_ms, "algorithmic_flops_per_eval": wl["per_eval"], "note": wl["note"],
             "fp64_dfma_peak_tflops_measured": fp64,
             "time_base": "kernel_ms spans every launch of the lock-step loop (advance kernels and ragged tail included)"}
@@ -516,6 +533,8 @@ def b200_arm(args):
     ev1.record()
     barrier()
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, res)
     ms_total = parallel.max_over_ranks(ev0.elapsed_time(ev1))
     evals = parallel.sum_over_ranks(float(evals_t.item()))
     all_evals = float(all_evals_t.item())
@@ -530,7 +549,7 @@ def b200_arm(args):
     # ---- e2e: public host API, pinned host buffers, H2D + D2H inside the timed region --------------
     e2e = None
     near = parallel.near_gpu(local)
-    if not args.no_e2e:
+    if not args.no_e2e and args.steps > 0:
         near.__enter__()  # pinned buffers are allocated on the GPU's NUMA node (restored before the CPU arm runs)
         T = draws
         pin = lambda shape, dt: torch.empty(shape, dtype=dt, pin_memory=True).numpy()  # noqa: E731
@@ -538,7 +557,7 @@ def b200_arm(args):
         mean0_p = None
         if mean0_host is not None:
             mean0_p = pin((C, n), torch.float64); mean0_p[:] = mean0_host
-        n_e2e = max(1, min(args.steps, 3))
+        n_e2e = args.steps
         st_e = states0.copy()
         # one untimed call: allocates the pooled pinned output buffers the timed calls reuse
         res_h = cm.nuts_run(q0_p, st_e, tune=tune, draws=draws, mean0=mean0_p, store_warmup=False,
@@ -612,26 +631,25 @@ def b200_arm(args):
             fp64 = tf.value
         if _lib.load().b200_measure_dmma_tflops(ctypes.byref(tf)) == 0:
             dmma = tf.value
-    roofline = make_roofline(args.workload, wl, per_launch, k_ms, fp64, dmma, measured_peaks(),
-                             ncu_traffic(args.workload, per_launch))
+    roofline = make_roofline(args.workload, wl, per_launch, k_ms, fp64, dmma, measured_peaks())
     if args.precision == "tc_fp16x2":
         # tensor-core performance mode: every fp64 product is three fp16 MMAs (hi*hi, hi*lo, lo*hi) -> issued tensor flops =
         # 3 x the algorithmic 4 N K per eval; peak = the dense bf16/fp16 rate in MEASURED_PEAKS.json (sustained figure: the
-        # kernel runs inside a long loop), else the nominal 2250
+        # kernel runs inside a long loop), else the H100 SXM data sheet's 989
         issued = 3.0 * wl["per_eval"] * per_launch / (k_ms * 1e-3) / 1e12
-        tpeak, tsrc = 2250.0, "nominal dense bf16/fp16 (MEASURED_PEAKS.json absent)"
+        tpeak, tsrc = 989.0, "H100 SXM data sheet dense fp16 (MEASURED_PEAKS.json absent)"
         try:
             mp_ = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
             tpeak, tsrc = float(mp_.get("bf16_tflops_sustained") or mp_["bf16_tflops"]), "MEASURED_PEAKS.json bf16_tflops_sustained"
         except Exception:
             pass
         roofline = {"bound": "tensor", "achieved": issued, "peak": tpeak, "unit": "TFLOP/s", "frac": issued / tpeak,
-                    "traffic": None, "peak_source": tsrc,
-                    "kernel": ("logistic_tc2_kernel" if args.workload == "logistic" else "gemm_tc_kernel") + " (tcgen05.mma kind::f16, TMEM, TMA)",
+                    "peak_source": tsrc,
+                    "kernel": ("logistic_tc_kernel" if args.workload == "logistic" else "gemm_tc_kernel") + " (wgmma m64n64k16 f16, TMA)",
                     "kernel_ms": k_ms, "algorithmic_flops_per_eval": wl["per_eval"], "issued_tensor_flops_per_eval": 3.0 * wl["per_eval"],
                     "fp64_equivalent_tflops": wl["per_eval"] * per_launch / (k_ms * 1e-3) / 1e12,
                     "accuracy": "gradient <= 1e-6 of its largest entry, logp <= 1e-8 relative vs the fp64 path "
-                                "(tests/test_gpu_tc.py; profiles/r2_parity_report.json)",
+                                "(tests/test_gpu_tc.py)",
                     "time_base": "kernel_ms spans every launch of the lock-step loop (advance kernels and ragged tail included)"}
 
     # ---- cpu_baseline (rank 0, N = 1 only): the oracle port on the host cores, bounded sample -----------

@@ -288,9 +288,10 @@ int b200_set_device(int device);
 int b200_model_create(const b200_model_desc* desc, b200_model** out);
 /* Arithmetic of the dense contractions of a GEMM-shaped model (affects b200_logp_dlogp and b200_nuts_run of that handle).
  *   B200_PRECISION_FP64      IEEE fp64 on the fp64 tensor path (DMMA) -- the parity mode, default.
- *   B200_PRECISION_TC_FP16X2 LOGISTIC only: X.beta and X^T r on the 5th-generation tensor cores (tcgen05, TMEM, TMA) with
+ *   B200_PRECISION_TC_FP16X2 LOGISTIC and MVGAUSS: the dense contractions on the fp16 tensor cores (wgmma, TMA) with
  *                            every fp64 operand split into two fp16 pieces and fp32 accumulation, drained into fp64 every
- *                            2048 rows; gradient ~1e-7 relative (measured: profiles/), ~10x the DMMA throughput.
+ *                            256 rows (logistic) / into compensated sums every 64 terms (GEMM); gradient within 1e-6 of
+ *                            its largest entry (tests/test_gpu_tc.py).
  * The reference computes in floatX = float64 (pymc/pytensorf.py); this is the "tensor cores where the logp really is a
  * dense matvec" performance mode of north_star, with its error stated next to the number. */
 #define B200_PRECISION_FP64 0

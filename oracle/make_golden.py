@@ -73,6 +73,22 @@ def noise(seed, T, n):
     return np.array([g.normal(size=n) for _ in range(T)])
 
 
+def shrink(name, draws=None):
+    """Keeps a golden file under 1 MB: drops the momentum noise z (tests/conftest.py regenerates it from the seeds with noise()
+    above) and, with `draws`, keeps only the first `draws` sampling iterations -- an exact prefix of a run with that many draws,
+    since nothing adapts after tuning (final_var and final_step_size are unchanged)."""
+    path = os.path.join(OUT, name + ".npz")
+    d = dict(np.load(path))
+    d.pop("z")
+    if draws is not None:
+        T_old, T = int(d["tune"]) + int(d["draws"]), int(d["tune"]) + draws
+        for k, v in d.items():
+            if v.ndim >= 2 and v.shape[1] == T_old:
+                d[k] = v[:, :T].copy()
+        d["draws"] = np.array(draws)
+    np.savez_compressed(path, **d)
+
+
 def case(name, spec_name, spec_args, q0s, seeds, *, tune, draws, adapt, var=None, eps=None, nuts_kwargs=None,
          init_var=None, dense=False):
     spec = models.BUILDERS[spec_name](**spec_args)
@@ -131,6 +147,7 @@ def main():
     # exercises dual averaging and both Welford window switches in the non-chaotic regime
     case("radon_warm_adapt", "radon", {}, warm_q[:1], [501], tune=250, draws=30, adapt=True, init_var=warm_var[:1],
          nuts_kwargs={"step_scale": float(warm_eps[0]) / 10 * rd.n**0.25})
+    shrink("radon_adapt", draws=20)  # the 50 draws above only seed the warm state of radon_fixed / radon_warm_adapt
     # small ragged radon (counties with 1..n obs, fewer counties than lanes), early treedepth cap exercised
     q0s = [np.zeros(2 * 7 + 5) + rng.uniform(-1, 1, 19)]
     case("radon_small_adapt", "radon", {"n_obs": 40, "n_counties": 7, "seed": 5}, q0s, [401], tune=250, draws=50,
@@ -194,6 +211,7 @@ def fullsize_cases():
     for k in ("var", "init_var", "pre_var", "final_var"):  # unused by a dense-mass replay
         d[k] = np.zeros(1)
     np.savez_compressed(os.path.join(OUT, "mvgauss_n10000_fixed.npz"), **d)
+    shrink("mvgauss_n10000_fixed")
 
 
 def run_reference_generic(spec, q0, *, seed, tune, draws, step_kind="nuts", potential, adapt=True, step_kwargs=None):

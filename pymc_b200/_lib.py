@@ -282,7 +282,7 @@ def check(rc: int) -> None:
 
 def require_gpu() -> None:
     if load().b200_device_count() < 1:
-        raise B200Error("no CUDA device visible: the B200 engine has no CPU fallback")
+        raise B200Error("no CUDA device visible: the CUDA engine has no CPU fallback")
 
 
 def ptr(a) -> int | None:

@@ -48,6 +48,23 @@ static int fail(const char* fmt, ...) {
                                            __FILE__, __LINE__);                                   \
     } while (0)
 
+// streaming multiprocessors of a device (132 on an H100 SXM): grid sizes and GEMM tile choices fill whole waves of them
+static int sm_count(int device) {
+    static int cached[64] = {0};
+    if (device < 0 || device >= 64) return 132;
+    if (!cached[device]) {
+        int sms = 0;
+        if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, device) != cudaSuccess || sms <= 0) sms = 132;
+        cached[device] = sms;
+    }
+    return cached[device];
+}
+static int current_sm_count() {
+    int dev = 0;
+    cudaGetDevice(&dev);
+    return sm_count(dev);
+}
+
 struct DevBuf {  // owning device allocation
     void* p = nullptr;
     ~DevBuf() { if (p) cudaFree(p); }
@@ -654,7 +671,7 @@ struct Staged {
 };
 // `direct`: an OUTPUT buffer in page-locked host memory (cudaHostAlloc / cudaHostRegister, e.g. a torch pinned tensor) is
 // written by the kernel itself through its device alias (UVA), so the device->host transfer overlaps the run instead of
-// following it (2.9 GB of draws per Radon bench step: 160 ms after the kernel vs ~0 inside it).
+// following it (2.9 GB of draws per Radon bench step).
 static int stage_in(Staged& s, const void* user, size_t bytes, int mem, bool copy_in, bool copy_out,
                     cudaStream_t st, bool direct = false) {
     s.user = const_cast<void*>(user);
@@ -699,7 +716,7 @@ struct LogpLaunch {
         const size_t smem = data + (size_t)wpb * (2 * 32 * W * NPL + (W > 1 ? 8 * W : 0)) * sizeof(double);
         auto kern = logp_grad_warp_kernel<Model, NPL, W>;
         CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        const int blocks = std::max(1, std::min((C + wpb - 1) / wpb, 148 * 8));
+        const int blocks = std::max(1, std::min((C + wpb - 1) / wpb, sm_count(m->device) * 8));
         typename Model::Params MPl;
         if (launch_params<Model>(m, MP, (long long)blocks * wpb, &MPl)) return -1;
         kern<<<blocks, (W == 1) ? wpb * 32 : 32 * W, smem, st>>>(MPl, m->n, C, q, logp, grad, ldq ? ldq : m->n, ldg ? ldg : m->n);
@@ -745,7 +762,7 @@ struct LeapLaunch {
         const size_t smem = data + (size_t)wpb * (2 * 32 * W * NPL + (W > 1 ? 8 * W : 0)) * sizeof(double);
         auto kern = leapfrog_warp_kernel<Model, NPL, W>;
         CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        const int blocks = std::max(1, std::min((C + wpb - 1) / wpb, 148 * 8));
+        const int blocks = std::max(1, std::min((C + wpb - 1) / wpb, sm_count(m->device) * 8));
         typename Model::Params MPl;
         if (launch_params<Model>(m, MP, (long long)blocks * wpb, &MPl)) return -1;
         kern<<<blocks, (W == 1) ? wpb * 32 : 32 * W, smem, st>>>(MPl, m->n, C, var, eps, n_steps, q, p, v, grad, energy, logp, idx);
@@ -804,7 +821,7 @@ static int launch_gemm(cudaStream_t st, const double* Q, long long ldq, int C, c
 }
 
 // D[C][Nout] = alpha * Q[C][K] . M[Nout][K]^T.  Tile shape picked per call: chains per CTA from C, outputs per CTA
-// (8 NB) so that the tile count fills whole waves of 148 SMs.
+// (8 NB) so that the tile count fills whole waves of the device's SMs.
 static int gemm_nt_tc(b200_model* m, cudaStream_t st, const double* Q, long long ldq, int C, const b200_model::TcMat& T, int Nout,
                       double alpha, double* D, long long ldd);
 
@@ -817,15 +834,16 @@ static int gemm_nt(b200_model* m, cudaStream_t st, const double* Q, long long ld
     }
     const int wm = C > 64 ? 8 : (C > 32 ? 4 : 2);
     const int cb = (C + 16 * wm - 1) / (16 * wm);
+    const int sms = m ? sm_count(m->device) : current_sm_count();
     int best_nb = 9;
     double best = -1.0;
     const int nbs[3] = {17, 9, 5};
     for (int i = 0; i < (wm == 8 ? 3 : 2); ++i) {
         const int nb = (wm == 8) ? nbs[i] : nbs[i + 1];
         const long long tiles = (long long)cb * ((Nout + 8 * nb - 1) / (8 * nb));
-        const long long waves = (tiles + 147) / 148;
+        const long long waves = (tiles + sms - 1) / sms;
         // useful work / occupied SM time; small bonus for wider tiles (fewer fragment loads per DMMA)
-        const double eff = (double)Nout * cb / ((double)waves * 148 * 8 * nb) + 1e-3 * nb;
+        const double eff = (double)Nout * cb / ((double)waves * sms * 8 * nb) + 1e-3 * nb;
         if (eff > best) { best = eff; best_nb = nb; }
     }
 #define B200_GEMM(WM_, NB_) return launch_gemm<WM_, NB_>(st, Q, ldq, C, M, ldm, Nout, K, alpha, D, ldd)
@@ -844,7 +862,7 @@ struct BatchScratch {  // logistic partial results
 
 
 // ------------------------------------------------------------------------------------------------
-// tensor-core performance mode of the logistic GLM (tcgen05 + TMEM + TMA, split fp16): preparation and launch
+// tensor-core performance mode of the logistic GLM and the dense Gaussian (wgmma + TMA, split fp16): preparation and launch
 // ------------------------------------------------------------------------------------------------
 typedef CUresult (*b200_encode_tiled_fn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                          const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -917,11 +935,11 @@ static int gemm_nt_tc(b200_model* m, cudaStream_t st, const double* Q, long long
     if (make_tc_map(&a_hi, m->tc_a_hi, rows_pad, m->tc_kpad, kGtM) || make_tc_map(&a_lo, m->tc_a_lo, rows_pad, m->tc_kpad, kGtM)) return -1;
     GemmTcArgs G{};
     G.C = C; G.Nout = Nout; G.n_kblocks = (int)(m->tc_kpad / kGtKB); G.alpha = alpha; G.D = D; G.ldd = ldd;
-    G.n_tiles_n = (int)(m->tc_npad / kGtN);
-    G.n_tiles = G.n_tiles_n * (int)(rows_pad / kGtM);
+    G.n_tiles_m = (int)(rows_pad / kGtM);
+    G.n_tiles = G.n_tiles_m * (int)(m->tc_npad / kGtN);
     auto kern = gemm_tc_kernel;
     CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kGtSmemBytes));
-    const int grid = std::min(G.n_tiles, 148);
+    const int grid = std::min(G.n_tiles, sm_count(m->device));
     kern<<<grid, kGtThreads, kGtSmemBytes, st>>>(a_hi, a_lo, T.map_hi, T.map_lo, G);
     CU(cudaGetLastError());
     return 0;
@@ -942,7 +960,7 @@ static int prepare_logistic_tc(b200_model* m) {
     CU(cudaDeviceSynchronize());
     m->Xh = (const __half*)h;
     m->Xl = (const __half*)l;
-    void* y32 = nullptr;  // labels as fp32, padded to whole slabs: travel with the slab (logistic_tc2_kernel)
+    void* y32 = nullptr;  // labels as fp32, padded to whole slabs: travel with the slab (logistic_tc_kernel)
     CU(cudaMalloc(&y32, (size_t)rows_pad * sizeof(float)));
     m->owned.push_back(y32);
     logistic_tc_y_kernel<<<(unsigned)((rows_pad + 255) / 256), 256>>>(m->y8, m->n_rows, (float*)y32, rows_pad);
@@ -997,34 +1015,31 @@ static int batch_eval(b200_model* m, int C, const double* Q, double* G, double* 
     }
     // logistic: one fused pass over X, then the fixed-order reduction of the row-CTA partials
     const int cb = (C + kLogiChains - 1) / kLogiChains;
-    const long long n_slabs = (m->n_rows + kLogiRows - 1) / kLogiRows;
-    const int gx = (int)std::max<long long>(1, std::min<long long>(n_slabs, 148 / std::min(cb, 148)));
+    const int sms = sm_count(m->device);
+    const bool tc = m->precision == B200_PRECISION_TC_FP16X2;
+    // row-CTAs per chain block: one wave of CTAs over the SMs (the tensor-core kernel's CTA holds half a chain block)
+    const long long n_slabs = tc ? m->tc_slabs : (m->n_rows + kLogiRows - 1) / kLogiRows;
+    const int cta_per_block = tc ? kLogiChains / kTcChains : 1;
+    const int gx = (int)std::max<long long>(1, std::min<long long>(n_slabs, sms / std::min(cb * cta_per_block, sms)));
     bs.gx = gx;
     bs.cpad = cb * kLogiChains;
     if ((long long)gx * bs.cpad > bs.cap_rows) {
         if (bs.gpart.p) { cudaFree(bs.gpart.p); bs.gpart.p = nullptr; }
         if (bs.lpart.p) { cudaFree(bs.lpart.p); bs.lpart.p = nullptr; }
-        bs.cap_rows = std::max<long long>((long long)gx * bs.cpad, 148LL * kLogiChains);
+        bs.cap_rows = std::max<long long>((long long)gx * bs.cpad, (long long)sms * kLogiChains);
         CU(bs.gpart.alloc((size_t)bs.cap_rows * m->KP * sizeof(double)));
         CU(bs.lpart.alloc((size_t)bs.cap_rows * sizeof(double)));
     }
     int rc = 0;
-    if (m->precision == B200_PRECISION_TC_FP16X2) {
-        // tcgen05 path: the same partial-result layout ([gx][Cpad][128] fp64), so the fixed-order finish below is shared
+    if (tc) {
+        // wgmma path: the same partial-result layout ([gx][128][Cpad] fp64), so the fixed-order finish below is shared
         if (m->KP != kTcK) {  // partials are [.][.][KP]: the tensor-core kernel writes 128-wide rows
             return fail("tensor-core mode needs the 128-feature layout (65..128 features); this model has %d", m->n);
         }
-        if (env_int("B200_LOGI_TC_V", 2) == 1) {  // version 1 of the kernel (8 epilogue warps, drains through global memory)
-            auto kern = logistic_tc_kernel;
-            CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmemBytes));
-            LogisticTcArgs A{m->y8, m->n_rows, m->tc_slabs, Q, ld, C, m->n, bs.gpart.as<double>(), bs.lpart.as<double>(), bs.cpad};
-            kern<<<dim3(bs.gx, bs.cpad / kLogiChains), kTcThreads, kTcSmemBytes, st>>>(m->map_hi, m->map_lo, A);
-        } else {
-            auto kern = logistic_tc2_kernel;
-            CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTc2SmemBytes));
-            LogisticTc2Args A{m->y32, m->n_rows, m->tc_slabs, Q, ld, C, m->n, bs.gpart.as<double>(), bs.lpart.as<double>(), bs.cpad};
-            kern<<<dim3(bs.gx, bs.cpad / kLogiChains), kTc2Threads, kTc2SmemBytes, st>>>(m->map_hi, m->map_lo, A);
-        }
+        auto kern = logistic_tc_kernel;
+        CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmemBytes));
+        LogisticTcArgs A{m->y32, m->n_rows, m->tc_slabs, Q, ld, C, m->n, bs.gpart.as<double>(), bs.lpart.as<double>(), bs.cpad};
+        kern<<<dim3(bs.gx, bs.cpad / kTcChains), kTcThreads, kTcSmemBytes, st>>>(m->map_hi, m->map_lo, A);
         CU(cudaGetLastError());
     } else
     switch (m->KP) {
@@ -1114,7 +1129,7 @@ static int run_lockstep(b200_model* m, LsDev P, cudaStream_t st) {
         P.fa_raw = reinterpret_cast<double*>(take(2 * b_fa));
     }
     // the padding columns of the request / result matrices must be zero (they are inside the GEMMs' k range) and the chain
-    // vectors start from zero: clearing is bandwidth-trivial (2.6 GB at HBM speed = 0.4 ms), unlike allocating
+    // vectors start from zero: clearing runs at HBM bandwidth, unlike allocating
     CU(cudaMemsetAsync(P.vecs, 0, b_vecs + n_mats * b_mat, st));
     P.logp_from_dot = (m->kind == B200_MODEL_MVGAUSS) ? 1 : 0;
     P.logp_const = m->logp_const;
@@ -1205,7 +1220,7 @@ struct NutsLaunch {
     int operator()(const typename Model::Params& MP) {
         constexpr int NP = 32 * W * NPL;
         constexpr bool SUBS = (W > 1) ? true : (B200_SUBTREE_SMEM != 0);
-        int wpb = (W == 1) ? env_int("B200_NUTS_WPB", 8) : 1;  // chains per CTA (8 warps, 1 CTA per SM: measured best, r2)
+        int wpb = (W == 1) ? env_int("B200_NUTS_WPB", 8) : 1;  // chains per CTA: 8 warps, 1 CTA per SM (see seg below)
         int hot = env_int("B200_NUTS_HOT", (W == 1) ? 2 : 1);
         wpb = std::max(1, std::min(wpb, B200_NUTS_THREADS / 32));
         hot = std::max(0, std::min(hot, P.max_td));
@@ -1233,7 +1248,7 @@ struct NutsLaunch {
         CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         // persistent grid: every CTA resident (teams take (chain, segment) units from the ticket counter)
         const int threads = (W == 1) ? wpb * 32 : 32 * W;
-        int per_sm = 0, sms = 148;
+        int per_sm = 0, sms = 0;
         CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem));
         CU(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, m->device));
         const int need = (P.C + wpb - 1) / wpb;
@@ -1241,7 +1256,8 @@ struct NutsLaunch {
         // iterations per work unit: fine enough to balance chains of different cost, coarse enough that the ~3 KB state
         // hand-over per unit is noise.  One unit per chain when every chain has its own resident team anyway.
         const int Ttot = P.n_iter;
-        int seg = env_int("B200_NUTS_SEG", 50);  // measured (r2): 10 -> 390 ms, 25 -> 370, 50 -> 361, 100 -> 367
+        int seg = env_int("B200_NUTS_SEG", 100);  // Radon bench step on an H100 SXM (700 W), wpb 8 / 4 / 2: seg 25 -> 377 / 386 / 391 ms,
+        // 50 -> 371 / 380 / 385, 100 -> 368 / 378 / 383, 200 -> 369 / 378 / 383 (medians of 3; the draws are identical)
         if (seg <= 0 || need <= blocks) seg = Ttot;
         P.seg_iters = std::max(1, std::min(seg, Ttot));
         typename Model::Params MPl;
@@ -1318,8 +1334,8 @@ extern "C" int b200_nuts_run(b200_model* m, const b200_nuts_cfg* cfg, const doub
     const size_t vb = (size_t)C * n * sizeof(double);
     Staged s_q0, s_var0, s_mean0, s_eps0, s_rng, s_z, s_draws;
     // Device staging of host arrays comes from ONE arena kept in the model handle: a steady-state call makes no cudaMalloc /
-    // cudaFree at all (measured on the bench boxes, call 8 of round 2: the per-call allocations of five small input arrays
-    // cost 0.2-90 ms, and a public-API call took 20-770 ms longer than its kernel).  Everything except the draws (direct
+    // cudaFree at all (per-call allocations of the small input arrays synchronise the device and make a public-API call
+    // take far longer than its kernel).  Everything except the draws (direct
     // host writes, or their own buffer) and a host momentum buffer (parity tests) is lent from it.
     const size_t ct_all = (size_t)C * (size_t)std::max<long long>(0, it0 + Ttot - rec_lo);
     char* lend_p = nullptr;
@@ -1458,8 +1474,6 @@ extern "C" int b200_nuts_run(b200_model* m, const b200_nuts_cfg* cfg, const doub
         if (run_lockstep(m, Q, st)) return -1;
     } else {
         NutsLaunch L{m, P, st};
-        // (a chain of the stochastic-volatility model spread over 16 warps instead of 8 was measured and rejected: 16.0 M vs
-        // 17.5 M grad-evals/s, the extra cross-warp reduction traffic outweighs the halved per-thread work; profiles/r2_variants.md)
         if (dispatch(m, L)) return -1;
     }
 
@@ -1492,7 +1506,7 @@ extern "C" int b200_pointwise_loglik(b200_model* m, int32_t lik, const double* d
         stage_in(s_out, out, (size_t)D * (size_t)L.N * sizeof(double), mem, false, true, st))
         return -1;
     const int wpb = 8;
-    const int blocks = (int)std::max<long long>(1, std::min<long long>((D + wpb - 1) / wpb, 148 * 8));
+    const int blocks = (int)std::max<long long>(1, std::min<long long>((D + wpb - 1) / wpb, sm_count(m->device) * 8));
     CU(m->ensure_ir_scratch((long long)blocks * wpb));
     Timer t(st);
     ir_pointwise_kernel<<<blocks, wpb * 32, 0, st>>>(m->ir, lik, D, (const double*)s_in.ptr(), (double*)s_out.ptr());
@@ -1525,7 +1539,7 @@ __global__ void __launch_bounds__(256) dfma_peak_kernel(double* out, int iters) 
 
 extern "C" int b200_measure_fp64_tflops(double* tflops) {
     if (!tflops) return fail("null argument");
-    const int blocks = 148 * 8, threads = 256, iters = 1 << 14;
+    const int blocks = current_sm_count() * 8, threads = 256, iters = 1 << 14;
     DevBuf out;
     CU(out.alloc((size_t)blocks * threads * sizeof(double)));
     dfma_peak_kernel<<<blocks, threads>>>(out.as<double>(), 64);
@@ -1563,7 +1577,7 @@ __global__ void __launch_bounds__(256) dmma_peak_kernel(double* out, int iters) 
 
 extern "C" int b200_measure_dmma_tflops(double* tflops) {
     if (!tflops) return fail("null argument");
-    const int blocks = 148 * 2, threads = 256, iters = 1 << 12;
+    const int blocks = current_sm_count() * 2, threads = 256, iters = 1 << 12;
     DevBuf out;
     CU(out.alloc((size_t)blocks * threads * sizeof(double)));
     dmma_peak_kernel<<<blocks, threads>>>(out.as<double>(), 16);

@@ -1,7 +1,6 @@
 // Dense fp64 contractions of the GEMM-shaped models, hand-written on the fp64 tensor-core path
-// (mma.sync.aligned.m8n8k4.f64, SASS DMMA.8x8x4; tcgen05 has no fp64 kind).  Measured on B200 (scripts/mb):
-// DMMA sustains 37.0 TFLOP/s = the DFMA peak (the fp64 pipe is the roof either way), but needs 1/8 of the issue
-// slots and no register-operand bandwidth, which leaves room for the shared-memory fragment loads.
+// (mma.sync.aligned.m8n8k4.f64, SASS DMMA.8x8x4; the fp16 tensor-core instructions have no fp64 kind).  DMMA needs 1/8 of
+// the issue slots of DFMA and no register-operand bandwidth, which leaves room for the shared-memory fragment loads.
 //
 //   gemm_nt_dmma_kernel     D[C][Nout] = alpha * Q[C][K] . M[Nout][K]^T        (config 5: grad = -P q, w = Sigma g,
 //                                                                              p0 = L^-T z, v0 = L z; chains are rows)
@@ -155,8 +154,8 @@ __host__ __device__ constexpr size_t logistic_smem_bytes() {
 }
 
 #ifndef B200_LOGI_MB
-#define B200_LOGI_MB 1  // 8-chain accumulator blocks per warp: 1 -> 16 warps x 8 chains per CTA (126 regs, 4 warps per scheduler:
-                        // 10.8 ms per 512-chain batch), 2 -> 8 warps x 16 chains (212 regs, 12.4 ms)
+#define B200_LOGI_MB 1  // 8-chain accumulator blocks per warp: 1 -> 16 warps x 8 chains per CTA (126 regs, 4 warps per
+                        // scheduler), 2 -> 8 warps x 16 chains (212 regs)
 #endif
 template <int KB, int MB = B200_LOGI_MB>
 __global__ void __launch_bounds__(32 * (kLogiChains / (8 * MB)), 1)
@@ -244,7 +243,7 @@ __global__ void __launch_bounds__(32 * (kLogiChains / (8 * MB)), 1)
                     const double ex = exp(-fabs(x));
                     const double rr = 1.0 / (1.0 + ex);
                     const double sg = x >= 0 ? rr : ex * rr;                 // sigmoid(x)
-                    const double sp = fmax(x, 0.0) + log1p(ex);             // softplus(x); log(1 + e) instead: no gain measured (r2)
+                    const double sp = fmax(x, 0.0) + log1p(ex);             // softplus(x)
                     lp[mb] += live ? fma(yi, x, -sp) : 0.0;
                     E[mb][nb][s] = live ? yi - sg : 0.0;
                 }
@@ -310,8 +309,7 @@ __global__ void __launch_bounds__(128) logistic_finish_kernel(const double* __re
 }
 
 // The same reduction for FEATURE-major partials Gpart[p][k][c] (the tensor-core kernels' layout: chains contiguous).  The
-// kernel above walks them with lane = feature, i.e. with a stride of Cpad doubles (measured: 74 us per 512-chain batch, 16 % of
-// the tensor-core lock-step loop, profiles/r2l_launches_logistic_tc_summary.csv).  Here a CTA owns a 32-chain x 16-feature tile:
+// kernel above walks them with lane = feature, i.e. with a stride of Cpad doubles.  Here a CTA owns a 32-chain x 16-feature tile:
 // lane = chain while summing (coalesced, 4 independent partial loads in flight per thread, the same fixed order over p as
 // above, so the same bits), a shared-memory transpose for the row-major gradient, and the blockIdx.y == 0 CTAs also produce
 // logp with the arithmetic of the kernel above.

@@ -38,8 +38,7 @@ constexpr int kLsLevels = 12;
 
 // A pass over a chain's vectors in tiles of U elements per thread: ALL loads of a tile, then the arithmetic and the stores.
 // Written as `for (i) { load; store; }` the compiler must keep every load behind the previous iteration's store (the vectors
-// are slots of one allocation, so it cannot rule out aliasing), and the pass runs one DRAM latency per element: measured
-// 1.3 TB/s for ls_advance_kernel<16> at n = 10^4 (profiles/r2_tc_launches_mvgauss_tc_summary.csv).  Element order per thread is
+// are slots of one allocation, so it cannot rule out aliasing), and the pass runs one DRAM latency per element.  Element order per thread is
 // unchanged (i = lane, lane + TS, ...), so every per-thread partial sum keeps its bits.
 template <int U, int TS, class Load, class Store>
 __device__ __forceinline__ void ls_tiled(int lane, int n, Load&& load, Store&& store) {

@@ -1,25 +1,23 @@
-// Logistic GLM, tensor-core PERFORMANCE mode (BASELINE config 3; VERDICT r1 item N2): the two contractions of one batched
-// leapfrog,  eta = X beta  and  G = X^T (y - sigmoid(eta)),  on the 5th-generation tensor cores (tcgen05.mma, accumulators
-// in TMEM, operands staged by TMA) instead of the fp64 DMMA path of dense.cuh.
+// Logistic GLM, tensor-core PERFORMANCE mode (BASELINE config 3): the two contractions of one batched leapfrog,
+// eta = X beta  and  G = X^T (y - sigmoid(eta)),  on the Hopper tensor cores (wgmma.mma_async, operands staged in shared
+// memory by TMA) instead of the fp64 DMMA path of dense.cuh.
 //
-// tcgen05 has no fp64 kind, so every fp64 operand is split into two fp16 pieces, v = hi + lo with hi = fp16(v) and
+// wgmma has no fp64 kind, so every fp64 operand is split into two fp16 pieces, v = hi + lo with hi = fp16(v) and
 // lo = fp16(v - hi) (22 significant bits; absolute floor 2^-25 where lo is subnormal), and a product is evaluated as
-// hi*hi + hi*lo + lo*hi in three kind::f16 MMAs with fp32 accumulation (the lo*lo term is below 2^-22 relative).
-// fp32 accumulators only ever cover one slab: X beta sums K = 128 terms, and the gradient accumulator in TMEM is drained
-// into fp64 after every 128-row slab, so neither fp32 rounding nor the tensor cores' one-sided accumulate rounding builds up.
-// Accuracy against the fp64 path is measured by tests/test_gpu_tc.py and reported in profiles/ (parity report).  The fp64
-// DMMA kernel stays the parity mode.
+// hi*hi + hi*lo + lo*hi in three f16 MMAs with fp32 accumulation (the lo*lo term is below 2^-22 relative).
+// fp32 accumulators only ever cover a bounded number of terms: X beta sums K = 128 terms, and the gradient accumulator is
+// drained into fp64 registers every kTcDrain slabs, so fp32 rounding does not build up over the rows of X.  The small
+// correction products (hi*lo, lo*hi) are issued first, while the accumulator is still small, and hi*hi last.
+// Accuracy against the fp64 path is measured by tests/test_gpu_tc.py.  The fp64 DMMA kernel stays the parity mode.
 //
-// One CTA = 128 chains x a strided set of 128-row slabs of X.  Per slab (FlashAttention-shaped, P kept in TMEM):
-//   TMA   : X_hi, X_lo slab [128 rows][128 features] fp16 -> smem (SWIZZLE_128B, two 64-column boxes each), 2 stages
-//   GEMM 1: D1[c][i] = sum_k beta[c][k] X[i][k]     A = beta pieces (smem, K-major), B = X pieces (smem, K-major)
-//   epilog: thread c (TMEM lane c) reads its 128 eta values (tcgen05.ld), computes r = y - sigmoid(eta) and the
-//           log-likelihood terms in fp32, splits r into fp16 pieces and writes them back to TMEM (tcgen05.st)
-//   GEMM 2: D2[c][k] += sum_i r[c][i] X[i][k]        A = r pieces (TMEM), B = the SAME X bytes read MN-major
-// Warp roles: warp 0 = TMA producer, warp 1 = MMA issuer (one elected lane), warps 2..9 = epilogue (two per TMEM
-// subpartition, 64 rows of the slab each: the elementwise sigmoid / softplus work is what bounds the kernel, so it gets two
-// warps per scheduler).  D1 is double-buffered so GEMM 1 of slab s+1 runs under the epilogue of slab s.
-// TMEM columns (512): D1[0] 0..127, D1[1] 128..255, D2 256..383, r_hi 384..447, r_lo 448..511.
+// One CTA = 64 chains x a strided set of 128-row slabs of X; two consumer warpgroups and a producer warp.  Per slab:
+//   TMA   : X_hi, X_lo slab [128 rows][128 features] fp16 -> smem (SWIZZLE_128B, two 64-column boxes each) + the slab's
+//           128 labels (fp32), 2 stages
+//   GEMM 1: warpgroup w: eta[c][i] = sum_k beta[c][k] X[i][k] for the slab rows 64w..64w+63 (m64n64k16; A = beta pieces,
+//           B = X pieces, both K-major in smem); r = y - sigmoid(eta) and the log-likelihood terms from the accumulator
+//           registers, in fp32; r split into fp16 pieces and stored as K-major tile [64 chains][128 rows] in smem
+//   GEMM 2: warpgroup w: G[c][k] += sum_i r[c][i] X[i][k] for the features 64w..64w+63 (A = r pieces, B = the SAME X
+//           bytes read MN-major: box w of the stage)
 #pragma once
 #include <cuda.h>
 #include <cuda_fp16.h>
@@ -28,17 +26,21 @@
 
 namespace b200 {
 
-constexpr int kTcRows = 128;      // rows of X per slab (N of GEMM 1, K of GEMM 2)
-constexpr int kTcChains = 128;    // chains per CTA (M of both GEMMs = TMEM lanes)
+constexpr int kTcRows = 128;      // rows of X per slab (N of GEMM 1 over both warpgroups, K of GEMM 2)
+constexpr int kTcChains = 64;     // chains per CTA (M of both GEMMs)
 constexpr int kTcK = 128;         // features (padded)
 constexpr int kTcStages = 2;      // X slab stages in shared memory
-constexpr int kTcThreads = 320;   // 10 warps: TMA producer, MMA issuer, 8 epilogue
-constexpr int kTcEpiThreads = 256;
-constexpr int kTcDrain = 2;       // slabs per fp32 gradient accumulation chunk (16 full-magnitude accumulate steps)
+constexpr int kTcConsumers = 256; // two warpgroups
+constexpr int kTcThreads = 32 + kTcConsumers;  // producer warp + consumers
+constexpr int kTcDrain = 2;       // slabs per fp32 gradient accumulation chunk
 constexpr uint32_t kTcBlockBytes = kTcRows * 64 * 2;          // one [128 rows][64 cols] fp16 box = 16 KB
-constexpr uint32_t kTcPieceBytes = 2 * kTcBlockBytes;         // one piece of a [128][128] tile = 32 KB
+constexpr uint32_t kTcPieceBytes = 2 * kTcBlockBytes;         // one piece of a [128][128] slab = 32 KB
 constexpr uint32_t kTcStageBytes = 2 * kTcPieceBytes;         // X_hi + X_lo = 64 KB
-constexpr size_t kTcSmemBytes = 1024 /*align*/ + 2 * kTcPieceBytes /*beta hi, lo*/ + kTcStages * kTcStageBytes + 256 /*barriers*/;
+constexpr uint32_t kTcABlockBytes = kTcChains * 64 * 2;       // one [64 chains][64 k] fp16 box = 8 KB
+constexpr uint32_t kTcAPieceBytes = 2 * kTcABlockBytes;       // one piece of a [64][128] operand tile = 16 KB
+constexpr uint32_t kTcYBytes = kTcRows * sizeof(float);
+constexpr size_t kTcSmemBytes = 1024 /*align*/ + 2 * kTcAPieceBytes /*beta*/ + 2 * kTcAPieceBytes /*r*/ +
+                                kTcStages * kTcStageBytes + kTcStages * kTcYBytes + 256 /*barriers*/;
 
 // ---- raw PTX wrappers ------------------------------------------------------------------------------------------------
 __device__ __forceinline__ void tc_mbar_arrive(uint64_t* bar) {
@@ -64,388 +66,57 @@ __device__ __forceinline__ void tc_tma_load_2d(void* dst, const CUtensorMap* map
         "l"(map), "r"(c0), "r"(c1), "r"(smem_u32(bar))
         : "memory");
 }
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint64_t* bar) {  // arrives on `bar` when every MMA issued so far has completed
-    asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-// D[tmem] (+)= A[smem] . B[smem]
-__device__ __forceinline__ void tc_mma_ss(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// D[tmem] (+)= A[tmem] . B[smem]
-__device__ __forceinline__ void tc_mma_ts(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n"
-        "}\n" ::"r"(d_tmem),
-        "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-// 32 consecutive TMEM columns of this thread's lane -> 32 registers
-__device__ __forceinline__ void tc_ld32(uint32_t taddr, uint32_t (&v)[32]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-          "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]), "=r"(v[17]), "=r"(v[18]),
-          "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]),
-          "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-        : "r"(taddr)
-        : "memory");
-}
-__device__ __forceinline__ void tc_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tc_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-// 16 registers -> 16 consecutive TMEM columns of this thread's lane
-__device__ __forceinline__ void tc_st16(uint32_t taddr, const uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], "
-        "{%1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16};" ::"r"(taddr),
-        "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]), "r"(v[8]), "r"(v[9]), "r"(v[10]),
-        "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15])
-        : "memory");
-}
+__device__ __forceinline__ void wg_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wg_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// the consumer warpgroups only (named barrier 1)
+__device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 1, %0;" ::"r"(kTcConsumers) : "memory"); }
 
-// shared-memory matrix descriptor (cute::UMMA::SmemDescriptor, mma_sm100_desc.hpp): start address, leading / stride byte
-// offsets (all >> 4), version 1 (Blackwell) at bit 46, layout type SWIZZLE_128B = 2 at bits 61..63
-__device__ __forceinline__ uint64_t tc_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
+// shared-memory matrix descriptor of wgmma (cute::GMMA::GmmaDescriptor): start address, leading / stride byte offsets
+// (all >> 4), layout type SWIZZLE_128B = 1 at bits 62..63
+__device__ __forceinline__ uint64_t wg_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
     return (uint64_t)((saddr & 0x3FFFF) >> 4) | ((uint64_t)(lbo_bytes >> 4) << 16) | ((uint64_t)(sbo_bytes >> 4) << 32) |
-           (1ull << 46) | (2ull << 61);
+           (1ull << 62);
 }
-// instruction descriptor (cute::UMMA::InstrDescriptor): D = F32 (bits 4..5 = 1), A = B = F16 (formats 0), N >> 3 at bit 17,
-// M >> 4 at bit 24; bit 16 = B is MN-major
-constexpr uint32_t kTcIdesc = (1u << 4) | ((uint32_t)(kTcRows >> 3) << 17) | ((uint32_t)(kTcChains >> 4) << 24);
-constexpr uint32_t kTcIdescBmn = kTcIdesc | (1u << 16);
 
-// byte offset of element (row r, column k) of a [128][128] fp16 tile stored as two [128][64] blocks, rows 128 B apart,
-// 16-byte chunks XOR-swizzled with the row (SWIZZLE_128B: what TMA writes and what the descriptors above describe)
-__device__ __forceinline__ uint32_t tc_tile_off(int r, int k) {
+// D[64][64] (+)= A[64][16] . B[16][64], fp16 operands from shared memory, fp32 accumulators in registers.
+// TRANS_B = 0: B is K-major ([n][k] in memory); 1: B is MN-major ([k][n]).  scale_d = 0 overwrites D.
+// Accumulator layout (per thread of the warpgroup, warp w, lane l): d[4j + h] is row 16w + l/4 + 8 (h >> 1), column
+// 8j + 2 (l % 4) + (h & 1).
+template <int TRANS_B>
+__device__ __forceinline__ void wg_mma_n64(float (&d)[32], uint64_t a_desc, uint64_t b_desc, int scale_d) {
+    asm volatile(
+        "{\n"
+        ".reg .pred p;\n"
+        "setp.ne.b32 p, %34, 0;\n"
+        "wgmma.mma_async.sync.aligned.m64n64k16.f32.f16.f16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
+        "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, "
+        "%32, %33, p, 1, 1, 0, %35;\n"
+        "}\n"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]),
+          "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]),
+          "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]),
+          "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+        : "l"(a_desc), "l"(b_desc), "r"(scale_d), "n"(TRANS_B)
+        : "memory");
+}
+
+// byte offset of element (row r, column k) of a [rows][128] fp16 tile stored as two [rows][64] blocks of block_bytes,
+// rows 128 B apart, 16-byte chunks XOR-swizzled with the row (SWIZZLE_128B: what TMA writes and what wg_desc describes)
+__device__ __forceinline__ uint32_t tc_tile_off(int r, int k, uint32_t block_bytes) {
     const int blk = k >> 6, kk = k & 63;
-    return (uint32_t)(blk * kTcBlockBytes + r * 128 + ((((kk >> 3) ^ (r & 7)) << 4) | ((kk & 7) << 1)));
+    return (uint32_t)(blk * block_bytes + r * 128 + ((((kk >> 3) ^ (r & 7)) << 4) | ((kk & 7) << 1)));
 }
-
-struct LogisticTcArgs {
-    const uint8_t* y;        // [N]
-    long long N;             // true rows
-    long long n_slabs;       // ceil(N / 128); X pieces are allocated with n_slabs * 128 rows (zero padded)
-    const double* Q;         // [C][ldq] beta per chain
-    long long ldq;
-    int C, K;
-    double* Gpart;           // [gridDim.x][128 features][Cpad]  (feature-major, see the drain)
-    double* lpart;           // [gridDim.x][Cpad]
-    int Cpad;
-};
-
-// Accumulation order and drain period are dictated by the tensor cores' fp32 accumulate, which rounds toward zero: every
-// tcgen05.mma into an accumulator of magnitude |D| loses ~2^-25 |D| one-sidedly (measured, round 2 call 3: 24 accumulate
-// steps per slab -> 8e-7, 384 steps -> 7.9e-6 relative).  So (i) the small correction products hi*lo and lo*hi are issued
-// FIRST, while the accumulator is still tiny, and hi*hi last: 8 full-magnitude steps per GEMM instead of 24; (ii) the
-// gradient accumulator is drained into fp64 every kTcDrain = 2 slabs.
-__global__ void __launch_bounds__(kTcThreads, 1)
-    logistic_tc_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ CUtensorMap map_lo, const LogisticTcArgs A) {
-    extern __shared__ char tc_smem_raw[];
-    char* base = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(tc_smem_raw) + 1023) & ~(uintptr_t)1023);
-    char* beta_s = base;                                   // [hi | lo] pieces, 32 KB each
-    char* x_s = base + 2 * kTcPieceBytes;                  // stages x [X_hi | X_lo]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(x_s + kTcStages * kTcStageBytes);
-    uint64_t* x_full = bars;          // [2] TMA -> MMA
-    uint64_t* x_empty = bars + 2;     // [2] MMA (GEMM 2 done) -> TMA
-    uint64_t* eta_full = bars + 4;    // [2] MMA (GEMM 1 done) -> epilogue
-    uint64_t* eta_empty = bars + 6;   // [2] epilogue (D1 read) -> MMA
-    uint64_t* r_full = bars + 8;      // epilogue (r written) -> MMA
-    uint64_t* r_empty = bars + 9;     // MMA (GEMM 2 done: r and the X stage are free) -> epilogue
-    uint64_t* g_full = bars + 10;     // MMA (drain point reached: D2 holds kTcDrain slabs) -> epilogue
-    uint64_t* g_empty = bars + 11;    // epilogue (D2 drained) -> MMA
-    __shared__ uint32_t tmem_base_s;
-    __shared__ double lp_half_s[kTcChains];
-
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-    const int c_base = blockIdx.y * kTcChains;
-    // slabs of this CTA: blockIdx.x, blockIdx.x + gridDim.x, ...
-    const long long my_slabs = (A.n_slabs > blockIdx.x) ? (A.n_slabs - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
-
-    if (tid == 0) {
-        for (int i = 0; i < 2; ++i) {
-            mbar_init(&x_full[i], 1);
-            mbar_init(&x_empty[i], 1);
-            mbar_init(&eta_full[i], 1);
-            mbar_init(&eta_empty[i], kTcEpiThreads);
-        }
-        mbar_init(r_full, kTcEpiThreads);
-        mbar_init(r_empty, 1);
-        mbar_init(g_full, 1);
-        mbar_init(g_empty, kTcEpiThreads);
-    }
-    if (warp == 1) {  // TMEM: all 512 columns (1 CTA per SM by construction: 193 KB of shared memory)
-        const uint32_t ncols = 512;
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)), "r"(ncols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    // beta pieces: fp64 -> fp16 hi / lo, written in the K-major SWIZZLE_128B image GEMM 1 reads as operand A
-    for (int e = tid; e < kTcChains * kTcK; e += kTcThreads) {
-        const int c = e >> 7, k = e & 127;
-        const double v = (c_base + c < A.C && k < A.K) ? A.Q[(long long)(c_base + c) * A.ldq + k] : 0.0;
-        const __half hi = __double2half(v);
-        const __half lo = __double2half(v - (double)__half2float(hi));
-        const uint32_t off = tc_tile_off(c, k);
-        *reinterpret_cast<__half*>(beta_s + off) = hi;
-        *reinterpret_cast<__half*>(beta_s + kTcPieceBytes + off) = lo;
-    }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes of beta -> visible to the MMA (async proxy)
-    tc_fence_before();
-    __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = tmem_base_s;
-    const uint32_t tD1[2] = {tmem + 0, tmem + 128}, tD2 = tmem + 256, tRh = tmem + 384, tRl = tmem + 448;
-
-    if (warp == 0) {
-        // ===== TMA producer =====
-        if (lane == 0) {
-            for (long long s = 0; s < my_slabs; ++s) {
-                const int st = (int)(s % kTcStages);
-                if (s >= kTcStages) tc_mbar_wait(&x_empty[st], (uint32_t)(((s / kTcStages) - 1) & 1));
-                const long long slab = blockIdx.x + s * gridDim.x;
-                const int row0 = (int)(slab * kTcRows);
-                char* dst = x_s + st * kTcStageBytes;
-                mbar_expect_tx(&x_full[st], kTcStageBytes);
-                tc_tma_load_2d(dst, &map_hi, 0, row0, &x_full[st]);
-                tc_tma_load_2d(dst + kTcBlockBytes, &map_hi, 64, row0, &x_full[st]);
-                tc_tma_load_2d(dst + kTcPieceBytes, &map_lo, 0, row0, &x_full[st]);
-                tc_tma_load_2d(dst + kTcPieceBytes + kTcBlockBytes, &map_lo, 64, row0, &x_full[st]);
-            }
-        }
-    } else if (warp == 1) {
-        // ===== MMA issuer (one lane) =====
-        if (lane == 0) {
-            const uint32_t beta_a = smem_u32(beta_s);
-            auto gemm1 = [&](long long s) {  // D1[s & 1] = beta . X^T   (3 products x 8 k-steps, small products first)
-                const int st = (int)(s % kTcStages), b = (int)(s & 1);
-                tc_mbar_wait(&x_full[st], (uint32_t)((s / kTcStages) & 1));
-                if (s >= 2) tc_mbar_wait(&eta_empty[b], (uint32_t)(((s >> 1) - 1) & 1));
-                tc_fence_after();
-                const uint32_t xa = smem_u32(x_s + st * kTcStageBytes);
-                uint32_t acc = 0;
-#pragma unroll
-                for (int prod = 0; prod < 3; ++prod) {  // hi*lo, lo*hi, hi*hi
-                    const uint32_t a0 = beta_a + (prod == 1 ? kTcPieceBytes : 0);
-                    const uint32_t b0 = xa + (prod == 0 ? kTcPieceBytes : 0);
-#pragma unroll
-                    for (int ks = 0; ks < 8; ++ks) {
-                        const uint32_t o = (uint32_t)((ks >> 2) * kTcBlockBytes + (ks & 3) * 32);
-                        tc_mma_ss(tD1[b], tc_desc(a0 + o, 16, 1024), tc_desc(b0 + o, 16, 1024), kTcIdesc, acc);
-                        acc = 1;
-                    }
-                }
-                tc_commit(&eta_full[b]);
-            };
-            if (my_slabs > 0) gemm1(0);
-            for (long long s = 0; s < my_slabs; ++s) {
-                if (s + 1 < my_slabs) gemm1(s + 1);
-                // GEMM 2 of slab s: D2 = r . X   (A = r pieces in TMEM, B = X pieces read MN-major); D2 was drained
-                tc_mbar_wait(r_full, (uint32_t)(s & 1));
-                const bool first = (s % kTcDrain) == 0;   // D2 was drained before this slab
-                if (first && s > 0) tc_mbar_wait(g_empty, (uint32_t)(((s / kTcDrain) - 1) & 1));
-                tc_fence_after();
-                const int st = (int)(s % kTcStages);
-                const uint32_t xa = smem_u32(x_s + st * kTcStageBytes);
-                uint32_t acc = first ? 0u : 1u;
-#pragma unroll
-                for (int prod = 0; prod < 3; ++prod) {  // r_hi X_lo, r_lo X_hi, r_hi X_hi
-                    const uint32_t ta = (prod == 1) ? tRl : tRh;
-                    const uint32_t b0 = xa + (prod == 0 ? kTcPieceBytes : 0);
-#pragma unroll
-                    for (int ks = 0; ks < 8; ++ks) {  // 16 rows of the slab per step: 2 KB of each 64-column block
-                        tc_mma_ts(tD2, ta + ks * 8, tc_desc(b0 + ks * 2048, kTcBlockBytes, 1024), kTcIdescBmn, acc);
-                        acc = 1;
-                    }
-                }
-                tc_commit(&x_empty[st]);
-                tc_commit(r_empty);
-                if ((s + 1) % kTcDrain == 0 || s + 1 == my_slabs) tc_commit(g_full);
-            }
-        }
-    } else {
-        // ===== epilogue: 8 warps; TMEM lane = chain (subpartition = warp % 4), the two warps of a subpartition split the
-        //       slab's 128 rows (and the 128 gradient columns of a drain) in halves =====
-        const int sub = warp & 3, half = (warp - 2) >> 2;
-        const int c = sub * 32 + lane;                       // chain inside the CTA = TMEM lane
-        const uint32_t lane_addr = (uint32_t)(sub * 32) << 16;
-        double lp = 0.0;
-        // this CTA's fp64 partial gradient, FEATURE-major [128 k][Cpad chains]: for a fixed k the 32 lanes of a warp touch 32
-        // consecutive chains (coalesced read-modify-write in L2; the chain-major layout cost 5 ms per batch, measured)
-        double* gp = A.Gpart + ((long long)blockIdx.x * kTcK + half * 64) * A.Cpad + c_base + c;
-        bool g_first = true;
-        long long n_drains = 0;
-        auto drain = [&]() {  // fp32 gradient accumulator -> fp64 partial
-            tc_mbar_wait(g_full, (uint32_t)(n_drains & 1));
-            tc_fence_after();
-#pragma unroll 1
-            for (int j = 0; j < 2; ++j) {
-                uint32_t v[32];
-                tc_ld32(tD2 + lane_addr + half * 64 + j * 32, v);
-                tc_wait_ld();
-#pragma unroll
-                for (int k = 0; k < 32; ++k) {
-                    const double add = (double)__uint_as_float(v[k]);
-                    double* e = gp + (long long)(j * 32 + k) * A.Cpad;
-                    *e = g_first ? add : *e + add;
-                }
-            }
-            g_first = false;
-            ++n_drains;
-            tc_fence_before();
-            tc_mbar_arrive(g_empty);
-        };
-        for (long long s = 0; s < my_slabs; ++s) {
-            const int b = (int)(s & 1);
-            const long long row0 = (blockIdx.x + s * gridDim.x) * kTcRows + half * 64;
-            tc_mbar_wait(&eta_full[b], (uint32_t)((s >> 1) & 1));
-            tc_fence_after();
-            float lp_s = 0.f;
-            uint32_t rh[2][16], rl[2][16];
-#pragma unroll
-            for (int j = 0; j < 2; ++j) {  // 32 rows of the slab at a time
-                uint32_t v[32];
-                tc_ld32(tD1[b] + lane_addr + half * 64 + j * 32, v);
-                tc_wait_ld();
-                if (j == 1) {  // this thread's share of D1[b] has been read: GEMM 1 of slab s + 2 may overwrite it
-                    tc_fence_before();
-                    tc_mbar_arrive(&eta_empty[b]);
-                }
-                const long long r_base = row0 + j * 32;
-                // y of these 32 rows: one 32-byte global read, the same address for every thread (L1 broadcast)
-                uint32_t yw[8];
-                if (r_base + 32 <= A.N && ((uintptr_t)(A.y + r_base) & 3) == 0) {
-#pragma unroll
-                    for (int w = 0; w < 8; ++w) yw[w] = __ldg(reinterpret_cast<const uint32_t*>(A.y + r_base) + w);
-                } else {
-#pragma unroll
-                    for (int w = 0; w < 8; ++w) {
-                        uint32_t p = 0;
-                        for (int bb = 0; bb < 4; ++bb) {
-                            const long long rr = r_base + 4 * w + bb;
-                            p |= (uint32_t)(rr < A.N ? A.y[rr] : 0) << (8 * bb);
-                        }
-                        yw[w] = p;
-                    }
-                }
-#pragma unroll
-                for (int i = 0; i < 32; i += 2) {
-                    float rr[2];
-#pragma unroll
-                    for (int u = 0; u < 2; ++u) {
-                        const float x = __uint_as_float(v[i + u]);
-                        const float yi = (float)((yw[(i + u) >> 2] >> (8 * ((i + u) & 3))) & 0xff);
-                        const bool live = r_base + i + u < A.N;
-                        const float e = __expf(-fabsf(x));                     // 2 ulp: unbiased, enters sigmoid and log1p only
-                        const float inv = __fdividef(1.f, 1.f + e);
-                        const float sg = x >= 0.f ? inv : e * inv;            // sigmoid(x)
-                        // softplus(x) = max(x, 0) + log(1 + e), 1 + e in (1, 2]: lg2.approx there is good to 2^-22 absolute, four
-                        // times coarser than log1pf but 25 instructions cheaper per element (the epilogue bounds this kernel);
-                        // summed over 1e6 rows that is ~3e-10 of logp, far below the tensor cores' accumulate rounding (1.5e-7)
-                        const float sp = fmaxf(x, 0.f) + __logf(1.f + e);
-                        lp_s += live ? fmaf(yi, x, -sp) : 0.f;
-                        rr[u] = live ? yi - sg : 0.f;
-                    }
-                    const __half2 h = __floats2half2_rn(rr[0], rr[1]);
-                    const float2 hf = __half22float2(h);
-                    const __half2 l = __floats2half2_rn(rr[0] - hf.x, rr[1] - hf.y);
-                    rh[j][i >> 1] = *reinterpret_cast<const uint32_t*>(&h);
-                    rl[j][i >> 1] = *reinterpret_cast<const uint32_t*>(&l);
-                }
-            }
-            // GEMM 2 of the previous slab has finished by now (it ran under the arithmetic above), which frees r for this slab;
-            // every kTcDrain slabs its accumulator goes to fp64
-            if (s > 0) {
-                if (s % kTcDrain == 0) drain();
-                else {
-                    tc_mbar_wait(r_empty, (uint32_t)((s - 1) & 1));
-                    tc_fence_after();
-                }
-            }
-#pragma unroll
-            for (int j = 0; j < 2; ++j) {
-                tc_st16(tRh + lane_addr + half * 32 + j * 16, rh[j]);
-                tc_st16(tRl + lane_addr + half * 32 + j * 16, rl[j]);
-            }
-            tc_wait_st();
-            tc_fence_before();
-            tc_mbar_arrive(r_full);
-            lp += (double)lp_s;
-        }
-        if (my_slabs > 0) drain();
-        else {
-            for (int k = 0; k < 64; ++k) gp[(long long)k * A.Cpad] = 0.0;
-        }
-        if (half == 1) lp_half_s[c] = lp;
-        __syncwarp();
-        asm volatile("bar.sync 1, %0;" ::"r"(kTcEpiThreads) : "memory");  // the 8 epilogue warps only
-        if (half == 0) A.lpart[(long long)blockIdx.x * A.Cpad + c_base + c] = lp + lp_half_s[c];
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        const uint32_t ncols = 512;
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(ncols) : "memory");
-    }
-}
-
-// =========================================================================================================================
-// Version 2 of the kernel above (round 2, second session).  Same GEMMs, same TMEM map, same accumulate order and drain period;
-// what changed is everything around them, after the ncu capture of version 1 (profiles/r2_tc_logistic_tc_ncu_summary.csv:
-// tensor pipe 14 % busy, 63 warp-instructions per (row, chain) element, 42 % of the stall samples on long-scoreboard waits):
-//   * 16 epilogue warps instead of 8 (four per TMEM subpartition, 32 rows of the slab each): 4 warps per scheduler hide the
-//     TMEM-load and MUFU latencies that 2 could not;
-//   * the gradient partials stay in REGISTERS as fp64 (32 per thread) across the drains and are written once at the end:
-//     version 1 added every drain into global memory (2 x 64 read-modify-writes per thread every 2 slabs = 2 GB of L2
-//     traffic per launch, the long-scoreboard stalls);
-//   * y travels with the slab: the TMA producer copies the slab's 128 labels (fp32, 512 B) into the stage next to the X pieces
-//     (version 1 read them from global memory inside the element loop and converted bytes to floats per element);
-//   * elementwise math on the MUFU units directly (ex2 / rcp / lg2 .approx.ftz): 12 instructions per element for
-//     sigmoid + softplus + log-likelihood + residual; fp16 pieces of the residual are packed in place;
-//   * rows past N need no masking: their X rows are zero, so eta = 0 exactly, the residual multiplies zero rows in GEMM 2, and
-//     the log-likelihood they add (-softplus(0) each) is added back per slab.
-constexpr int kTc2EpiWarps = 16;
-constexpr int kTc2EpiThreads = 32 * kTc2EpiWarps;
-constexpr int kTc2Threads = 64 + kTc2EpiThreads;  // TMA producer, MMA issuer, 16 epilogue warps
-constexpr uint32_t kTc2YBytes = kTcRows * sizeof(float);
-constexpr size_t kTc2SmemBytes = kTcSmemBytes + kTcStages * kTc2YBytes;
 
 __device__ __forceinline__ float tc_ex2(float x) { float r; asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x)); return r; }
 __device__ __forceinline__ float tc_rcp(float x) { float r; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x)); return r; }
 __device__ __forceinline__ float tc_lg2(float x) { float r; asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x)); return r; }
-__device__ __forceinline__ void tc_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]), "=r"(v[9]),
-          "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-        : "r"(taddr)
-        : "memory");
-}
-// 8 registers -> 8 consecutive TMEM columns of this thread's lane
-__device__ __forceinline__ void tc_st8(uint32_t taddr, uint32_t a0, uint32_t a1, uint32_t a2, uint32_t a3, uint32_t a4, uint32_t a5,
-                                       uint32_t a6, uint32_t a7) {
-    asm volatile("tcgen05.st.sync.aligned.32x32b.x8.b32 [%0], {%1, %2, %3, %4, %5, %6, %7, %8};" ::"r"(taddr), "r"(a0), "r"(a1),
-                 "r"(a2), "r"(a3), "r"(a4), "r"(a5), "r"(a6), "r"(a7)
-                 : "memory");
-}
 
-struct LogisticTc2Args {
+struct LogisticTcArgs {
     const float* y32;        // [n_slabs * 128] labels as fp32, zero padded
     long long N;             // true rows
-    long long n_slabs;
+    long long n_slabs;       // ceil(N / 128); X pieces are allocated with n_slabs * 128 rows (zero padded)
     const double* Q;         // [C][ldq] beta per chain
     long long ldq;
     int C, K;
@@ -454,256 +125,190 @@ struct LogisticTc2Args {
     int Cpad;
 };
 
-// 18 warps on 4 schedulers: one scheduler hosts 5 of them, and the register file is per scheduler (16 K entries), so the
-// kernel gets 96 registers per thread, not 65536 / 576 = 113 (a 112-register build fails to launch: measured, call 11)
-__global__ void __launch_bounds__(kTc2Threads, 1)
-    logistic_tc2_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ CUtensorMap map_lo, const LogisticTc2Args A) {
+// 3 products x 8 k-steps of 16: hi*lo, lo*hi, then hi*hi.  a0/b0: shared addresses of the hi pieces; the lo pieces follow
+// at +a_piece / +b_piece.  a_off / b_off give the byte offset of k-step ks inside a piece.
+template <int TRANS_B, class AOff, class BOff>
+__device__ __forceinline__ void tc_split_gemm(float (&d)[32], uint32_t a0, uint32_t a_piece, uint32_t b0, uint32_t b_piece,
+                                              uint32_t b_lbo, AOff a_off, BOff b_off, bool accumulate) {
+    int scale = accumulate ? 1 : 0;
+#pragma unroll
+    for (int prod = 0; prod < 3; ++prod) {
+        const uint32_t a = a0 + (prod == 1 ? a_piece : 0u), b = b0 + (prod == 0 ? b_piece : 0u);
+#pragma unroll
+        for (int ks = 0; ks < 8; ++ks) {
+            wg_mma_n64<TRANS_B>(d, wg_desc(a + a_off(ks), 16, 1024), wg_desc(b + b_off(ks), b_lbo, 1024), scale);
+            scale = 1;
+        }
+    }
+}
+
+__global__ void __launch_bounds__(kTcThreads, 1)
+    logistic_tc_kernel(const __grid_constant__ CUtensorMap map_hi, const __grid_constant__ CUtensorMap map_lo, const LogisticTcArgs A) {
     extern __shared__ char tc_smem_raw[];
     char* base = reinterpret_cast<char*>((reinterpret_cast<uintptr_t>(tc_smem_raw) + 1023) & ~(uintptr_t)1023);
-    char* beta_s = base;                                   // [hi | lo] pieces, 32 KB each
-    char* x_s = base + 2 * kTcPieceBytes;                  // stages x [X_hi | X_lo]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(x_s + kTcStages * kTcStageBytes);
-    float* y_s = reinterpret_cast<float*>(reinterpret_cast<char*>(bars) + 256);  // stages x [128] labels
-    uint64_t* x_full = bars;          // [2] TMA -> MMA (and the epilogue: y)
-    uint64_t* x_empty = bars + 2;     // [2] MMA (GEMM 2 done) -> TMA
-    uint64_t* eta_full = bars + 4;    // [2] MMA (GEMM 1 done) -> epilogue
-    uint64_t* eta_empty = bars + 6;   // [2] epilogue (D1 read) -> MMA
-    uint64_t* r_full = bars + 8;      // epilogue (r written) -> MMA
-    uint64_t* r_empty = bars + 9;     // MMA (GEMM 2 done: r and the X stage are free) -> epilogue
-    uint64_t* g_full = bars + 10;     // MMA (drain point reached: D2 holds kTcDrain slabs) -> epilogue
-    uint64_t* g_empty = bars + 11;    // epilogue (D2 drained) -> MMA
-    __shared__ uint32_t tmem_base_s;
-    __shared__ double lp_q_s[3][kTcChains];
+    char* beta_s = base;                                   // [hi | lo] pieces, 16 KB each
+    char* r_s = beta_s + 2 * kTcAPieceBytes;               // [hi | lo] pieces of the residual tile, 16 KB each
+    char* x_s = r_s + 2 * kTcAPieceBytes;                  // stages x [X_hi | X_lo]
+    float* y_s = reinterpret_cast<float*>(x_s + kTcStages * kTcStageBytes);  // stages x [128] labels
+    uint64_t* bars = reinterpret_cast<uint64_t*>(reinterpret_cast<char*>(y_s) + kTcStages * kTcYBytes);
+    uint64_t* x_full = bars;          // [2] TMA -> consumers
+    uint64_t* x_empty = bars + 2;     // [2] consumers (GEMM 2 done) -> TMA
+    __shared__ double lp_wg_s[2][kTcChains];
 
-    const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+    const int tid = threadIdx.x;
     const int c_base = blockIdx.y * kTcChains;
+    // slabs of this CTA: blockIdx.x, blockIdx.x + gridDim.x, ...
     const long long my_slabs = (A.n_slabs > blockIdx.x) ? (A.n_slabs - blockIdx.x + gridDim.x - 1) / gridDim.x : 0;
 
     if (tid == 0) {
-        for (int i = 0; i < 2; ++i) {
+        for (int i = 0; i < kTcStages; ++i) {
             mbar_init(&x_full[i], 1);
-            mbar_init(&x_empty[i], 1);
-            mbar_init(&eta_full[i], 1);
-            mbar_init(&eta_empty[i], kTc2EpiThreads);
+            mbar_init(&x_empty[i], kTcConsumers);
         }
-        mbar_init(r_full, kTc2EpiThreads);
-        mbar_init(r_empty, 1);
-        mbar_init(g_full, 1);
-        mbar_init(g_empty, kTc2EpiThreads);
     }
-    if (warp == 1) {
-        const uint32_t ncols = 512;
-        asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_base_s)), "r"(ncols) : "memory");
-        asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-    }
-    for (int e = tid; e < kTcChains * kTcK; e += kTc2Threads) {
+    // beta pieces: fp64 -> fp16 hi / lo, written in the K-major SWIZZLE_128B image GEMM 1 reads as operand A
+    for (int e = tid; e < kTcChains * kTcK; e += kTcThreads) {
         const int c = e >> 7, k = e & 127;
         const double v = (c_base + c < A.C && k < A.K) ? A.Q[(long long)(c_base + c) * A.ldq + k] : 0.0;
         const __half hi = __double2half(v);
         const __half lo = __double2half(v - (double)__half2float(hi));
-        const uint32_t off = tc_tile_off(c, k);
+        const uint32_t off = tc_tile_off(c, k, kTcABlockBytes);
         *reinterpret_cast<__half*>(beta_s + off) = hi;
-        *reinterpret_cast<__half*>(beta_s + kTcPieceBytes + off) = lo;
+        *reinterpret_cast<__half*>(beta_s + kTcAPieceBytes + off) = lo;
     }
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    tc_fence_before();
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes of beta -> visible to wgmma
     __syncthreads();
-    tc_fence_after();
-    const uint32_t tmem = tmem_base_s;
-    const uint32_t tD1[2] = {tmem + 0, tmem + 128}, tD2 = tmem + 256, tRh = tmem + 384, tRl = tmem + 448;
 
-    if (warp == 0) {
+    // warps 0..7: the two consumer warpgroups (wgmma needs warpgroup-aligned warps), warp 8: the producer
+    if (tid >= kTcConsumers) {
         // ===== TMA producer: X_hi, X_lo (two 64-column boxes each) and the slab's labels =====
-        if (lane == 0) {
+        if (tid == kTcConsumers) {
             for (long long s = 0; s < my_slabs; ++s) {
                 const int st = (int)(s % kTcStages);
                 if (s >= kTcStages) tc_mbar_wait(&x_empty[st], (uint32_t)(((s / kTcStages) - 1) & 1));
                 const long long slab = blockIdx.x + s * gridDim.x;
                 const int row0 = (int)(slab * kTcRows);
                 char* dst = x_s + st * kTcStageBytes;
-                mbar_expect_tx(&x_full[st], kTcStageBytes + kTc2YBytes);
+                mbar_expect_tx(&x_full[st], kTcStageBytes + kTcYBytes);
                 tc_tma_load_2d(dst, &map_hi, 0, row0, &x_full[st]);
                 tc_tma_load_2d(dst + kTcBlockBytes, &map_hi, 64, row0, &x_full[st]);
                 tc_tma_load_2d(dst + kTcPieceBytes, &map_lo, 0, row0, &x_full[st]);
                 tc_tma_load_2d(dst + kTcPieceBytes + kTcBlockBytes, &map_lo, 64, row0, &x_full[st]);
-                tma_bulk_g2s(y_s + st * kTcRows, A.y32 + (long long)row0, kTc2YBytes, &x_full[st]);
-            }
-        }
-    } else if (warp == 1) {
-        // ===== MMA issuer (one lane): identical to version 1 =====
-        if (lane == 0) {
-            const uint32_t beta_a = smem_u32(beta_s);
-            auto gemm1 = [&](long long s) {
-                const int st = (int)(s % kTcStages), b = (int)(s & 1);
-                tc_mbar_wait(&x_full[st], (uint32_t)((s / kTcStages) & 1));
-                if (s >= 2) tc_mbar_wait(&eta_empty[b], (uint32_t)(((s >> 1) - 1) & 1));
-                tc_fence_after();
-                const uint32_t xa = smem_u32(x_s + st * kTcStageBytes);
-                uint32_t acc = 0;
-#pragma unroll
-                for (int prod = 0; prod < 3; ++prod) {  // hi*lo, lo*hi, hi*hi
-                    const uint32_t a0 = beta_a + (prod == 1 ? kTcPieceBytes : 0);
-                    const uint32_t b0 = xa + (prod == 0 ? kTcPieceBytes : 0);
-#pragma unroll
-                    for (int ks = 0; ks < 8; ++ks) {
-                        const uint32_t o = (uint32_t)((ks >> 2) * kTcBlockBytes + (ks & 3) * 32);
-                        tc_mma_ss(tD1[b], tc_desc(a0 + o, 16, 1024), tc_desc(b0 + o, 16, 1024), kTcIdesc, acc);
-                        acc = 1;
-                    }
-                }
-                tc_commit(&eta_full[b]);
-            };
-            if (my_slabs > 0) gemm1(0);
-            for (long long s = 0; s < my_slabs; ++s) {
-                if (s + 1 < my_slabs) gemm1(s + 1);
-                tc_mbar_wait(r_full, (uint32_t)(s & 1));
-                const bool first = (s % kTcDrain) == 0;
-                if (first && s > 0) tc_mbar_wait(g_empty, (uint32_t)(((s / kTcDrain) - 1) & 1));
-                tc_fence_after();
-                const int st = (int)(s % kTcStages);
-                const uint32_t xa = smem_u32(x_s + st * kTcStageBytes);
-                uint32_t acc = first ? 0u : 1u;
-#pragma unroll
-                for (int prod = 0; prod < 3; ++prod) {  // r_hi X_lo, r_lo X_hi, r_hi X_hi
-                    const uint32_t ta = (prod == 1) ? tRl : tRh;
-                    const uint32_t b0 = xa + (prod == 0 ? kTcPieceBytes : 0);
-#pragma unroll
-                    for (int ks = 0; ks < 8; ++ks) {
-                        tc_mma_ts(tD2, ta + ks * 8, tc_desc(b0 + ks * 2048, kTcBlockBytes, 1024), kTcIdescBmn, acc);
-                        acc = 1;
-                    }
-                }
-                tc_commit(&x_empty[st]);
-                tc_commit(r_empty);
-                if ((s + 1) % kTcDrain == 0 || s + 1 == my_slabs) tc_commit(g_full);
+                tma_bulk_g2s(y_s + st * kTcRows, A.y32 + (long long)row0, kTcYBytes, &x_full[st]);
             }
         }
     } else {
-        // ===== epilogue: 16 warps; TMEM lane = chain (subpartition = warp % 4); the four warps of a subpartition take a
-        //       quarter of the slab's rows (32) and a quarter of the gradient's columns (32 features) each =====
-        const int sub = warp & 3, quarter = (warp - 2) >> 2;
-        const int c = sub * 32 + lane;
-        const uint32_t lane_addr = (uint32_t)(sub * 32) << 16;
-        double lp = 0.0;
-        double gacc[32];  // this thread's gradient partials: features quarter*32 .. +31 of chain c, over all slabs of the CTA
+        // ===== consumers: warpgroup wg owns slab rows 64 wg.. in GEMM 1 and features 64 wg.. in GEMM 2 =====
+        const int t = tid, wg = t >> 7, wt = t & 127, warp = wt >> 5, lane = wt & 31;
+        const int r0 = 16 * warp + (lane >> 2);        // chains r0 and r0 + 8 of this CTA
+        const int col = 2 * (lane & 3);                // + 8 j + {0, 1}: column inside the warpgroup's 64
+        const uint32_t beta_a = smem_u32(beta_s), r_a = smem_u32(r_s);
+        double lp[2] = {0.0, 0.0};
+        double gacc[32];  // fp64 gradient partials: d-layout of GEMM 2 (features 64 wg + 8j + col + {0,1}), all slabs
 #pragma unroll
         for (int k = 0; k < 32; ++k) gacc[k] = 0.0;
-        long long n_drains = 0;
-        auto drain = [&]() {  // fp32 gradient accumulator (kTcDrain slabs) -> the fp64 registers
-            tc_mbar_wait(g_full, (uint32_t)(n_drains & 1));
-            tc_fence_after();
+        float g[32];
 #pragma unroll
-            for (int j = 0; j < 2; ++j) {
-                uint32_t v[16];
-                tc_ld16(tD2 + lane_addr + quarter * 32 + j * 16, v);
-                tc_wait_ld();
-#pragma unroll
-                for (int k = 0; k < 16; ++k) gacc[j * 16 + k] += (double)__uint_as_float(v[k]);
-            }
-            ++n_drains;
-            tc_fence_before();
-            tc_mbar_arrive(g_empty);
-        };
-        // softplus(0) as the element formula computes it: what every padded row (eta = 0 exactly) subtracts from lp
-        const float sp0 = tc_lg2(2.0f) * 0.69314718055994530942f;
+        for (int k = 0; k < 32; ++k) g[k] = 0.0f;
         for (long long s = 0; s < my_slabs; ++s) {
-            const int b = (int)(s & 1), st = (int)(s % kTcStages);
-            const long long row0 = (blockIdx.x + s * gridDim.x) * kTcRows + quarter * 32;
-            tc_mbar_wait(&eta_full[b], (uint32_t)((s >> 1) & 1));
-            // the labels arrived with the X pieces of this stage (same mbarrier; completed before GEMM 1 was issued)
+            const int st = (int)(s % kTcStages);
             tc_mbar_wait(&x_full[st], (uint32_t)((s / kTcStages) & 1));
-            tc_fence_after();
-            const float4* yq = reinterpret_cast<const float4*>(y_s + st * kTcRows + quarter * 32);
-            float lp_s = 0.f;
+            const uint32_t xa = smem_u32(x_s + st * kTcStageBytes);
+            // GEMM 1: eta for slab rows 64 wg .. 64 wg + 63 (row r of the slab is at r * 128 B inside each 64-column box)
+            float eta[32];
 #pragma unroll
-            for (int j = 0; j < 2; ++j) {  // 16 rows of the slab at a time
-                uint32_t v[16];
-                tc_ld16(tD1[b] + lane_addr + quarter * 32 + j * 16, v);
-                tc_wait_ld();
-                if (j == 1) {  // this thread's share of D1[b] has been read: GEMM 1 of slab s + 2 may overwrite it
-                    tc_fence_before();
-                    tc_mbar_arrive(&eta_empty[b]);
-                }
+            for (int k = 0; k < 32; ++k) eta[k] = 0.0f;
+            wg_fence();
+            tc_split_gemm<0>(eta, beta_a, kTcAPieceBytes, xa + wg * 64 * 128, kTcPieceBytes, 16,
+                             [](int ks) { return (uint32_t)((ks >> 2) * kTcABlockBytes + (ks & 3) * 32); },
+                             [](int ks) { return (uint32_t)((ks >> 2) * kTcBlockBytes + (ks & 3) * 32); }, false);
+            wg_commit();
+            wg_wait_all();
+            // residuals and log-likelihood terms
+            const long long row_base = (blockIdx.x + s * gridDim.x) * kTcRows + 64 * wg;
+            const float* ys = y_s + st * kTcRows + 64 * wg;
+            float lp_s[2] = {0.f, 0.f};
+            uint32_t rh[16], rl[16];
 #pragma unroll
-                for (int i4 = 0; i4 < 4; ++i4) {
-                    const float4 y4 = yq[j * 4 + i4];  // same address in every lane: one broadcast LDS.128 per 4 rows
-                    const float yv[4] = {y4.x, y4.y, y4.z, y4.w};
-                    float rr[4];
+            for (int j = 0; j < 8; ++j) {
 #pragma unroll
-                    for (int u = 0; u < 4; ++u) {
-                        const float x = __uint_as_float(v[4 * i4 + u]);
-                        const float t = tc_ex2(-1.4426950408889634f * fabsf(x));   // e^-|x|
-                        const float w = 1.f + t;
+                for (int hh = 0; hh < 2; ++hh) {
+                    float rr[2];
+#pragma unroll
+                    for (int u = 0; u < 2; ++u) {
+                        const int i = 8 * j + col + u;
+                        const float x = eta[4 * j + 2 * hh + u];
+                        const float yv = ys[i];
+                        const float tt = tc_ex2(-1.4426950408889634f * fabsf(x));   // e^-|x|
+                        const float w = 1.f + tt;
                         const float inv = tc_rcp(w);
-                        const float sg = x >= 0.f ? inv : t * inv;                  // sigmoid(x)
+                        const float sg = x >= 0.f ? inv : tt * inv;                  // sigmoid(x)
                         const float sp = fmaf(tc_lg2(w), 0.69314718055994530942f, fmaxf(x, 0.f));  // softplus(x)
-                        lp_s += fmaf(yv[u], x, -sp);
-                        rr[u] = yv[u] - sg;
+                        // rows past N: X rows are zero (eta = 0), so the residual multiplies zero rows in GEMM 2
+                        lp_s[hh] += (row_base + i < A.N) ? fmaf(yv, x, -sp) : 0.f;
+                        rr[u] = yv - sg;
                     }
-#pragma unroll
-                    for (int u = 0; u < 4; u += 2) {  // fp16 pieces of two residuals, packed in place of their eta values
-                        const __half2 h = __floats2half2_rn(rr[u], rr[u + 1]);
-                        const float2 hf = __half22float2(h);
-                        const __half2 l = __floats2half2_rn(rr[u] - hf.x, rr[u + 1] - hf.y);
-                        v[4 * i4 + u] = *reinterpret_cast<const uint32_t*>(&h);
-                        v[4 * i4 + u + 1] = *reinterpret_cast<const uint32_t*>(&l);
-                    }
-                }
-                // GEMM 2 of the previous slab (it ran under the arithmetic above) frees r; every kTcDrain slabs its accumulator
-                // goes to the fp64 registers first
-                const bool drain_now = (j == 0 && s > 0 && s % kTcDrain == 0);
-                if (j == 0 && s > 0) {
-                    if (drain_now) tc_mbar_wait(g_full, (uint32_t)(n_drains & 1));  // GEMM 2 of slab s-1 done: r free, D2 complete
-                    else tc_mbar_wait(r_empty, (uint32_t)((s - 1) & 1));
-                    tc_fence_after();
-                }
-                // 16 rows -> 8 packed columns of r_hi and of r_lo
-                tc_st8(tRh + lane_addr + quarter * 16 + j * 8, v[0], v[2], v[4], v[6], v[8], v[10], v[12], v[14]);
-                tc_st8(tRl + lane_addr + quarter * 16 + j * 8, v[1], v[3], v[5], v[7], v[9], v[11], v[13], v[15]);
-                if (drain_now) {
-                    // the drain: both TMEM loads first, D2 handed back to the MMA issuer as soon as they have landed; the fp64
-                    // conversions and sums run afterwards, off the GEMM 2 -> GEMM 2 critical path
-                    uint32_t d0[16], d1[16];
-                    tc_ld16(tD2 + lane_addr + quarter * 32, d0);
-                    tc_ld16(tD2 + lane_addr + quarter * 32 + 16, d1);
-                    tc_wait_ld();
-                    ++n_drains;
-                    tc_fence_before();
-                    tc_mbar_arrive(g_empty);
-#pragma unroll
-                    for (int k = 0; k < 16; ++k) gacc[k] += (double)__uint_as_float(d0[k]);
-#pragma unroll
-                    for (int k = 0; k < 16; ++k) gacc[16 + k] += (double)__uint_as_float(d1[k]);
+                    const __half2 h = __floats2half2_rn(rr[0], rr[1]);
+                    const float2 hf = __half22float2(h);
+                    const __half2 l = __floats2half2_rn(rr[0] - hf.x, rr[1] - hf.y);
+                    rh[2 * j + hh] = *reinterpret_cast<const uint32_t*>(&h);
+                    rl[2 * j + hh] = *reinterpret_cast<const uint32_t*>(&l);
                 }
             }
-            tc_wait_st();
-            tc_fence_before();
-            tc_mbar_arrive(r_full);
-            const long long over = row0 + 32 - A.N;  // padded rows of this quarter (the last slab only)
-            if (over > 0) lp_s += (float)(over < 32 ? over : 32) * sp0;
-            lp += (double)lp_s;
-        }
-        if (my_slabs > 0) drain();
-        // the CTA's fp64 partial gradient, FEATURE-major [128 k][Cpad chains]: for a fixed k the 32 lanes of a warp write 32
-        // consecutive chains (coalesced), once
-        double* gp = A.Gpart + ((long long)blockIdx.x * kTcK + quarter * 32) * A.Cpad + c_base + c;
+            lp[0] += (double)lp_s[0];
+            lp[1] += (double)lp_s[1];
+            consumers_sync();  // both warpgroups are past GEMM 2 of the previous slab: the residual tile is free
 #pragma unroll
-        for (int k = 0; k < 32; ++k) gp[(long long)k * A.Cpad] = gacc[k];
-        if (quarter > 0) lp_q_s[quarter - 1][c] = lp;
-        __syncwarp();
-        asm volatile("bar.sync 1, %0;" ::"r"(kTc2EpiThreads) : "memory");  // the 16 epilogue warps only
-        if (quarter == 0) A.lpart[(long long)blockIdx.x * A.Cpad + c_base + c] = ((lp + lp_q_s[0][c]) + lp_q_s[1][c]) + lp_q_s[2][c];
-    }
-    tc_fence_before();
-    __syncthreads();
-    if (warp == 1) {
-        tc_fence_after();
-        const uint32_t ncols = 512;
-        asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem), "r"(ncols) : "memory");
+            for (int j = 0; j < 8; ++j) {
+#pragma unroll
+                for (int hh = 0; hh < 2; ++hh) {
+                    const uint32_t off = tc_tile_off(r0 + 8 * hh, 64 * wg + 8 * j + col, kTcABlockBytes);
+                    *reinterpret_cast<uint32_t*>(r_s + off) = rh[2 * j + hh];
+                    *reinterpret_cast<uint32_t*>(r_s + kTcAPieceBytes + off) = rl[2 * j + hh];
+                }
+            }
+            asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+            consumers_sync();  // the whole residual tile [64 chains][128 rows] is written
+            // GEMM 2: g[c][k] += sum_i r[c][i] X[i][64 wg + k]; B = box wg of the stage, MN-major (16 rows = 2 KB per k-step)
+            const bool first = (s % kTcDrain) == 0;
+            wg_fence();
+            tc_split_gemm<1>(g, r_a, kTcAPieceBytes, xa + wg * kTcBlockBytes, kTcPieceBytes, kTcBlockBytes,
+                             [](int ks) { return (uint32_t)((ks >> 2) * kTcABlockBytes + (ks & 3) * 32); },
+                             [](int ks) { return (uint32_t)(ks * 2048); }, !first);
+            wg_commit();
+            wg_wait_all();
+            tc_mbar_arrive(&x_empty[st]);
+            if ((s + 1) % kTcDrain == 0 || s + 1 == my_slabs) {
+#pragma unroll
+                for (int k = 0; k < 32; ++k) gacc[k] += (double)g[k];
+            }
+        }
+        // row sums of the log-likelihood over the four lanes that share a chain (fixed order: deterministic)
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+            lp[hh] += __shfl_xor_sync(B200_FULL_MASK, lp[hh], 1);
+            lp[hh] += __shfl_xor_sync(B200_FULL_MASK, lp[hh], 2);
+        }
+        if ((lane & 3) == 0) {
+            lp_wg_s[wg][r0] = lp[0];
+            lp_wg_s[wg][r0 + 8] = lp[1];
+        }
+        // the CTA's fp64 partial gradient, FEATURE-major [128 k][Cpad chains]
+        double* gp = A.Gpart + (long long)blockIdx.x * kTcK * A.Cpad + c_base;
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+#pragma unroll
+            for (int h = 0; h < 4; ++h) {
+                const int k = 64 * wg + 8 * j + col + (h & 1), c = r0 + 8 * (h >> 1);
+                gp[(long long)k * A.Cpad + c] = gacc[4 * j + h];
+            }
+        }
+        consumers_sync();
+        if (t < kTcChains) A.lpart[(long long)blockIdx.x * A.Cpad + c_base + t] = lp_wg_s[0][t] + lp_wg_s[1][t];
     }
 }
 
-// labels as fp32, zero padded to whole slabs (version 2 copies them into shared memory with the slab)
+// labels as fp32, zero padded to whole slabs (copied into shared memory with the slab)
 __global__ void __launch_bounds__(256) logistic_tc_y_kernel(const uint8_t* __restrict__ y, long long N, float* __restrict__ y32,
                                                             long long rows_pad) {
     const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;

@@ -166,9 +166,8 @@ struct RadonModel {
             const double a_c = q_s[4 + ci], b_c = q_s[4 + J + ci];
             const double al = fma(sa, a_c, mu_a), be = fma(sb, b_c, mu_b);
             double Ga0 = 0.0, Gb0 = 0.0, S20 = 0.0, Ga1 = 0.0, Gb1 = 0.0, S21 = 0.0;
-            // SMALL: no unrolling inside the persistent NUTS kernel, whose hot code must stay inside the instruction cache
-            // (measured: 511 vs 562 ms per bench step; ping-ponging the prefetch registers with an unroll of 2: 526 vs 506);
-            // the stand-alone leapfrog/logp kernels unroll (540 vs 393 M evals/s).
+            // SMALL: no unrolling inside the persistent NUTS kernel, whose hot code must stay inside the instruction cache;
+            // the stand-alone leapfrog/logp kernels unroll.
             // Padding slots hold (x, y) = (0, 0): their residual is -alpha exactly, so instead of masking every slot
             // (2 selects + a compare per observation: a fifth of the loop's issue slots) the lane removes its padding's
             // contribution after the row:  Ga += npad alpha,  S2 -= npad alpha^2,  Gb untouched (x = 0).

@@ -34,8 +34,8 @@ constexpr int kMaxLevels = 12;  // pending-subtree levels (max_treedepth <= 12)
 // A subtree's multinomial weight is carried as the pair (m, s), log-weight = m + log(s), instead of one log-weight.  A
 // leaf is (-dE, 1); merging (m1, s1) and (m2, s2) gives m = max(m1, m2), s = s1 e^(m1-m) + s2 e^(m2-m): one exp and no log
 // per merge, and no overflow for any energy change because m carries the scale and 1 <= s <= number of leaves.  The pick
-// probabilities are the numbers logaddexp gives (nuts.py:465-467, :370-376) up to rounding; measured on the bench
-// workload (round 2, profiles/r2_variants.md): 481.6 vs 506.3 ms per step, every golden tree decision unchanged.
+// probabilities are the numbers logaddexp gives (nuts.py:465-467, :370-376) up to rounding; every golden tree decision is
+// unchanged.
 
 struct NutsDev {
     int C, n, tune, draws, max_td, early_td, adapt_step, mass_kind, momentum_source, store_warmup;
@@ -116,8 +116,6 @@ __host__ __device__ inline size_t nuts_warp_smem_bytes(int NP, int hot, bool sub
 #define B200_NUTS_MINBLOCKS 1  // __launch_bounds__ min CTAs/SM: the register budget knob
 #endif
 // W = warps per chain (team).  SUBS = subtree-under-construction vectors in shared memory instead of registers.
-// Register caps below the ~240 the kernel wants were measured and rejected (round 2, profiles/r2_variants.md): 224 registers
-// (9 warps/SM) 460 ms, 200 (10 warps/SM, 264 B of spills) 521 ms, 168 (12 warps/SM) 685 ms vs 370 ms at 2 x 4 warps per SM.
 #define B200_NUTS_BOUNDS __launch_bounds__(W > 1 ? 32 * W : B200_NUTS_THREADS, W > 1 ? 1 : B200_NUTS_MINBLOCKS)
 template <class Model, int NPL, int W, bool SUBS>
 __global__ void B200_NUTS_BOUNDS

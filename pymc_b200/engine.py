@@ -159,8 +159,8 @@ class CompiledModel:
         _lib.check(self._lib.b200_model_set_dense_mass(self._h, S.ctypes.data, mp0.ctypes.data, mv0.ctypes.data))
 
     def set_precision(self, mode: str) -> None:
-        """"fp64" (parity mode, default) or "tc_fp16x2": the dense contractions of the logistic GLM on the tcgen05 tensor
-        cores with split-fp16 operands (performance mode; gradient ~1e-7 relative, see include/b200nuts.h)."""
+        """"fp64" (parity mode, default) or "tc_fp16x2": the dense contractions of the logistic GLM or the dense Gaussian on
+        the fp16 tensor cores with split-fp16 operands (performance mode; error bounds in include/b200nuts.h)."""
         code = {"fp64": _lib.PRECISION_FP64, "tc_fp16x2": _lib.PRECISION_TC_FP16X2}[mode]
         _lib.check(self._lib.b200_model_set_precision(self._h, code))
         self.precision = mode

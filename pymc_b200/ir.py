@@ -405,7 +405,7 @@ def specialise(ir: ModelIR, extended: bool = False):
 
     Recognised: the non-centred varying-intercept/varying-slope Normal regression of benchmarks.py:34-45 (Radon; any data),
     non-centred Eight Schools (any J), the AR(1) stochastic-volatility model of BASELINE config 4 (any T) and the logistic GLM
-    of config 3 (beta ~ Normal(0, 1), up to 128 features: the fused design-matrix kernels, fp64 DMMA or tcgen05) -- these two
+    of config 3 (beta ~ Normal(0, 1), up to 128 features: the fused design-matrix kernels, fp64 DMMA or wgmma) -- these two
     only with ``extended=True`` (``CompiledModel(ir, specialise="all")``): the routes were added after the round's last GPU run
     and are checked on the CPU only (the specialised spec has the IR's density, tests/test_ir.py), so the default keeps such
     models on the generic function.  Everything else runs on the generic IR device function."""

@@ -174,7 +174,7 @@ def sample_b200_nuts(
     step: str = "nuts",
     gather: str = "rank0",
 ) -> SampleResult:
-    """Draw samples from the posterior using the B200 engine.
+    """Draw samples from the posterior using the CUDA engine.
 
     Arguments follow ``sample_jax_nuts`` (pymc/sampling/jax.py:495-517).  ``model``: a ``pymc_b200.ir.ModelIR`` (any model
     of the closed factor set; ``from_pymc`` lowers a ``pm.Model`` to one), a ``ModelSpec`` naming a hand-written kernel, or

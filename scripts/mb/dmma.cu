@@ -1,6 +1,5 @@
 // DMMA (mma.sync m8n8k4.f64 and m16n8k16.f64) throughput micro-benchmark used to decide between DFMA and DMMA kernels:
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -DTRY_M16 -o scripts/mb/dmma_bench scripts/mb/dmma.cu
-// Measured on B200: 36.7-37.0 TFLOP/s for every shape = the DFMA peak; a dependent DMMA issues every ~35 cycles per warp.
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -DTRY_M16 -o scripts/mb/dmma_bench scripts/mb/dmma.cu
 #include <cstdio>
 #include <cuda_runtime.h>
 __device__ __forceinline__ void dmma884(double& c0, double& c1, double a, double b) {
@@ -40,10 +39,12 @@ __global__ void __launch_bounds__(256) k_dmma16(double* out, int iters) {
 #endif
 template <class F> float timeit(F f) { cudaEvent_t a, b; cudaEventCreate(&a); cudaEventCreate(&b); f(); cudaDeviceSynchronize(); float best = 1e30; for (int r = 0; r < 3; ++r) { cudaEventRecord(a); f(); cudaEventRecord(b); cudaEventSynchronize(b); float ms; cudaEventElapsedTime(&ms, a, b); if (ms < best) best = ms; } return best; }
 int main() {
-    double* out; cudaMalloc(&out, 148 * 8 * 256 * 8);
+    int sms = 0;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, 0);
+    double* out; cudaMalloc(&out, (size_t)sms * 4 * 256 * 8);  // largest grid below: 4 CTAs of 256 threads per SM
     const int iters = 4096;
     for (int bps : {1, 2, 4}) {
-        int blocks = 148 * bps;
+        int blocks = sms * bps;
         float ms = timeit([&] { k_dmma<8><<<blocks, 256>>>(out, iters); });
         printf("m8n8k4 NACC=8 blocks/SM=%d: %.2f TFLOP/s\n", bps, 2.0 * 256 * 8 * iters * (double)blocks * 8 / ms / 1e9);
         ms = timeit([&] { k_dmma<1><<<blocks, 256>>>(out, iters); });

@@ -27,20 +27,20 @@ def test_roofline_objects():
     import bench
 
     wl = bench.WORKLOADS["radon"]
-    r = bench.make_roofline("radon", wl, per_launch=9.0e7, k_ms=500.0, fp64=36.0, dmma=37.0, peaks=(6563.9, "measured"),
-                            traffic=(5.3e9, "ncu"))
+    r = bench.make_roofline("radon", wl, per_launch=9.0e7, k_ms=500.0, fp64=36.0, dmma=37.0, peaks=(6563.9, "measured"))
     # the top level is the BINDING resource of the on-chip kernels: the fp64 pipe (VERDICT r1 weak #3)
-    assert r["bound"] == "fp64" and r["unit"] == "TFLOP/s" and r["peak"] == 36.0 and r["traffic"] == 5.3e9
+    assert r["bound"] == "fp64" and r["unit"] == "TFLOP/s" and r["peak"] == 36.0
     assert abs(r["achieved"] - (919 * 30 + 175 * 12) * 9.0e7 / 0.5 / 1e12) < 1e-9 and abs(r["frac"] - r["achieved"] / 36.0) < 1e-12
     h = r["hbm_by_algorithmic_bytes"]  # SURVEY 8(d)'s second figure, secondary
     assert h["unit"] == "GB/s" and abs(h["achieved"] - 28180 * 9.0e7 / 0.5 / 1e9) < 1e-6 and h["peak_source"] == "measured"
-    assert abs(h["frac"] - h["achieved"] / 6563.9) < 1e-12 and h["dram_bytes_measured"] == 5.3e9
-    assert bench.make_roofline("radon", wl, 9.0e7, 500.0, None, None, (6650.0, "fallback"), None)["peak"] == 36.0
+    assert abs(h["frac"] - h["achieved"] / 6563.9) < 1e-12
+    # no measurement in the run: the H100 SXM data sheet's fp64 rates
+    assert bench.make_roofline("radon", wl, 9.0e7, 500.0, None, None, (3350.0, "fallback"))["peak"] == 34.0
     t = bench.make_roofline("logistic", bench.WORKLOADS["logistic"], per_launch=4.0e5, k_ms=12000.0, fp64=36.0, dmma=37.0,
-                            peaks=(6563.9, "measured"), traffic=None)
+                            peaks=(6563.9, "measured"))
     assert t["bound"] == "tensor" and t["unit"] == "TFLOP/s" and abs(t["achieved"] - 512e6 * 4.0e5 / 12.0 / 1e12) < 1e-9
-    assert t["peak"] == 37.0 and t["traffic"] is None
-    assert bench.make_roofline("mvgauss", bench.WORKLOADS["mvgauss"], 1e5, 1e4, None, None, (6563.9, "measured"), None)["peak"] == 37.0
+    assert t["peak"] == 37.0
+    assert bench.make_roofline("mvgauss", bench.WORKLOADS["mvgauss"], 1e5, 1e4, None, None, (6563.9, "measured"))["peak"] == 67.0
     json.dumps([r, t])
 
 

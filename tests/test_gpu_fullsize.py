@@ -99,7 +99,7 @@ def test_logistic_full_design_matrix_points(logistic_full):
 
 
 def test_logistic_sharding_drift_is_bounded(logistic_full):
-    """The fused pass splits the rows over 148 / ceil(C/128) row-CTAs, so the partial-sum grouping of a chain's
+    """The fused pass splits the rows over SMs / ceil(C/128) row-CTAs, so the partial-sum grouping of a chain's
     gradient depends on how many chains share the launch (DESIGN section 6).  Bound: <= 1e-12 relative."""
     cm = logistic_full
     rng = np.random.default_rng(2)
@@ -115,7 +115,7 @@ def test_logistic_sharding_drift_is_bounded(logistic_full):
 
 @pytest.mark.parametrize("C", [256, 64, 32])
 def test_mvgauss_full_logp_grad(mvgauss_full, C):
-    """C = 256 -> gemm_nt_dmma_kernel<8,17,3>, 64 -> <4,*>, 32 -> <2,*> (one wave of 148 SMs each)."""
+    """C = 256 -> gemm_nt_dmma_kernel<8,17,3>, 64 -> <4,*>, 32 -> <2,*> (tile counts chosen to fill whole waves of the SMs)."""
     cm = mvgauss_full
     rng = np.random.default_rng(C)
     L = cm.spec.data["L"]

@@ -1,9 +1,9 @@
-"""-m gpu: the tensor-core performance mode of the logistic GLM (tcgen05.mma + TMEM + TMA, split fp16; csrc/logistic_tc.cuh)
+"""-m gpu: the tensor-core performance mode of the logistic GLM (wgmma + TMA, split fp16; csrc/logistic_tc.cuh)
 against the fp64 parity path and the oracle.  SURVEY section 7 ("fp64 parity vs tensor cores"): the performance mode states
-its measured error next to its throughput -- both land in gpurun_out/parity_report.json (copied to profiles/).
+its measured error next to its throughput -- both land in the parity report the tests write.
 
-Tolerances: gradient <= 1e-6 of its largest entry per chain (north_star's logp/grad bound); logp <= 1e-6 relative (the
-tensor cores' fp32 accumulate rounds toward zero, which shrinks eta = X.beta by ~2e-7 systematically: logistic_tc.cuh);
+Tolerances: gradient <= 1e-6 of its largest entry per chain (north_star's logp/grad bound); logp <= 1e-6 relative (fp16
+pieces carry 22 significant bits and the tensor cores accumulate in fp32);
 sampler level: the fixed-step golden keeps its tree statistics, and an adaptive run's posterior agrees with the fp64
 run's within Monte Carlo error.
 """
@@ -87,8 +87,7 @@ def test_tc_full_design_matrix_error_and_speed():
         "fp64_equivalent_tflops_tc": flops / (mstc * 1e-3) / 1e12, "fp64_tflops_dmma": flops / (ms64 * 1e-3) / 1e12,
         "tensor_flops_issued_tflops": 3 * flops / (mstc * 1e-3) / 1e12})
     assert eg <= 1e-6 and el <= 1e-6, (eg, el)
-    # (speed: the call-level timer includes per-call allocations; the kernel-level comparison is the ncu launch list in
-    # profiles/: 2.6 ms vs 10.8-12 ms per 512-chain batch)
+    # (speed: the call-level timer includes per-call allocations; the times are reported, not asserted)
 
 
 def test_tc_fixed_step_golden_keeps_its_trees(pair128, golden):
@@ -130,7 +129,7 @@ def test_tc_adaptive_run_posterior_matches_fp64_run(pair128):
 
 
 # ------------------------------------------------------------------------------------------------------------------------
-# dense Gaussian (config #5): the four n x n contractions on tcgen05 (csrc/gemm_tc.cuh)
+# dense Gaussian (config #5): the four n x n contractions on wgmma (csrc/gemm_tc.cuh)
 # ------------------------------------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("n,C", [(300, 40), (1000, 130)])
 def test_tc_gemm_dense_gaussian_error(n, C):
@@ -168,7 +167,7 @@ def test_tc_gemm_dense_mass_golden_keeps_its_trees(golden):
 
 
 def test_tc_gemm_full_size_error_and_speed():
-    """n = 10^4, 256 chains: one wave of 140 tiles; error and time against the fp64 DMMA GEMM."""
+    """n = 10^4, 256 chains: error and time against the fp64 DMMA GEMM."""
     from pymc_b200 import _lib, engine, models
 
     spec = models.mvgauss(cache_dir="/dev/shm/b200_cache")
@@ -187,6 +186,5 @@ def test_tc_gemm_full_size_error_and_speed():
     _report("tc_fp16x2/mvgauss_n10000_256chains", {
         "grad_rel_to_max_vs_fp64": eg, "logp_rel_vs_fp64": el, "fp64_dmma_ms": ms64, "tc_ms_incl_operand_split": mstc,
         "speedup": ms64 / mstc, "fp64_equivalent_tflops_tc": flops / (mstc * 1e-3) / 1e12})
-    # 10^4-term contractions: 1.2e-6 of the largest gradient entry measured (n = 300 / 1000: 5e-7); stated, not hidden
+    # 10^4-term contractions: 1.2e-6 of the largest gradient entry measured on an H100 (n = 300 / 1000: 5e-7); stated, not hidden
     assert eg <= 2e-6 and el <= 1e-6, (eg, el)
-    # (speed: profiles/ launch lists: gemm_tc_kernel 0.30 ms vs gemm_nt_dmma_kernel 1.67 ms per 256-chain GEMM)

@@ -3,16 +3,15 @@
 
 CPU: the device engine is replaced by a stand-in with the ``CompiledModel.nuts_run`` interface that runs the oracle
 (bit-identical to the reference, tests/test_oracle_vs_reference.py), which pins the protocol glue: stream derivation
-(``rng`` / ``rng.spawn(1)[0]``), tune/draw schedule, point (un)raveling, stats keys.  GPU: the real engine."""
+(``rng`` / ``rng.spawn(1)[0]``), tune/draw schedule, point (un)raveling, stats keys.  The reference chain driven the same
+way is stored in tests/golden/reference_chains.npz (oracle/make_reference_chains.py).  GPU: the real engine."""
 import numpy as np
 import pytest
 
 from b200_helpers import OracleEngine
-from oracle import logp_numpy, ref_loader
+from oracle.make_reference_chains import SEAM_STATS
 from pymc_b200 import models
 from pymc_b200.step import B200NUTS
-
-needs_reference = pytest.mark.skipif(not ref_loader.available(), reason="/root/reference is not present")
 
 
 def drive(step, start, rng, tune, draws):
@@ -30,29 +29,29 @@ def drive(step, start, rng, tune, draws):
     return np.array(out), stats
 
 
-@needs_reference
-def test_b200nuts_protocol_matches_reference_nuts_with_oracle_engine():
+def test_b200nuts_protocol_matches_reference_nuts_with_oracle_engine(golden):
     spec = models.eight_schools()
-    f = logp_numpy.make_logp(spec)
     q0 = spec.initial_point() + np.random.default_rng(3).uniform(-1, 1, spec.n)
     start = {v.name: q0[v.offset : v.offset + v.size].copy() for v in spec.vars}
     tune, draws, seed = 60, 25, 20240922
 
-    ref, _ = ref_loader.make_nuts(f, spec.var_sizes, start, step_rng=0)  # default potential: DiagAdapt(zeros, ones, 10)
-    want_q, want_st = drive(ref, dict(start), np.random.default_rng(seed), tune, draws)
-    rng_ref_after = ref.rng.bit_generator.state["state"]["state"]
+    # the reference NUTS with its default potential, DiagAdapt(zeros, ones, 10), driven by the same loop
+    ref = golden("reference_chains")
+    hi, lo = (int(x) for x in ref["seam_rng_after"])
+    rng_ref_after = (hi << 64) | lo
 
     mine = B200NUTS(OracleEngine(spec))
     rng = np.random.default_rng(seed)
     got_q, got_st = drive(mine, dict(start), rng, tune, draws)
 
-    assert np.array_equal(got_q, want_q)
+    assert np.array_equal(got_q, ref["seam_q"])
     for k in ("depth", "tree_size", "index_in_trajectory", "diverging", "reached_max_treedepth", "divergences"):
-        assert [s[k] for s in got_st] == [w[k] for w in want_st], k
+        assert [s[k] for s in got_st] == list(ref[f"seam_{k}"]), k
     for k in ("step_size", "step_size_bar", "mean_tree_accept", "energy", "energy_error", "max_energy_error", "model_logp"):
-        np.testing.assert_allclose([s[k] for s in got_st], [w[k] for w in want_st], rtol=1e-12, atol=1e-12, err_msg=k)
-    assert set(B200NUTS.stats_dtypes_shapes) == set(type(ref).stats_dtypes_shapes)
-    assert set(got_st[0]) == set(want_st[0])
+        np.testing.assert_allclose([s[k] for s in got_st], ref[f"seam_{k}"], rtol=1e-12, atol=1e-12, err_msg=k)
+    assert set(SEAM_STATS) <= set(got_st[0])
+    assert set(B200NUTS.stats_dtypes_shapes) == set(ref["seam_stats_keys"])
+    assert set(got_st[0]) == set(ref["seam_point_keys"])
     # the caller's generator is left exactly where the reference leaves its own
     assert rng.bit_generator.state["state"]["state"] == rng_ref_after
     # shape of a point entry is preserved, other keys pass through

@@ -77,6 +77,14 @@ extern "C" {
 #define B200_IR_L_POISSON_LOG 2     /* y ~ Poisson(exp(eta))                     discrete.py:581-586    */
 #define B200_IR_L_STUDENTT 3        /* y ~ StudentT(nu, eta, sigma)              continuous.py:1936-1944 */
 #define B200_IR_L_NORMAL_LOGVAR 4   /* y ~ Normal(0, exp(eta / 2))                                      */
+/* The three families below carry their parameter in the likelihood's `sigma` slot:
+ *   BINOMIAL_LOGIT     trials n: CONST (sigma.value) or OBS (sigma_obs[N]), integer >= 0; integer 0 <= y <= n
+ *   NEGBINOMIAL_LOG    dispersion alpha: CONST (> 0) or REF (a scalar variable with positive support); integer y >= 0.
+ *                      Above alpha = 1e10 the density is the Poisson(exp(eta)) limit, as in the reference.
+ *   GAMMA_LOG          shape alpha: CONST (> 0) or REF; y > 0                                                        */
+#define B200_IR_L_BINOMIAL_LOGIT 5  /* y ~ Binomial(n, logit_p = eta)            discrete.py:141-152    */
+#define B200_IR_L_NEGBINOMIAL_LOG 6 /* y ~ NegativeBinomial(mu = exp(eta), alpha) discrete.py:700-745   */
+#define B200_IR_L_GAMMA_LOG 7       /* y ~ Gamma(alpha, beta = alpha exp(-eta))  continuous.py:2478-2521 */
 #define B200_IR_S_NONE 0
 #define B200_IR_S_CONST 1 /* sigma.value               */
 #define B200_IR_S_REF 2   /* sigma = x[sigma.ref]      */
@@ -111,7 +119,7 @@ typedef struct b200_ir_lik {
     const b200_ir_term* terms;
     int32_t sigma_kind, reserved;
     b200_ir_param sigma;
-    const double* sigma_obs; /* [N] when sigma_kind == B200_IR_S_OBS */
+    const double* sigma_obs; /* [N] when sigma_kind == B200_IR_S_OBS (Binomial: trials per observation) */
     double nu;
 } b200_ir_lik;
 typedef struct b200_ir_ar1 { /* h_0 ~ Normal(0, init_sigma); h_t - phi h_{t-1} ~ Normal(0, sigma)  (timeseries.py:646-676) */

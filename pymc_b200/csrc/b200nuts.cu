@@ -8,6 +8,7 @@
 #include <cstdio>
 #include <cmath>
 #include <cstring>
+#include <map>
 #include <numeric>
 #include <string>
 #include <type_traits>
@@ -441,10 +442,68 @@ static int prepare_ir(b200_model* m, const b200_model_desc* d) {
                 if (!(L.nu > 0)) return fail("ir: likelihood %d: StudentT nu must be > 0", l);
                 D.c0 = (double)N * (std::lgamma(0.5 * (L.nu + 1.0)) - std::lgamma(0.5 * L.nu) - 0.5 * std::log(L.nu) - 0.5 * LOG_PI);
                 break;
+            case B200_IR_L_BINOMIAL_LOGIT: {  // c0 = sum_i binomln(n_i, y_i)
+                if (L.sigma_kind != B200_IR_S_CONST && L.sigma_kind != B200_IR_S_OBS)
+                    return fail("ir: likelihood %d: Binomial trials must be a constant or one per observation", l);
+                double c = 0;
+                for (long long i = 0; i < N; ++i) {
+                    const double nt = L.sigma_kind == B200_IR_S_OBS ? L.sigma_obs[i] : L.sigma.value, y = L.y[i];
+                    if (!std::isfinite(nt) || !(nt >= 0) || nt != std::floor(nt)) return fail("ir: likelihood %d: Binomial trials must be integers >= 0 (at %lld)", l, i);
+                    if (!(y >= 0 && y <= nt) || y != std::floor(y)) return fail("ir: likelihood %d: Binomial y must be an integer in [0, n] (at %lld)", l, i);
+                    c += std::lgamma(nt + 1.0) - std::lgamma(y + 1.0) - std::lgamma(nt - y + 1.0);
+                }
+                D.c0 = c;
+            } break;
+            case B200_IR_L_NEGBINOMIAL_LOG: {
+                if (L.sigma_kind != B200_IR_S_CONST && L.sigma_kind != B200_IR_S_REF)
+                    return fail("ir: likelihood %d: NegativeBinomial alpha must be a constant or a scalar variable", l);
+                if (L.sigma_kind == B200_IR_S_CONST && !(L.sigma.value > 0 && std::isfinite(L.sigma.value))) return fail("ir: likelihood %d: NegativeBinomial alpha must be finite and > 0", l);
+                const double a = L.sigma.value;
+                const bool fold = L.sigma_kind == B200_IR_S_CONST && a <= kNegBinPoissonAlpha;
+                double c = 0;
+                std::map<double, double> count;  // distinct nonzero y -> multiplicity, ascending
+                for (long long i = 0; i < N; ++i) {
+                    const double y = L.y[i];
+                    if (!(y >= 0) || y != std::floor(y) || std::isinf(y)) return fail("ir: likelihood %d: NegativeBinomial y must be an integer >= 0 (at %lld)", l, i);
+                    c -= std::lgamma(y + 1.0);
+                    if (fold) c += std::lgamma(y + a) - std::lgamma(a);
+                    if (y > 0) count[y] += 1.0;
+                }
+                D.c0 = c;
+                if (L.sigma_kind == B200_IR_S_REF) {
+                    std::vector<double> u, cnt;
+                    for (const auto& kv : count) { u.push_back(kv.first); cnt.push_back(kv.second); }
+                    D.n_tab = (int)u.size();
+                    if (upload(m, u, &D.tab_u) || upload(m, cnt, &D.tab_cnt)) return -1;
+                }
+            } break;
+            case B200_IR_L_GAMMA_LOG: {
+                if (L.sigma_kind != B200_IR_S_CONST && L.sigma_kind != B200_IR_S_REF)
+                    return fail("ir: likelihood %d: Gamma alpha must be a constant or a scalar variable", l);
+                if (L.sigma_kind == B200_IR_S_CONST && !(L.sigma.value > 0 && std::isfinite(L.sigma.value))) return fail("ir: likelihood %d: Gamma alpha must be finite and > 0", l);
+                double sly = 0;
+                for (long long i = 0; i < N; ++i) {
+                    if (!(L.y[i] > 0) || std::isinf(L.y[i])) return fail("ir: likelihood %d: Gamma y must be > 0 (at %lld)", l, i);
+                    sly += std::log(L.y[i]);
+                }
+                if (L.sigma_kind == B200_IR_S_CONST) {
+                    const double a = L.sigma.value;
+                    D.c0 = (double)N * (a * std::log(a) - std::lgamma(a)) + (a - 1.0) * sly;
+                } else {
+                    D.sum_log_y = sly;
+                }
+            } break;
             default: return fail("ir: likelihood %d: density %d is not in the closed set", l, L.dist);
         }
         if ((L.dist == B200_IR_L_NORMAL || L.dist == B200_IR_L_STUDENTT) && L.sigma_kind == B200_IR_S_NONE)
             return fail("ir: likelihood %d needs sigma", l);
+        if ((L.dist == B200_IR_L_NEGBINOMIAL_LOG || L.dist == B200_IR_L_GAMMA_LOG) && L.sigma_kind == B200_IR_S_REF) {
+            bool positive = false;  // the referenced scalar must have positive support: log, or interval with lo >= 0
+            for (const IrVarD& V : vars)
+                if (L.sigma.ref >= V.offset && L.sigma.ref < V.offset + V.size)
+                    positive = V.size == 1 && (V.transform == B200_IR_T_LOG || (V.transform == B200_IR_T_INTERVAL && V.lo >= 0));
+            if (!positive) return fail("ir: likelihood %d: a random alpha must be a scalar variable with positive support", l);
+        }
         for (int t = 0; t < L.n_terms; ++t) {
             const b200_ir_term& T = L.terms[t];
             if (T.n_factors < 0 || T.n_factors > 3) return fail("ir: likelihood %d term %d: 0..3 variable factors", l, t);

@@ -13,6 +13,10 @@
 //
 // Team scratch in global memory (L1/L2 resident), one slice per resident team: x[n] and the per-observation
 // d loglik / d eta of the likelihood being processed.
+//
+// A random dispersion alpha (NegativeBinomial, Gamma) reaches its slot through the same team reduction as a likelihood's
+// sigma.  Its normalising terms are not per observation: Gamma's once per evaluation, NegativeBinomial's over a table of
+// the distinct nonzero counts (csrc/b200nuts.cu: prepare_ir), with digamma() of common.cuh for the gradient.
 #pragma once
 #include "common.cuh"
 
@@ -21,16 +25,21 @@ namespace b200 {
 enum { IRT_NONE = 0, IRT_LOG = 1, IRT_INTERVAL = 2 };
 enum { IRP_FLAT = 0, IRP_NORMAL, IRP_HALFNORMAL, IRP_CAUCHY, IRP_HALFCAUCHY, IRP_EXPONENTIAL, IRP_STUDENTT, IRP_UNIFORM,
        IRP_GAMMA, IRP_BETA, IRP_LOGNORMAL };
-enum { IRL_NORMAL = 0, IRL_BERNOULLI_LOGIT, IRL_POISSON_LOG, IRL_STUDENTT, IRL_NORMAL_LOGVAR };
+enum { IRL_NORMAL = 0, IRL_BERNOULLI_LOGIT, IRL_POISSON_LOG, IRL_STUDENTT, IRL_NORMAL_LOGVAR, IRL_BINOMIAL_LOGIT,
+       IRL_NEGBINOMIAL_LOG, IRL_GAMMA_LOG };
 enum { IRS_NONE = 0, IRS_CONST, IRS_REF, IRS_OBS };
+constexpr double kNegBinPoissonAlpha = 1e10;  // above: NegativeBinomial -> Poisson(mu) limit (discrete.py:727-735)
 
 struct IrParamD { int kind, ref; double value; };                     // kind 0: constant; 1: x[ref] (a scalar variable)
 struct IrVarD { int offset, size, transform, pad; double lo, hi; };
 struct IrPriorD { int dist, offset, size, pad; IrParamD p[3]; double c0; };      // c0: per-element constant of the density
 struct IrFactorD { int offset, size; const int* idx; const int* rowptr; const int* rowobs; };  // CSR: element -> observations
 struct IrTermD { const double* coef; int n_factors, pad; IrFactorD f[3]; };
+// c0: sum of the constant parts over i.  Random dispersion (sigma_kind REF): Gamma keeps sum_i log y_i in sum_log_y;
+// NegativeBinomial keeps the distinct nonzero y values u[k] with their counts cnt[k] (n_tab of them), over which the
+// alpha-dependent normalising terms sum_i lgamma(y_i + a) - lgamma(a) and their digamma gradient are evaluated.
 struct IrLikD { int dist, n_terms, term0, sigma_kind; long long N; const double* y; const double* sigma_obs; IrParamD sigma;
-                double nu, c0; };                                                 // c0: sum of the constant parts over i
+                double nu, c0, sum_log_y; const double* tab_u; const double* tab_cnt; int n_tab, pad; };
 struct IrAr1D { int offset, size; IrParamD phi, sigma; double init_sigma; };
 
 struct IrModel {
@@ -153,6 +162,8 @@ struct IrModel {
             const IrLikD L = P.liks[l];
             const int N = (int)L.N;
             const double sg_s = (L.sigma_kind == IRS_REF) ? x[L.sigma.ref] : L.sigma.value;
+            const bool disp = L.dist == IRL_NEGBINOMIAL_LOG || L.dist == IRL_GAMMA_LOG;  // sg_s is the dispersion alpha
+            const double la = disp ? log(sg_s) : 0.0;
             double s_sig = 0.0;
             for (int i = tid; i < N; i += TS) {
                 double eta = 0.0;
@@ -194,9 +205,58 @@ struct IrModel {
                         lp += -0.5 * w - 0.5 * eta;
                         ri = 0.5 * w - 0.5;
                     } break;
+                    case IRL_BINOMIAL_LOGIT: {  // discrete.py:141-152 in PyTensor's stabilised forms; binomln(n, y) is in c0
+                        const double nt = (L.sigma_kind == IRS_OBS) ? L.sigma_obs[i] : sg_s;
+                        lp += yi * eta - nt * softplus(eta);
+                        ri = yi - nt * sigmoid(eta);
+                    } break;
+                    case IRL_NEGBINOMIAL_LOG:  // discrete.py:700-745, n = a, p = a / (mu + a); the lgamma part is in c0 / below
+                        if (sg_s > kNegBinPoissonAlpha) {  // uniform branch: the Poisson(mu) limit
+                            const double mu = exp(eta);
+                            lp += yi * eta - mu;
+                            ri = yi - mu;
+                        } else {
+                            // d = eta - log a: lse = logaddexp(eta, log a) = log a + softplus(d) = eta + softplus(-d), with
+                            // s = mu / (mu + a) and sc = a / (mu + a) from one exp, so nothing overflows for any finite eta
+                            const double d = eta - la, e = exp(-fabs(d)), l1 = log1p(e), h = 1.0 / (1.0 + e);
+                            const double s = d >= 0 ? h : e * h, sc = d >= 0 ? e * h : h;
+                            const double sp = fmax(d, 0.0) + l1;  // lse - log a
+                            lp -= yi * (fmax(-d, 0.0) + l1) + sg_s * sp;
+                            ri = yi * sc - sg_s * s;                         // a (y - mu) / (mu + a)
+                            s_sig += 1.0 - sp - sc * (1.0 + yi / sg_s);      // d/da except psi(y + a) - psi(a)
+                        }
+                        break;
+                    case IRL_GAMMA_LOG: {  // continuous.py:2512-2521, beta = a exp(-eta); the eta-free part once below
+                        const double w = yi * exp(-eta);
+                        lp -= sg_s * (eta + w);
+                        ri = sg_s * (w - 1.0);
+                        s_sig -= eta + w;
+                    } break;
                     default: break;
                 }
                 r[i] = ri;
+            }
+            if (disp && L.sigma_kind == IRS_REF) {  // uniform branch: the alpha-dependent normalising terms
+                const double a = sg_s;
+                const IrLikD& Lt = P.liks[l];  // read here, not kept live through the observation loop
+                if (L.dist == IRL_GAMMA_LOG) {
+                    if (tid == 0) {
+                        const double sly = Lt.sum_log_y;
+                        lp += (double)N * (a * la - lgamma(a)) + (a - 1.0) * sly;
+                        s_sig += (double)N * (la + 1.0 - digamma(a)) + sly;
+                    }
+                } else if (a <= kNegBinPoissonAlpha) {
+                    // sum_i lgamma(y_i + a) - lgamma(a) over the distinct values: team-strided, fixed order
+                    const double lga = lgamma(a), pa = digamma(a);
+                    const double* tu = Lt.tab_u;
+                    const double* tc = Lt.tab_cnt;
+                    const int n_tab = Lt.n_tab;
+                    for (int k = tid; k < n_tab; k += TS) {
+                        const double u = tu[k], c = tc[k];
+                        lp = fma(c, lgamma(u + a) - lga, lp);
+                        s_sig = fma(c, digamma(u + a) - pa, s_sig);
+                    }
+                }
             }
             if (tid == 0) lp += L.c0;
             team_sync<W>();
@@ -322,6 +382,7 @@ __global__ void __launch_bounds__(256) ir_pointwise_kernel(const IrModel::Params
         }
         __syncwarp();
         const double sg_s = (L.sigma_kind == IRS_REF) ? x[L.sigma.ref] : L.sigma.value;
+        const double la = (L.dist == IRL_NEGBINOMIAL_LOG || L.dist == IRL_GAMMA_LOG) ? log(sg_s) : 0.0;
         for (int i = lane; i < N; i += 32) {
             double eta = 0.0;
             for (int t = 0; t < L.n_terms; ++t) {
@@ -348,6 +409,19 @@ __global__ void __launch_bounds__(256) ir_pointwise_kernel(const IrModel::Params
                          0.5 * (L.nu + 1.0) * log1p(z * z / L.nu);
                 } break;
                 case IRL_NORMAL_LOGVAR: lp = -0.5 * yi * yi * exp(-eta) - 0.5 * eta - B200_HALF_LOG_2PI; break;
+                case IRL_BINOMIAL_LOGIT: {
+                    const double nt = (L.sigma_kind == IRS_OBS) ? L.sigma_obs[i] : sg_s;
+                    lp = lgamma(nt + 1.0) - lgamma(yi + 1.0) - lgamma(nt - yi + 1.0) + yi * eta - nt * softplus(eta);
+                } break;
+                case IRL_NEGBINOMIAL_LOG:
+                    if (sg_s > kNegBinPoissonAlpha) {
+                        lp = yi * eta - exp(eta) - lgamma(yi + 1.0);
+                    } else {
+                        const double d = eta - la, l1 = log1p(exp(-fabs(d)));
+                        lp = lgamma(yi + sg_s) - lgamma(sg_s) - lgamma(yi + 1.0) - yi * (fmax(-d, 0.0) + l1) - sg_s * (fmax(d, 0.0) + l1);
+                    }
+                    break;
+                case IRL_GAMMA_LOG: lp = sg_s * (la - eta) - lgamma(sg_s) + (sg_s - 1.0) * log(yi) - sg_s * yi * exp(-eta); break;
                 default: break;
             }
             out[d * N + i] = lp;

@@ -10,7 +10,9 @@ pymc/model/fgraph.py:76-81, :139) -- and pattern-matches them onto the closed fa
                      AR(1) / GaussianRandomWalk -> ir.AR1
     observed RV  ->  ir.Likelihood; its location parameter is parsed into linear-predictor terms
                      (Add / Sub / Neg / Mul / division by a constant / indexing by constant integer arrays / Dot with a
-                     constant matrix / broadcasts); Normal(0, exp(eta / 2)) with a linear eta -> the log-variance likelihood
+                     constant matrix / broadcasts); Normal(0, exp(eta / 2)) with a linear eta -> the log-variance likelihood;
+                     Binomial(n, logit_p = eta) with constant trials, NegativeBinomial(mu = exp(eta), alpha) and
+                     Gamma(alpha, beta = alpha / exp(eta) | alpha * exp(-eta)), alpha a constant or a scalar free RV
 
 Anything outside the closed set raises ``NotImplementedError`` naming the offending op, so a model either lowers exactly
 or not at all.  PyMC and PyTensor are NOT importable in the build image (SURVEY 8c); this module imports them lazily and
@@ -240,6 +242,23 @@ def from_pymc(model) -> _ir.ModelIR:
             return x.owner.inputs[0]
         return None
 
+    def inputs_of(x, want):
+        """inputs of the Elemwise `want` (add / truediv / exp ...) that x is, under any DimShuffle layers, or None"""
+        while x.owner is not None and isinstance(x.owner.op, DimShuffle):
+            x = x.owner.inputs[0]
+        if x.owner is not None and scalar_op_name(x.owner) == want:
+            return list(x.owner.inputs)
+        return None
+
+    def same_param(x, p):
+        """x (under DimShuffle layers) is the constant or scalar free RV p"""
+        while x.owner is not None and isinstance(x.owner.op, DimShuffle):
+            x = x.owner.inputs[0]
+        try:
+            return param(x, "") == p
+        except NotImplementedError:
+            return False
+
     liks = []
     for rv in model.observed_RVs:
         y = _const_value(model.rvs_to_values[rv])
@@ -285,6 +304,54 @@ def from_pymc(model) -> _ir.ModelIR:
             if eta is None:
                 raise NotImplementedError(f"{rv.name}: write the rate as pm.math.exp(linear predictor)")
             liks.append(_ir.Likelihood("poisson_log", y, make_terms(eta, N), name=rv.name))
+        elif op == "binomial":  # RV parameters (n, p); logit_p= and p=invlogit(eta) both give p = sigmoid(eta)
+            form = "pm.Binomial(n=trials, logit_p=linear predictor) with constant trials"
+            nt = _const_value(ps[0])
+            eta = inputs_of(ps[1], "sigmoid")
+            if nt is None or eta is None:
+                raise NotImplementedError(f"{rv.name}: write the likelihood as {form}")
+            trials = float(nt.reshape(())) if nt.size == 1 else np.ravel(np.broadcast_to(nt, (N,))).astype(np.float64)
+            liks.append(_ir.Likelihood("binomial_logit", y, make_terms(eta[0], N), trials=trials, name=rv.name))
+        elif op in ("negbinomial", "nbinom"):  # RV parameters (n = alpha, p = alpha / (mu + alpha)), discrete.py:700-723
+            form = "pm.NegativeBinomial(mu=pm.math.exp(linear predictor), alpha=constant or scalar free RV)"
+            try:
+                alpha = param(ps[0], rv.name + ".alpha")
+            except NotImplementedError:
+                raise NotImplementedError(f"{rv.name}: write the likelihood as {form}") from None
+            div, eta = inputs_of(ps[1], "truediv"), None
+            den = inputs_of(div[1], "add") if div is not None and same_param(div[0], alpha) else None
+            if den is not None and len(den) == 2:
+                for mu_, a_ in (den, den[::-1]):
+                    e = inputs_of(mu_, "exp")
+                    if e is not None and same_param(a_, alpha):
+                        eta = e[0]
+                        break
+            if eta is None:
+                raise NotImplementedError(f"{rv.name}: write the likelihood as {form}")
+            liks.append(_ir.Likelihood("negative_binomial_log", y, make_terms(eta, N), alpha=alpha, name=rv.name))
+        elif op == "gamma":  # RV parameters (alpha, scale = reciprocal(beta)), continuous.py:2478-2510
+            form = ("pm.Gamma(alpha=a, beta=a / pm.math.exp(linear predictor)) or beta=a * pm.math.exp(-linear predictor), "
+                    "a a constant or scalar free RV")
+            try:
+                alpha = param(ps[0], rv.name + ".alpha")
+            except NotImplementedError:
+                raise NotImplementedError(f"{rv.name}: write the likelihood as {form}") from None
+            beta, eta = inputs_of(ps[1], "reciprocal"), None
+            if beta is not None:
+                div, mul = inputs_of(beta[0], "truediv"), inputs_of(beta[0], "mul")
+                if div is not None and same_param(div[0], alpha):  # a / exp(eta)
+                    e = inputs_of(div[1], "exp")
+                    eta = e[0] if e is not None else None
+                elif mul is not None and len(mul) == 2:  # a * exp(-eta), either order
+                    for a_, e_ in (mul, mul[::-1]):
+                        e = inputs_of(e_, "exp")
+                        ng = inputs_of(e[0], "neg") if e is not None else None
+                        if ng is not None and same_param(a_, alpha):
+                            eta = ng[0]
+                            break
+            if eta is None:
+                raise NotImplementedError(f"{rv.name}: write the likelihood as {form}")
+            liks.append(_ir.Likelihood("gamma_log", y, make_terms(eta, N), alpha=alpha, name=rv.name))
         else:
             raise NotImplementedError(f"{rv.name}: likelihood {type(rv.owner.op).__name__} is outside the closed set "
                                       f"{sorted(_ir.LIK_DISTS)}")

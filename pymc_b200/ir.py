@@ -47,7 +47,12 @@ LIK_DISTS = {
     "poisson_log": 2,        # y_i ~ Poisson(mu = exp(eta_i))                           discrete.py:581-586
     "studentt": 3,           # y_i ~ StudentT(nu, eta_i, sigma)                         continuous.py:1936-1944
     "normal_logvar": 4,      # y_i ~ Normal(0, exp(eta_i / 2))   (stochastic volatility observation)
+    "binomial_logit": 5,     # y_i ~ Binomial(trials, logit_p = eta_i)                  discrete.py:141-152 (stabilised forms)
+    "negative_binomial_log": 6,  # y_i ~ NegativeBinomial(mu = exp(eta_i), alpha)       discrete.py:700-745
+    "gamma_log": 7,          # y_i ~ Gamma(alpha, beta = alpha exp(-eta_i))             continuous.py:2478-2521
 }
+DISPERSION_LIKS = ("negative_binomial_log", "gamma_log")  # their `alpha` is a constant or a Ref
+NEGBIN_POISSON_ALPHA = 1e10  # above: the NegativeBinomial density is its Poisson(mu) limit (discrete.py:727-735)
 SIGMA_NONE, SIGMA_CONST, SIGMA_REF, SIGMA_OBS = 0, 1, 2, 3
 MAX_TERM_FACTORS = 3
 
@@ -93,6 +98,8 @@ class Likelihood:
     sigma: float | Ref | np.ndarray | None = None
     nu: float = 0.0
     name: str = "y"
+    alpha: float | Ref | None = None           # negative_binomial_log / gamma_log: dispersion (shape)
+    trials: float | np.ndarray | None = None   # binomial_logit: number of trials, one for all or one per observation
 
 
 @dataclass
@@ -191,12 +198,49 @@ class ModelIR:
                 raise ValueError(f"{L.dist} likelihood needs sigma")
             if isinstance(L.sigma, Ref) and self.var(L.sigma.var).size != 1:
                 raise ValueError("likelihood sigma must be a scalar variable")
+            self._validate_family(L)
         for a in self.ar1:
             if self.var(a.var).size < 2:
                 raise ValueError("AR1 needs at least two steps")
             for r in (a.phi, a.sigma):
                 if isinstance(r, Ref) and self.var(r.var).size != 1:
                     raise ValueError("AR1 parameters must be scalar variables or constants")
+
+    def _validate_family(self, L) -> None:
+        """Support and parameter rules of the count / positive families (the same checks prepare_ir makes)."""
+        y = np.asarray(L.y, dtype=np.float64)
+        integer = lambda a: bool(np.all(np.isfinite(a)) and np.all(a == np.floor(a)))  # noqa: E731
+        if L.dist == "binomial_logit":
+            if L.trials is None or isinstance(L.trials, Ref):
+                raise ValueError("binomial_logit: trials must be a constant scalar or a constant array")
+            n = np.asarray(L.trials, dtype=np.float64)
+            if n.ndim > 1 or (n.ndim == 1 and len(n) != len(y)):
+                raise ValueError("binomial_logit: trials must be a scalar or one per observation")
+            if not integer(n) or np.any(n < 0):
+                raise ValueError("binomial_logit: trials must be integers >= 0")
+            if not integer(y) or np.any(y < 0) or np.any(y > n):
+                raise ValueError("binomial_logit: y must be integers with 0 <= y <= trials")
+        elif L.trials is not None:
+            raise ValueError(f"{L.dist}: trials belong to binomial_logit")
+        if L.dist in DISPERSION_LIKS:
+            if L.alpha is None:
+                raise ValueError(f"{L.dist} needs alpha")
+            if isinstance(L.alpha, Ref):
+                v = self.var(L.alpha.var)
+                if v.size != 1:
+                    raise ValueError(f"{L.dist}: alpha must be a scalar variable")
+                if not (v.transform == "log" or (v.transform == "interval" and v.bounds[0] >= 0)):
+                    raise ValueError(f"{L.dist}: alpha {v.name} needs positive support (a log transform, or an interval with lo >= 0)")
+            elif not (np.ndim(L.alpha) == 0 and np.isfinite(float(L.alpha)) and float(L.alpha) > 0):
+                raise ValueError(f"{L.dist}: a constant alpha must be a finite scalar > 0")
+            if L.dist == "negative_binomial_log" and (not integer(y) or np.any(y < 0)):
+                raise ValueError("negative_binomial_log: y must be integers >= 0")
+            if L.dist == "gamma_log" and not (np.all(np.isfinite(y)) and np.all(y > 0)):
+                raise ValueError("gamma_log: y must be > 0")
+        elif L.alpha is not None:
+            raise ValueError(f"{L.dist}: alpha belongs to the negative_binomial_log / gamma_log likelihoods")
+        if L.dist in ("binomial_logit",) + DISPERSION_LIKS and L.sigma is not None:
+            raise ValueError(f"{L.dist} has no sigma (its parameter is {'trials' if L.dist == 'binomial_logit' else 'alpha'})")
 
     # ---- host-side post-processing (f1): unconstrained draws -> named constrained RVs --------------------------------
     def constrain(self, q: np.ndarray) -> dict:
@@ -247,6 +291,8 @@ class ModelIR:
                 for vn, idx in t.factors:
                     if idx is not None:
                         out[f"{L.name}_{vn}_idx"] = np.asarray(idx)
+            if L.trials is not None and np.ndim(L.trials) == 1:
+                out[f"{L.name}_trials"] = np.asarray(L.trials)
         return out
 
 
@@ -327,6 +373,69 @@ def varying_intercept_logistic_ir(n_obs: int = 600, n_groups: int = 12, n_featur
     )
 
 
+def binomial_logit_ir(n_obs: int = 150, n_groups: int = 10, seed: int = 29) -> ModelIR:
+    """Varying-intercept binomial regression on simulated data (rat-tumour / seeds shape): a_g ~ Normal(mu, sigma) (centred),
+    beta ~ Normal(0, 1), y_i ~ Binomial(trials_i, logit_p = a[g_i] + beta x_i) with 1..40 trials per observation."""
+    rng = np.random.default_rng(seed)
+    g = rng.integers(0, n_groups, n_obs).astype(np.int32)
+    x = rng.standard_normal(n_obs)
+    trials = rng.integers(1, 41, n_obs).astype(np.float64)
+    a = rng.normal(-0.5, 0.7, n_groups)
+    eta = a[g] + 0.4 * x
+    y = rng.binomial(trials.astype(np.int64), 1.0 / (1.0 + np.exp(-eta))).astype(np.float64)
+    return ModelIR(
+        name="binomial_logit",
+        vars=[Var("mu", "mu", 1), Var("sigma_log__", "sigma", 1, "log"), Var("a", "a", n_groups), Var("beta", "beta", 1)],
+        priors=[Prior("normal", "mu", (0.0, 2.0)), Prior("halfnormal", "sigma_log__", (1.0,)),
+                Prior("normal", "a", (Ref("mu"), Ref("sigma_log__"))), Prior("normal", "beta", (0.0, 1.0))],
+        likelihoods=[Likelihood("binomial_logit", y, [Term([("a", g)]), Term([("beta", None)], coef=x)], trials=trials)],
+    )
+
+
+def negative_binomial_ir(n_obs: int = 300, n_groups: int = 8, seed: int = 31, alpha: float | None = None) -> ModelIR:
+    """Hierarchical negative-binomial regression on simulated overdispersed counts: z_g ~ Normal(0, 1) (non-centred),
+    beta ~ Normal(0, 1)^2, alpha ~ Exponential(1) (or the constant `alpha`),
+    y_i ~ NegativeBinomial(mu = exp(mu_a + sigma_a z[g_i] + x_i . beta), alpha)."""
+    rng = np.random.default_rng(seed)
+    g = rng.integers(0, n_groups, n_obs).astype(np.int32)
+    X = rng.standard_normal((n_obs, 2))
+    z = rng.standard_normal(n_groups)
+    eta = 1.2 + 0.5 * z[g] + X @ np.array([0.3, -0.2])
+    a_true = 2.5
+    mu = np.exp(eta)
+    y = rng.negative_binomial(a_true, a_true / (mu + a_true)).astype(np.float64)
+    vars_ = [Var("mu_a", "mu_a", 1), Var("sigma_a_log__", "sigma_a", 1, "log"), Var("z", "z", n_groups), Var("beta", "beta", 2)]
+    priors = [Prior("normal", "mu_a", (0.0, 2.0)), Prior("halfnormal", "sigma_a_log__", (1.0,)), Prior("normal", "z", (0.0, 1.0)),
+              Prior("normal", "beta", (0.0, 1.0))]
+    if alpha is None:
+        vars_.append(Var("alpha_log__", "alpha", 1, "log"))
+        priors.append(Prior("exponential", "alpha_log__", (1.0,)))
+    terms = [Term([("mu_a", None)]), Term([("sigma_a_log__", None), ("z", g)])] + \
+        [Term([("beta", np.full(n_obs, k, dtype=np.int32))], coef=X[:, k].copy()) for k in range(2)]
+    return ModelIR(name="negative_binomial", vars=vars_, priors=priors,
+                   likelihoods=[Likelihood("negative_binomial_log", y, terms,
+                                           alpha=Ref("alpha_log__") if alpha is None else float(alpha))])
+
+
+def gamma_regression_ir(n_obs: int = 200, n_features: int = 3, seed: int = 37, alpha: float | None = None) -> ModelIR:
+    """Gamma regression with a log link on simulated positive data: b0 ~ Normal(0, 2), beta ~ Normal(0, 1)^K,
+    alpha ~ HalfNormal(2) (or the constant `alpha`), y_i ~ Gamma(alpha, beta = alpha / exp(b0 + x_i . beta))."""
+    rng = np.random.default_rng(seed)
+    X = rng.standard_normal((n_obs, n_features))
+    eta = 0.7 + X @ rng.normal(0.0, 0.4, n_features)
+    a_true = 3.0
+    y = rng.gamma(a_true, np.exp(eta) / a_true)
+    vars_ = [Var("b0", "b0", 1), Var("beta", "beta", n_features)]
+    priors = [Prior("normal", "b0", (0.0, 2.0)), Prior("normal", "beta", (0.0, 1.0))]
+    if alpha is None:
+        vars_.append(Var("alpha_log__", "alpha", 1, "log"))
+        priors.append(Prior("halfnormal", "alpha_log__", (2.0,)))
+    terms = [Term([("b0", None)])] + [Term([("beta", np.full(n_obs, k, dtype=np.int32))], coef=X[:, k].copy())
+                                      for k in range(n_features)]
+    return ModelIR(name="gamma_regression", vars=vars_, priors=priors,
+                   likelihoods=[Likelihood("gamma_log", y, terms, alpha=Ref("alpha_log__") if alpha is None else float(alpha))])
+
+
 # ------------------------------------------------------------------------------------------------------------------------
 # lowering: ModelIR -> flat arrays of the C ABI (include/b200nuts.h: b200_ir)
 # ------------------------------------------------------------------------------------------------------------------------
@@ -384,13 +493,15 @@ def lower(ir: ModelIR) -> LoweredIR:
                 v = ir.var(vn)
                 fs.append((off[v.name], v.size, None if idx is None else np.ascontiguousarray(idx, dtype=np.int32)))
             terms.append(dict(coef=coef, factors=fs))
+        # the likelihood's one parameter slot: sigma, or the trials / alpha of the count and positive families
+        par = L.trials if L.dist == "binomial_logit" else (L.alpha if L.dist in DISPERSION_LIKS else L.sigma)
         sk, sv, sr, so = SIGMA_NONE, 0.0, -1, None
-        if isinstance(L.sigma, Ref):
-            sk, sr = SIGMA_REF, off[ir.var(L.sigma.var).name]
-        elif L.sigma is not None and np.ndim(L.sigma) == 1:
-            sk, so = SIGMA_OBS, np.ascontiguousarray(L.sigma, dtype=np.float64)
-        elif L.sigma is not None:
-            sk, sv = SIGMA_CONST, float(L.sigma)
+        if isinstance(par, Ref):
+            sk, sr = SIGMA_REF, off[ir.var(par.var).name]
+        elif par is not None and np.ndim(par) == 1:
+            sk, so = SIGMA_OBS, np.ascontiguousarray(par, dtype=np.float64)
+        elif par is not None:
+            sk, sv = SIGMA_CONST, float(par)
         liks.append(dict(dist=LIK_DISTS[L.dist], N=N, y=np.ascontiguousarray(L.y, dtype=np.float64), terms=terms,
                          sigma_kind=sk, sigma_value=sv, sigma_ref=sr, sigma_obs=so, nu=float(L.nu)))
     ar1 = [(index[ir.var(a.var).name], _param(ir, a.phi, off), _param(ir, a.sigma, off), float(a.init_sigma)) for a in ir.ar1]

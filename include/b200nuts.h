@@ -85,6 +85,11 @@ extern "C" {
 #define B200_IR_L_BINOMIAL_LOGIT 5  /* y ~ Binomial(n, logit_p = eta)            discrete.py:141-152    */
 #define B200_IR_L_NEGBINOMIAL_LOG 6 /* y ~ NegativeBinomial(mu = exp(eta), alpha) discrete.py:700-745   */
 #define B200_IR_L_GAMMA_LOG 7       /* y ~ Gamma(alpha, beta = alpha exp(-eta))  continuous.py:2478-2521 */
+/* The support rule b200_model_create enforces (as ModelIR.validate does): HalfNormal, HalfCauchy, Exponential, Gamma and
+ * LogNormal priors sit on a LOG variable or an INTERVAL with lo >= 0, Beta on an INTERVAL inside [0, 1], Uniform(a, b) on an
+ * INTERVAL inside [a, b]; every scale (a prior's sigma / beta / lam, Normal and StudentT sigma including each sigma_obs, an
+ * AR(1) sigma, alpha) is a finite constant > 0 or a REF to a scalar of positive support; Poisson y are integers >= 0,
+ * Bernoulli y are 0 or 1. */
 #define B200_IR_S_NONE 0
 #define B200_IR_S_CONST 1 /* sigma.value               */
 #define B200_IR_S_REF 2   /* sigma = x[sigma.ref]      */

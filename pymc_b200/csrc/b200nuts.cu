@@ -362,6 +362,21 @@ static int ir_param(const b200_ir_param& p, int n, IrParamD* out, const char* wh
     return 0;
 }
 
+// The support rule (pymc_b200/ir.py: ModelIR.validate, same wording): the device evaluates a density's formula wherever
+// it is asked to, so a variable must be kept inside its prior's support by its transform, and every scale parameter must
+// be positive.  A variable has positive support under a log transform or an interval with lo >= 0.
+static bool ir_positive_support(const IrVarD& V) { return V.transform == IRT_LOG || (V.transform == IRT_INTERVAL && V.lo >= 0); }
+
+// A scale slot (a prior's sigma / beta / lam, a likelihood's sigma, an AR(1) sigma, a dispersion alpha): a finite constant
+// > 0, or a reference to a scalar variable with positive support.
+static bool ir_scale_ok(const b200_ir_param& p, const std::vector<IrVarD>& vars) {
+    if (p.kind == 0) return std::isfinite(p.value) && p.value > 0;
+    for (const IrVarD& V : vars)
+        if (p.ref >= V.offset && p.ref < V.offset + V.size) return V.size == 1 && ir_positive_support(V);
+    return false;
+}
+#define B200_IR_SCALE_RULE "must be a finite constant > 0 or a scalar variable with positive support (a log transform, or an interval with lo >= 0)"
+
 static int prepare_ir(b200_model* m, const b200_model_desc* d) {
     const b200_ir* R = d->ir;
     if (!R) return fail("ir: desc.ir is null");
@@ -388,6 +403,19 @@ static int prepare_ir(b200_model* m, const b200_model_desc* d) {
         for (int a = 0; a < 3; ++a)
             if (ir_param(F.p[a], n, &P.p[a], "prior")) return -1;
         auto cst = [&](int a) { return F.p[a].kind == 0; };
+        const IrVarD& PV = vars[F.var];
+        int scale = -1;  // which parameter is the prior's scale
+        switch (F.dist) {
+            case B200_IR_P_NORMAL: case B200_IR_P_LOGNORMAL: case B200_IR_P_CAUCHY: scale = 1; break;
+            case B200_IR_P_HALFNORMAL: case B200_IR_P_HALFCAUCHY: case B200_IR_P_EXPONENTIAL: scale = 0; break;
+            case B200_IR_P_STUDENTT: scale = 2; break;
+            default: break;
+        }
+        if (scale >= 0 && !ir_scale_ok(F.p[scale], vars)) return fail("ir: prior %d: parameter %d (the scale) " B200_IR_SCALE_RULE, k, scale);
+        const bool positive = F.dist == B200_IR_P_HALFNORMAL || F.dist == B200_IR_P_HALFCAUCHY || F.dist == B200_IR_P_EXPONENTIAL ||
+                              F.dist == B200_IR_P_GAMMA || F.dist == B200_IR_P_LOGNORMAL;
+        if (positive && !ir_positive_support(PV))
+            return fail("ir: prior %d: the variable needs a log transform or an interval with lo >= 0 (positive support)", k);
         switch (F.dist) {
             case B200_IR_P_FLAT: break;
             case B200_IR_P_NORMAL: case B200_IR_P_LOGNORMAL: P.c0 = -B200_HALF_LOG_2PI; break;
@@ -402,6 +430,8 @@ static int prepare_ir(b200_model* m, const b200_model_desc* d) {
             } break;
             case B200_IR_P_UNIFORM:
                 if (!cst(0) || !cst(1) || !(F.p[0].value < F.p[1].value)) return fail("ir: prior %d: Uniform bounds must be constants lo < hi", k);
+                if (!(PV.transform == IRT_INTERVAL && PV.lo >= F.p[0].value && PV.hi <= F.p[1].value))
+                    return fail("ir: prior %d: the variable needs an interval inside the Uniform bounds", k);
                 P.c0 = -std::log(F.p[1].value - F.p[0].value);
                 break;
             case B200_IR_P_GAMMA:
@@ -410,6 +440,7 @@ static int prepare_ir(b200_model* m, const b200_model_desc* d) {
                 break;
             case B200_IR_P_BETA:
                 if (!cst(0) || !cst(1) || !(F.p[0].value > 0) || !(F.p[1].value > 0)) return fail("ir: prior %d: Beta needs constant alpha, beta > 0", k);
+                if (!(PV.transform == IRT_INTERVAL && PV.lo >= 0 && PV.hi <= 1)) return fail("ir: prior %d: the variable needs an interval inside [0, 1]", k);
                 P.c0 = -(std::lgamma(F.p[0].value) + std::lgamma(F.p[1].value) - std::lgamma(F.p[0].value + F.p[1].value));
                 break;
             default: return fail("ir: prior %d: density %d is not in the closed set", k, F.dist);
@@ -430,14 +461,27 @@ static int prepare_ir(b200_model* m, const b200_model_desc* d) {
         if (upload_raw(m, L.y, (size_t)N, &D.y)) return -1;
         if (ir_param(L.sigma, n, &D.sigma, "likelihood sigma")) return -1;
         if (L.sigma_kind == B200_IR_S_REF && L.sigma.kind != 1) return fail("ir: likelihood %d: sigma_kind REF needs a reference", l);
+        b200_ir_param slot = L.sigma;  // the parameter slot as the device reads it: x[ref] for REF, else the value
+        slot.kind = L.sigma_kind == B200_IR_S_REF ? 1 : 0;
         if (L.sigma_kind == B200_IR_S_OBS) {
             if (!L.sigma_obs) return fail("ir: likelihood %d: sigma_obs missing", l);
             if (upload_raw(m, L.sigma_obs, (size_t)N, &D.sigma_obs)) return -1;
         }
         switch (L.dist) {
             case B200_IR_L_NORMAL: case B200_IR_L_NORMAL_LOGVAR: D.c0 = -(double)N * B200_HALF_LOG_2PI; break;
-            case B200_IR_L_BERNOULLI_LOGIT: break;
-            case B200_IR_L_POISSON_LOG: { double c = 0; for (long long i = 0; i < N; ++i) c -= std::lgamma(L.y[i] + 1.0); D.c0 = c; } break;
+            case B200_IR_L_BERNOULLI_LOGIT:
+                for (long long i = 0; i < N; ++i)
+                    if (L.y[i] != 0.0 && L.y[i] != 1.0) return fail("ir: likelihood %d: bernoulli_logit: y must be 0 or 1 (at %lld)", l, i);
+                break;
+            case B200_IR_L_POISSON_LOG: {
+                double c = 0;
+                for (long long i = 0; i < N; ++i) {
+                    const double y = L.y[i];
+                    if (!(y >= 0) || y != std::floor(y) || std::isinf(y)) return fail("ir: likelihood %d: poisson_log: y must be integers >= 0 (at %lld)", l, i);
+                    c -= std::lgamma(y + 1.0);
+                }
+                D.c0 = c;
+            } break;
             case B200_IR_L_STUDENTT:
                 if (!(L.nu > 0)) return fail("ir: likelihood %d: StudentT nu must be > 0", l);
                 D.c0 = (double)N * (std::lgamma(0.5 * (L.nu + 1.0)) - std::lgamma(0.5 * L.nu) - 0.5 * std::log(L.nu) - 0.5 * LOG_PI);
@@ -457,7 +501,7 @@ static int prepare_ir(b200_model* m, const b200_model_desc* d) {
             case B200_IR_L_NEGBINOMIAL_LOG: {
                 if (L.sigma_kind != B200_IR_S_CONST && L.sigma_kind != B200_IR_S_REF)
                     return fail("ir: likelihood %d: NegativeBinomial alpha must be a constant or a scalar variable", l);
-                if (L.sigma_kind == B200_IR_S_CONST && !(L.sigma.value > 0 && std::isfinite(L.sigma.value))) return fail("ir: likelihood %d: NegativeBinomial alpha must be finite and > 0", l);
+                if (!ir_scale_ok(slot, vars)) return fail("ir: likelihood %d: NegativeBinomial alpha " B200_IR_SCALE_RULE, l);
                 const double a = L.sigma.value;
                 const bool fold = L.sigma_kind == B200_IR_S_CONST && a <= kNegBinPoissonAlpha;
                 double c = 0;
@@ -480,7 +524,7 @@ static int prepare_ir(b200_model* m, const b200_model_desc* d) {
             case B200_IR_L_GAMMA_LOG: {
                 if (L.sigma_kind != B200_IR_S_CONST && L.sigma_kind != B200_IR_S_REF)
                     return fail("ir: likelihood %d: Gamma alpha must be a constant or a scalar variable", l);
-                if (L.sigma_kind == B200_IR_S_CONST && !(L.sigma.value > 0 && std::isfinite(L.sigma.value))) return fail("ir: likelihood %d: Gamma alpha must be finite and > 0", l);
+                if (!ir_scale_ok(slot, vars)) return fail("ir: likelihood %d: Gamma alpha " B200_IR_SCALE_RULE, l);
                 double sly = 0;
                 for (long long i = 0; i < N; ++i) {
                     if (!(L.y[i] > 0) || std::isinf(L.y[i])) return fail("ir: likelihood %d: Gamma y must be > 0 (at %lld)", l, i);
@@ -497,12 +541,14 @@ static int prepare_ir(b200_model* m, const b200_model_desc* d) {
         }
         if ((L.dist == B200_IR_L_NORMAL || L.dist == B200_IR_L_STUDENTT) && L.sigma_kind == B200_IR_S_NONE)
             return fail("ir: likelihood %d needs sigma", l);
-        if ((L.dist == B200_IR_L_NEGBINOMIAL_LOG || L.dist == B200_IR_L_GAMMA_LOG) && L.sigma_kind == B200_IR_S_REF) {
-            bool positive = false;  // the referenced scalar must have positive support: log, or interval with lo >= 0
-            for (const IrVarD& V : vars)
-                if (L.sigma.ref >= V.offset && L.sigma.ref < V.offset + V.size)
-                    positive = V.size == 1 && (V.transform == B200_IR_T_LOG || (V.transform == B200_IR_T_INTERVAL && V.lo >= 0));
-            if (!positive) return fail("ir: likelihood %d: a random alpha must be a scalar variable with positive support", l);
+        if (L.dist == B200_IR_L_NORMAL || L.dist == B200_IR_L_STUDENTT) {
+            if (L.sigma_kind == B200_IR_S_OBS) {
+                for (long long i = 0; i < N; ++i)
+                    if (!(std::isfinite(L.sigma_obs[i]) && L.sigma_obs[i] > 0))
+                        return fail("ir: likelihood %d: sigma must be a finite constant > 0 for every observation (at %lld)", l, i);
+            } else if (!ir_scale_ok(slot, vars)) {
+                return fail("ir: likelihood %d: sigma " B200_IR_SCALE_RULE, l);
+            }
         }
         for (int t = 0; t < L.n_terms; ++t) {
             const b200_ir_term& T = L.terms[t];
@@ -542,6 +588,7 @@ static int prepare_ir(b200_model* m, const b200_model_desc* d) {
         IrAr1D D{};
         D.offset = vars[A.var].offset; D.size = vars[A.var].size; D.init_sigma = A.init_sigma;
         if (ir_param(A.phi, n, &D.phi, "ar1 phi") || ir_param(A.sigma, n, &D.sigma, "ar1 sigma")) return -1;
+        if (!ir_scale_ok(A.sigma, vars)) return fail("ir: ar1 %d: sigma " B200_IR_SCALE_RULE, k);
         ars[k] = D;
     }
     IrModel::Params& P = m->ir;

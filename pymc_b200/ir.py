@@ -52,9 +52,19 @@ LIK_DISTS = {
     "gamma_log": 7,          # y_i ~ Gamma(alpha, beta = alpha exp(-eta_i))             continuous.py:2478-2521
 }
 DISPERSION_LIKS = ("negative_binomial_log", "gamma_log")  # their `alpha` is a constant or a Ref
+# The support rule.  The device evaluates a density's formula wherever it is asked to, so every variable must be kept
+# inside its prior's support by its transform, and every scale parameter must be positive:
+POSITIVE_PRIORS = ("halfnormal", "halfcauchy", "exponential", "gamma", "lognormal")  # a log transform, or interval lo >= 0
+SCALE_PARAMS = {"normal": {1: "sigma"}, "lognormal": {1: "sigma"}, "halfnormal": {0: "sigma"}, "cauchy": {1: "beta"},
+                "halfcauchy": {0: "beta"}, "exponential": {0: "lam"}, "studentt": {2: "sigma"}}
+POSITIVE_SUPPORT = "a scalar variable with positive support (a log transform, or an interval with lo >= 0)"
 NEGBIN_POISSON_ALPHA = 1e10  # above: the NegativeBinomial density is its Poisson(mu) limit (discrete.py:727-735)
 SIGMA_NONE, SIGMA_CONST, SIGMA_REF, SIGMA_OBS = 0, 1, 2, 3
 MAX_TERM_FACTORS = 3
+
+
+def _positive_support(v) -> bool:
+    return v.transform == "log" or (v.transform == "interval" and v.bounds[0] >= 0.0)
 
 
 @dataclass(frozen=True)
@@ -172,13 +182,16 @@ class ModelIR:
                 raise ValueError(f"prior {p.dist!r} is not in the closed set {sorted(PRIOR_DISTS)}")
             if len(p.params) != PRIOR_DISTS[p.dist][1]:
                 raise ValueError(f"prior {p.dist} on {p.var}: expected {PRIOR_DISTS[p.dist][1]} parameters")
-            self.var(p.var)
+            v = self.var(p.var)
             for k, a in enumerate(p.params):
                 if isinstance(a, Ref):
                     if self.var(a.var).size != 1:
                         raise ValueError(f"prior on {p.var}: parameter {a.var} must be a scalar variable")
                     if p.dist in ("uniform", "gamma", "beta") or (p.dist == "studentt" and k == 0):
                         raise ValueError(f"prior {p.dist} on {p.var}: parameter {k} must be a constant")
+                if k in SCALE_PARAMS.get(p.dist, {}):
+                    self._check_scale(a, f"prior {p.dist} on {v.name}: {SCALE_PARAMS[p.dist][k]}")
+            self._check_prior_support(p, v)
         for L in self.likelihoods:
             if L.dist not in LIK_DISTS:
                 raise ValueError(f"likelihood {L.dist!r} is not in the closed set {sorted(LIK_DISTS)}")
@@ -198,6 +211,22 @@ class ModelIR:
                 raise ValueError(f"{L.dist} likelihood needs sigma")
             if isinstance(L.sigma, Ref) and self.var(L.sigma.var).size != 1:
                 raise ValueError("likelihood sigma must be a scalar variable")
+            if L.dist in ("normal", "studentt"):
+                if not isinstance(L.sigma, Ref) and np.ndim(L.sigma) == 1:
+                    s = np.asarray(L.sigma, dtype=np.float64)
+                    if len(s) != N:
+                        raise ValueError(f"{L.dist} likelihood {L.name}: sigma must be a scalar or one per observation")
+                    if not (np.all(np.isfinite(s)) and np.all(s > 0)):
+                        raise ValueError(f"{L.dist} likelihood {L.name}: sigma must be a finite constant > 0 for every observation")
+                else:
+                    self._check_scale(L.sigma, f"{L.dist} likelihood {L.name}: sigma")
+            if L.dist == "studentt" and not (np.isfinite(L.nu) and L.nu > 0):
+                raise ValueError(f"studentt likelihood {L.name}: StudentT nu must be > 0")
+            y = np.asarray(L.y, dtype=np.float64)
+            if L.dist == "poisson_log" and not (np.all(np.isfinite(y)) and np.all(y == np.floor(y)) and np.all(y >= 0)):
+                raise ValueError("poisson_log: y must be integers >= 0")
+            if L.dist == "bernoulli_logit" and not np.all((y == 0.0) | (y == 1.0)):
+                raise ValueError("bernoulli_logit: y must be 0 or 1")
             self._validate_family(L)
         for a in self.ar1:
             if self.var(a.var).size < 2:
@@ -205,6 +234,39 @@ class ModelIR:
             for r in (a.phi, a.sigma):
                 if isinstance(r, Ref) and self.var(r.var).size != 1:
                     raise ValueError("AR1 parameters must be scalar variables or constants")
+            self._check_scale(a.sigma, f"AR1 on {a.var}: sigma")
+            if not (np.isfinite(a.init_sigma) and a.init_sigma > 0):
+                raise ValueError(f"AR1 on {a.var}: init_sigma must be > 0")
+
+    def _check_scale(self, a, what: str) -> None:
+        """A scale slot (a prior's sigma / beta / lam, a likelihood's sigma, an AR(1) sigma, a dispersion alpha): a finite
+        constant > 0, or a Ref to a scalar variable whose transform keeps it positive."""
+        if isinstance(a, Ref):
+            v = self.var(a.var)
+            if v.size == 1 and _positive_support(v):
+                return
+        elif np.ndim(a) == 0 and np.isfinite(float(a)) and float(a) > 0:
+            return
+        raise ValueError(f"{what} must be a finite constant > 0 or {POSITIVE_SUPPORT}")
+
+    def _check_prior_support(self, p, v) -> None:
+        """The variable's transform keeps it inside the prior's support; the constant parameters are in their domain."""
+        lo, hi = v.bounds if v.transform == "interval" else (None, None)
+        if p.dist in POSITIVE_PRIORS and not _positive_support(v):
+            raise ValueError(f"prior {p.dist} on {v.name}: the variable needs a log transform or an interval with lo >= 0 "
+                             "(positive support)")
+        if p.dist == "studentt" and not (np.isfinite(float(p.params[0])) and float(p.params[0]) > 0):
+            raise ValueError(f"prior studentt on {v.name}: StudentT nu must be a positive constant")
+        if p.dist in ("gamma", "beta") and not all(np.isfinite(float(a)) and float(a) > 0 for a in p.params):
+            raise ValueError(f"prior {p.dist} on {v.name}: {p.dist.capitalize()} needs constant alpha, beta > 0")
+        if p.dist == "beta" and not (lo is not None and lo >= 0.0 and hi <= 1.0):
+            raise ValueError(f"prior beta on {v.name}: the variable needs an interval inside [0, 1]")
+        if p.dist == "uniform":
+            a, b = float(p.params[0]), float(p.params[1])
+            if not a < b:
+                raise ValueError(f"prior uniform on {v.name}: Uniform bounds must be constants lo < hi")
+            if not (lo is not None and lo >= a and hi <= b):
+                raise ValueError(f"prior uniform on {v.name}: the variable needs an interval inside the Uniform bounds")
 
     def _validate_family(self, L) -> None:
         """Support and parameter rules of the count / positive families (the same checks prepare_ir makes)."""
@@ -225,14 +287,9 @@ class ModelIR:
         if L.dist in DISPERSION_LIKS:
             if L.alpha is None:
                 raise ValueError(f"{L.dist} needs alpha")
-            if isinstance(L.alpha, Ref):
-                v = self.var(L.alpha.var)
-                if v.size != 1:
-                    raise ValueError(f"{L.dist}: alpha must be a scalar variable")
-                if not (v.transform == "log" or (v.transform == "interval" and v.bounds[0] >= 0)):
-                    raise ValueError(f"{L.dist}: alpha {v.name} needs positive support (a log transform, or an interval with lo >= 0)")
-            elif not (np.ndim(L.alpha) == 0 and np.isfinite(float(L.alpha)) and float(L.alpha) > 0):
-                raise ValueError(f"{L.dist}: a constant alpha must be a finite scalar > 0")
+            if isinstance(L.alpha, Ref) and self.var(L.alpha.var).size != 1:
+                raise ValueError(f"{L.dist}: alpha must be a scalar variable")
+            self._check_scale(L.alpha, f"{L.dist}: alpha")
             if L.dist == "negative_binomial_log" and (not integer(y) or np.any(y < 0)):
                 raise ValueError("negative_binomial_log: y must be integers >= 0")
             if L.dist == "gamma_log" and not (np.all(np.isfinite(y)) and np.all(y > 0)):

@@ -812,22 +812,30 @@ static int env_int(const char* name, int dflt) {
 // ------------------------------------------------------------------------------------------------
 // b200_logp_dlogp
 // ------------------------------------------------------------------------------------------------
+// Launch of a one-point-per-team kernel (logp_grad_warp_kernel, leapfrog_warp_kernel) over C points: 8 chains per CTA at
+// chain = warp, one at chain = CTA; shared memory = the model's data + q, g and the team's reduction pad per chain.
+template <class Model, int NPL, int W, class Kern, class... Args>
+static int launch_point_kernel(Kern kern, const b200_model* m, const typename Model::Params& MP, int C, cudaStream_t st,
+                               Args... args) {
+    const int wpb = (W == 1) ? 8 : 1;  // chains per CTA
+    const size_t data = (Model::shared_bytes(MP) + 15) & ~(size_t)15;
+    const size_t smem = data + (size_t)wpb * (2 * 32 * W * NPL + (W > 1 ? 8 * W : 0)) * sizeof(double);
+    CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+    const int blocks = std::max(1, std::min((C + wpb - 1) / wpb, sm_count(m->device) * 8));
+    typename Model::Params MPl;
+    if (launch_params<Model>(m, MP, (long long)blocks * wpb, &MPl)) return -1;
+    kern<<<blocks, (W == 1) ? wpb * 32 : 32 * W, smem, st>>>(MPl, m->n, C, args...);
+    CU(cudaGetLastError());
+    return 0;
+}
+
 struct LogpLaunch {
     const b200_model* m; int C; const double* q; double* logp; double* grad; cudaStream_t st;
     long long ldq = 0, ldg = 0;  // row strides (0: contiguous rows of n)
     template <class Model, int NPL, int W>
     int operator()(const typename Model::Params& MP) const {
-        const int wpb = (W == 1) ? 8 : 1;  // chains per CTA
-        const size_t data = (Model::shared_bytes(MP) + 15) & ~(size_t)15;
-        const size_t smem = data + (size_t)wpb * (2 * 32 * W * NPL + (W > 1 ? 8 * W : 0)) * sizeof(double);
-        auto kern = logp_grad_warp_kernel<Model, NPL, W>;
-        CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        const int blocks = std::max(1, std::min((C + wpb - 1) / wpb, sm_count(m->device) * 8));
-        typename Model::Params MPl;
-        if (launch_params<Model>(m, MP, (long long)blocks * wpb, &MPl)) return -1;
-        kern<<<blocks, (W == 1) ? wpb * 32 : 32 * W, smem, st>>>(MPl, m->n, C, q, logp, grad, ldq ? ldq : m->n, ldg ? ldg : m->n);
-        CU(cudaGetLastError());
-        return 0;
+        return launch_point_kernel<Model, NPL, W>(logp_grad_warp_kernel<Model, NPL, W>, m, MP, C, st, q, logp, grad,
+                                                  ldq ? ldq : (long long)m->n, ldg ? ldg : (long long)m->n);
     }
 };
 
@@ -863,17 +871,8 @@ struct LeapLaunch {
     long long* idx; cudaStream_t st;
     template <class Model, int NPL, int W>
     int operator()(const typename Model::Params& MP) const {
-        const int wpb = (W == 1) ? 8 : 1;
-        const size_t data = (Model::shared_bytes(MP) + 15) & ~(size_t)15;
-        const size_t smem = data + (size_t)wpb * (2 * 32 * W * NPL + (W > 1 ? 8 * W : 0)) * sizeof(double);
-        auto kern = leapfrog_warp_kernel<Model, NPL, W>;
-        CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        const int blocks = std::max(1, std::min((C + wpb - 1) / wpb, sm_count(m->device) * 8));
-        typename Model::Params MPl;
-        if (launch_params<Model>(m, MP, (long long)blocks * wpb, &MPl)) return -1;
-        kern<<<blocks, (W == 1) ? wpb * 32 : 32 * W, smem, st>>>(MPl, m->n, C, var, eps, n_steps, q, p, v, grad, energy, logp, idx);
-        CU(cudaGetLastError());
-        return 0;
+        return launch_point_kernel<Model, NPL, W>(leapfrog_warp_kernel<Model, NPL, W>, m, MP, C, st, var, eps, n_steps, q, p,
+                                                  v, grad, energy, logp, idx);
     }
 };
 
@@ -1540,45 +1539,39 @@ extern "C" int b200_nuts_run(b200_model* m, const b200_nuts_cfg* cfg, const doub
         if (stage_state(cfg->resume, &d_resume, true) || stage_state(cfg->save, &d_save, false)) return -1;
     }
 
-    NutsDev P{};
-    P.it0 = (int)it0; P.n_iter = (int)Ttot; P.resume = d_resume; P.save = d_save;
-    P.C = C; P.n = n; P.tune = cfg->tune; P.draws = cfg->draws;
-    P.max_td = cfg->max_treedepth; P.early_td = cfg->early_max_treedepth;
-    P.adapt_step = cfg->adapt_step_size; P.mass_kind = cfg->mass_kind;
-    P.momentum_source = cfg->momentum_source; P.store_warmup = cfg->store_warmup;
-    P.window = cfg->adaptation_window; P.discard = cfg->discard_window;
-    P.eps0 = cfg->step_scale / std::pow((double)n, 0.25);  // base_hmc.py:161
-    P.target = cfg->target_accept; P.gamma = cfg->gamma; P.kappa = cfg->k; P.t0 = cfg->t0;
-    P.Emax = cfg->Emax; P.init_weight = cfg->mass_initial_weight;
-    P.philox_seed = cfg->philox_seed; P.chain_offset = cfg->chain_offset;
-    P.sampler = cfg->sampler; P.max_steps = cfg->max_steps; P.path_length = cfg->path_length;
-    P.mass_alpha = cfg->mass_alpha; P.stop_adaptation = cfg->stop_adaptation < 0 ? 0x7fffffff : cfg->stop_adaptation;
-    P.q0 = (const double*)s_q0.ptr(); P.var0 = (const double*)s_var0.ptr();
-    P.mean0 = (const double*)s_mean0.ptr(); P.eps0c = (const double*)s_eps0.ptr(); P.z = (const double*)s_z.ptr();
-    P.rng = (b200_pcg64*)s_rng.ptr(); P.draws_out = (double*)s_draws.ptr();
-    P.st = ds; P.sm = dsum;
+    RunCfg R{};
+    R.it0 = (int)it0; R.n_iter = (int)Ttot;
+    R.C = C; R.n = n; R.tune = cfg->tune; R.draws = cfg->draws;
+    R.max_td = cfg->max_treedepth; R.early_td = cfg->early_max_treedepth;
+    R.adapt_step = cfg->adapt_step_size; R.mass_kind = cfg->mass_kind;
+    R.momentum_source = cfg->momentum_source; R.store_warmup = cfg->store_warmup;
+    R.window = cfg->adaptation_window; R.discard = cfg->discard_window;
+    R.eps0 = cfg->step_scale / std::pow((double)n, 0.25);  // base_hmc.py:161
+    R.target = cfg->target_accept; R.gamma = cfg->gamma; R.kappa = cfg->k; R.t0 = cfg->t0;
+    R.Emax = cfg->Emax; R.init_weight = cfg->mass_initial_weight;
+    R.philox_seed = cfg->philox_seed; R.chain_offset = cfg->chain_offset;
+    R.q0 = (const double*)s_q0.ptr(); R.var0 = (const double*)s_var0.ptr();
+    R.mean0 = (const double*)s_mean0.ptr(); R.eps0c = (const double*)s_eps0.ptr(); R.z = (const double*)s_z.ptr();
+    R.rng = (b200_pcg64*)s_rng.ptr(); R.draws_out = (double*)s_draws.ptr();
+    R.st = ds; R.sm = dsum;
     if (cfg->constrain_draws) {
         if (!m->tr_kind) return fail("b200_nuts_run: constrain_draws needs b200_model_set_transforms first");
-        P.tr_kind = m->tr_kind; P.tr_lo = m->tr_lo; P.tr_hi = m->tr_hi;
+        R.tr_kind = m->tr_kind; R.tr_lo = m->tr_lo; R.tr_hi = m->tr_hi;
     }
 
     const double tr_stage = trace ? since(tr0) : 0.0;
     const auto tr1 = std::chrono::steady_clock::now();
     if (lockstep) {
-        LsDev Q{};
-        Q.C = C; Q.n = n; Q.tune = P.tune; Q.draws = P.draws; Q.max_td = P.max_td; Q.early_td = P.early_td;
-        Q.adapt_step = P.adapt_step; Q.mass_kind = P.mass_kind; Q.momentum_source = P.momentum_source;
-        Q.store_warmup = P.store_warmup; Q.window = P.window; Q.discard = P.discard; Q.chain_offset = P.chain_offset;
+        LsDev Q{R};
         Q.dense = (cfg->mass_kind == B200_MASS_DENSE || cfg->mass_kind == B200_MASS_DENSE_ADAPT) ? 1 : 0;
         Q.upd_window = cfg->mass_update_window > 0 ? cfg->mass_update_window : 1;
         Q.win_mult = cfg->adaptation_window_multiplier > 0 ? cfg->adaptation_window_multiplier : 2.0;
-        Q.eps0 = P.eps0; Q.target = P.target; Q.gamma = P.gamma; Q.kappa = P.kappa; Q.t0 = P.t0; Q.Emax = P.Emax;
-        Q.init_weight = P.init_weight; Q.philox_seed = P.philox_seed;
-        Q.q0 = P.q0; Q.var0 = P.var0; Q.mean0 = P.mean0; Q.eps0c = P.eps0c; Q.z = P.z; Q.rng = P.rng;
-        Q.draws_out = P.draws_out; Q.st = P.st; Q.sm = P.sm;
-        Q.tr_kind = P.tr_kind; Q.tr_lo = P.tr_lo; Q.tr_hi = P.tr_hi;
         if (run_lockstep(m, Q, st)) return -1;
     } else {
+        NutsDev P{R};
+        P.resume = d_resume; P.save = d_save;
+        P.sampler = cfg->sampler; P.max_steps = cfg->max_steps; P.path_length = cfg->path_length;
+        P.mass_alpha = cfg->mass_alpha; P.stop_adaptation = cfg->stop_adaptation < 0 ? 0x7fffffff : cfg->stop_adaptation;
         NutsLaunch L{m, P, st};
         if (dispatch(m, L)) return -1;
     }

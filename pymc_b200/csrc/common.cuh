@@ -208,24 +208,6 @@ __device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t phase) {
         : "memory");
 }
 
-// Stats of an iteration that never ran (chain frozen by "Bad initial energy"): zeros / NaN, so caller-provided output
-// buffers need no clearing before a run and a reused buffer never shows values of an earlier run.
-__device__ __forceinline__ void stats_sentinel(const b200_stats& st, long long o) {
-    const double qnan = nan("");
-    if (st.depth) st.depth[o] = 0;
-    if (st.tree_size) st.tree_size[o] = 0;
-    if (st.index_in_trajectory) st.index_in_trajectory[o] = 0;
-    if (st.diverging) st.diverging[o] = 0;
-    if (st.reached_max_treedepth) st.reached_max_treedepth[o] = 0;
-    if (st.step_size) st.step_size[o] = qnan;
-    if (st.step_size_bar) st.step_size_bar[o] = qnan;
-    if (st.mean_tree_accept) st.mean_tree_accept[o] = qnan;
-    if (st.energy) st.energy[o] = qnan;
-    if (st.energy_error) st.energy_error[o] = qnan;
-    if (st.max_energy_error) st.max_energy_error[o] = qnan;
-    if (st.model_logp) st.model_logp[o] = qnan;
-}
-
 // Draw post-processing fused into the record step (SURVEY 8f-1): the backward transform of one element, what the reference
 // evaluates per draw through a compiled function (backends/ndarray.py:108; transforms logprob/transforms.py:880-891,
 // :1026-1045).  kind == null: the unconstrained value is recorded.

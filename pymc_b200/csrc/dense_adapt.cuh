@@ -105,9 +105,10 @@ __global__ void __launch_bounds__(kFaThreads) fa_update_momentum_kernel(const Ls
     const int chain = P.mom_list[jj], n = P.n, tid = threadIdx.x;
     const long long nn = (long long)n * n;
     LsState* SP = P.state + chain;
-    // scalars of the chain (identical in every thread; thread 0 writes them back)
-    int k_samples = SP->k_samples, window = SP->window, prev = SP->prev_update, fa_fg = SP->fa_fg, fg_m = SP->fg_m, bg_m = SP->bg_m;
-    double fg_n = SP->fg_n, bg_n = SP->bg_n;
+    // scalars of the chain (identical in every thread; thread 0 writes them back).  Only the window's mean slots are used:
+    // dw.swap() also exchanges the variance slot ids, which nothing reads under DENSE_ADAPT.
+    DiagWindow dw = SP->dw;
+    int prev = SP->prev_update, fa_fg = SP->fa_fg;
     const int upd = SP->upd_pending, it = SP->mom_it;
     int chol_bad = SP->chol_bad;
     double* vb = P.vecs + (long long)chain * P.vec_stride;
@@ -117,25 +118,21 @@ __global__ void __launch_bounds__(kFaThreads) fa_update_momentum_kernel(const Ls
 
     if (upd) {
         // ---- QuadPotentialFullAdapt.update (quadpotential.py:818-843), sample = the accepted position ------------------
-        const int delta = k_samples - prev;
+        const int delta = dw.k_samples - prev;
         const double* x = vb + (long long)LV_Q * n;
-        double* fm = vb + (long long)fg_m * n;
-        double* bm = vb + (long long)bg_m * n;
-        fg_n += 1.0; bg_n += 1.0;  // _WeightedCovariance.add_sample :887-893
+        double* fm = vb + (long long)dw.fg_m * n;
+        double* bm = vb + (long long)dw.bg_m * n;
+        dw.fg_n += 1.0; dw.bg_n += 1.0;  // _WeightedCovariance.add_sample :887-893
         for (int i = tid; i < n; i += blockDim.x) {
             const double xi = x[i];
-            double mean = fm[i], d0 = xi - mean;
-            mean = __dadd_rn(mean, d0 / fg_n);
-            fm[i] = mean; before_f[i] = d0; after_f[i] = xi - mean;
-            mean = bm[i]; d0 = xi - mean;
-            mean = __dadd_rn(mean, d0 / bg_n);
-            bm[i] = mean; before_b[i] = d0; after_b[i] = xi - mean;
+            before_f[i] = welford_mean(xi, dw.fg_n, fm[i]); after_f[i] = xi - fm[i];
+            before_b[i] = welford_mean(xi, dw.bg_n, bm[i]); after_b[i] = xi - bm[i];
         }
         __syncthreads();
         const bool refresh = ((delta + 1) % P.upd_window) == 0;
         double* F = P.fa_raw + (2LL * chain + fa_fg) * nn;
         double* B = P.fa_raw + (2LL * chain + (fa_fg ^ 1)) * nn;
-        const double denom = fg_n - 1.0;  // current_covariance :895-901
+        const double denom = dw.fg_n - 1.0;  // current_covariance :895-901
         for (long long idx = tid; idx < nn; idx += blockDim.x) {
             const int i = (int)(idx / n), j = (int)(idx - (long long)i * n);
             const double f = __dadd_rn(F[idx], __dmul_rn(after_f[i], before_f[j]));
@@ -155,28 +152,23 @@ __global__ void __launch_bounds__(kFaThreads) fa_update_momentum_kernel(const Ls
             fa_matvec(cov, tmp, vb + (long long)LV_W * n, n);
             __syncthreads();
         }
-        if (delta >= window) {  // the background estimator takes over; a fresh one starts (:833-841)
+        if (delta >= dw.window) {  // the background estimator takes over; a fresh one starts (:833-841)
             fa_fg ^= 1;
-            const int t = fg_m; fg_m = bg_m; bg_m = t;
-            fg_n = bg_n; bg_n = 0.0;
+            dw.swap();
             double* nb = P.fa_raw + (2LL * chain + (fa_fg ^ 1)) * nn;
             for (long long idx = tid; idx < nn; idx += blockDim.x) nb[idx] = 0.0;  // eye * n_samples(0)
-            double* nm = vb + (long long)bg_m * n;
+            double* nm = vb + (long long)dw.bg_m * n;
             for (int i = tid; i < n; i += blockDim.x) nm[i] = 0.0;
-            prev = k_samples;
-            window = (int)(window * P.win_mult);
+            prev = dw.k_samples;
+            dw.window = (int)(dw.window * P.win_mult);
         }
-        ++k_samples;
+        ++dw.k_samples;
     }
 
     // ---- potential.random() for draw `it`: p0 = solve_triangular(chol^T, z) (quadpotential.py:710-713) ---------------------
     double* b = before_f;   // right-hand side, updated in place
     double* px = after_f;   // solution
-    const int Ttot = P.tune + P.draws;
-    for (int i = tid; i < n; i += blockDim.x)
-        b[i] = (P.momentum_source == B200_MOMENTUM_HOST_BUFFER)
-                   ? P.z[((long long)chain * Ttot + it) * n + i]
-                   : philox_normal(P.philox_seed, (uint32_t)(chain + P.chain_offset), (uint32_t)it, (uint32_t)i);
+    for (int i = tid; i < n; i += blockDim.x) b[i] = momentum_z(P, chain, it, i);
     __syncthreads();
     for (int j = n - 1; j >= 0; --j) {  // back substitution, row j of the factor is column j of its transpose (contiguous)
         const double* Lj = chol + (long long)j * n;
@@ -191,8 +183,7 @@ __global__ void __launch_bounds__(kFaThreads) fa_update_momentum_kernel(const Ls
     fa_matvec(cov, px, P.V0n + (long long)chain * P.ld, n);
 
     if (tid == 0) {
-        SP->k_samples = k_samples; SP->window = window; SP->prev_update = prev; SP->fa_fg = fa_fg;
-        SP->fg_m = fg_m; SP->bg_m = bg_m; SP->fg_n = fg_n; SP->bg_n = bg_n; SP->upd_pending = 0; SP->chol_bad = chol_bad;
+        SP->dw = dw; SP->prev_update = prev; SP->fa_fg = fa_fg; SP->upd_pending = 0; SP->chol_bad = chol_bad;
         SP->mom_have = it;
     }
 }

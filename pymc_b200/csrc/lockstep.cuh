@@ -9,7 +9,8 @@
 // doubling, end-of-draw adaptation), writes the next position into the dense request matrix and returns.
 // The logic and the order of random-number consumption are those of nuts_warp.cuh (same reference citations:
 // hmc/nuts.py:204-489, hmc/integration.py:68-145, hmc/base_hmc.py:196-288, step_sizes.py:41-84,
-// hmc/quadpotential.py:211-355 diag-adapt, :680-725 QuadPotentialFull).
+// hmc/quadpotential.py:211-355 diag-adapt, :680-725 QuadPotentialFull); the per-draw bookkeeping around the tree (step
+// size, Welford windows, statistics, momentum noise) is the same code, in sampler_state.cuh.
 //
 // Dense mass matrix (QuadPotentialFull): v = Sigma p is a GEMM.  By linearity ONE mass GEMM per leapfrog is
 // enough: every state carries w = Sigma.grad, then  v(p + dt g) = v + dt w  and  v(p' ) = v_half + dt w'.
@@ -20,9 +21,7 @@
 // chain = warp; all vectors live in HBM ([C][n] row-major, coalesced lane-strided loops); the O(n) vector work
 // per leaf is negligible next to the O(n^2) or O(N K) contraction.
 #pragma once
-#include "../../include/b200nuts.h"
-#include "common.cuh"
-#include "rng.cuh"
+#include "sampler_state.cuh"
 
 namespace b200 {
 
@@ -56,11 +55,12 @@ struct LsState {  // per-chain scalars, resident in HBM between calls
                   //     always stops here for the potential's update; a fixed dense mass only when its prefetch is still
                   //     queued, see "deferred momentum" in b200nuts.cu run_lockstep)
     int it, d_iter, maxd, depth, leaf, n_leaf, dir, w_idx, L_idx, R_idx, n_prop, m_pidx, c_pidx;
-    int da_count, k_samples, window, fg_m, fg_v, bg_m, bg_v, bad_at, diverged, need_mom, mom_it;
+    int bad_at, diverged, need_mom, mom_it;
     int prev_update, fa_fg, upd_pending, chol_bad;  // DENSE_ADAPT (dense_adapt.cuh): window start, foreground slot, flags
     int mom_have;  // dense mass: the iteration whose momentum (p0, v0) currently sits in the chain's rows of P0n / V0n
     double eps, E0, accept_sum, max_de, m_logw, m_pe, m_plogp, c_logw, c_pe, c_plogp, cur_logp;
-    double log_step, log_bar, hbar, da_mu, fg_n, bg_n;
+    StepSize ss;
+    DiagWindow dw;
     unsigned long long rs_hi, rs_lo, ri_hi, ri_lo;
     long long n_grad;
     double sc_logw[kLsLevels], sc_pe[kLsLevels], sc_plogp[kLsLevels];
@@ -78,17 +78,9 @@ enum {
 };
 __host__ __device__ inline long long ls_vec_count(int levels) { return LV_STACK + 8LL * levels; }
 
-struct LsDev {
-    int C, n, tune, draws, max_td, early_td, adapt_step, mass_kind, momentum_source, store_warmup;
-    int window, discard, chain_offset, dense;
-    double eps0, target, gamma, kappa, t0, Emax, init_weight, logp_const;
-    unsigned long long philox_seed;
-    const double* q0; const double* var0; const double* mean0; const double* eps0c; const double* z;
-    b200_pcg64* rng;
-    double* draws_out;
-    const signed char* tr_kind; const double* tr_lo; const double* tr_hi;  // record constrained values (common.cuh)
-    b200_stats st;
-    b200_chain_summary sm;
+struct LsDev : RunCfg {  // a whole schedule per run: it0 = 0, n_iter = tune + draws
+    int dense;
+    double logp_const;
     LsState* state;
     double* vecs; long long vec_stride;     // per-chain vector block
     long long ld;                              // row stride (doubles) of the request / result matrices: n rounded up to 4
@@ -244,11 +236,8 @@ __global__ void __launch_bounds__(W == 1 ? 128 : 32 * W) ls_advance_kernel(const
                 team_sum_n<W>(dots, lane, red);
                 bool turn = (dots[0] <= 0) || (dots[1] <= 0);
                 if (h > 0) turn = turn || (dots[2] <= 0) || (dots[3] <= 0) || (dots[4] <= 0) || (dots[5] <= 0);
-                const double t_logw = S.sc_logw[h];
-                const double dlw = S.c_logw - t_logw;
-                const double e_w = exp(-fabs(dlw));
-                const double logw = (dlw == 0.0) ? S.c_logw + 0.69314718055994530942
-                                                 : (isnan(dlw) ? S.c_logw + t_logw : fmax(S.c_logw, t_logw) + log1p_abs(e_w));
+                double dlw, e_w;
+                const double logw = merge_logw(S.c_logw, S.sc_logw[h], dlw, e_w);
                 const double u = rng.next_double();
                 if (!(u * (1.0 + e_w) < (dlw >= 0.0 ? 1.0 : e_w))) {  // keep tree1's proposal
                     const double* t_pq = LVL(h, 5); const double* t_pqg = LVL(h, 6); const double* t_pqw = LVL(h, 7);
@@ -307,8 +296,8 @@ __global__ void __launch_bounds__(W == 1 ? 128 : 32 * W) ls_advance_kernel(const
                 // biased progressive pick (nuts.py:370-374)
                 {
                     const double u = rng.next_double();
-                    const double dlw = S.c_logw - S.m_logw;
-                    const double e_w = exp(-fabs(dlw));
+                    double dlw, e_w;
+                    const double logw = merge_logw(S.c_logw, S.m_logw, dlw, e_w);
                     if (dlw >= 0.0 || u < e_w) {
                         double a_[U], b_[U], c_[U];
                         ls_tiled<U, TS>(lane, n,
@@ -316,8 +305,7 @@ __global__ void __launch_bounds__(W == 1 ? 128 : 32 * W) ls_advance_kernel(const
                             [&](int u, int i) { V(LV_PQ)[i] = a_[u]; V(LV_PQG)[i] = b_[u]; if (dense) V(LV_PQW)[i] = c_[u]; });
                         S.m_pe = S.c_pe; S.m_plogp = S.c_plogp; S.m_pidx = S.c_pidx;
                     }
-                    S.m_logw = (dlw == 0.0) ? S.c_logw + 0.69314718055994530942
-                                            : (isnan(dlw) ? S.c_logw + S.m_logw : fmax(S.c_logw, S.m_logw) + log1p_abs(e_w));
+                    S.m_logw = logw;
                 }
                 // U-turn checks on the whole tree (nuts.py:376-390)
                 {
@@ -379,61 +367,35 @@ __global__ void __launch_bounds__(W == 1 ? 128 : 32 * W) ls_advance_kernel(const
                 });
         }
         S.cur_logp = S.m_plogp;
-        if (adapting) {  // step_sizes.py:66-78
-            const double w = 1.0 / (S.da_count + P.t0);
-            S.hbar = __dadd_rn(__dmul_rn(1.0 - w, S.hbar), __dmul_rn(w, P.target - accept));
-            S.log_step = S.da_mu - __dmul_rn(S.hbar, sqrt((double)S.da_count)) / P.gamma;
-            const double mk = pow((double)S.da_count, -P.kappa);
-            S.log_bar = __dadd_rn(__dmul_rn(mk, S.log_step), __dmul_rn(1.0 - mk, S.log_bar));
-            ++S.da_count;
-        }
+        if (adapting) S.ss.update(P, accept);
         if (tuning && P.mass_kind == B200_MASS_DIAG_ADAPT) {  // quadpotential.py:335-355
-            if (S.k_samples > P.discard) {
-                S.fg_n += 1.0; S.bg_n += 1.0;
-                double* fm = V(S.fg_m); double* fv = V(S.fg_v); double* bm = V(S.bg_m); double* bv = V(S.bg_v);
+            if (S.dw.add_sample(P.discard)) {
+                double* fm = V(S.dw.fg_m); double* fv = V(S.dw.fg_v); double* bm = V(S.dw.bg_m); double* bv = V(S.dw.bg_v);
                 double x_[U], fm_[U], fv_[U], bm_[U], bv_[U];
                 ls_tiled<U, TS>(lane, n,
                     [&](int u, int i) { x_[u] = V(LV_Q)[i]; fm_[u] = fm[i]; fv_[u] = fv[i]; bm_[u] = bm[i]; bv_[u] = bv[i]; },
                     [&](int u, int i) {
-                        const double x = x_[u];
-                        double mean = fm_[u], d0 = x - mean;
-                        mean = __dadd_rn(mean, d0 / S.fg_n); fm[i] = mean;
-                        fv[i] = __dadd_rn(fv_[u], __dmul_rn(d0, x - mean));
-                        mean = bm_[u]; d0 = x - mean;
-                        mean = __dadd_rn(mean, d0 / S.bg_n); bm[i] = mean;
-                        bv[i] = __dadd_rn(bv_[u], __dmul_rn(d0, x - mean));
+                        welford_add(x_[u], S.dw.fg_n, fm_[u], fv_[u]);
+                        welford_add(x_[u], S.dw.bg_n, bm_[u], bv_[u]);
+                        fm[i] = fm_[u]; fv[i] = fv_[u]; bm[i] = bm_[u]; bv[i] = bv_[u];
                     });
             }
-            if (S.k_samples > S.window) {
-                const double* fv = V(S.fg_v);
+            if (S.dw.var_ready()) {
+                const double* fv = V(S.dw.fg_v);
                 double f_[U];
                 ls_tiled<U, TS>(lane, n, [&](int u, int i) { f_[u] = fv[i]; },
-                                [&](int u, int i) { V(LV_VAR)[i] = fmin(fmax(f_[u] / S.fg_n, 1e-12), 1e12); });
+                                [&](int u, int i) { V(LV_VAR)[i] = S.dw.variance(f_[u]); });
             }
-            if (S.k_samples > 0 && S.k_samples % S.window == 0) {
-                const int tm = S.fg_m, tv = S.fg_v;
-                S.fg_m = S.bg_m; S.fg_v = S.bg_v; S.fg_n = S.bg_n;
-                S.bg_m = tm; S.bg_v = tv; S.bg_n = 0.0;
+            if (S.dw.swap_due()) {
+                S.dw.swap();
                 B200_LS_UNROLL
-                for (int i = lane; i < n; i += TS) { V(S.bg_m)[i] = 0.0; V(S.bg_v)[i] = 0.0; }
+                for (int i = lane; i < n; i += TS) { V(S.dw.bg_m)[i] = 0.0; V(S.dw.bg_v)[i] = 0.0; }
             }
-            ++S.k_samples;
+            ++S.dw.k_samples;
         }
-        if (rec && lane == 0) {
-            const long long o = (long long)chain * T_out + t_out;
-            if (P.st.depth) P.st.depth[o] = S.depth;
-            if (P.st.tree_size) P.st.tree_size[o] = S.n_prop;
-            if (P.st.index_in_trajectory) P.st.index_in_trajectory[o] = S.m_pidx;
-            if (P.st.diverging) P.st.diverging[o] = S.diverged ? 1 : 0;
-            if (P.st.reached_max_treedepth) P.st.reached_max_treedepth[o] = hit_max ? 1 : 0;
-            if (P.st.step_size) P.st.step_size[o] = exp(S.log_step);
-            if (P.st.step_size_bar) P.st.step_size_bar[o] = exp(S.log_bar);
-            if (P.st.mean_tree_accept) P.st.mean_tree_accept[o] = accept;
-            if (P.st.energy) P.st.energy[o] = S.m_pe;
-            if (P.st.energy_error) P.st.energy_error[o] = S.m_pe - S.E0;
-            if (P.st.max_energy_error) P.st.max_energy_error[o] = S.max_de;
-            if (P.st.model_logp) P.st.model_logp[o] = S.m_plogp;
-        }
+        if (rec && lane == 0)
+            record_draw_stats(P.st, (long long)chain * T_out + t_out, S.depth, S.n_prop, S.m_pidx, S.diverged, hit_max, S.ss,
+                              accept, S.m_pe, S.m_pe - S.E0, S.max_de, S.m_plogp);
         ++S.it;
         if (S.it >= Ttot) S.phase = 2;
         else if (fa) {
@@ -467,10 +429,7 @@ __global__ void __launch_bounds__(W == 1 ? 128 : 32 * W) ls_advance_kernel(const
                 const double* var = V(LV_VAR);
                 B200_LS_UNROLL
                 for (int i = lane; i < n; i += TS) {
-                    const double zz = (P.momentum_source == B200_MOMENTUM_HOST_BUFFER)
-                                          ? P.z[((long long)chain * Ttot + S.it) * n + i]
-                                          : philox_normal(P.philox_seed, (uint32_t)(chain + P.chain_offset), (uint32_t)S.it, (uint32_t)i);
-                    const double pi = (1.0 / sqrt(var[i])) * zz, vi = var[i] * pi;
+                    const double pi = (1.0 / sqrt(var[i])) * momentum_z(P, chain, S.it, i), vi = var[i] * pi;
                     p[i] = pi; v[i] = vi; kin = fma(pi, vi, kin);
                 }
             }
@@ -480,15 +439,9 @@ __global__ void __launch_bounds__(W == 1 ? 128 : 32 * W) ls_advance_kernel(const
         if (!isfinite(S.E0) || S.chol_bad) {  // "Bad initial energy" (base_hmc.py:205-224): freeze; the iterations that never ran are NaN
             S.bad_at = S.it;
             S.phase = 2;
-            for (int t = S.it; t < Ttot; ++t) {
-                if (!(P.store_warmup || t >= P.tune)) continue;
-                const int t_o = P.store_warmup ? t : t - P.tune;
-                B200_LS_UNROLL
-                for (int i = lane; i < n; i += TS) P.draws_out[((long long)chain * T_out + t_o) * n + i] = nan("");
-                if (lane == 0) stats_sentinel(P.st, (long long)chain * T_out + t_o);
-            }
+            freeze_outputs<TS>(P, chain, S.it, Ttot, P.store_warmup ? 0 : P.tune, T_out, lane);
         } else {
-            S.eps = exp(adapting ? S.log_step : S.log_bar);
+            S.eps = S.ss.current(adapting);
             S.maxd = (tuning && S.it < 200) ? P.early_td : P.max_td;
             {
                 double q_[U], p_[U], g_[U], v_[U], w_[U];
@@ -568,9 +521,7 @@ __global__ void __launch_bounds__(W == 1 ? 128 : 32 * W) ls_advance_kernel(const
             b200_pcg64 r;
             r.state_hi = S.rs_hi; r.state_lo = S.rs_lo; r.inc_hi = S.ri_hi; r.inc_lo = S.ri_lo;
             P.rng[chain] = r;
-            if (P.sm.grad_evals) P.sm.grad_evals[chain] = S.n_grad;
-            if (P.sm.bad_energy_at) P.sm.bad_energy_at[chain] = S.bad_at;
-            if (P.sm.final_step_size) P.sm.final_step_size[chain] = exp(S.log_bar);
+            record_chain_summary(P.sm, chain, S.n_grad, S.bad_at, S.ss);
         }
         S.need_mom = 0;  // the host serves the request before the next advance
         *SP = S;
@@ -605,11 +556,9 @@ __global__ void __launch_bounds__(128) ls_init_kernel(const LsDev P) {
         memset(&S, 0, sizeof(S));
         S.phase = 0;
         S.bad_at = -1;
-        const double e0 = P.eps0c ? P.eps0c[chain] : P.eps0;
-        S.log_step = log(e0); S.log_bar = S.log_step; S.hbar = 0.0; S.da_mu = log(10.0 * e0); S.da_count = 1;
-        S.window = P.window; S.fg_m = LV_FGM; S.fg_v = LV_FGV; S.bg_m = LV_BGM; S.bg_v = LV_BGV;
+        S.ss.init(P.eps0c ? P.eps0c[chain] : P.eps0);
+        S.dw.init(LV_FGM, P.init_weight, P.window);
         S.prev_update = 0; S.fa_fg = 0; S.upd_pending = 0; S.chol_bad = 0; S.mom_have = -1;
-        S.fg_n = P.init_weight; S.bg_n = 0.0;
         const b200_pcg64 r = P.rng[chain];
         S.rs_hi = r.state_hi; S.rs_lo = r.state_lo; S.ri_hi = r.inc_hi; S.ri_lo = r.inc_lo;
         if (P.dense) { S.need_mom = 0; S.mom_it = 0; P.mom_list[chain] = chain; }
@@ -665,11 +614,7 @@ __global__ void __launch_bounds__(256) ls_gather_z_kernel(const LsDev P, int m, 
     if (j >= m) return;
     const int chain = P.mom_list[j];
     const int it = P.state[chain].mom_it;
-    const int n = P.n, Ttot = P.tune + P.draws;
-    for (int i = threadIdx.x; i < n; i += blockDim.x)
-        Zb[(long long)j * P.ld + i] = (P.momentum_source == B200_MOMENTUM_HOST_BUFFER)
-                                       ? P.z[((long long)chain * Ttot + it) * n + i]
-                                       : philox_normal(P.philox_seed, (uint32_t)(chain + P.chain_offset), (uint32_t)it, (uint32_t)i);
+    for (int i = threadIdx.x; i < P.n; i += blockDim.x) Zb[(long long)j * P.ld + i] = momentum_z(P, chain, it, i);
 }
 __global__ void __launch_bounds__(256) ls_scatter_mom_kernel(const LsDev P, int m, const double* P0b, const double* V0b) {
     const int j = blockIdx.x;

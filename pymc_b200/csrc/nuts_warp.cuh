@@ -23,9 +23,7 @@
 //   global/L2 : the colder stack levels, the main tree (both edge states, p_sum, proposal q) and the
 //               Welford accumulators -- touched once per doubling / per draw
 #pragma once
-#include "../../include/b200nuts.h"
-#include "common.cuh"
-#include "rng.cuh"
+#include "sampler_state.cuh"
 
 namespace b200 {
 
@@ -37,27 +35,11 @@ constexpr int kMaxLevels = 12;  // pending-subtree levels (max_treedepth <= 12)
 // probabilities are the numbers logaddexp gives (nuts.py:465-467, :370-376) up to rounding; every golden tree decision is
 // unchanged.
 
-struct NutsDev {
-    int C, n, tune, draws, max_td, early_td, adapt_step, mass_kind, momentum_source, store_warmup;
-    int window, discard, hot_levels, chain_offset;
-    int it0, n_iter;                           // this call runs the iterations [it0, it0 + n_iter) of the chain's schedule
+struct NutsDev : RunCfg {
+    int hot_levels;
     b200_chain_state resume, save;             // optional per-chain state in / out (null pointers: not used)
     int sampler, max_steps, stop_adaptation;   // B200_SAMPLER_*; HMC: max leapfrogs; DIAG_ADAPT_GRAD: stop after this many
     double path_length, mass_alpha;            // HMC trajectory length; DIAG_ADAPT_GRAD decay rate
-    double eps0, target, gamma, kappa, t0, Emax, init_weight;
-    unsigned long long philox_seed;
-    const double* q0;     // [C][n]
-    const double* var0;   // [C][n] or null
-    const double* mean0;  // [C][n] or null
-    const double* eps0c;  // [C] or null: per-chain initial step size
-    const double* z;      // [C][Ttot][n] or null
-    b200_pcg64* rng;      // [C]
-    double* draws_out;    // [C][T][n]
-    const signed char* tr_kind;  // [n] or null: record CONSTRAINED values (0 identity, 1 exp, 2 lo + (hi - lo) sigmoid)
-    const double* tr_lo;         // [n]
-    const double* tr_hi;         // [n]
-    b200_stats st;
-    b200_chain_summary sm;
     double* scratch;            // per-chain global scratch
     long long scratch_stride;   // doubles per chain
     // dynamic scheduling (see "Scheduling" below)
@@ -78,9 +60,10 @@ struct NutsDev {
 // step sizes make the slowest chain 1.7x the mean).  A chain's arithmetic and stream consumption are unchanged, so
 // results stay bit-identical and independent of the schedule.
 struct ChainCtx {
-    double log_step, log_bar, hbar, fg_n, bg_n;
+    StepSize ss;
+    DiagWindow dw;
     long long n_grad;
-    int da_count, k_samples, window, fg_m, fg_v, bg_m, bg_v, bad_at;
+    int bad_at;
 };
 
 __device__ __forceinline__ int ld_acquire_i32(const int* p) {
@@ -115,6 +98,21 @@ __host__ __device__ inline size_t nuts_warp_smem_bytes(int NP, int hot, bool sub
 #ifndef B200_NUTS_MINBLOCKS
 #define B200_NUTS_MINBLOCKS 1  // __launch_bounds__ min CTAs/SM: the register budget knob
 #endif
+// CTA prologue of the model kernels: stage the model's observed data into the start of the dynamic shared memory (bulk
+// TMA).  Returns the bytes it occupies, padded to 16.
+template <class Model>
+__device__ __forceinline__ size_t stage_model_data(const typename Model::Params& M, char* smem) {
+    __shared__ __align__(8) uint64_t tma_bar;
+    const size_t data_bytes = (Model::shared_bytes(M) + 15) & ~(size_t)15;
+    if (data_bytes) {
+        if (threadIdx.x == 0) mbar_init(&tma_bar, 1);
+        __syncthreads();
+        Model::stage(M, smem, &tma_bar);
+        mbar_wait(&tma_bar, 0);
+    }
+    return data_bytes;
+}
+
 // W = warps per chain (team).  SUBS = subtree-under-construction vectors in shared memory instead of registers.
 #define B200_NUTS_BOUNDS __launch_bounds__(W > 1 ? 32 * W : B200_NUTS_THREADS, W > 1 ? 1 : B200_NUTS_MINBLOCKS)
 template <class Model, int NPL, int W, bool SUBS>
@@ -123,16 +121,7 @@ __global__ void B200_NUTS_BOUNDS
     constexpr int TS = 32 * W;      // threads per chain
     constexpr int NP = TS * NPL;    // padded vector length
     extern __shared__ __align__(16) char smem_raw[];
-    __shared__ __align__(8) uint64_t tma_bar;
-
-    // ---- CTA prologue: stage the observed data into shared memory (bulk TMA) -------------------
-    const size_t data_bytes = (Model::shared_bytes(M) + 15) & ~(size_t)15;
-    if (data_bytes) {
-        if (threadIdx.x == 0) mbar_init(&tma_bar, 1);
-        __syncthreads();
-        Model::stage(M, smem_raw, &tma_bar);
-        mbar_wait(&tma_bar, 0);
-    }
+    const size_t data_bytes = stage_model_data<Model>(M, smem_raw);
     const char* data_s = smem_raw;
 
     // `lane` is the thread's index inside its team (0 .. TS-1)
@@ -200,11 +189,10 @@ __global__ void B200_NUTS_BOUNDS
 
     // ---- per-chain state: initialised by the first segment, carried through global memory afterwards ------------
     double var[NPL], p[NPL];
-    int fg_m, fg_v, bg_m, bg_v, k_samples, window, da_count, bad_at;
-    double fg_n, bg_n, log_step, log_bar, hbar;
+    StepSize ss;
+    DiagWindow dw;
+    int bad_at;
     long long n_grad;
-    const double eps_init = P.eps0c ? P.eps0c[chain] : P.eps0;
-    const double da_mu = log(10.0 * eps_init);  // dual averaging (step_sizes.py:50-57)
     if (seg == 0) {
 #pragma unroll
         for (int k = 0; k < NPL; ++k) {
@@ -220,18 +208,15 @@ __global__ void B200_NUTS_BOUNDS
                 gvec(G_BGV)[i] = 0.0;
             }
         }
-        fg_m = G_FGM; fg_v = G_FGV; bg_m = G_BGM; bg_v = G_BGV;
-        fg_n = P.init_weight; bg_n = 0.0;
-        k_samples = 0; window = P.window;
-        log_step = log(eps_init); log_bar = log_step; hbar = 0.0;
-        da_count = 1;
+        dw.init(G_FGM, P.init_weight, P.window);
+        ss.init(P.eps0c ? P.eps0c[chain] : P.eps0);
         n_grad = 0;
         bad_at = -1;
         if (P.resume.log_step) {  // continue a chain from an exported state (BaseHMC / potential / step_adapt sampling_state)
             const b200_chain_state& R = P.resume;
-            log_step = R.log_step[chain]; log_bar = R.log_bar[chain]; hbar = R.hbar[chain]; da_count = R.da_count[chain];
-            k_samples = R.n_samples[chain]; window = R.window[chain];
-            fg_n = R.fg_n[chain]; bg_n = R.bg_n[chain]; n_grad = R.n_grad[chain];
+            ss.log_step = R.log_step[chain]; ss.log_bar = R.log_bar[chain]; ss.hbar = R.hbar[chain]; ss.count = R.da_count[chain];
+            dw.k_samples = R.n_samples[chain]; dw.window = R.window[chain];
+            dw.fg_n = R.fg_n[chain]; dw.bg_n = R.bg_n[chain]; n_grad = R.n_grad[chain];
 #pragma unroll
             for (int k = 0; k < NPL; ++k) {
                 const int i = lane + TS * k;
@@ -247,10 +232,7 @@ __global__ void B200_NUTS_BOUNDS
         }
     } else {
         const ChainCtx cx = P.ctx[chain];
-        fg_m = cx.fg_m; fg_v = cx.fg_v; bg_m = cx.bg_m; bg_v = cx.bg_v;
-        fg_n = cx.fg_n; bg_n = cx.bg_n; k_samples = cx.k_samples; window = cx.window;
-        log_step = cx.log_step; log_bar = cx.log_bar; hbar = cx.hbar; da_count = cx.da_count;
-        n_grad = cx.n_grad; bad_at = cx.bad_at;
+        ss = cx.ss; dw = cx.dw; n_grad = cx.n_grad; bad_at = cx.bad_at;
         const double* sq = gvec(G_Q); const double* sv = gvec(G_VAR);
 #pragma unroll
         for (int k = 0; k < NPL; ++k) {
@@ -270,9 +252,9 @@ __global__ void B200_NUTS_BOUNDS
     // QuadPotentialDiagAdaptExp.update with use_grads (quadpotential.py:531-579); sample = q_s, grad = g_s.  The four
     // Welford slots of the scratch hold (mean, var) of the draws and of the gradients.
     auto grad_mass_update = [&](double* em, double* ev, double* gm, double* gv) {
-        if (k_samples >= P.stop_adaptation) return;
+        if (dw.k_samples >= P.stop_adaptation) return;
         const double al = P.mass_alpha, om = 1.0 - P.mass_alpha;
-        if (k_samples > P.discard) {
+        if (dw.k_samples > P.discard) {
 #pragma unroll
             for (int k = 0; k < NPL; ++k) {
                 const int i = lane + TS * k;
@@ -283,21 +265,21 @@ __global__ void B200_NUTS_BOUNDS
                 gm[i] = __dadd_rn(gm[i], __dmul_rn(al, d));
                 gv[i] = __dmul_rn(om, __dadd_rn(gv[i], __dmul_rn(al, __dmul_rn(d, d))));
             }
-        } else if (k_samples == P.discard) {
+        } else if (dw.k_samples == P.discard) {
 #pragma unroll
             for (int k = 0; k < NPL; ++k) {
                 const int i = lane + TS * k;
                 em[i] = q_s[i]; ev[i] = 0.0; gm[i] = g_s[i]; gv[i] = 0.0;
             }
         }
-        if (k_samples > 2 * P.discard) {  // _update_from_variances :569-575: var = sqrt(var_draws / var_grads), no clipping
+        if (dw.k_samples > 2 * P.discard) {  // _update_from_variances :569-575: var = sqrt(var_draws / var_grads), no clipping
 #pragma unroll
             for (int k = 0; k < NPL; ++k) {
                 const int i = lane + TS * k;
                 if (i < n) VAR(k) = sqrt(ev[i] / gv[i]);
             }
         }
-        ++k_samples;
+        ++dw.k_samples;
     };
 
     for (int it = it_begin; it < it_end && bad_at < 0; ++it) {
@@ -320,12 +302,7 @@ __global__ void B200_NUTS_BOUNDS
 #pragma unroll
         for (int k = 0; k < NPL; ++k) {
             const int i = lane + TS * k;
-            double zz = 0.0;
-            if (i < n) {
-                zz = (P.momentum_source == B200_MOMENTUM_HOST_BUFFER)
-                         ? P.z[((long long)chain * P.n_iter + (it - it_lo)) * n + i]
-                         : philox_normal(P.philox_seed, (uint32_t)(chain + P.chain_offset), (uint32_t)it, (uint32_t)i);
-            }
+            const double zz = (i < n) ? momentum_z(P, chain, it, i) : 0.0;
             p[k] = (1.0 / sqrt(VAR(k))) * zz;
         }
         double kin = 0.0;
@@ -336,7 +313,7 @@ __global__ void B200_NUTS_BOUNDS
             bad_at = it;
             break;
         }
-        const double eps = exp(adapting ? log_step : log_bar);  // step_adapt.current (step_sizes.py:60-64)
+        const double eps = ss.current(adapting);  // step_adapt.current (step_sizes.py:60-64)
         const int maxd = (tuning && it < 200) ? P.early_td : P.max_td;  // nuts.py:205-208
 
         double m_logw = 0.0, m_pe = E0, m_plogp = logp0;
@@ -369,7 +346,6 @@ __global__ void B200_NUTS_BOUNDS
                 team_sync<W>();
                 logp = Model::template eval<NPL, W, true>(M, data_s, q_s, g_s, lane, red);
                 team_sync<W>();
-                ++n_grad;
                 double kk = 0.0;
 #pragma unroll
                 for (int k = 0; k < NPL; ++k) {
@@ -440,7 +416,6 @@ __global__ void B200_NUTS_BOUNDS
                     team_sync<W>();
                     const double logp = Model::template eval<NPL, W, true>(M, data_s, q_s, g_s, lane, red);
                     team_sync<W>();
-                    ++n_grad;
                     double kk = 0.0;
     #pragma unroll
                     for (int k = 0; k < NPL; ++k) {
@@ -630,6 +605,7 @@ __global__ void B200_NUTS_BOUNDS
             }
         }
         if (d_iter == maxd) hit_max = !tuning;  // for/else of nuts.py:220-221
+        n_grad += n_prop;  // one gradient per leapfrog
 
         // ---- the accepted position becomes the chain state -------------------------------------------
         const double accept = (P.sampler == B200_SAMPLER_HMC) ? hmc_accept : accept_sum / n_prop;  // nuts.py:479
@@ -643,92 +619,46 @@ __global__ void B200_NUTS_BOUNDS
             PQ(k) = qi;
             if (rec && i < n) P.draws_out[((long long)chain * T_out + t_out) * n + i] = constrained(qi, i, P.tr_kind, P.tr_lo, P.tr_hi);
         }
-        // ---- step_adapt.update (step_sizes.py:66-78); products/sums kept unfused like the Python scalars
-        if (adapting) {
-            const double w = 1.0 / (da_count + P.t0);
-            hbar = __dadd_rn(__dmul_rn(1.0 - w, hbar), __dmul_rn(w, P.target - accept));
-            log_step = da_mu - __dmul_rn(hbar, sqrt((double)da_count)) / P.gamma;
-            const double mk = pow((double)da_count, -P.kappa);
-            log_bar = __dadd_rn(__dmul_rn(mk, log_step), __dmul_rn(1.0 - mk, log_bar));
-            ++da_count;
-        }
-        // ---- potential.update (quadpotential.py:335-355, _WeightedVariance.add_sample :431-437) --------
+        if (adapting) ss.update(P, accept);
+        // ---- potential.update (quadpotential.py:335-355) -----------------------------------------------
         if (tuning && P.mass_kind == B200_MASS_DIAG_ADAPT) {
-            if (k_samples > P.discard) {
-                fg_n += 1.0;
-                bg_n += 1.0;
-                double* fm = gvec(fg_m); double* fv = gvec(fg_v);
-                double* bm = gvec(bg_m); double* bv = gvec(bg_v);
+            if (dw.add_sample(P.discard)) {
+                double* fm = gvec(dw.fg_m); double* fv = gvec(dw.fg_v);
+                double* bm = gvec(dw.bg_m); double* bv = gvec(dw.bg_v);
 #pragma unroll
                 for (int k = 0; k < NPL; ++k) {
                     const int i = lane + TS * k;
-                    const double x = PQ(k);
-                    double mean = fm[i];
-                    double d0 = x - mean;
-                    mean = __dadd_rn(mean, d0 / fg_n);
-                    fm[i] = mean;
-                    fv[i] = __dadd_rn(fv[i], __dmul_rn(d0, x - mean));
-                    mean = bm[i];
-                    d0 = x - mean;
-                    mean = __dadd_rn(mean, d0 / bg_n);
-                    bm[i] = mean;
-                    bv[i] = __dadd_rn(bv[i], __dmul_rn(d0, x - mean));
+                    welford_add(PQ(k), dw.fg_n, fm[i], fv[i]);
+                    welford_add(PQ(k), dw.bg_n, bm[i], bv[i]);
                 }
             }
-            if (k_samples > window) {
-                const double* fv = gvec(fg_v);
+            if (dw.var_ready()) {
+                const double* fv = gvec(dw.fg_v);
 #pragma unroll
                 for (int k = 0; k < NPL; ++k) {
                     const int i = lane + TS * k;
-                    if (i < n) VAR(k) = fmin(fmax(fv[i] / fg_n, 1e-12), 1e12);
+                    if (i < n) VAR(k) = dw.variance(fv[i]);
                 }
             }
-            if (k_samples > 0 && k_samples % window == 0) {
-                const int tm = fg_m, tv = fg_v;
-                fg_m = bg_m; fg_v = bg_v; fg_n = bg_n;
-                bg_m = tm; bg_v = tv; bg_n = 0.0;
-                double* bm = gvec(bg_m); double* bv = gvec(bg_v);
+            if (dw.swap_due()) {
+                dw.swap();
+                double* bm = gvec(dw.bg_m); double* bv = gvec(dw.bg_v);
 #pragma unroll
                 for (int k = 0; k < NPL; ++k) {
                     bm[lane + TS * k] = 0.0;
                     bv[lane + TS * k] = 0.0;
                 }
             }
-            ++k_samples;
+            ++dw.k_samples;
         }
-        // ---- stats (nuts.py:478-489, base_hmc.py:275-286) --------------------------------------------
-        if (rec && lane == 0) {
-            const long long o = (long long)chain * T_out + t_out;
-            if (P.st.depth) P.st.depth[o] = depth;
-            if (P.st.tree_size) P.st.tree_size[o] = n_prop;
-            if (P.st.index_in_trajectory) P.st.index_in_trajectory[o] = m_pidx;
-            if (P.st.diverging) P.st.diverging[o] = diverged ? 1 : 0;
-            if (P.st.reached_max_treedepth) P.st.reached_max_treedepth[o] = hit_max ? 1 : 0;
-            if (P.st.step_size) P.st.step_size[o] = exp(log_step);
-            if (P.st.step_size_bar) P.st.step_size_bar[o] = exp(log_bar);
-            if (P.st.mean_tree_accept) P.st.mean_tree_accept[o] = accept;
-            if (P.st.energy) P.st.energy[o] = m_pe;
-            if (P.st.energy_error) P.st.energy_error[o] = (P.sampler == B200_SAMPLER_HMC) ? max_de : m_pe - E0;
-            if (P.st.max_energy_error) P.st.max_energy_error[o] = max_de;
-            if (P.st.model_logp) P.st.model_logp[o] = m_plogp;
-        }
+        if (rec && lane == 0)
+            record_draw_stats(P.st, (long long)chain * T_out + t_out, depth, n_prop, m_pidx, diverged, hit_max, ss, accept, m_pe,
+                              (P.sampler == B200_SAMPLER_HMC) ? max_de : m_pe - E0, max_de, m_plogp);
         (void)turned;
         team_sync<W>();
     }
 
-    // ---- a frozen chain ("Bad initial energy"): the iterations that never ran are NaN in the output --------------
-    if (bad_at >= 0) {
-        for (int t = max(bad_at, it_begin); t < it_end; ++t) {
-            if (!(P.store_warmup || t >= P.tune)) continue;
-            const int t_out = t - rec_lo;
-#pragma unroll
-            for (int k = 0; k < NPL; ++k) {
-                const int i = lane + TS * k;
-                if (i < n) P.draws_out[((long long)chain * T_out + t_out) * n + i] = nan("");
-            }
-            if (lane == 0) stats_sentinel(P.st, (long long)chain * T_out + t_out);
-        }
-    }
+    if (bad_at >= 0) freeze_outputs<TS>(P, chain, max(bad_at, it_begin), it_end, rec_lo, T_out, lane);
     // ---- end of the segment: the stream position goes back to the caller's array (it is also where the next segment
     //      picks it up); last segment: adaptation results; otherwise: the chain's state for the next segment ------------
     const bool last_seg = it_end >= it_hi;
@@ -737,26 +667,17 @@ __global__ void B200_NUTS_BOUNDS
         r.state_hi = (uint64_t)(rng.state >> 64); r.state_lo = (uint64_t)rng.state;
         r.inc_hi = (uint64_t)(rng.inc >> 64); r.inc_lo = (uint64_t)rng.inc;
         P.rng[chain] = r;
-        if (last_seg) {
-            if (P.sm.grad_evals) P.sm.grad_evals[chain] = n_grad;
-            if (P.sm.bad_energy_at) P.sm.bad_energy_at[chain] = bad_at;
-            if (P.sm.final_step_size) P.sm.final_step_size[chain] = exp(log_bar);
-        } else {
-            ChainCtx cx;
-            cx.log_step = log_step; cx.log_bar = log_bar; cx.hbar = hbar; cx.fg_n = fg_n; cx.bg_n = bg_n;
-            cx.n_grad = n_grad; cx.da_count = da_count; cx.k_samples = k_samples; cx.window = window;
-            cx.fg_m = fg_m; cx.fg_v = fg_v; cx.bg_m = bg_m; cx.bg_v = bg_v; cx.bad_at = bad_at;
-            P.ctx[chain] = cx;
-        }
+        if (last_seg) record_chain_summary(P.sm, chain, n_grad, bad_at, ss);
+        else P.ctx[chain] = ChainCtx{ss, dw, n_grad, bad_at};
     }
     if (last_seg && P.save.log_step) {  // export the chain's state (the pending DIAG_ADAPT_GRAD update stays pending)
         const b200_chain_state& S = P.save;
         if (lane == 0) {
-            S.log_step[chain] = log_step; S.log_bar[chain] = log_bar; S.hbar[chain] = hbar; S.da_count[chain] = da_count;
-            S.n_samples[chain] = k_samples; S.window[chain] = window;
-            S.fg_n[chain] = fg_n; S.bg_n[chain] = bg_n; S.n_grad[chain] = n_grad;
+            S.log_step[chain] = ss.log_step; S.log_bar[chain] = ss.log_bar; S.hbar[chain] = ss.hbar; S.da_count[chain] = ss.count;
+            S.n_samples[chain] = dw.k_samples; S.window[chain] = dw.window;
+            S.fg_n[chain] = dw.fg_n; S.bg_n[chain] = dw.bg_n; S.n_grad[chain] = n_grad;
         }
-        const double* fm = gvec(fg_m); const double* fv = gvec(fg_v); const double* bm = gvec(bg_m); const double* bv = gvec(bg_v);
+        const double* fm = gvec(dw.fg_m); const double* fv = gvec(dw.fg_v); const double* bm = gvec(dw.bg_m); const double* bv = gvec(dw.bg_v);
 #pragma unroll
         for (int k = 0; k < NPL; ++k) {
             const int i = lane + TS * k;
@@ -812,14 +733,7 @@ __global__ void __launch_bounds__(256) logp_grad_warp_kernel(const typename Mode
     constexpr int TS = 32 * W;
     constexpr int NP = TS * NPL;
     extern __shared__ __align__(16) char smem_raw[];
-    __shared__ __align__(8) uint64_t tma_bar;
-    const size_t data_bytes = (Model::shared_bytes(M) + 15) & ~(size_t)15;
-    if (data_bytes) {
-        if (threadIdx.x == 0) mbar_init(&tma_bar, 1);
-        __syncthreads();
-        Model::stage(M, smem_raw, &tma_bar);
-        mbar_wait(&tma_bar, 0);
-    }
+    const size_t data_bytes = stage_model_data<Model>(M, smem_raw);
     const int lane = (W == 1) ? (threadIdx.x & 31) : (int)threadIdx.x;
     const int wib = (W == 1) ? (threadIdx.x >> 5) : 0, wpb = (W == 1) ? (blockDim.x >> 5) : 1;
     double* q_s = reinterpret_cast<double*>(smem_raw + data_bytes) + (size_t)wib * (2 * NP + (W > 1 ? 8 * W : 0));
@@ -857,14 +771,7 @@ __global__ void __launch_bounds__(256)
     constexpr int TS = 32 * W;
     constexpr int NP = TS * NPL;
     extern __shared__ __align__(16) char smem_raw[];
-    __shared__ __align__(8) uint64_t tma_bar;
-    const size_t data_bytes = (Model::shared_bytes(M) + 15) & ~(size_t)15;
-    if (data_bytes) {
-        if (threadIdx.x == 0) mbar_init(&tma_bar, 1);
-        __syncthreads();
-        Model::stage(M, smem_raw, &tma_bar);
-        mbar_wait(&tma_bar, 0);
-    }
+    const size_t data_bytes = stage_model_data<Model>(M, smem_raw);
     const int lane = (W == 1) ? (threadIdx.x & 31) : (int)threadIdx.x;
     const int wib = (W == 1) ? (threadIdx.x >> 5) : 0, wpb = (W == 1) ? (blockDim.x >> 5) : 1;
     double* q_s = reinterpret_cast<double*>(smem_raw + data_bytes) + (size_t)wib * (2 * NP + (W > 1 ? 8 * W : 0));

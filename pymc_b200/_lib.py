@@ -259,15 +259,12 @@ def load() -> C.CDLL:
             raise B200Error(f"{LIB_PATH} is missing: build the CUDA engine first (./build.sh); there is no CPU fallback")
         lib = C.CDLL(LIB_PATH)
         for name, restype, argtypes in SYMBOLS:
-            if name in ("b200_struct_size", "b200_model_set_precision", "b200_model_set_transforms",
-                        "b200_model_set_dense_mass", "b200_pointwise_loglik") and not hasattr(lib, name):
-                continue  # an A/B build (B200_LIB=...) older than ABI 0.2.0; tests/test_abi.py requires it of the in-tree library
             fn = getattr(lib, name)
             fn.restype = restype
             fn.argtypes = argtypes
         mirrors = [ModelDesc, NutsCfg, Stats, ChainSummary, Pcg64State, Ir, IrVar, IrPrior, IrTerm, IrLik, IrAr1, IrParam, IrFactor,
                    ChainStateC]
-        for which, cls in enumerate(mirrors if hasattr(lib, "b200_struct_size") else []):
+        for which, cls in enumerate(mirrors):
             if lib.b200_struct_size(which) != C.sizeof(cls):
                 raise B200Error(f"ABI mismatch: {cls.__name__} is {C.sizeof(cls)} bytes here, {lib.b200_struct_size(which)} in "
                                 f"{LIB_PATH} (rebuild with ./build.sh)")

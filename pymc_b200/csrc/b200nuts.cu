@@ -8,6 +8,7 @@
 #include <cstdio>
 #include <cmath>
 #include <cstring>
+#include <deque>
 #include <map>
 #include <numeric>
 #include <string>
@@ -66,10 +67,23 @@ static int current_sm_count() {
     return sm_count(dev);
 }
 
-struct DevBuf {  // owning device allocation
+struct DevBuf {  // owning, grow-only device allocation
     void* p = nullptr;
+    size_t bytes = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
     ~DevBuf() { if (p) cudaFree(p); }
-    cudaError_t alloc(size_t bytes) { return cudaMalloc(&p, bytes ? bytes : 16); }
+    // keeps the allocation when it already holds `b` bytes; otherwise frees it and allocates `b` (at least 16)
+    cudaError_t reserve(size_t b) {
+        if (p && b <= bytes) return cudaSuccess;
+        if (p) cudaFree(p);
+        p = nullptr;
+        bytes = 0;
+        const cudaError_t e = cudaMalloc(&p, std::max<size_t>(b, 16));
+        if (e == cudaSuccess) bytes = b;
+        return e;
+    }
     template <class T> T* as() const { return static_cast<T*>(p); }
 };
 
@@ -85,21 +99,7 @@ struct b200_model {
     const double* tr_hi = nullptr;
     IrModel::Params ir{};
     long long ir_max_obs = 0;
-    void* ir_scratch = nullptr;   // per-team scratch of the generic IR device function: [slots][n_pad + max N] doubles
-    size_t ir_scratch_bytes = 0;
-    cudaError_t ensure_ir_scratch(long long slots) {
-        const size_t bytes = (size_t)slots * (size_t)ir.stride * sizeof(double);
-        if (bytes > ir_scratch_bytes) {
-            if (ir_scratch) cudaFree(ir_scratch);
-            ir_scratch = nullptr;
-            ir_scratch_bytes = 0;
-            cudaError_t e = cudaMalloc(&ir_scratch, bytes);
-            if (e != cudaSuccess) return e;
-            ir_scratch_bytes = bytes;
-        }
-        ir.scratch = static_cast<double*>(ir_scratch);
-        return cudaSuccess;
-    }
+    DevBuf ir_scratch;  // per-team scratch of the generic IR device function: [teams][n_pad + max N] doubles
     // lock-step (GEMM-shaped) models; every matrix is row-major with rows `ld` doubles apart (n rounded up to 4, zero pad)
     long long ld = 0;
     const double* prec = nullptr;   // MVGAUSS: precision P [n][ld]
@@ -124,52 +124,13 @@ struct b200_model {
     struct TcMat { const double* src = nullptr; const __half* hi = nullptr; const __half* lo = nullptr; CUtensorMap map_hi{}, map_lo{}; };
     TcMat tc_mats[4];
     long long tc_kpad = 0, tc_npad = 0;
-    __half* tc_a_hi = nullptr; __half* tc_a_lo = nullptr;   // [tc_a_rows][tc_kpad]
-    long long tc_a_rows = 0;
-    // per-chain tree scratch of the persistent kernel, kept between runs (cudaMalloc/cudaFree of 100+ MB per call costs
-    // tens of milliseconds of host time on the end-to-end path)
-    void* scratch = nullptr;
-    size_t scratch_bytes = 0;
-    void* ls_arena = nullptr;  // lock-step engine: per-chain state machines, vectors, request matrices (kept between runs)
-    size_t ls_arena_bytes = 0;
-    cudaError_t ensure_ls_arena(size_t bytes) {
-        if (bytes <= ls_arena_bytes) return cudaSuccess;
-        if (ls_arena) cudaFree(ls_arena);
-        ls_arena = nullptr;
-        ls_arena_bytes = 0;
-        cudaError_t e = cudaMalloc(&ls_arena, bytes);
-        if (e == cudaSuccess) ls_arena_bytes = bytes;
-        return e;
-    }
-    void* stage_arena = nullptr;  // device staging of per-draw sampler statistics bound for host memory (kept between runs)
-    size_t stage_bytes = 0;
-    cudaError_t ensure_stage(size_t bytes) {
-        if (bytes <= stage_bytes) return cudaSuccess;
-        if (stage_arena) cudaFree(stage_arena);
-        stage_arena = nullptr;
-        stage_bytes = 0;
-        cudaError_t e = cudaMalloc(&stage_arena, bytes);
-        if (e == cudaSuccess) stage_bytes = bytes;
-        return e;
-    }
-    cudaError_t ensure_scratch(size_t bytes) {
-        if (bytes <= scratch_bytes) return cudaSuccess;
-        if (scratch) cudaFree(scratch);
-        scratch = nullptr;
-        scratch_bytes = 0;
-        cudaError_t e = cudaMalloc(&scratch, bytes);
-        if (e == cudaSuccess) scratch_bytes = bytes;
-        return e;
-    }
-    ~b200_model() {
-        if (ls_arena) cudaFree(ls_arena);
-        if (stage_arena) cudaFree(stage_arena);
-        if (tc_a_hi) cudaFree(tc_a_hi);
-        if (tc_a_lo) cudaFree(tc_a_lo);
-        if (ir_scratch) cudaFree(ir_scratch);
-        if (scratch) cudaFree(scratch);
-        for (void* p : owned) cudaFree(p);
-    }
+    DevBuf tc_a_hi, tc_a_lo;  // fp16 [rows][tc_kpad]
+    // Kept between runs (cudaMalloc/cudaFree of 100+ MB per call costs tens of milliseconds of host time on the end-to-end
+    // path, and per-call allocations of small arrays synchronise the device):
+    DevBuf scratch;      // persistent engine: per-chain tree scratch, chain contexts, work-unit tickets
+    DevBuf ls_arena;     // lock-step engine: per-chain state machines, vectors, request matrices
+    DevBuf stage_arena;  // device copies of the host arrays of a call (Staging)
+    ~b200_model() { for (void* p : owned) cudaFree(p); }
 };
 
 static bool is_lockstep_kind(int kind);
@@ -177,14 +138,16 @@ template <class F> static int dispatch(const b200_model* m, F&& f);
 static int lockstep_logp(b200_model* m, const double* q_dev, int C, double* logp_dev, double* grad_dev, cudaStream_t st);
 
 template <class T>
-static int upload(b200_model* m, const std::vector<T>& h, const T** out) {
+static int upload_raw(b200_model* m, const T* h, size_t count, const T** out) {
     void* d = nullptr;
-    CU(cudaMalloc(&d, std::max<size_t>(h.size() * sizeof(T), 16)));
+    CU(cudaMalloc(&d, std::max<size_t>(count * sizeof(T), 16)));
     m->owned.push_back(d);
-    if (!h.empty()) CU(cudaMemcpy(d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice));
+    if (count) CU(cudaMemcpy(d, h, count * sizeof(T), cudaMemcpyHostToDevice));
     *out = static_cast<const T*>(d);
     return 0;
 }
+template <class T>
+static int upload(b200_model* m, const std::vector<T>& h, const T** out) { return upload_raw(m, h.data(), h.size(), out); }
 
 extern "C" int b200_version(void) { return B200NUTS_VERSION; }
 extern "C" const char* b200_last_error(void) { return g_err.c_str(); }
@@ -301,16 +264,6 @@ static int prepare_stochvol(b200_model* m, const b200_model_desc* d) {
     for (int t = 0; t < T; ++t) y2[t] = d->y[t] * d->y[t];
     m->stochvol.T = T;
     return upload(m, y2, &m->stochvol.y2);
-}
-
-template <class T>
-static int upload_raw(b200_model* m, const T* h, size_t count, const T** out) {
-    void* d = nullptr;
-    CU(cudaMalloc(&d, std::max<size_t>(count * sizeof(T), 16)));
-    m->owned.push_back(d);
-    CU(cudaMemcpy(d, h, count * sizeof(T), cudaMemcpyHostToDevice));
-    *out = static_cast<const T*>(d);
-    return 0;
 }
 
 // host matrix [rows][cols] -> device [rows_pad][ld], zero padded
@@ -737,7 +690,8 @@ static int launch_params(const b200_model* m, const typename Model::Params& MP, 
     *out = MP;
     if constexpr (std::is_same_v<Model, IrModel>) {
         b200_model* mm = const_cast<b200_model*>(m);
-        CU(mm->ensure_ir_scratch(teams));
+        CU(mm->ir_scratch.reserve((size_t)teams * (size_t)mm->ir.stride * sizeof(double)));
+        mm->ir.scratch = mm->ir_scratch.as<double>();
         *out = mm->ir;
     }
     return 0;
@@ -765,44 +719,87 @@ struct Timer {
     }
 };
 
-// Host<->device staging of one array.
-struct Staged {
-    DevBuf dev;
-    void* lent = nullptr;  // device staging lent by the caller (an arena in the model handle) instead of `dev`
-    void* user = nullptr;
-    size_t bytes = 0;
-    bool host = false, out = false;
-    void* dptr() const { return lent ? lent : dev.p; }
-    void* ptr() const { return host ? dptr() : user; }
-};
-// `direct`: an OUTPUT buffer in page-locked host memory (cudaHostAlloc / cudaHostRegister, e.g. a torch pinned tensor) is
-// written by the kernel itself through its device alias (UVA), so the device->host transfer overlaps the run instead of
-// following it (2.9 GB of draws per Radon bench step).
-static int stage_in(Staged& s, const void* user, size_t bytes, int mem, bool copy_in, bool copy_out,
-                    cudaStream_t st, bool direct = false) {
-    s.user = const_cast<void*>(user);
-    s.bytes = bytes;
-    s.host = (mem == B200_MEM_HOST) && user != nullptr;
-    s.out = copy_out;
-    if (s.host && direct && !copy_in && !getenv("B200_NO_DIRECT_HOST_WRITES")) {
-        cudaPointerAttributes at{};
-        if (cudaPointerGetAttributes(&at, user) == cudaSuccess && at.type == cudaMemoryTypeHost && at.devicePointer) {
-            s.user = at.devicePointer;
-            s.host = false;
-            return 0;
+// The array arguments of one C-ABI call.  With B200_MEM_DEVICE the kernels use the caller's pointers; with B200_MEM_HOST
+// every non-null array gets a device copy.  Those copies are lent from ONE arena in the model handle, sized in commit() from
+// the requests themselves, so a steady-state call makes no cudaMalloc / cudaFree at all (per-call allocations synchronise
+// the device and make a public-API call take far longer than its kernel).
+//   DIRECT: an OUTPUT in page-locked host memory (cudaHostAlloc / cudaHostRegister, e.g. a torch pinned tensor) is written
+//           by the kernel itself through its device alias (UVA), so the device->host transfer overlaps the run instead of
+//           following it (2.9 GB of draws per Radon bench step).
+//   OWN:    a per-call allocation instead of arena space, for arrays the arena must not grow to (the draws).
+// Usage: add() every array, commit() before the launch, finish() after it.
+class Staging {
+  public:
+    enum Dir { IN = 1, OUT = 2, INOUT = 3 };
+    enum Flag { DIRECT = 1, OWN = 2 };
+    Staging(b200_model* m, int mem, cudaStream_t st) : m_(m), host_(mem == B200_MEM_HOST), st_(st) {}
+    // `count` elements at `user`; commit() stores the pointer the kernels use in *dst
+    template <class T>
+    void add(T** dst, T* user, size_t count, Dir dir, int flags = 0) {
+        reqs_.push_back(Req{dst, &put<T>, const_cast<void*>(static_cast<const void*>(user)), count * sizeof(T), dir, flags});
+    }
+    int commit() {
+        size_t lent = 0;
+        for (Req& r : reqs_) {
+            r.copy = host_ && r.user;
+            if (r.copy && (r.flags & DIRECT) && r.dir == OUT) {
+                cudaPointerAttributes at{};
+                if (cudaPointerGetAttributes(&at, r.user) == cudaSuccess && at.type == cudaMemoryTypeHost && at.devicePointer) {
+                    r.dev = at.devicePointer;
+                    r.copy = false;
+                } else {
+                    cudaGetLastError();  // pageable memory: not an error, fall back to a device copy
+                }
+            }
+            if (r.copy && !(r.flags & OWN)) {
+                r.off = lent;
+                lent += (r.bytes + 255) & ~(size_t)255;
+            }
         }
-        cudaGetLastError();  // pageable memory: not an error, fall back to staging
+        if (lent) CU(m_->stage_arena.reserve(lent));
+        for (Req& r : reqs_) {
+            if (r.copy) {
+                if (r.flags & OWN) {
+                    own_.emplace_back();
+                    CU(own_.back().reserve(r.bytes));
+                    r.dev = own_.back().p;
+                } else {
+                    r.dev = m_->stage_arena.as<char>() + r.off;
+                }
+                if (r.dir & IN) CU(cudaMemcpyAsync(r.dev, r.user, r.bytes, cudaMemcpyHostToDevice, st_));
+            } else if (!r.dev) {
+                r.dev = r.user;
+            }
+            r.put(r.dst, r.dev);
+        }
+        return 0;
     }
-    if (s.host) {
-        if (!s.lent) CU(s.dev.alloc(bytes));
-        if (copy_in) CU(cudaMemcpyAsync(s.dptr(), user, bytes, cudaMemcpyHostToDevice, st));
+    // device->host copies of the outputs, then wait for the stream
+    int finish() {
+        for (const Req& r : reqs_)
+            if (r.copy && (r.dir & OUT)) CU(cudaMemcpyAsync(r.user, r.dev, r.bytes, cudaMemcpyDeviceToHost, st_));
+        CU(cudaStreamSynchronize(st_));
+        return 0;
     }
-    return 0;
-}
-static int stage_out(Staged& s, cudaStream_t st) {
-    if (s.host && s.out) CU(cudaMemcpyAsync(s.user, s.dptr(), s.bytes, cudaMemcpyDeviceToHost, st));
-    return 0;
-}
+
+  private:
+    struct Req {
+        void* dst;
+        void (*put)(void* dst, void* dev);
+        void* user;
+        size_t bytes;
+        int dir, flags;
+        bool copy = false;  // a device copy of a host array
+        size_t off = 0;     // its place in the arena
+        void* dev = nullptr;
+    };
+    template <class T> static void put(void* dst, void* dev) { *static_cast<T**>(dst) = static_cast<T*>(dev); }
+    b200_model* m_;
+    bool host_;
+    cudaStream_t st_;
+    std::vector<Req> reqs_;
+    std::deque<DevBuf> own_;
+};
 
 static int env_int(const char* name, int dflt) {
     const char* v = getenv(name);
@@ -845,22 +842,17 @@ extern "C" int b200_logp_dlogp(b200_model* m, const double* q, int32_t C, double
     if (C <= 0) return 0;
     CU(cudaSetDevice(m->device));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const size_t vb = (size_t)C * m->n * sizeof(double);
-    Staged sq, sl, sg;
-    if (stage_in(sq, q, vb, mem, true, false, st)) return -1;
-    if (stage_in(sl, logp, (size_t)C * sizeof(double), mem, false, true, st)) return -1;
-    if (stage_in(sg, grad, vb, mem, false, true, st)) return -1;
+    const size_t vn = (size_t)C * m->n;
+    LogpLaunch L{m, C, nullptr, nullptr, nullptr, st};
+    Staging sg(m, mem, st);
+    sg.add(&L.q, q, vn, Staging::IN);
+    sg.add(&L.logp, logp, C, Staging::OUT);
+    sg.add(&L.grad, grad, vn, Staging::OUT);
+    if (sg.commit()) return -1;
     Timer t(st);
-    if (is_lockstep_kind(m->kind)) {
-        if (lockstep_logp(m, (const double*)sq.ptr(), C, (double*)sl.ptr(), (double*)sg.ptr(), st)) return -1;
-    } else {
-        LogpLaunch L{m, C, (const double*)sq.ptr(), (double*)sl.ptr(), (double*)sg.ptr(), st};
-        if (dispatch(m, L)) return -1;
-    }
+    if (is_lockstep_kind(m->kind) ? lockstep_logp(m, L.q, C, L.logp, L.grad, st) : dispatch(m, L)) return -1;
     t.stop(1);
-    if (stage_out(sl, st) || stage_out(sg, st)) return -1;
-    CU(cudaStreamSynchronize(st));
-    return 0;
+    return sg.finish();
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -886,25 +878,24 @@ extern "C" int b200_leapfrog(b200_model* m, const double* var, const double* eps
     if (C <= 0) return 0;
     CU(cudaSetDevice(m->device));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    const size_t vb = (size_t)C * m->n * sizeof(double), sb = (size_t)C * sizeof(double);
-    Staged s_var, s_eps, s_q, s_p, s_v, s_g, s_e, s_l, s_i;
-    if (stage_in(s_var, var, vb, mem, true, false, st) || stage_in(s_eps, eps, sb, mem, true, false, st) ||
-        stage_in(s_q, q, vb, mem, true, true, st) || stage_in(s_p, p, vb, mem, true, true, st) ||
-        stage_in(s_v, v, vb, mem, true, true, st) || stage_in(s_g, grad, vb, mem, true, true, st) ||
-        stage_in(s_e, energy, sb, mem, true, true, st) || stage_in(s_l, logp, sb, mem, true, true, st) ||
-        stage_in(s_i, idx, (size_t)C * sizeof(int64_t), mem, true, true, st))
-        return -1;
+    const size_t vn = (size_t)C * m->n;
+    LeapLaunch L{m, C, n_steps};
+    L.st = st;
+    Staging sg(m, mem, st);
+    sg.add(&L.var, var, vn, Staging::IN);
+    sg.add(&L.eps, eps, C, Staging::IN);
+    sg.add(&L.q, q, vn, Staging::INOUT);
+    sg.add(&L.p, p, vn, Staging::INOUT);
+    sg.add(&L.v, v, vn, Staging::INOUT);
+    sg.add(&L.grad, grad, vn, Staging::INOUT);
+    sg.add(&L.energy, energy, C, Staging::INOUT);
+    sg.add(&L.logp, logp, C, Staging::INOUT);
+    sg.add(&L.idx, reinterpret_cast<long long*>(idx), C, Staging::INOUT);
+    if (sg.commit()) return -1;
     Timer t(st);
-    LeapLaunch L{m, C, n_steps, (const double*)s_var.ptr(), (const double*)s_eps.ptr(), (double*)s_q.ptr(),
-                 (double*)s_p.ptr(), (double*)s_v.ptr(), (double*)s_g.ptr(), (double*)s_e.ptr(),
-                 (double*)s_l.ptr(), (long long*)s_i.ptr(), st};
     if (dispatch(m, L)) return -1;
     t.stop(1);
-    if (stage_out(s_q, st) || stage_out(s_p, st) || stage_out(s_v, st) || stage_out(s_g, st) ||
-        stage_out(s_e, st) || stage_out(s_l, st) || stage_out(s_i, st))
-        return -1;
-    CU(cudaStreamSynchronize(st));
-    return 0;
+    return sg.finish();
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -962,7 +953,6 @@ static int gemm_nt(b200_model* m, cudaStream_t st, const double* Q, long long ld
 struct BatchScratch {  // logistic partial results
     DevBuf gpart, lpart;
     int gx = 0, cpad = 0;
-    long long cap_rows = 0;  // allocated gx * cpad (the product barely changes when the batch shrinks: more row CTAs per chain block)
 };
 
 
@@ -1024,20 +1014,15 @@ static int prepare_mvgauss_tc(b200_model* m) {
 static int gemm_nt_tc(b200_model* m, cudaStream_t st, const double* Q, long long ldq, int C, const b200_model::TcMat& T, int Nout,
                       double alpha, double* D, long long ldd) {
     const long long rows_pad = ((long long)C + kGtM - 1) / kGtM * kGtM;
-    if (rows_pad > m->tc_a_rows) {
-        if (m->tc_a_hi) cudaFree(m->tc_a_hi);
-        if (m->tc_a_lo) cudaFree(m->tc_a_lo);
-        m->tc_a_hi = m->tc_a_lo = nullptr;
-        m->tc_a_rows = 0;
-        CU(cudaMalloc((void**)&m->tc_a_hi, (size_t)rows_pad * m->tc_kpad * sizeof(__half)));
-        CU(cudaMalloc((void**)&m->tc_a_lo, (size_t)rows_pad * m->tc_kpad * sizeof(__half)));
-        m->tc_a_rows = rows_pad;
-    }
     const long long total = rows_pad * m->tc_kpad;
-    gemm_tc_split_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(Q, C, m->n, ldq, m->tc_a_hi, m->tc_a_lo, rows_pad, m->tc_kpad);
+    CU(m->tc_a_hi.reserve((size_t)total * sizeof(__half)));
+    CU(m->tc_a_lo.reserve((size_t)total * sizeof(__half)));
+    __half* a_hi_p = m->tc_a_hi.as<__half>();
+    __half* a_lo_p = m->tc_a_lo.as<__half>();
+    gemm_tc_split_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(Q, C, m->n, ldq, a_hi_p, a_lo_p, rows_pad, m->tc_kpad);
     CU(cudaGetLastError());
     CUtensorMap a_hi, a_lo;
-    if (make_tc_map(&a_hi, m->tc_a_hi, rows_pad, m->tc_kpad, kGtM) || make_tc_map(&a_lo, m->tc_a_lo, rows_pad, m->tc_kpad, kGtM)) return -1;
+    if (make_tc_map(&a_hi, a_hi_p, rows_pad, m->tc_kpad, kGtM) || make_tc_map(&a_lo, a_lo_p, rows_pad, m->tc_kpad, kGtM)) return -1;
     GemmTcArgs G{};
     G.C = C; G.Nout = Nout; G.n_kblocks = (int)(m->tc_kpad / kGtKB); G.alpha = alpha; G.D = D; G.ldd = ldd;
     G.n_tiles_m = (int)(rows_pad / kGtM);
@@ -1096,8 +1081,8 @@ static int launch_logistic(const b200_model* m, int C, const double* Q, long lon
     auto kern = logistic_fused_kernel<KB>;
     const size_t smem = logistic_smem_bytes<KB>();
     CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-    kern<<<dim3(bs.gx, bs.cpad / kLogiChains), 32 * (kLogiChains / (8 * B200_LOGI_MB)), smem, st>>>(m->X, m->y8, m->n_rows, Q, ldq, C, m->n, bs.gpart.as<double>(),
-                                                               bs.lpart.as<double>(), bs.cpad);
+    kern<<<dim3(bs.gx, bs.cpad / kLogiChains), kLogiThreads, smem, st>>>(m->X, m->y8, m->n_rows, Q, ldq, C, m->n, bs.gpart.as<double>(),
+                                                                        bs.lpart.as<double>(), bs.cpad);
     CU(cudaGetLastError());
     return 0;
 }
@@ -1128,13 +1113,10 @@ static int batch_eval(b200_model* m, int C, const double* Q, double* G, double* 
     const int gx = (int)std::max<long long>(1, std::min<long long>(n_slabs, sms / std::min(cb * cta_per_block, sms)));
     bs.gx = gx;
     bs.cpad = cb * kLogiChains;
-    if ((long long)gx * bs.cpad > bs.cap_rows) {
-        if (bs.gpart.p) { cudaFree(bs.gpart.p); bs.gpart.p = nullptr; }
-        if (bs.lpart.p) { cudaFree(bs.lpart.p); bs.lpart.p = nullptr; }
-        bs.cap_rows = std::max<long long>((long long)gx * bs.cpad, (long long)sms * kLogiChains);
-        CU(bs.gpart.alloc((size_t)bs.cap_rows * m->KP * sizeof(double)));
-        CU(bs.lpart.alloc((size_t)bs.cap_rows * sizeof(double)));
-    }
+    // at least one wave of chain blocks: gx * cpad barely changes when the batch shrinks (more row CTAs per chain block)
+    const size_t rows = (size_t)std::max<long long>((long long)gx * bs.cpad, (long long)sms * kLogiChains);
+    CU(bs.gpart.reserve(rows * m->KP * sizeof(double)));
+    CU(bs.lpart.reserve(rows * sizeof(double)));
     int rc = 0;
     if (tc) {
         // wgmma path: the same partial-result layout ([gx][128][Cpad] fp64), so the fixed-order finish below is shared
@@ -1169,8 +1151,8 @@ static int lockstep_logp(b200_model* m, const double* q_dev, int C, double* logp
     const int n = m->n;
     const long long ld = m->ld;
     DevBuf Qp, Gp;
-    CU(Qp.alloc((size_t)C * ld * sizeof(double)));
-    CU(Gp.alloc((size_t)C * ld * sizeof(double)));
+    CU(Qp.reserve((size_t)C * ld * sizeof(double)));
+    CU(Gp.reserve((size_t)C * ld * sizeof(double)));
     CU(cudaMemsetAsync(Qp.p, 0, (size_t)C * ld * sizeof(double), st));
     CU(cudaMemcpy2DAsync(Qp.p, ld * sizeof(double), q_dev, n * sizeof(double), n * sizeof(double), C, cudaMemcpyDeviceToDevice, st));
     BatchScratch bs;
@@ -1205,8 +1187,8 @@ static int run_lockstep(b200_model* m, LsDev P, cudaStream_t st) {
     // DENSE_ADAPT: four n x n matrices per chain (covariance, Cholesky factor, two raw scatter matrices; dense_adapt.cuh)
     const bool fa = P.mass_kind == B200_MASS_DENSE_ADAPT;
     const size_t b_fa = fa ? up((size_t)C * n * n * sizeof(double)) : 0;
-    CU(m->ensure_ls_arena(b_state + b_vecs + n_mats * b_mat + b_l + b_cnt + 3 * b_mom + 4 * b_fa));
-    char* a = static_cast<char*>(m->ls_arena);
+    CU(m->ls_arena.reserve(b_state + b_vecs + n_mats * b_mat + b_l + b_cnt + 3 * b_mom + 4 * b_fa));
+    char* a = m->ls_arena.as<char>();
     auto take = [&](size_t b) { char* p = a; a += b; return p; };
     P.state = reinterpret_cast<LsState*>(take(b_state));
     P.vecs = reinterpret_cast<double*>(take(b_vecs));
@@ -1257,8 +1239,8 @@ static int run_lockstep(b200_model* m, LsDev P, cudaStream_t st) {
     // requesting rows (for n = 10^4 they cost as much as the gradient and mass GEMMs of ALL chains), so requests are queued on
     // the device and served in batches: when half of the live chains are waiting in the queue, or as soon as a chain reaches
     // the end of its draw without its momentum (it then idles for one round: LsState phase 3).  The noise z of (chain, draw)
-    // does not depend on when it is served, so results are identical for every threshold.  B200_LS_MOM_DEFER=0: serve every round.
-    const double defer = fa ? 0.0 : std::max(0.0, std::min(1.0, env_int("B200_LS_MOM_DEFER", 50) / 100.0));
+    // does not depend on when it is served, so results are identical for every threshold.
+    const double defer = fa ? 0.0 : 0.5;
     CU(cudaMemsetAsync(P.counters, 0, 4 * sizeof(int), st));
     int C_eval = C;             // rows of the request matrices in use (shrinks when finished chains free a tile)
     for (;;) {
@@ -1290,10 +1272,8 @@ static int run_lockstep(b200_model* m, LsDev P, cudaStream_t st) {
             }
         }
         CU(cudaMemsetAsync(P.counters, 0, 2 * sizeof(int), st));
-#ifndef B200_ADV_W
-#define B200_ADV_W 16  // warps per chain of the lock-step advance kernel for long state vectors (16: 5 % faster than 8 at n = 10^4)
-#endif
-        if (n > 512) ls_advance_kernel<B200_ADV_W><<<C, 32 * B200_ADV_W, 0, st>>>(P);
+        constexpr int kAdvW = 16;  // warps per chain of the advance kernel for long state vectors (16: 5 % faster than 8 at n = 10^4)
+        if (n > 512) ls_advance_kernel<kAdvW><<<C, 32 * kAdvW, 0, st>>>(P);
         else ls_advance_kernel<1><<<blocks, 128, 0, st>>>(P);
         CU(cudaGetLastError());
         ++launches;
@@ -1324,16 +1304,13 @@ struct NutsLaunch {
     template <class Model, int NPL, int W>
     int operator()(const typename Model::Params& MP) {
         constexpr int NP = 32 * W * NPL;
-        constexpr bool SUBS = (W > 1) ? true : (B200_SUBTREE_SMEM != 0);
-        int wpb = (W == 1) ? env_int("B200_NUTS_WPB", 8) : 1;  // chains per CTA: 8 warps, 1 CTA per SM (see seg below)
-        int hot = env_int("B200_NUTS_HOT", (W == 1) ? 2 : 1);
-        wpb = std::max(1, std::min(wpb, B200_NUTS_THREADS / 32));
-        hot = std::max(0, std::min(hot, P.max_td));
+        constexpr int wpb = (W == 1) ? kNutsWarpChains : 1;  // chains per CTA (see seg below)
+        int hot = std::min((W == 1) ? 2 : 1, P.max_td);      // tree levels whose vectors live in shared memory
         const size_t data = (Model::shared_bytes(MP) + 15) & ~(size_t)15;
-        size_t smem = data + (size_t)wpb * nuts_warp_smem_bytes(NP, hot, SUBS, W);
+        size_t smem = data + (size_t)wpb * nuts_warp_smem_bytes(NP, hot, W);
         while (smem > 227 * 1024 && hot > 0) {  // shrink the hot window until the CTA fits
             --hot;
-            smem = data + (size_t)wpb * nuts_warp_smem_bytes(NP, hot, SUBS, W);
+            smem = data + (size_t)wpb * nuts_warp_smem_bytes(NP, hot, W);
         }
         if (smem > 227 * 1024) return fail("nuts: shared memory request %zu B exceeds 227 KB", smem);
         P.hot_levels = hot;
@@ -1342,14 +1319,14 @@ struct NutsLaunch {
         const size_t tree_bytes = ((size_t)P.C * P.scratch_stride * sizeof(double) + 255) & ~(size_t)255;
         const size_t ctx_bytes = ((size_t)P.C * sizeof(ChainCtx) + 255) & ~(size_t)255;
         const size_t sched_bytes = ((size_t)(P.C + 1) * sizeof(int) + 255) & ~(size_t)255;
-        CU(m->ensure_scratch(tree_bytes + ctx_bytes + sched_bytes));
-        char* base = static_cast<char*>(m->scratch);
+        CU(m->scratch.reserve(tree_bytes + ctx_bytes + sched_bytes));
+        char* base = m->scratch.as<char>();
         P.scratch = reinterpret_cast<double*>(base);
         P.ctx = reinterpret_cast<ChainCtx*>(base + tree_bytes);
         P.done = reinterpret_cast<int*>(base + tree_bytes + ctx_bytes);
         P.ticket = reinterpret_cast<unsigned int*>(P.done + P.C);
         CU(cudaMemsetAsync(P.done, 0, sched_bytes, st));
-        auto kern = nuts_warp_kernel<Model, NPL, W, SUBS>;
+        auto kern = nuts_warp_kernel<Model, NPL, W>;
         CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         // persistent grid: every CTA resident (teams take (chain, segment) units from the ticket counter)
         const int threads = (W == 1) ? wpb * 32 : 32 * W;
@@ -1361,9 +1338,9 @@ struct NutsLaunch {
         // iterations per work unit: fine enough to balance chains of different cost, coarse enough that the ~3 KB state
         // hand-over per unit is noise.  One unit per chain when every chain has its own resident team anyway.
         const int Ttot = P.n_iter;
-        int seg = env_int("B200_NUTS_SEG", 100);  // Radon bench step on an H100 SXM (700 W), wpb 8 / 4 / 2: seg 25 -> 377 / 386 / 391 ms,
+        int seg = 100;  // Radon bench step on an H100 SXM (700 W), wpb 8 / 4 / 2: seg 25 -> 377 / 386 / 391 ms,
         // 50 -> 371 / 380 / 385, 100 -> 368 / 378 / 383, 200 -> 369 / 378 / 383 (medians of 3; the draws are identical)
-        if (seg <= 0 || need <= blocks) seg = Ttot;
+        if (need <= blocks) seg = Ttot;
         P.seg_iters = std::max(1, std::min(seg, Ttot));
         typename Model::Params MPl;
         if (launch_params<Model>(m, MP, (long long)blocks * wpb, &MPl)) return -1;
@@ -1376,6 +1353,14 @@ struct NutsLaunch {
         return 0;
     }
 };
+
+// The arrays of b200_stats, and those of b200_chain_state with their elements per chain (include/b200nuts.h)
+#define B200_STATS_FIELDS(X)                                                                                         \
+    X(depth) X(tree_size) X(index_in_trajectory) X(diverging) X(reached_max_treedepth) X(step_size) X(step_size_bar) \
+    X(mean_tree_accept) X(energy) X(energy_error) X(max_energy_error) X(model_logp)
+#define B200_CHAIN_STATE_FIELDS(X)                                                                                       \
+    X(q, n) X(log_step, 1) X(log_bar, 1) X(hbar, 1) X(da_count, 1) X(n_samples, 1) X(window, 1) X(var, n) X(fg_n, 1)     \
+    X(fg_mean, n) X(fg_m2, n) X(bg_n, 1) X(bg_mean, n) X(bg_m2, n) X(n_grad, 1)
 
 extern "C" int b200_nuts_run(b200_model* m, const b200_nuts_cfg* cfg, const double* q0, const double* var0,
                              const double* mean0, const double* eps0, b200_pcg64* rng, const double* z,
@@ -1436,109 +1421,6 @@ extern "C" int b200_nuts_run(b200_model* m, const b200_nuts_cfg* cfg, const doub
         return fail("b200_nuts_run: partial schedules / chain-state export are implemented by the persistent engine only");
     const long long rec_lo = cfg->store_warmup ? it0 : std::max<long long>(cfg->tune, it0);
     const long long T = std::max<long long>(0, it0 + Ttot - rec_lo);
-    const size_t vb = (size_t)C * n * sizeof(double);
-    Staged s_q0, s_var0, s_mean0, s_eps0, s_rng, s_z, s_draws;
-    // Device staging of host arrays comes from ONE arena kept in the model handle: a steady-state call makes no cudaMalloc /
-    // cudaFree at all (per-call allocations of the small input arrays synchronise the device and make a public-API call
-    // take far longer than its kernel).  Everything except the draws (direct
-    // host writes, or their own buffer) and a host momentum buffer (parity tests) is lent from it.
-    const size_t ct_all = (size_t)C * (size_t)std::max<long long>(0, it0 + Ttot - rec_lo);
-    char* lend_p = nullptr;
-    size_t lend_left = 0;
-    auto up256 = [](size_t b) { return (b + 255) & ~(size_t)255; };
-    if (mem == B200_MEM_HOST) {
-        size_t need = 3 * up256(vb) + up256((size_t)C * sizeof(double)) + up256((size_t)C * sizeof(b200_pcg64));
-        if (stats) need += 12 * up256(ct_all * sizeof(double));
-        const size_t state_bytes = 6 * up256(vb) + 9 * up256((size_t)C * sizeof(double));
-        if (cfg->resume) need += state_bytes;
-        if (cfg->save) need += state_bytes;
-        CU(m->ensure_stage(need));
-        lend_p = static_cast<char*>(m->stage_arena);
-        lend_left = m->stage_bytes;
-    }
-    auto lend = [&](Staged& s, const void* user, size_t bytes) {
-        const size_t b = up256(bytes);
-        if (user && lend_p && b <= lend_left) { s.lent = lend_p; lend_p += b; lend_left -= b; }
-    };
-    lend(s_q0, q0, vb); lend(s_var0, var0, vb); lend(s_mean0, mean0, vb);
-    lend(s_eps0, eps0, (size_t)C * sizeof(double)); lend(s_rng, rng, (size_t)C * sizeof(b200_pcg64));
-    if (stage_in(s_q0, q0, vb, mem, true, false, st) || stage_in(s_var0, var0, vb, mem, true, false, st) ||
-        stage_in(s_mean0, mean0, vb, mem, true, false, st) ||
-        stage_in(s_eps0, eps0, (size_t)C * sizeof(double), mem, true, false, st) ||
-        stage_in(s_rng, rng, (size_t)C * sizeof(b200_pcg64), mem, true, true, st) ||
-        stage_in(s_z, cfg->momentum_source == B200_MOMENTUM_HOST_BUFFER ? z : nullptr, vb * Ttot, mem, true, false, st) ||
-        stage_in(s_draws, T > 0 ? draws_out : nullptr, vb * T, mem, false, true, st, /*direct=*/true))
-        return -1;
-    // stats / summary arrays
-    b200_stats ds{};
-    b200_chain_summary dsum{};
-    Staged st_arr[12], sm_arr[5];
-    const size_t ct = (size_t)C * T;
-    if (stats) {
-        // Sampler statistics are ONE 1-8 byte value per (chain, draw) and array: written straight into host memory they are
-        // 12 x C x T single-value PCIe write transactions (24 M for the Radon bench), which costs more link time than the
-        // draws themselves.  They are staged in HBM (one arena in the model handle) and leave with 12 DMA copies at the end
-        // (143 MB for the Radon bench).  The draws -- 256-byte coalesced row segments -- keep the direct path.
-        const bool direct_stats = getenv("B200_DIRECT_STATS") != nullptr;
-#define B200_ST(i, field, type)                                                              \
-    if (stats->field) {                                                                      \
-        if (!direct_stats) lend(st_arr[i], stats->field, ct * sizeof(type));                 \
-        if (stage_in(st_arr[i], stats->field, ct * sizeof(type), mem, false, true, st, /*direct=*/direct_stats)) return -1; \
-        ds.field = (type*)st_arr[i].ptr();                                                   \
-    }
-        B200_ST(0, depth, int32_t) B200_ST(1, tree_size, int32_t) B200_ST(2, index_in_trajectory, int32_t)
-        B200_ST(3, diverging, uint8_t) B200_ST(4, reached_max_treedepth, uint8_t) B200_ST(5, step_size, double)
-        B200_ST(6, step_size_bar, double) B200_ST(7, mean_tree_accept, double) B200_ST(8, energy, double)
-        B200_ST(9, energy_error, double) B200_ST(10, max_energy_error, double) B200_ST(11, model_logp, double)
-#undef B200_ST
-    }
-    if (summary) {
-        if (summary->grad_evals) {
-            if (stage_in(sm_arr[0], summary->grad_evals, (size_t)C * sizeof(int64_t), mem, false, true, st, true)) return -1;
-            dsum.grad_evals = (int64_t*)sm_arr[0].ptr();
-        }
-        if (summary->bad_energy_at) {
-            if (stage_in(sm_arr[1], summary->bad_energy_at, (size_t)C * sizeof(int32_t), mem, false, true, st, true)) return -1;
-            dsum.bad_energy_at = (int32_t*)sm_arr[1].ptr();
-        }
-        if (summary->final_step_size) {
-            if (stage_in(sm_arr[2], summary->final_step_size, (size_t)C * sizeof(double), mem, false, true, st, true)) return -1;
-            dsum.final_step_size = (double*)sm_arr[2].ptr();
-        }
-        if (summary->final_var) {
-            if (stage_in(sm_arr[3], summary->final_var, vb, mem, false, true, st, true)) return -1;
-            dsum.final_var = (double*)sm_arr[3].ptr();
-        }
-        if (summary->final_cov && cfg->mass_kind == B200_MASS_DENSE_ADAPT) {
-            if (stage_in(sm_arr[4], summary->final_cov, vb * n, mem, false, true, st, true)) return -1;
-            dsum.final_cov = (double*)sm_arr[4].ptr();
-        }
-    }
-    // draws of a frozen chain ("bad initial energy") from the failing iteration on are set to NaN by the kernels
-
-    // per-chain state in / out (b200_chain_state): 15 arrays each, staged like every other buffer
-    b200_chain_state d_resume{}, d_save{};
-    Staged st_state[30];
-    {
-        const size_t sb = (size_t)C * sizeof(double), ib = (size_t)C * sizeof(int32_t), lb = (size_t)C * sizeof(int64_t);
-        int slot = 0;
-        auto stage_state = [&](const b200_chain_state* src, b200_chain_state* dst, bool in) -> int {
-            if (!src) return 0;
-#define B200_SF(field, bytes, type)                                                                       \
-    if (!src->field) return fail("b200_nuts_run: chain state field `" #field "` is null");               \
-    lend(st_state[slot], src->field, bytes);                                                             \
-    if (stage_in(st_state[slot], src->field, bytes, mem, in, !in, st)) return -1;                        \
-    dst->field = (type*)st_state[slot++].ptr();
-            B200_SF(q, vb, double) B200_SF(log_step, sb, double) B200_SF(log_bar, sb, double) B200_SF(hbar, sb, double)
-            B200_SF(da_count, ib, int32_t) B200_SF(n_samples, ib, int32_t) B200_SF(window, ib, int32_t) B200_SF(var, vb, double)
-            B200_SF(fg_n, sb, double) B200_SF(fg_mean, vb, double) B200_SF(fg_m2, vb, double) B200_SF(bg_n, sb, double)
-            B200_SF(bg_mean, vb, double) B200_SF(bg_m2, vb, double) B200_SF(n_grad, lb, int64_t)
-#undef B200_SF
-            return 0;
-        };
-        if (stage_state(cfg->resume, &d_resume, true) || stage_state(cfg->save, &d_save, false)) return -1;
-    }
-
     RunCfg R{};
     R.it0 = (int)it0; R.n_iter = (int)Ttot;
     R.C = C; R.n = n; R.tune = cfg->tune; R.draws = cfg->draws;
@@ -1550,14 +1432,52 @@ extern "C" int b200_nuts_run(b200_model* m, const b200_nuts_cfg* cfg, const doub
     R.target = cfg->target_accept; R.gamma = cfg->gamma; R.kappa = cfg->k; R.t0 = cfg->t0;
     R.Emax = cfg->Emax; R.init_weight = cfg->mass_initial_weight;
     R.philox_seed = cfg->philox_seed; R.chain_offset = cfg->chain_offset;
-    R.q0 = (const double*)s_q0.ptr(); R.var0 = (const double*)s_var0.ptr();
-    R.mean0 = (const double*)s_mean0.ptr(); R.eps0c = (const double*)s_eps0.ptr(); R.z = (const double*)s_z.ptr();
-    R.rng = (b200_pcg64*)s_rng.ptr(); R.draws_out = (double*)s_draws.ptr();
-    R.st = ds; R.sm = dsum;
     if (cfg->constrain_draws) {
         if (!m->tr_kind) return fail("b200_nuts_run: constrain_draws needs b200_model_set_transforms first");
         R.tr_kind = m->tr_kind; R.tr_lo = m->tr_lo; R.tr_hi = m->tr_hi;
     }
+
+    const size_t vn = (size_t)C * n, ct = (size_t)C * T;
+    Staging sg(m, mem, st);
+    sg.add(&R.q0, q0, vn, Staging::IN);
+    sg.add(&R.var0, var0, vn, Staging::IN);
+    sg.add(&R.mean0, mean0, vn, Staging::IN);
+    sg.add(&R.eps0c, eps0, C, Staging::IN);
+    sg.add(&R.rng, rng, C, Staging::INOUT);
+    // the draws and a host momentum buffer (parity tests) are the large arrays: the arena is not grown to hold them
+    sg.add(&R.z, cfg->momentum_source == B200_MOMENTUM_HOST_BUFFER ? z : nullptr, vn * Ttot, Staging::IN, Staging::OWN);
+    sg.add(&R.draws_out, T > 0 ? draws_out : nullptr, vn * T, Staging::OUT, Staging::DIRECT | Staging::OWN);
+    // draws of a frozen chain ("bad initial energy") from the failing iteration on are set to NaN by the kernels
+    if (stats) {
+        // Sampler statistics are ONE 1-8 byte value per (chain, draw) and array: written straight into host memory they are
+        // 12 x C x T single-value PCIe write transactions (24 M for the Radon bench), which costs more link time than the
+        // draws themselves.  They are staged in HBM (the arena) and leave with 12 DMA copies at the end (143 MB for the
+        // Radon bench).  The draws -- 256-byte coalesced row segments -- keep the direct path.
+#define B200_STAGE_STAT(field) sg.add(&R.st.field, stats->field, ct, Staging::OUT);
+        B200_STATS_FIELDS(B200_STAGE_STAT)
+#undef B200_STAGE_STAT
+    }
+    if (summary) {
+        const int flags = Staging::DIRECT | Staging::OWN;
+        sg.add(&R.sm.grad_evals, summary->grad_evals, C, Staging::OUT, flags);
+        sg.add(&R.sm.bad_energy_at, summary->bad_energy_at, C, Staging::OUT, flags);
+        sg.add(&R.sm.final_step_size, summary->final_step_size, C, Staging::OUT, flags);
+        sg.add(&R.sm.final_var, summary->final_var, vn, Staging::OUT, flags);
+        if (cfg->mass_kind == B200_MASS_DENSE_ADAPT) sg.add(&R.sm.final_cov, summary->final_cov, vn * n, Staging::OUT, flags);
+    }
+    // per-chain state in / out (b200_chain_state)
+    b200_chain_state d_resume{}, d_save{};
+    auto stage_state = [&](const b200_chain_state* src, b200_chain_state* dst, Staging::Dir dir) -> int {
+        if (!src) return 0;
+#define B200_STAGE_STATE(field, per_chain)                                                    \
+    if (!src->field) return fail("b200_nuts_run: chain state field `" #field "` is null");   \
+    sg.add(&dst->field, src->field, (size_t)C * (per_chain), dir);
+        B200_CHAIN_STATE_FIELDS(B200_STAGE_STATE)
+#undef B200_STAGE_STATE
+        return 0;
+    };
+    if (stage_state(cfg->resume, &d_resume, Staging::IN) || stage_state(cfg->save, &d_save, Staging::OUT)) return -1;
+    if (sg.commit()) return -1;
 
     const double tr_stage = trace ? since(tr0) : 0.0;
     const auto tr1 = std::chrono::steady_clock::now();
@@ -1578,11 +1498,7 @@ extern "C" int b200_nuts_run(b200_model* m, const b200_nuts_cfg* cfg, const doub
 
     const double tr_run = trace ? since(tr1) : 0.0;
     const auto tr2 = std::chrono::steady_clock::now();
-    if (stage_out(s_rng, st) || stage_out(s_draws, st)) return -1;
-    for (auto& s : st_arr) if (stage_out(s, st)) return -1;
-    for (auto& s : sm_arr) if (stage_out(s, st)) return -1;
-    for (auto& s : st_state) if (stage_out(s, st)) return -1;
-    CU(cudaStreamSynchronize(st));
+    if (sg.finish()) return -1;
     if (trace)
         fprintf(stderr, "[b200_nuts_run] staging %.2f ms | run %.2f ms (kernels %.2f ms) | copy-out %.2f ms | mem=%s\n", tr_stage, tr_run,
                 g_last_ms, since(tr2), mem == B200_MEM_HOST ? "host" : "device");
@@ -1600,20 +1516,21 @@ extern "C" int b200_pointwise_loglik(b200_model* m, int32_t lik, const double* d
     // the IR tables live on the device: read the number of observations of this factor back
     IrLikD L;
     CU(cudaMemcpy(&L, m->ir.liks + lik, sizeof L, cudaMemcpyDeviceToHost));
-    Staged s_in, s_out;
-    if (stage_in(s_in, draws, (size_t)D * m->n * sizeof(double), mem, true, false, st) ||
-        stage_in(s_out, out, (size_t)D * (size_t)L.N * sizeof(double), mem, false, true, st))
-        return -1;
+    const double* d_draws = nullptr;
+    double* d_out = nullptr;
+    Staging sg(m, mem, st);
+    sg.add(&d_draws, draws, (size_t)D * m->n, Staging::IN, Staging::OWN);
+    sg.add(&d_out, out, (size_t)D * (size_t)L.N, Staging::OUT, Staging::OWN);
+    if (sg.commit()) return -1;
     const int wpb = 8;
     const int blocks = (int)std::max<long long>(1, std::min<long long>((D + wpb - 1) / wpb, sm_count(m->device) * 8));
-    CU(m->ensure_ir_scratch((long long)blocks * wpb));
+    CU(m->ir_scratch.reserve((size_t)blocks * wpb * (size_t)m->ir.stride * sizeof(double)));
+    m->ir.scratch = m->ir_scratch.as<double>();
     Timer t(st);
-    ir_pointwise_kernel<<<blocks, wpb * 32, 0, st>>>(m->ir, lik, D, (const double*)s_in.ptr(), (double*)s_out.ptr());
+    ir_pointwise_kernel<<<blocks, wpb * 32, 0, st>>>(m->ir, lik, D, d_draws, d_out);
     CU(cudaGetLastError());
     t.stop(1);
-    if (stage_out(s_out, st)) return -1;
-    CU(cudaStreamSynchronize(st));
-    return 0;
+    return sg.finish();
 }
 
 extern "C" int b200_last_kernel_ms(double* ms, int32_t* launches) {
@@ -1640,7 +1557,7 @@ extern "C" int b200_measure_fp64_tflops(double* tflops) {
     if (!tflops) return fail("null argument");
     const int blocks = current_sm_count() * 8, threads = 256, iters = 1 << 14;
     DevBuf out;
-    CU(out.alloc((size_t)blocks * threads * sizeof(double)));
+    CU(out.reserve((size_t)blocks * threads * sizeof(double)));
     dfma_peak_kernel<<<blocks, threads>>>(out.as<double>(), 64);
     CU(cudaDeviceSynchronize());
     double best = 0.0;
@@ -1678,7 +1595,7 @@ extern "C" int b200_measure_dmma_tflops(double* tflops) {
     if (!tflops) return fail("null argument");
     const int blocks = current_sm_count() * 2, threads = 256, iters = 1 << 12;
     DevBuf out;
-    CU(out.alloc((size_t)blocks * threads * sizeof(double)));
+    CU(out.reserve((size_t)blocks * threads * sizeof(double)));
     dmma_peak_kernel<<<blocks, threads>>>(out.as<double>(), 16);
     CU(cudaDeviceSynchronize());
     double best = 0.0;

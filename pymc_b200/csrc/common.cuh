@@ -8,9 +8,7 @@
 
 #define B200_FULL_MASK 0xffffffffu
 
-#ifndef B200_HALF_LOG_2PI
 #define B200_HALF_LOG_2PI 0.91893853320467274178032973640562
-#endif
 
 namespace b200 {
 

@@ -153,17 +153,16 @@ __host__ __device__ constexpr size_t logistic_smem_bytes() {
     return ((size_t)kLogiChains * (8 * KB + 4) + 2 * (size_t)kLogiRows * (8 * KB + 4)) * sizeof(double) + 64;
 }
 
-#ifndef B200_LOGI_MB
-#define B200_LOGI_MB 1  // 8-chain accumulator blocks per warp: 1 -> 16 warps x 8 chains per CTA (126 regs, 4 warps per
-                        // scheduler), 2 -> 8 warps x 16 chains (212 regs)
-#endif
-template <int KB, int MB = B200_LOGI_MB>
-__global__ void __launch_bounds__(32 * (kLogiChains / (8 * MB)), 1)
+constexpr int kLogiThreads = 32 * (kLogiChains / 8);  // one warp per 8 chains: 16 warps (126 regs, 4 warps per scheduler)
+
+template <int KB>
+__global__ void __launch_bounds__(kLogiThreads, 1)
     logistic_fused_kernel(const double* __restrict__ X /*[Npad][8KB]*/, const uint8_t* __restrict__ y, long long N,
                           const double* __restrict__ Q, long long ldq, int C, int K,
                           double* __restrict__ Gpart /*[gridDim.x][Cpad][8KB]*/, double* __restrict__ lpart /*[gridDim.x][Cpad]*/,
                           int Cpad) {
-    constexpr int KP = 8 * KB, LD = KP + 4, NT = 32 * (kLogiChains / (8 * MB));
+    constexpr int MB = 1;  // 8-chain accumulator blocks per warp
+    constexpr int KP = 8 * KB, LD = KP + 4, NT = kLogiThreads;
     extern __shared__ __align__(16) char smem_raw[];
     double* Qs = reinterpret_cast<double*>(smem_raw);
     double* Xs = Qs + kLogiChains * LD;                       // 2 slabs

@@ -28,12 +28,7 @@ namespace b200 {
 constexpr int kLsLevels = 12;
 
 // the O(n) vector passes of the advance kernel are latency-bound strided loops: unrolling keeps several loads in flight
-#ifndef B200_LS_UNROLL_N
-#define B200_LS_UNROLL_N 4
-#endif
-#define B200_LS_PRAGMA(x) _Pragma(#x)
-#define B200_LS_UNROLL_(n) B200_LS_PRAGMA(unroll n)
-#define B200_LS_UNROLL B200_LS_UNROLL_(B200_LS_UNROLL_N)
+constexpr int kLsUnroll = 4;
 
 // A pass over a chain's vectors in tiles of U elements per thread: ALL loads of a tile, then the arithmetic and the stores.
 // Written as `for (i) { load; store; }` the compiler must keep every load behind the previous iteration's store (the vectors
@@ -102,7 +97,7 @@ struct LsDev : RunCfg {  // a whole schedule per run: it0 = 0, n_iter = tune + d
 // thread of the team (common.cuh), so every thread carries an identical private copy of the scalar state.
 template <int W>
 __global__ void __launch_bounds__(W == 1 ? 128 : 32 * W) ls_advance_kernel(const LsDev P) {
-    constexpr int TS = 32 * W, U = B200_LS_UNROLL_N;
+    constexpr int TS = 32 * W, U = kLsUnroll;
     __shared__ double red_s[W == 1 ? 1 : 8 * W];
     double* red = red_s;
     const int lane = (W == 1) ? (threadIdx.x & 31) : (int)threadIdx.x;  // index inside the team
@@ -129,7 +124,7 @@ __global__ void __launch_bounds__(W == 1 ? 128 : 32 * W) ls_advance_kernel(const
     auto req_logp = [&]() -> double {
         if (P.logp_from_dot) {
             double s = 0.0;
-            B200_LS_UNROLL
+#pragma unroll kLsUnroll
             for (int i = lane; i < n; i += TS) s = fma(qreq[i], greq[i], s);
             return P.logp_const + 0.5 * team_sum<W>(s, lane, red);
         }
@@ -144,7 +139,7 @@ __global__ void __launch_bounds__(W == 1 ? 128 : 32 * W) ls_advance_kernel(const
     } else if (S.phase == 0) {
         // ---- evaluation at q0 has arrived: the start state of the first draw --------------------------------
         S.cur_logp = req_logp();
-        B200_LS_UNROLL
+#pragma unroll kLsUnroll
         for (int i = lane; i < n; i += TS) {
             V(LV_Q)[i] = qreq[i];
             V(LV_G)[i] = greq[i];
@@ -388,7 +383,7 @@ __global__ void __launch_bounds__(W == 1 ? 128 : 32 * W) ls_advance_kernel(const
             }
             if (S.dw.swap_due()) {
                 S.dw.swap();
-                B200_LS_UNROLL
+#pragma unroll kLsUnroll
                 for (int i = lane; i < n; i += TS) { V(S.dw.bg_m)[i] = 0.0; V(S.dw.bg_v)[i] = 0.0; }
             }
             ++S.dw.k_samples;
@@ -427,7 +422,7 @@ __global__ void __launch_bounds__(W == 1 ? 128 : 32 * W) ls_advance_kernel(const
                                 [&](int u, int i) { p[i] = a_[u]; v[i] = b_[u]; kin = fma(a_[u], b_[u], kin); });
             } else {
                 const double* var = V(LV_VAR);
-                B200_LS_UNROLL
+#pragma unroll kLsUnroll
                 for (int i = lane; i < n; i += TS) {
                     const double pi = (1.0 / sqrt(var[i])) * momentum_z(P, chain, S.it, i), vi = var[i] * pi;
                     p[i] = pi; v[i] = vi; kin = fma(pi, vi, kin);
@@ -527,7 +522,7 @@ __global__ void __launch_bounds__(W == 1 ? 128 : 32 * W) ls_advance_kernel(const
         *SP = S;
     }
     if (S.phase == 2 && P.sm.final_var)
-        B200_LS_UNROLL
+#pragma unroll kLsUnroll
         for (int i = lane; i < n; i += TS) P.sm.final_var[(long long)chain * n + i] = V(LV_VAR)[i];
     if (S.phase == 2 && fa && P.sm.final_cov) {
         const long long nn = (long long)n * n;

@@ -81,23 +81,16 @@ enum { G_LQ = 0, G_LP, G_LG, G_RQ, G_RP, G_RG, G_PS, G_PQ, G_NEARP, G_FGM, G_FGV
 __host__ __device__ inline long long nuts_scratch_doubles(int NP, int levels) {
     return (long long)(G_STACK + 4 * levels) * NP;
 }
-// shared memory per warp (bytes): q, g, hot stack levels (level 0: 2 vectors, others: 4), scalars
-#ifndef B200_SUBTREE_SMEM
-#define B200_SUBTREE_SMEM 0  // 1: left.p / p_sum / proposal q of the subtree under construction live in shared memory
-#endif                       //    (frees 6*NPL registers per lane -> more resident warps); 0: in registers
-// (per chain; + 3 vectors when the subtree under construction is kept in shared memory; + the team's reduction pad)
-__host__ __device__ inline size_t nuts_warp_smem_bytes(int NP, int hot, bool subs = B200_SUBTREE_SMEM, int W = 1) {
-    const int vecs = 2 + (subs ? 3 : 0) + (hot > 0 ? 2 + 4 * (hot - 1) : 0);
+// shared memory per chain (bytes): q, g, hot stack levels (level 0: 2 vectors, others: 4), scalars; a team (W > 1) also
+// keeps the subtree under construction there (left.p, p_sum, proposal q: 3 vectors; SUBS below) and its reduction pad
+__host__ __device__ inline size_t nuts_warp_smem_bytes(int NP, int hot, int W) {
+    const int vecs = 2 + (W > 1 ? 3 : 0) + (hot > 0 ? 2 + 4 * (hot - 1) : 0);
     return (size_t)vecs * NP * sizeof(double) + 5 * kMaxLevels * sizeof(double) +
            (W > 1 ? W * 8 * sizeof(double) : 0);
 }
 
-#ifndef B200_NUTS_THREADS
-#define B200_NUTS_THREADS 256  // CTA size cap of the NUTS kernel (warps per CTA <= THREADS/32)
-#endif
-#ifndef B200_NUTS_MINBLOCKS
-#define B200_NUTS_MINBLOCKS 1  // __launch_bounds__ min CTAs/SM: the register budget knob
-#endif
+constexpr int kNutsWarpChains = 8;  // chain = warp (W = 1): chains per CTA (256 threads, one CTA per SM)
+
 // CTA prologue of the model kernels: stage the model's observed data into the start of the dynamic shared memory (bulk
 // TMA).  Returns the bytes it occupies, padded to 16.
 template <class Model>
@@ -113,11 +106,12 @@ __device__ __forceinline__ size_t stage_model_data(const typename Model::Params&
     return data_bytes;
 }
 
-// W = warps per chain (team).  SUBS = subtree-under-construction vectors in shared memory instead of registers.
-#define B200_NUTS_BOUNDS __launch_bounds__(W > 1 ? 32 * W : B200_NUTS_THREADS, W > 1 ? 1 : B200_NUTS_MINBLOCKS)
-template <class Model, int NPL, int W, bool SUBS>
-__global__ void B200_NUTS_BOUNDS
+// W = warps per chain (team).
+template <class Model, int NPL, int W>
+__global__ void __launch_bounds__(W > 1 ? 32 * W : 32 * kNutsWarpChains, 1)
     nuts_warp_kernel(const NutsDev P, const typename Model::Params M) {
+    // subtree-under-construction vectors in shared memory (a team: frees 6 NPL registers per thread) or in registers
+    constexpr bool SUBS = W > 1;
     constexpr int TS = 32 * W;      // threads per chain
     constexpr int NP = TS * NPL;    // padded vector length
     extern __shared__ __align__(16) char smem_raw[];
@@ -130,7 +124,7 @@ __global__ void B200_NUTS_BOUNDS
     __shared__ unsigned int ticket_s;  // W > 1: the CTA's current ticket
 
     const int hot = P.hot_levels;
-    double* ws = reinterpret_cast<double*>(smem_raw + data_bytes + wib * nuts_warp_smem_bytes(NP, hot, SUBS, W));
+    double* ws = reinterpret_cast<double*>(smem_raw + data_bytes + wib * nuts_warp_smem_bytes(NP, hot, W));
     double* q_s = ws;
     double* g_s = ws + NP;
     double* sub_s = ws + 2 * NP + lane;            // SUBS: left.p, p_sum, proposal q of the subtree under construction

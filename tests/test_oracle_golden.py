@@ -101,9 +101,9 @@ def test_dense_mass_step_adaptation_prefix_reproduces_golden(golden):
 
 
 def test_ms_weight_candidate_takes_the_reference_decisions(golden, monkeypatch):
-    """The (m, s) multinomial-weight arithmetic prepared for the CUDA kernel (nuts_warp.cuh, B200_MS_WEIGHTS: log-weight =
-    m + log s, one exp and no log per merge) restated here on top of the oracle: it must take exactly the decisions of
-    the reference's logaddexp arithmetic on the golden chains."""
+    """The (m, s) multinomial-weight arithmetic of the persistent CUDA kernel (nuts_warp.cuh: log-weight = m + log s, one
+    exp and no log per merge) restated here on top of the oracle: it must take exactly the decisions of the reference's
+    logaddexp arithmetic on the golden chains."""
     import math
 
     class MSTrajectory(nuts_numpy._Trajectory):

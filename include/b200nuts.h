@@ -112,9 +112,12 @@ typedef struct b200_ir_factor {
     int32_t offset, size; /* the variable's slice of q */
     const int32_t* idx;   /* [N] gather index into the variable, or NULL (scalar: broadcast; size == N: elementwise) */
 } b200_ir_factor;
+/* A term is coef[i] * prod_f x_f[idx_f[i]] when n_cols == 0.  n_cols > 0 makes it a design term,
+ * eta_i += sum_k X[i][k] x[f[0].offset + k]: coef is X, row-major [N][n_cols], finite; n_factors == 1, f[0].size == n_cols
+ * and f[0].idx == NULL.  b200_model_create refuses any other design table with the words ModelIR.validate uses. */
 typedef struct b200_ir_term {
-    const double* coef; /* [N] or NULL (= 1) */
-    int32_t n_factors, reserved;
+    const double* coef; /* [N] or NULL (= 1); a design term: X [N][n_cols] */
+    int32_t n_factors, n_cols;
     b200_ir_factor f[3];
 } b200_ir_term;
 typedef struct b200_ir_lik {

@@ -64,7 +64,7 @@ class IrFactor(C.Structure):
 
 
 class IrTerm(C.Structure):
-    _fields_ = [("coef", C.c_void_p), ("n_factors", C.c_int32), ("reserved", C.c_int32), ("f", IrFactor * 3)]
+    _fields_ = [("coef", C.c_void_p), ("n_factors", C.c_int32), ("n_cols", C.c_int32), ("f", IrFactor * 3)]
 
 
 class IrLik(C.Structure):
@@ -112,6 +112,7 @@ def build_ir(low):
         for t, T in enumerate(L["terms"]):
             terms[t].coef = addr(T["coef"])
             terms[t].n_factors = len(T["factors"])
+            terms[t].n_cols = int(T.get("n_cols", 0))  # > 0: a design term, coef = X [N][n_cols]
             for f, (o, sz, idx) in enumerate(T["factors"]):
                 terms[t].f[f] = IrFactor(int(o), int(sz), addr(idx))
         keep.append(terms)

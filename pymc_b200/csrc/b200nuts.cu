@@ -403,6 +403,7 @@ static int prepare_ir(b200_model* m, const b200_model_desc* d) {
     std::vector<IrLikD> liks(std::max(R->n_liks, 0));
     std::vector<IrTermD> terms;
     long long max_obs = 0;
+    bool has_design = false;
     for (int l = 0; l < R->n_liks; ++l) {
         const b200_ir_lik& L = R->liks[l];
         if (L.N <= 0 || L.N > 0x7fffffff || !L.y) return fail("ir: likelihood %d: missing observations", l);
@@ -508,6 +509,27 @@ static int prepare_ir(b200_model* m, const b200_model_desc* d) {
             if (T.n_factors < 0 || T.n_factors > 3) return fail("ir: likelihood %d term %d: 0..3 variable factors", l, t);
             IrTermD TD{};
             TD.n_factors = T.n_factors;
+            if (T.n_cols != 0) {  // design term: coef is X [N][n_cols]; the same checks and words as ModelIR.validate()
+                const int K = T.n_cols;
+                if (T.n_factors != 1) return fail("ir: likelihood %d term %d: a design term has exactly one factor", l, t);
+                if (T.f[0].idx) return fail("ir: likelihood %d term %d: a design term's factor takes no index", l, t);
+                if (K < 0 || T.f[0].size != K || !T.coef)
+                    return fail("ir: likelihood %d term %d: X must have shape (N, size of the variable)", l, t);
+                if (T.f[0].offset < 0 || T.f[0].offset + K > n) return fail("ir: likelihood %d term %d: factor slice outside q", l, t);
+                std::vector<double> xt((size_t)N * K);
+                for (long long i = 0; i < N; ++i)
+                    for (int k = 0; k < K; ++k) {
+                        const double v = T.coef[i * K + k];
+                        if (!std::isfinite(v)) return fail("ir: likelihood %d term %d: X must be finite (at row %lld, column %d)", l, t, i, k);
+                        xt[(size_t)k * N + i] = v;
+                    }
+                TD.n_cols = K;
+                TD.f[0] = IrFactorD{T.f[0].offset, K, nullptr, nullptr, nullptr};
+                if (upload_raw(m, T.coef, (size_t)N * K, &TD.coef) || upload(m, xt, &TD.xt)) return -1;
+                has_design = true;
+                terms.push_back(TD);
+                continue;
+            }
             if (T.coef && upload_raw(m, T.coef, (size_t)N, &TD.coef)) return -1;
             for (int f = 0; f < T.n_factors; ++f) {
                 const b200_ir_factor& F = T.f[f];
@@ -550,7 +572,7 @@ static int prepare_ir(b200_model* m, const b200_model_desc* d) {
         upload(m, ars, &P.ar1))
         return -1;
     P.n_pad = (n + 3) & ~3;
-    P.stride = P.n_pad + ((max_obs + 3) & ~3LL);
+    P.stride = P.n_pad + ((max_obs + 3) & ~3LL) + (has_design ? kIrPartDoubles : 0);
     m->ir_max_obs = max_obs;
     return 0;
 }

@@ -34,7 +34,56 @@ struct IrParamD { int kind, ref; double value; };                     // kind 0:
 struct IrVarD { int offset, size, transform, pad; double lo, hi; };
 struct IrPriorD { int dist, offset, size, pad; IrParamD p[3]; double c0; };      // c0: per-element constant of the density
 struct IrFactorD { int offset, size; const int* idx; const int* rowptr; const int* rowobs; };  // CSR: element -> observations
-struct IrTermD { const double* coef; int n_factors, pad; IrFactorD f[3]; };
+// n_cols > 0: a design term, eta_i += sum_k X[i][k] x[f[0].offset + k], with coef = X row-major [N][n_cols] (the gradient
+// reads it) and xt = X column-major [n_cols][N] (the forward pass reads it: consecutive threads take consecutive rows).
+struct IrTermD { const double* coef; int n_factors, n_cols; IrFactorD f[3]; const double* xt; };
+constexpr int kIrPartDoubles = 256;  // per-team slice partials of a design term's gradient, at the end of the team scratch
+
+// sum_k X[i][k] b[k], k ascending
+__device__ __forceinline__ double ir_design_row(const IrTermD& Tm, const double* b, int i, int N) {
+    const double* xt = Tm.xt + i;
+    double s = 0.0;
+    for (int k = 0; k < Tm.n_cols; ++k) s = fma(xt[(long long)k * N], b[k], s);
+    return s;
+}
+
+// g[k] += sum_i X[i][k] r[i] with the whole team, no atomics.  Columns go TS at a time; a block of kc < TS columns (the last
+// one) splits the rows into S = TS / kc interleaved slices, thread t taking column t % kc and rows i = t / kc (mod S), so a
+// warp reads adjacent rows of row-major X.  The slice partials meet in `part` and are added in slice order.  Every sum
+// has a fixed order, so the result does not depend on the run or on the other teams.
+template <int W>
+__device__ __forceinline__ void ir_design_grad(const IrTermD& Tm, const double* r, int N, double* g, double* part, int tid) {
+    constexpr int TS = 32 * W;
+    const int K = Tm.n_cols;
+    const double* X = Tm.coef;
+    for (int c0 = 0; c0 < K; c0 += TS) {
+        const int kc = min(K - c0, TS), S = TS / kc, c = tid % kc, s = tid / kc;
+        double a0 = 0.0, a1 = 0.0, a2 = 0.0, a3 = 0.0;  // four independent chains, combined in a fixed order
+        if (s < S) {
+            const double* xc = X + c0 + c;
+            int i = s;
+            for (; i + 3 * S < N; i += 4 * S) {
+                a0 = fma(xc[(long long)i * K], r[i], a0);
+                a1 = fma(xc[(long long)(i + S) * K], r[i + S], a1);
+                a2 = fma(xc[(long long)(i + 2 * S) * K], r[i + 2 * S], a2);
+                a3 = fma(xc[(long long)(i + 3 * S) * K], r[i + 3 * S], a3);
+            }
+            for (; i < N; i += S) a0 = fma(xc[(long long)i * K], r[i], a0);
+        }
+        const double a = (a0 + a1) + (a2 + a3);
+        if (S == 1) {
+            if (s == 0) g[c0 + c] += a;
+        } else {  // uniform branch; only the last block can take it
+            if (s < S) part[tid] = a;
+            team_sync<W>();
+            if (tid < kc) {
+                double tot = part[c];
+                for (int j = 1; j < S; ++j) tot += part[j * kc + c];
+                g[c0 + c] += tot;
+            }
+        }
+    }
+}
 // c0: sum of the constant parts over i.  Random dispersion (sigma_kind REF): Gamma keeps sum_i log y_i in sum_log_y;
 // NegativeBinomial keeps the distinct nonzero y values u[k] with their counts cnt[k] (n_tab of them), over which the
 // alpha-dependent normalising terms sum_i lgamma(y_i + a) - lgamma(a) and their digamma gradient are evaluated.
@@ -47,7 +96,7 @@ struct IrModel {
         const IrVarD* vars; const IrPriorD* priors; const IrLikD* liks; const IrTermD* terms; const IrAr1D* ar1;
         int n_vars, n_priors, n_liks, n_ar1, n;
         double* scratch;            // [slots][stride]
-        long long stride;           // doubles per team: n_pad + max N
+        long long stride;           // doubles per team: n_pad + max N (+ kIrPartDoubles with a design term)
         int n_pad;
     };
     __host__ __device__ static size_t shared_bytes(const Params&) { return 0; }
@@ -169,6 +218,10 @@ struct IrModel {
                 double eta = 0.0;
                 for (int t = 0; t < L.n_terms; ++t) {
                     const IrTermD& Tm = P.terms[L.term0 + t];
+                    if (Tm.n_cols) {
+                        eta += ir_design_row(Tm, x + Tm.f[0].offset, i, N);
+                        continue;
+                    }
                     double pr = Tm.coef ? Tm.coef[i] : 1.0;
                     for (int f = 0; f < Tm.n_factors; ++f) {
                         const IrFactorD& Fc = Tm.f[f];
@@ -268,6 +321,11 @@ struct IrModel {
             // gradient of every (term, factor): d eta_i / d x_f = coef * (other factors)
             for (int t = 0; t < L.n_terms; ++t) {
                 const IrTermD& Tm = P.terms[L.term0 + t];
+                if (Tm.n_cols) {  // uniform branch: the residuals r are complete after the barrier above
+                    ir_design_grad<W>(Tm, r, N, g_s + Tm.f[0].offset, x + P.stride - kIrPartDoubles, tid);
+                    team_sync<W>();
+                    continue;
+                }
                 for (int f = 0; f < Tm.n_factors; ++f) {
                     const IrFactorD& Fc = Tm.f[f];
                     auto others = [&](int i) -> double {
@@ -387,6 +445,10 @@ __global__ void __launch_bounds__(256) ir_pointwise_kernel(const IrModel::Params
             double eta = 0.0;
             for (int t = 0; t < L.n_terms; ++t) {
                 const IrTermD& Tm = P.terms[L.term0 + t];
+                if (Tm.n_cols) {
+                    eta += ir_design_row(Tm, x + Tm.f[0].offset, i, N);
+                    continue;
+                }
                 double pr = Tm.coef ? Tm.coef[i] : 1.0;
                 for (int f = 0; f < Tm.n_factors; ++f) {
                     const IrFactorD& Fc = Tm.f[f];

@@ -54,15 +54,22 @@ class CompiledModel:
 
     ``spec`` is either a ``pymc_b200.ir.ModelIR`` (the general interface: any model of the closed factor set; routed to
     a hand-specialised kernel when ``ir.specialise`` recognises its shape, otherwise evaluated by the generic IR device
-    function) or a ``models.ModelSpec`` naming one of the hand-written kernels directly (the GEMM-shaped configs)."""
+    function) or a ``models.ModelSpec`` naming one of the hand-written kernels directly (the GEMM-shaped configs).
+
+    On the generic function, ``specialise`` (the default) also evaluates ``ir.fuse_design_columns(spec)``: a design matrix
+    written one column per term runs as one team-parallel design term.  ``specialise=False`` evaluates the IR exactly as
+    written."""
 
     def __init__(self, spec, device: int | None = None, specialise: bool | str = True):
         from . import ir as _ir
 
         self.ir = None
+        lowered = None  # the IR the generic device function evaluates
         if isinstance(spec, _ir.ModelIR):
-            self.ir = spec
+            self.ir = lowered = spec
             fast = _ir.specialise(spec, extended=(specialise == "all")) if specialise else None
+            if fast is None and specialise:  # X beta written one column per term runs as one design term
+                lowered = _ir.fuse_design_columns(spec)
             spec = fast if fast is not None else _ir_spec(spec)
         self.spec = spec
         self.n = spec.n
@@ -103,7 +110,7 @@ class CompiledModel:
             d.m1, d.m2 = hold(LinvT, np.float64), hold(L, np.float64)
             d.scalar0 = spec.meta["logdet_L"]
         elif spec.name == "ir":
-            c_ir, keep_ir = _lib.build_ir(_ir.lower(self.ir))
+            c_ir, keep_ir = _lib.build_ir(_ir.lower(lowered))
             keep += keep_ir + [c_ir]
             d.ir = C.addressof(c_ir)
         handle = C.c_void_p()

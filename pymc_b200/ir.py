@@ -20,6 +20,7 @@ needs no new CUDA.  Models whose IR matches a hand-specialised kernel (Eight Sch
 """
 from __future__ import annotations
 
+import copy
 from dataclasses import dataclass, field
 
 import numpy as np
@@ -67,6 +68,11 @@ def _positive_support(v) -> bool:
     return v.transform == "log" or (v.transform == "interval" and v.bounds[0] >= 0.0)
 
 
+def is_design(t) -> bool:
+    """A design term: its coef is a 2-D X [N][K] (see ``Term``)."""
+    return t.coef is not None and np.ndim(t.coef) == 2
+
+
 @dataclass(frozen=True)
 class Ref:
     """A parameter that is another (scalar) value variable, seen through its transform (e.g. sigma_a)."""
@@ -94,7 +100,10 @@ class Prior:
 @dataclass
 class Term:
     """coef[i] * prod_f x_f[idx_f[i]].  A factor's idx is None for a scalar variable (broadcast) or for a vector variable of
-    the likelihood's own length (elementwise)."""
+    the likelihood's own length (elementwise).
+
+    A design term has a 2-D coef X of shape [N][K] and exactly one factor, a variable of size K with no index:
+    it adds sum_k X[i, k] * x[k], i.e. ``pm.math.dot(X, beta)``, evaluated on the device as one team-parallel term."""
 
     factors: list  # [(var_name, idx or None), ...]
     coef: np.ndarray | float | None = None
@@ -197,6 +206,9 @@ class ModelIR:
                 raise ValueError(f"likelihood {L.dist!r} is not in the closed set {sorted(LIK_DISTS)}")
             N = len(L.y)
             for t in L.terms:
+                if is_design(t):
+                    self._check_design(t, N, f"likelihood {L.name}")
+                    continue
                 if len(t.factors) > MAX_TERM_FACTORS:  # no factor: a constant offset coef[i]
                     raise ValueError(f"a term has at most {MAX_TERM_FACTORS} variable factors")
                 for vn, idx in t.factors:
@@ -237,6 +249,21 @@ class ModelIR:
             self._check_scale(a.sigma, f"AR1 on {a.var}: sigma")
             if not (np.isfinite(a.init_sigma) and a.init_sigma > 0):
                 raise ValueError(f"AR1 on {a.var}: init_sigma must be > 0")
+
+    def _check_design(self, t, N: int, where: str) -> None:
+        """A design term: X [N][K] of finite values, one factor on a variable of size K, no index (the checks prepare_ir
+        makes, in the same words)."""
+        if len(t.factors) != 1:
+            raise ValueError(f"{where}: a design term has exactly one factor (got {len(t.factors)})")
+        vn, idx = t.factors[0]
+        if idx is not None:
+            raise ValueError(f"{where}: a design term's factor takes no index ({vn})")
+        X = np.asarray(t.coef)
+        K = self.var(vn).size
+        if X.shape != (N, K):
+            raise ValueError(f"{where}: X must have shape (N, size of the variable): X is {X.shape}, N = {N}, {vn} has size {K}")
+        if not np.all(np.isfinite(X)):
+            raise ValueError(f"{where}: X must be finite")
 
     def _check_scale(self, a, what: str) -> None:
         """A scale slot (a prior's sigma / beta / lam, a likelihood's sigma, an AR(1) sigma, a dispersion alpha): a finite
@@ -321,6 +348,13 @@ class ModelIR:
             lead = None
             total = 0.0
             for t in d.terms:
+                if is_design(t):  # X @ x
+                    v = self.var(t.factors[0][0])
+                    x = np.asarray(posterior[v.rv_name])
+                    x = x[..., None] if v.size == 1 else x
+                    lead = x.shape[:-1]
+                    total = total + x @ np.asarray(t.coef, dtype=np.float64).T
+                    continue
                 term = 1.0 if t.coef is None else np.asarray(t.coef, dtype=np.float64)
                 for vn, idx in t.factors:
                     v = self.var(vn)
@@ -343,7 +377,7 @@ class ModelIR:
         out = {}
         for L in self.likelihoods:
             for k, t in enumerate(L.terms):
-                if t.coef is not None and np.ndim(t.coef) == 1:
+                if t.coef is not None and np.ndim(t.coef) in (1, 2):  # 2: a design term's X
                     out[f"{L.name}_coef{k}"] = np.asarray(t.coef)
                 for vn, idx in t.factors:
                     if idx is not None:
@@ -505,6 +539,7 @@ class LoweredIR:
     var_bounds: np.ndarray  # [n_vars][2]
     priors: list            # [(dist, var, [(kind, value, ref_offset)] * 3)]
     liks: list              # [dict(dist, N, y, terms=[dict(coef, factors=[(offset, size, idx)])], sigma_kind, sigma_value, sigma_ref, sigma_obs, nu)]
+                            # a design term's dict also has n_cols = K, with coef = X [N][K]
     ar1: list               # [(var, phi(kind, value, ref), sigma(kind, value, ref), init_sigma)]
 
 
@@ -536,6 +571,11 @@ def lower(ir: ModelIR) -> LoweredIR:
         N = len(L.y)
         terms = []
         for t in L.terms:
+            if is_design(t):  # one ABI design term: coef = X row-major, n_cols = K
+                v = ir.var(t.factors[0][0])
+                terms.append(dict(coef=np.ascontiguousarray(t.coef, dtype=np.float64), factors=[(off[v.name], v.size, None)],
+                                  n_cols=v.size))
+                continue
             coef = None
             scale = 1.0
             if t.coef is not None:
@@ -563,6 +603,54 @@ def lower(ir: ModelIR) -> LoweredIR:
                          sigma_kind=sk, sigma_value=sv, sigma_ref=sr, sigma_obs=so, nu=float(L.nu)))
     ar1 = [(index[ir.var(a.var).name], _param(ir, a.phi, off), _param(ir, a.sigma, off), float(a.init_sigma)) for a in ir.ar1]
     return LoweredIR(ir.n, vars_, bounds, priors, liks, ar1)
+
+
+def _column_of(t, N: int, ir: ModelIR):
+    """(variable name, k) when term t is column k of a design matrix written out: one factor on a vector variable of size
+    K >= 2, gathered at the constant index k, times a 1-D coefficient of length N, a scalar or nothing; else None."""
+    if len(t.factors) != 1 or t.factors[0][1] is None:
+        return None
+    vn, idx = t.factors[0]
+    v = ir.var(vn)
+    idx = np.asarray(idx)
+    if v.size < 2 or idx.shape != (N,) or N == 0:
+        return None
+    k = int(idx[0])
+    if not (0 <= k < v.size and np.all(idx == k)):
+        return None
+    if t.coef is not None and not (np.ndim(t.coef) == 0 or (np.ndim(t.coef) == 1 and len(t.coef) == N)):
+        return None
+    return v.name, k
+
+
+def fuse_design_columns(model: ModelIR) -> ModelIR:
+    """A copy of ``model`` in which, per likelihood, each complete run of column terms -- one term per column k = 0..K-1 of
+    the same vector variable of size K, as ``from_pymc`` lowers ``pm.math.dot(X, beta)`` -- is one design term with
+    X[:, k] = the column's coefficient, placed where the run's first term was.  Partial or duplicated runs, indexed group
+    effects, multi-factor terms and Deterministics stay as written; ``model`` itself is not changed."""
+    out = copy.deepcopy(model)
+    for L in out.likelihoods:
+        N = len(L.y)
+        runs = {}  # variable -> [(term position, k)]
+        for j, t in enumerate(L.terms):
+            ck = _column_of(t, N, out)
+            if ck is not None:
+                runs.setdefault(ck[0], []).append((j, ck[1]))
+        fused, drop = {}, set()
+        for vn, cols in runs.items():
+            K = out.var(vn).size
+            if sorted(k for _, k in cols) != list(range(K)):
+                continue
+            X = np.empty((N, K))
+            for j, k in cols:
+                c = L.terms[j].coef
+                X[:, k] = 1.0 if c is None else np.asarray(c, dtype=np.float64)
+            first = min(j for j, _ in cols)
+            fused[first] = Term([(vn, None)], coef=X)
+            drop.update(j for j, _ in cols)
+        if fused:
+            L.terms = [fused[j] if j in fused else t for j, t in enumerate(L.terms) if j in fused or j not in drop]
+    return out
 
 
 # ------------------------------------------------------------------------------------------------------------------------
@@ -619,24 +707,31 @@ def specialise(ir: ModelIR, extended: bool = False):
         return None
     # ---- logistic GLM (BASELINE config 3): beta ~ Normal(0, 1)^K, y ~ Bernoulli(logit_p = X beta), K <= 128 --------------
     if extended and L.dist == "bernoulli_logit":
-        if not (len(names) == 1 and tr == [None] and 1 <= sizes[0] <= 128 and len(L.terms) == sizes[0]):
+        design = len(L.terms) == 1 and is_design(L.terms[0])  # X beta as one design term, or as one term per column
+        if not (len(names) == 1 and tr == [None] and 1 <= sizes[0] <= 128 and (design or len(L.terms) == sizes[0])):
             return None
         beta, K, N = names[0], sizes[0], len(L.y)
         if not (beta in pri and pri[beta].dist == "normal" and const(pri[beta], 0, 0.0) and const(pri[beta], 1, 1.0)):
             return None
         if not np.all((np.asarray(L.y) == 0) | (np.asarray(L.y) == 1)):
             return None
-        X = np.empty((N, K))
-        seen = set()
-        for t in L.terms:
-            if len(t.factors) != 1 or t.factors[0][0] != beta or t.factors[0][1] is None or np.ndim(t.coef) != 1 or len(t.coef) != N:
+        if design:
+            t = L.terms[0]
+            if ir.var(t.factors[0][0]).name != beta or np.shape(t.coef) != (N, K):
                 return None
-            ix = np.asarray(t.factors[0][1])
-            k = int(ix[0])
-            if k in seen or not (0 <= k < K) or not np.all(ix == k):
-                return None
-            seen.add(k)
-            X[:, k] = t.coef
+            X = np.array(t.coef, dtype=np.float64)
+        else:
+            X = np.empty((N, K))
+            seen = set()
+            for t in L.terms:
+                if len(t.factors) != 1 or t.factors[0][0] != beta or t.factors[0][1] is None or np.ndim(t.coef) != 1 or len(t.coef) != N:
+                    return None
+                ix = np.asarray(t.factors[0][1])
+                k = int(ix[0])
+                if k in seen or not (0 <= k < K) or not np.all(ix == k):
+                    return None
+                seen.add(k)
+                X[:, k] = t.coef
         spec = models.logistic(n_rows=4, n_features=2)  # layout donor
         spec.n = K
         spec.vars, _ = models._layout([(beta, ir.vars[0].rv_name, K, None, None)])

@@ -59,7 +59,10 @@ __device__ __forceinline__ double digamma(double x) {
 __device__ __forceinline__ void halfcauchy_log(double z, double x, double beta, double log_beta,
                                                double& val, double& dz) {
     const double t = x * (1.0 / beta);
-    const double u = t * t;
+    // rounded product: an unmarked t * t lets ptxas fuse it into 1 + t * t below at some inlining sites and not at others
+    // (it did so in the batched Eight Schools logp kernel but not in its NUTS kernel), so one model's logp at one point
+    // would differ between kernels by an ulp
+    const double u = __dmul_rn(t, t);
     val = (0.69314718055994530942 - 1.1447298858494001741 /* log pi */) - log_beta - log1p_abs(u) + z;
     dz = 1.0 - 2.0 * u / (1.0 + u);
 }

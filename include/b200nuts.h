@@ -306,8 +306,10 @@ int b200_model_create(const b200_model_desc* desc, b200_model** out);
  *   B200_PRECISION_FP64      IEEE fp64 on the fp64 tensor path (DMMA) -- the parity mode, default.
  *   B200_PRECISION_TC_FP16X2 LOGISTIC and MVGAUSS: the dense contractions on the fp16 tensor cores (wgmma, TMA) with
  *                            every fp64 operand split into two fp16 pieces and fp32 accumulation, drained into fp64 every
- *                            256 rows (logistic) / into compensated sums every 64 terms (GEMM); gradient within 1e-6 of
- *                            its largest entry (tests/test_gpu_tc.py).
+ *                            256 rows (logistic) / into compensated sums every 64 terms (GEMM); operands are scaled by
+ *                            exact powers of two per row / column first, so at any data scale every output is within
+ *                            2^-18 S of the exact value, S = the sum of |terms| it is made of (tests/test_gpu_contractions.py;
+ *                            gradient within 1e-6 of its largest entry at unit-scale data, tests/test_gpu_tc.py).
  * The reference computes in floatX = float64 (pymc/pytensorf.py); this is the "tensor cores where the logp really is a
  * dense matvec" performance mode of north_star, with its error stated next to the number. */
 #define B200_PRECISION_FP64 0

@@ -117,14 +117,19 @@ struct b200_model {
     const __half* Xh = nullptr;
     const __half* Xl = nullptr;
     const float* y32 = nullptr;
+    const int* x_exp = nullptr;     // [128] power-of-two column exponents of the X pieces
     long long tc_slabs = 0;
     CUtensorMap map_hi{}, map_lo{};
-    // dense Gaussian, tensor-core performance mode (csrc/gemm_tc.cuh): fp16 pieces of the n x n matrices (B operands) and the
-    // per-call pieces of the chains' vectors (A operand)
-    struct TcMat { const double* src = nullptr; const __half* hi = nullptr; const __half* lo = nullptr; CUtensorMap map_hi{}, map_lo{}; };
+    // dense Gaussian, tensor-core performance mode (csrc/gemm_tc.cuh): fp16 pieces of the n x n matrices (B operands, with
+    // their power-of-two row exponents) and the per-call pieces of the chains' vectors (A operand)
+    struct TcMat {
+        const double* src = nullptr; const __half* hi = nullptr; const __half* lo = nullptr; const int* exp = nullptr;
+        CUtensorMap map_hi{}, map_lo{};
+    };
     TcMat tc_mats[4];
     long long tc_kpad = 0, tc_npad = 0;
     DevBuf tc_a_hi, tc_a_lo;  // fp16 [rows][tc_kpad]
+    DevBuf tc_a_exp;          // int [rows]
     // Kept between runs (cudaMalloc/cudaFree of 100+ MB per call costs tens of milliseconds of host time on the end-to-end
     // path, and per-call allocations of small arrays synchronise the device):
     DevBuf scratch;      // persistent engine: per-chain tree scratch, chain contexts, work-unit tickets
@@ -1015,17 +1020,18 @@ static int prepare_mvgauss_tc(b200_model* m) {
     m->tc_npad = (n + kGtN - 1) / kGtN * kGtN;
     const double* src[4] = {m->prec, m->cov, m->linvT, m->chol};
     for (int i = 0; i < 4; ++i) {
-        void *h = nullptr, *l = nullptr;
+        void *h = nullptr, *l = nullptr, *e = nullptr;
         const size_t bytes = (size_t)m->tc_npad * m->tc_kpad * sizeof(__half);
         CU(cudaMalloc(&h, bytes));
         m->owned.push_back(h);
         CU(cudaMalloc(&l, bytes));
         m->owned.push_back(l);
-        const long long total = m->tc_npad * m->tc_kpad;
-        gemm_tc_split_kernel<<<(unsigned)((total + 255) / 256), 256>>>(src[i], n, n, m->ld, (__half*)h, (__half*)l, m->tc_npad, m->tc_kpad);
+        CU(cudaMalloc(&e, (size_t)m->tc_npad * sizeof(int)));
+        m->owned.push_back(e);
+        gemm_tc_split_kernel<<<(unsigned)m->tc_npad, kGtSplitThreads>>>(src[i], n, n, m->ld, (int*)e, (__half*)h, (__half*)l, m->tc_kpad);
         CU(cudaGetLastError());
         b200_model::TcMat& T = m->tc_mats[i];
-        T.src = src[i]; T.hi = (const __half*)h; T.lo = (const __half*)l;
+        T.src = src[i]; T.hi = (const __half*)h; T.lo = (const __half*)l; T.exp = (const int*)e;
         if (make_tc_map(&T.map_hi, T.hi, m->tc_npad, m->tc_kpad, kGtN) || make_tc_map(&T.map_lo, T.lo, m->tc_npad, m->tc_kpad, kGtN)) return -1;
     }
     CU(cudaDeviceSynchronize());
@@ -1039,14 +1045,17 @@ static int gemm_nt_tc(b200_model* m, cudaStream_t st, const double* Q, long long
     const long long total = rows_pad * m->tc_kpad;
     CU(m->tc_a_hi.reserve((size_t)total * sizeof(__half)));
     CU(m->tc_a_lo.reserve((size_t)total * sizeof(__half)));
+    CU(m->tc_a_exp.reserve((size_t)rows_pad * sizeof(int)));
     __half* a_hi_p = m->tc_a_hi.as<__half>();
     __half* a_lo_p = m->tc_a_lo.as<__half>();
-    gemm_tc_split_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(Q, C, m->n, ldq, a_hi_p, a_lo_p, rows_pad, m->tc_kpad);
+    int* a_exp_p = m->tc_a_exp.as<int>();
+    gemm_tc_split_kernel<<<(unsigned)rows_pad, kGtSplitThreads, 0, st>>>(Q, C, m->n, ldq, a_exp_p, a_hi_p, a_lo_p, m->tc_kpad);
     CU(cudaGetLastError());
     CUtensorMap a_hi, a_lo;
     if (make_tc_map(&a_hi, a_hi_p, rows_pad, m->tc_kpad, kGtM) || make_tc_map(&a_lo, a_lo_p, rows_pad, m->tc_kpad, kGtM)) return -1;
     GemmTcArgs G{};
     G.C = C; G.Nout = Nout; G.n_kblocks = (int)(m->tc_kpad / kGtKB); G.alpha = alpha; G.D = D; G.ldd = ldd;
+    G.ea = a_exp_p; G.eb = T.exp;
     G.n_tiles_m = (int)(rows_pad / kGtM);
     G.n_tiles = G.n_tiles_m * (int)(m->tc_npad / kGtN);
     auto kern = gemm_tc_kernel;
@@ -1066,8 +1075,20 @@ static int prepare_logistic_tc(b200_model* m) {
     m->owned.push_back(h);
     CU(cudaMalloc(&l, (size_t)rows_pad * kTcK * sizeof(__half)));
     m->owned.push_back(l);
+    // power-of-two column exponents of X (its column maxima, then tc_split_exponent)
+    void *colmax = nullptr, *sx = nullptr;
+    CU(cudaMalloc(&colmax, kTcK * sizeof(unsigned long long)));
+    m->owned.push_back(colmax);
+    CU(cudaMalloc(&sx, kTcK * sizeof(int)));
+    m->owned.push_back(sx);
+    CU(cudaMemset(colmax, 0, kTcK * sizeof(unsigned long long)));
+    const unsigned colmax_blocks = (unsigned)std::min<long long>(std::max<long long>(1, (m->n_rows + 1) / 2), 8LL * sm_count(m->device));
+    logistic_tc_colmax_kernel<<<colmax_blocks, 256>>>(m->X, m->n_rows, m->n, m->KP, (unsigned long long*)colmax);
+    tc_exponent_kernel<<<1, kTcK>>>((const unsigned long long*)colmax, kTcK, (int*)sx);
+    m->x_exp = (const int*)sx;
     const long long total = rows_pad * kTcK;
-    logistic_tc_split_kernel<<<(unsigned)((total + 255) / 256), 256>>>(m->X, m->n_rows, m->n, m->KP, (__half*)h, (__half*)l, rows_pad);
+    logistic_tc_split_kernel<<<(unsigned)((total + 255) / 256), 256>>>(m->X, m->n_rows, m->n, m->KP, m->x_exp, (__half*)h, (__half*)l,
+                                                                       rows_pad);
     CU(cudaGetLastError());
     CU(cudaDeviceSynchronize());
     m->Xh = (const __half*)h;
@@ -1147,7 +1168,7 @@ static int batch_eval(b200_model* m, int C, const double* Q, double* G, double* 
         }
         auto kern = logistic_tc_kernel;
         CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kTcSmemBytes));
-        LogisticTcArgs A{m->y32, m->n_rows, m->tc_slabs, Q, ld, C, m->n, bs.gpart.as<double>(), bs.lpart.as<double>(), bs.cpad};
+        LogisticTcArgs A{m->y32, m->n_rows, m->tc_slabs, Q, ld, m->x_exp, C, m->n, bs.gpart.as<double>(), bs.lpart.as<double>(), bs.cpad};
         kern<<<dim3(bs.gx, bs.cpad / kTcChains), kTcThreads, kTcSmemBytes, st>>>(m->map_hi, m->map_lo, A);
         CU(cudaGetLastError());
     } else
@@ -1159,7 +1180,7 @@ static int batch_eval(b200_model* m, int C, const double* Q, double* G, double* 
     if (rc) return rc;
     if (m->precision == B200_PRECISION_TC_FP16X2)  // feature-major partials: the coalesced reduction
         logistic_finish_fm_kernel<<<dim3((C + 31) / 32, (m->KP + 15) / 16), 256, 0, st>>>(Q, ld, G, ld, n, m->KP, C, bs.cpad, bs.gpart.as<double>(),
-                                                                                         bs.lpart.as<double>(), gx, logp);
+                                                                                         bs.lpart.as<double>(), gx, logp, m->x_exp);
     else
         logistic_finish_kernel<<<(C + 3) / 4, 128, 0, st>>>(Q, ld, G, ld, n, m->KP, C, bs.cpad, bs.gpart.as<double>(),
                                                             bs.lpart.as<double>(), gx, logp, 0);

@@ -311,11 +311,12 @@ __global__ void __launch_bounds__(128) logistic_finish_kernel(const double* __re
 // kernel above walks them with lane = feature, i.e. with a stride of Cpad doubles.  Here a CTA owns a 32-chain x 16-feature tile:
 // lane = chain while summing (coalesced, 4 independent partial loads in flight per thread, the same fixed order over p as
 // above, so the same bits), a shared-memory transpose for the row-major gradient, and the blockIdx.y == 0 CTAs also produce
-// logp with the arithmetic of the kernel above.
+// logp with the arithmetic of the kernel above.  The tensor-core kernel contracts X_k 2^sx[k] (logistic_tc.cuh), so feature
+// k's summed partial is multiplied by 2^-sx[k] (exact) before beta is subtracted.
 __global__ void __launch_bounds__(256) logistic_finish_fm_kernel(const double* __restrict__ Q, long long ldq, double* __restrict__ G,
                                                                  long long ldg, int K, int KP, int C, int Cpad,
                                                                  const double* __restrict__ Gpart, const double* __restrict__ lpart,
-                                                                 int nparts, double* __restrict__ logp) {
+                                                                 int nparts, double* __restrict__ logp, const int* __restrict__ sx) {
     __shared__ double tile[16][33];
     const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;  // 8 warps: features 2 w, 2 w + 1 of the tile
     const int c0 = blockIdx.x * 32, k0 = blockIdx.y * 16;
@@ -334,6 +335,7 @@ __global__ void __launch_bounds__(256) logistic_finish_fm_kernel(const double* _
                 a += x0; a += x1; a += x2; a += x3;
             }
             for (; p < nparts; ++p) a += src[(long long)p * step];
+            a = ldexp(a, -sx[k]);
         }
         tile[2 * w + u][lane] = a;
     }

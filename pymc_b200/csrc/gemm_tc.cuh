@@ -5,7 +5,10 @@
 // drained into compensated fp32 register sums (kahan_add).  The fp64 DMMA kernel of dense.cuh stays the parity mode.
 //
 // B (the model's n x n matrices) is split once at b200_model_set_precision; A (the chains' vectors) is split by
-// gemm_tc_split_kernel before every GEMM.  Both are K-major fp16 [rows][Kpad] in HBM, TMA-loaded in 64-wide k-blocks with
+// gemm_tc_split_kernel before every GEMM.  Each row is first scaled by an exact power of two that puts its maximum in
+// [2^14, 2^15) (tc_split_exponent: fp16 keeps 2^-14 .. 65504 only): eb[j] for row j of B, once; ea[c] for row c of A, found
+// by the split kernel itself (one CTA per row: row maximum, then the pieces) before every GEMM.  The epilogue multiplies
+// by 2^-(ea[c] + eb[j]), so the result does not depend on the scale of the data.  Both are K-major fp16 [rows][Kpad] in HBM, TMA-loaded in 64-wide k-blocks with
 // SWIZZLE_128B.  CTA tile = 128 chains x 64 outputs: two consumer warpgroups (64 chains each, sharing
 // the B tile) and a producer warp; tiles are walked output-block-major so that the chain tiles of one output block run together and share B
 // through L2.
@@ -34,11 +37,19 @@ __device__ __forceinline__ void kahan_add(float& s, float& c, float x) {
     s = t;
 }
 
+// 2^e as a double, exactly (a multiply by it is ldexp); a few integer instructions in the normal range instead of ldexp's
+// general path, which matters in an epilogue that runs once per output
+__device__ __forceinline__ double tc_pow2(int e) {
+    return (e >= -1022 && e <= 1023) ? __longlong_as_double((long long)(e + 1023) << 52) : ldexp(1.0, e);
+}
+
 struct GemmTcArgs {
     int C, Nout, n_kblocks;   // chains, outputs, k-blocks of 64 (operands are zero padded to that)
     double alpha;
     double* D;                // [C][ldd]
     long long ldd;
+    const int* ea;            // [C] row exponents of the A pieces (A_c 2^ea[c])
+    const int* eb;            // [Nout] row exponents of the B pieces
     int n_tiles_m, n_tiles;   // chain tiles per output block, total tiles
 };
 
@@ -114,30 +125,60 @@ __global__ void __launch_bounds__(kGtThreads, 1)
 #pragma unroll
                 for (int k = 0; k < 32; ++k) kahan_add(sum[k], comp[k], d[k]);
             }
+            // the row exponents of this thread's 2 chains and 16 outputs, loaded before any store (D may alias them as far as
+            // the compiler knows, which would serialise one load round trip per stored element)
+            int ea[2], eb[16];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) ea[h] = (c0 + r0 + 8 * h < G.C) ? G.ea[c0 + r0 + 8 * h] : 0;
+#pragma unroll
+            for (int j = 0; j < 16; ++j) {
+                const int jj = j0 + 8 * (j >> 1) + col + (j & 1);
+                eb[j] = (jj < G.Nout) ? G.eb[jj] : 0;
+            }
 #pragma unroll
             for (int j = 0; j < 8; ++j) {
 #pragma unroll
                 for (int h = 0; h < 4; ++h) {
                     const int c = c0 + r0 + 8 * (h >> 1), jj = j0 + 8 * j + col + (h & 1);
                     if (c < G.C && jj < G.Nout)
-                        G.D[(long long)c * G.ldd + jj] = G.alpha * ((double)sum[4 * j + h] - (double)comp[4 * j + h]);
+                        G.D[(long long)c * G.ldd + jj] =
+                            G.alpha * (((double)sum[4 * j + h] - (double)comp[4 * j + h]) * tc_pow2(-(ea[h >> 1] + eb[2 * j + (h & 1)])));
                 }
             }
         }
     }
 }
 
-// fp64 [rows][ld] (first `cols` columns) -> fp16 pieces [rows_pad][kpad], zero padded
-__global__ void __launch_bounds__(256) gemm_tc_split_kernel(const double* __restrict__ X, long long rows, long long cols, long long ld,
-                                                            __half* __restrict__ Xh, __half* __restrict__ Xl, long long rows_pad,
-                                                            long long kpad) {
-    const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (e >= rows_pad * kpad) return;
-    const long long r = e / kpad, k = e % kpad;
-    const double v = (r < rows && k < cols) ? X[r * ld + k] : 0.0;
-    const __half hi = __double2half(v);
-    Xh[e] = hi;
-    Xl[e] = __double2half(v - (double)__half2float(hi));
+// fp64 [rows][ld] (first `cols` columns) -> fp16 pieces of row r times 2^e_row[r], [rows_pad][kpad], zero padded, and
+// e_row[r] = tc_split_exponent(max_k |X[r][k]|) (0 for rows .. rows_pad).  One CTA of kGtSplitThreads threads per row: the row
+// maximum first, then the pieces from the same row, now in L1 / L2 (a row of 10^4 doubles is 10 elements per thread).
+constexpr int kGtSplitThreads = 1024;
+__global__ void __launch_bounds__(kGtSplitThreads) gemm_tc_split_kernel(const double* __restrict__ X, long long rows, long long cols,
+                                                                        long long ld, int* __restrict__ e_row, __half* __restrict__ Xh,
+                                                                        __half* __restrict__ Xl, long long kpad) {
+    __shared__ double wmax[kGtSplitThreads / 32];
+    const long long r = blockIdx.x;
+    const double* x = X + r * ld;
+    double m = 0.0;
+    if (r < rows) {
+#pragma unroll 4
+        for (long long k = threadIdx.x; k < cols; k += kGtSplitThreads) m = fmax(m, fabs(x[k]));
+    }
+    for (int o = 16; o > 0; o >>= 1) m = fmax(m, __shfl_xor_sync(B200_FULL_MASK, m, o));
+    if ((threadIdx.x & 31) == 0) wmax[threadIdx.x >> 5] = m;
+    __syncthreads();
+#pragma unroll
+    for (int w = 0; w < kGtSplitThreads / 32; ++w) m = fmax(m, wmax[w]);
+    const int es = tc_split_exponent(m);
+    if (threadIdx.x == 0) e_row[r] = es;
+    const double sc = ldexp(1.0, es);  // exact scaling: every scaled entry is <= 2^15
+#pragma unroll 4
+    for (long long k = threadIdx.x; k < kpad; k += kGtSplitThreads) {
+        const double v = (r < rows && k < cols) ? x[k] * sc : 0.0;
+        const __half hi = __double2half(v);
+        Xh[r * kpad + k] = hi;
+        Xl[r * kpad + k] = __double2half(v - (double)__half2float(hi));
+    }
 }
 
 }  // namespace b200

@@ -3,8 +3,13 @@
 // memory by TMA) instead of the fp64 DMMA path of dense.cuh.
 //
 // wgmma has no fp64 kind, so every fp64 operand is split into two fp16 pieces, v = hi + lo with hi = fp16(v) and
-// lo = fp16(v - hi) (22 significant bits; absolute floor 2^-25 where lo is subnormal), and a product is evaluated as
-// hi*hi + hi*lo + lo*hi in three f16 MMAs with fp32 accumulation (the lo*lo term is below 2^-22 relative).
+// lo = fp16(v - hi) (22 significant bits), and a product is evaluated as hi*hi + hi*lo + lo*hi in three f16 MMAs with fp32
+// accumulation (the lo*lo term is below 2^-22 relative).  fp16 holds magnitudes 2^-14 .. 65504 only, so every operand is
+// first scaled by an exact power of two: X column k by 2^sx[k] (once, at b200_model_set_precision), beta by 2^-sx[k] (which
+// keeps eta) and then by 2^tau[c] per chain, each chosen so that the column / row maximum lies in [2^14, 2^15)
+// (tc_split_exponent).  eta is unscaled by 2^-tau[c] in fp32 before the sigmoid, and the finish kernel
+// (logistic_finish_fm_kernel) multiplies feature k's gradient by 2^-sx[k].  The accuracy is then independent of the data's
+// scale: an entry keeps 22 bits down to 2^-14 of its row / column maximum, and an absolute floor of 2^-39 of it below that.
 // fp32 accumulators only ever cover a bounded number of terms: X beta sums K = 128 terms, and the gradient accumulator is
 // drained into fp64 registers every kTcDrain slabs, so fp32 rounding does not build up over the rows of X.  The small
 // correction products (hi*lo, lo*hi) are issued first, while the accumulator is still small, and hi*hi last.
@@ -113,12 +118,22 @@ __device__ __forceinline__ float tc_ex2(float x) { float r; asm("ex2.approx.ftz.
 __device__ __forceinline__ float tc_rcp(float x) { float r; asm("rcp.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x)); return r; }
 __device__ __forceinline__ float tc_lg2(float x) { float r; asm("lg2.approx.ftz.f32 %0, %1;" : "=f"(r) : "f"(x)); return r; }
 
+// The power-of-two exponent e that puts a row's (column's) largest magnitude m in [2^14, 2^15): every fp16 hi piece of
+// v 2^e is finite and normal down to 2^-14 of m.  0 for an all-zero row; inf / NaN pass through unscaled.
+__host__ __device__ __forceinline__ int tc_split_exponent(double m) {
+    if (!(m > 0.0) || !(m < INFINITY)) return 0;
+    int E;
+    frexp(m, &E);  // m in [2^(E-1), 2^E)
+    return 15 - E;
+}
+
 struct LogisticTcArgs {
     const float* y32;        // [n_slabs * 128] labels as fp32, zero padded
     long long N;             // true rows
     long long n_slabs;       // ceil(N / 128); X pieces are allocated with n_slabs * 128 rows (zero padded)
     const double* Q;         // [C][ldq] beta per chain
     long long ldq;
+    const int* sx;           // [128] column exponents of the X pieces (X_k 2^sx[k])
     int C, K;
     double* Gpart;           // [gridDim.x][128 features][Cpad]  (feature-major)
     double* lpart;           // [gridDim.x][Cpad]
@@ -154,6 +169,7 @@ __global__ void __launch_bounds__(kTcThreads, 1)
     uint64_t* x_full = bars;          // [2] TMA -> consumers
     uint64_t* x_empty = bars + 2;     // [2] consumers (GEMM 2 done) -> TMA
     __shared__ double lp_wg_s[2][kTcChains];
+    __shared__ float unscale_s[kTcChains];  // 2^-tau of each chain: eta = GEMM 1 accumulator * 2^-tau
 
     const int tid = threadIdx.x;
     const int c_base = blockIdx.y * kTcChains;
@@ -166,15 +182,45 @@ __global__ void __launch_bounds__(kTcThreads, 1)
             mbar_init(&x_empty[i], kTcConsumers);
         }
     }
-    // beta pieces: fp64 -> fp16 hi / lo, written in the K-major SWIZZLE_128B image GEMM 1 reads as operand A
-    for (int e = tid; e < kTcChains * kTcK; e += kTcThreads) {
-        const int c = e >> 7, k = e & 127;
-        const double v = (c_base + c < A.C && k < A.K) ? A.Q[(long long)(c_base + c) * A.ldq + k] : 0.0;
-        const __half hi = __double2half(v);
-        const __half lo = __double2half(v - (double)__half2float(hi));
-        const uint32_t off = tc_tile_off(c, k, kTcABlockBytes);
-        *reinterpret_cast<__half*>(beta_s + off) = hi;
-        *reinterpret_cast<__half*>(beta_s + kTcAPieceBytes + off) = lo;
+    // beta pieces.  Warp w stages chains w, w + 9, ... (lane: features lane + 32 j), four chains' loads in flight at a time:
+    // beta_k 2^-sx[k] keeps eta = sum_k beta_k X_k, its per-chain maximum sets tau, and the fp16 hi / lo pieces of
+    // beta_k 2^(tau - sx[k]) are written in the K-major SWIZZLE_128B image GEMM 1 reads as operand A
+    constexpr int kWarps = kTcThreads / 32, kPer = 4;
+    for (int c0 = tid >> 5; c0 < kTcChains; c0 += kPer * kWarps) {
+        const int lane = tid & 31;
+        double xs[4];  // 2^-sx[k] of this lane's features
+#pragma unroll
+        for (int j = 0; j < 4; ++j) xs[j] = ldexp(1.0, -A.sx[lane + 32 * j]);
+        double v[kPer][4];
+#pragma unroll
+        for (int i = 0; i < kPer; ++i) {
+            const int c = c0 + kWarps * i;
+#pragma unroll
+            for (int j = 0; j < 4; ++j) {
+                const int k = lane + 32 * j;
+                v[i][j] = (c < kTcChains && c_base + c < A.C && k < A.K) ? A.Q[(long long)(c_base + c) * A.ldq + k] * xs[j] : 0.0;
+            }
+        }
+#pragma unroll
+        for (int i = 0; i < kPer; ++i) {
+            const int c = c0 + kWarps * i;
+            double mx = fmax(fmax(fabs(v[i][0]), fabs(v[i][1])), fmax(fabs(v[i][2]), fabs(v[i][3])));
+            for (int o = 16; o > 0; o >>= 1) mx = fmax(mx, __shfl_xor_sync(B200_FULL_MASK, mx, o));
+            const int tau = tc_split_exponent(mx);
+            if (c < kTcChains) {
+                if (lane == 0) unscale_s[c] = ldexpf(1.0f, -tau);
+                const double sc = ldexp(1.0, tau);
+#pragma unroll
+                for (int j = 0; j < 4; ++j) {
+                    const double x = v[i][j] * sc;
+                    const __half hi = __double2half(x);
+                    const __half lo = __double2half(x - (double)__half2float(hi));
+                    const uint32_t off = tc_tile_off(c, lane + 32 * j, kTcABlockBytes);
+                    *reinterpret_cast<__half*>(beta_s + off) = hi;
+                    *reinterpret_cast<__half*>(beta_s + kTcAPieceBytes + off) = lo;
+                }
+            }
+        }
     }
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");  // generic-proxy writes of beta -> visible to wgmma
     __syncthreads();
@@ -237,7 +283,7 @@ __global__ void __launch_bounds__(kTcThreads, 1)
 #pragma unroll
                     for (int u = 0; u < 2; ++u) {
                         const int i = 8 * j + col + u;
-                        const float x = eta[4 * j + 2 * hh + u];
+                        const float x = eta[4 * j + 2 * hh + u] * unscale_s[r0 + 8 * hh];  // shared: no register held over the loop
                         const float yv = ys[i];
                         const float tt = tc_ex2(-1.4426950408889634f * fabsf(x));   // e^-|x|
                         const float w = 1.f + tt;
@@ -315,14 +361,32 @@ __global__ void __launch_bounds__(256) logistic_tc_y_kernel(const uint8_t* __res
     if (e < rows_pad) y32[e] = (e < N) ? (float)y[e] : 0.f;
 }
 
-// fp64 design matrix [N][K] (row stride ldx) -> fp16 pieces [n_slabs * 128][128], zero padded
+// colmax[k] = max_i |X[i][k]| over the N rows and K columns of the fp64 design matrix (row stride ldx), 0 for k >= K;
+// colmax[128] zeroed by the caller.  The bit patterns of non-negative doubles order like their values: the result does not
+// depend on the order of the atomics.
+__global__ void __launch_bounds__(256) logistic_tc_colmax_kernel(const double* __restrict__ X, long long N, int K, long long ldx,
+                                                                 unsigned long long* __restrict__ colmax) {
+    const int k = threadIdx.x & 127;
+    double m = 0.0;
+    if (k < K)
+        for (long long r = 2LL * blockIdx.x + (threadIdx.x >> 7); r < N; r += 2LL * gridDim.x) m = fmax(m, fabs(X[r * ldx + k]));
+    atomicMax(colmax + k, (unsigned long long)__double_as_longlong(m));
+}
+
+__global__ void tc_exponent_kernel(const unsigned long long* __restrict__ mx, int n, int* __restrict__ e) {
+    const int i = blockIdx.x * blockDim.x + threadIdx.x;
+    if (i < n) e[i] = tc_split_exponent(__longlong_as_double((long long)mx[i]));
+}
+
+// fp64 design matrix [N][K] (row stride ldx) -> fp16 pieces of X_k 2^sx[k], [n_slabs * 128][128], zero padded
 __global__ void __launch_bounds__(256) logistic_tc_split_kernel(const double* __restrict__ X, long long N, int K, long long ldx,
-                                                                __half* __restrict__ Xh, __half* __restrict__ Xl, long long rows_pad) {
+                                                                const int* __restrict__ sx, __half* __restrict__ Xh,
+                                                                __half* __restrict__ Xl, long long rows_pad) {
     const long long e = (long long)blockIdx.x * blockDim.x + threadIdx.x;
     if (e >= rows_pad * kTcK) return;
     const long long r = e >> 7;
     const int k = (int)(e & 127);
-    const double v = (r < N && k < K) ? X[r * ldx + k] : 0.0;
+    const double v = (r < N && k < K) ? ldexp(X[r * ldx + k], sx[k]) : 0.0;
     const __half hi = __double2half(v);
     Xh[e] = hi;
     Xl[e] = __double2half(v - (double)__half2float(hi));

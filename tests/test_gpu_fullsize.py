@@ -6,8 +6,9 @@ verbatim reference (oracle/make_golden.py fullsize):
 
   * logistic_fused_kernel<16> (K = 128): 8192 x 128 with 130 chains (two chain-CTAs, row-CTA split), the 3-draw
     fixed-step golden, and points on the real 1e6 x 128 design matrix of BASELINE config #3;
-  * gemm_nt_dmma_kernel<8,17|9|5,3>, <4,*>, <2,*> and ls_advance_kernel<16> at n = 10^4 (config #5): logp/grad at
-    C in {256, 64, 32} and the 3-draw dense-mass golden;
+  * gemm_nt_dmma_kernel at n = 10^4 (config #5) and ls_advance_kernel<16>: logp/grad at C in {256, 64, 32} and the 3-draw
+    dense-mass golden.  On an H100 (132 SMs) the tile rule picks NB = 5 for all of these (<8,5>, <4,5>, <2,5>); the other
+    instantiations are reached at the shapes of tests/test_gpu_contractions.py;
   * the sharding drift of the fused logistic pass (row-CTA count depends on the chains per launch) is bounded;
   * the bench path of config #2 (device Philox momentum, cold jitter+adapt_diag) against posterior moments of an
     independent oracle CPU run (tests/golden/radon_posterior_oracle.npz), within 4 MCSE.
@@ -115,7 +116,8 @@ def test_logistic_sharding_drift_is_bounded(logistic_full):
 
 @pytest.mark.parametrize("C", [256, 64, 32])
 def test_mvgauss_full_logp_grad(mvgauss_full, C):
-    """C = 256 -> gemm_nt_dmma_kernel<8,17,3>, 64 -> <4,*>, 32 -> <2,*> (tile counts chosen to fill whole waves of the SMs)."""
+    """C = 256 -> gemm_nt_dmma_kernel<8,NB,3>, 64 -> <4,NB>, 32 -> <2,NB>, NB chosen to fill whole waves of the SMs: 5 for
+    all three on an H100 (132 SMs); a 148-SM part runs <8,17>, <4,9> and <2,9> here."""
     cm = mvgauss_full
     rng = np.random.default_rng(C)
     L = cm.spec.data["L"]

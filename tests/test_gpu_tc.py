@@ -186,5 +186,6 @@ def test_tc_gemm_full_size_error_and_speed():
     _report("tc_fp16x2/mvgauss_n10000_256chains", {
         "grad_rel_to_max_vs_fp64": eg, "logp_rel_vs_fp64": el, "fp64_dmma_ms": ms64, "tc_ms_incl_operand_split": mstc,
         "speedup": ms64 / mstc, "fp64_equivalent_tflops_tc": flops / (mstc * 1e-3) / 1e12})
-    # 10^4-term contractions: 1.2e-6 of the largest gradient entry measured on an H100 (n = 300 / 1000: 5e-7); stated, not hidden
+    # 10^4-term contractions: 8.1e-7 of the largest gradient entry measured on an H100 with the operands scaled per row
+    # (1.2e-6 without; n = 300: 3.4e-7); stated, not hidden
     assert eg <= 2e-6 and el <= 1e-6, (eg, el)

@@ -120,12 +120,18 @@ typedef struct b200_ir_term {
     int32_t n_factors, n_cols;
     b200_ir_factor f[3];
 } b200_ir_term;
+/* y_var selects what the factor observes:
+ *   0      y[N] is observed data (every zero-initialised table);
+ *   v + 1  a LATENT factor: the values are the constrained values of variable v (N == its size; y may be NULL).  This is a
+ *          Normal or StudentT prior on variable v whose location is the linear predictor of the terms, e.g. centred group
+ *          effects a_j ~ Normal(g0 + g1 u_j + r[region_j], sigma); sigma as above (CONST, REF or OBS: one per element).
+ *          The y checks are skipped; b200_pointwise_loglik refuses its index, since it is not a likelihood. */
 typedef struct b200_ir_lik {
     int32_t dist, n_terms;
     int64_t N;
-    const double* y; /* [N] */
+    const double* y; /* [N]; NULL allowed when y_var > 0 */
     const b200_ir_term* terms;
-    int32_t sigma_kind, reserved;
+    int32_t sigma_kind, y_var;
     b200_ir_param sigma;
     const double* sigma_obs; /* [N] when sigma_kind == B200_IR_S_OBS (Binomial: trials per observation) */
     double nu;

@@ -69,7 +69,7 @@ class IrTerm(C.Structure):
 
 class IrLik(C.Structure):
     _fields_ = [("dist", C.c_int32), ("n_terms", C.c_int32), ("N", C.c_int64), ("y", C.c_void_p), ("terms", C.c_void_p),
-                ("sigma_kind", C.c_int32), ("reserved", C.c_int32), ("sigma", IrParam), ("sigma_obs", C.c_void_p),
+                ("sigma_kind", C.c_int32), ("y_var", C.c_int32), ("sigma", IrParam), ("sigma_obs", C.c_void_p),
                 ("nu", C.c_double)]
 
 
@@ -118,7 +118,7 @@ def build_ir(low):
         keep.append(terms)
         liks[k].dist, liks[k].n_terms, liks[k].N = int(L["dist"]), len(L["terms"]), int(L["N"])
         liks[k].y, liks[k].terms = addr(L["y"]), C.addressof(terms)
-        liks[k].sigma_kind = int(L["sigma_kind"])
+        liks[k].sigma_kind, liks[k].y_var = int(L["sigma_kind"]), int(L.get("y_var", 0))  # y_var > 0: latent, y is None
         liks[k].sigma = IrParam(1 if L["sigma_kind"] == 2 else 0, int(L["sigma_ref"]), float(L["sigma_value"]))
         liks[k].sigma_obs, liks[k].nu = addr(L["sigma_obs"]), float(L["nu"])
     ars = (IrAr1 * max(1, len(low.ar1)))()

@@ -411,13 +411,21 @@ static int prepare_ir(b200_model* m, const b200_model_desc* d) {
     bool has_design = false;
     for (int l = 0; l < R->n_liks; ++l) {
         const b200_ir_lik& L = R->liks[l];
-        if (L.N <= 0 || L.N > 0x7fffffff || !L.y) return fail("ir: likelihood %d: missing observations", l);
+        // y_var = v + 1: a latent factor, a Normal / StudentT prior on variable v with a linear-predictor location
+        if (L.y_var < 0 || L.y_var > R->n_vars) return fail("ir: likelihood %d: y_var %d outside [0, n_vars = %d]", l, L.y_var, R->n_vars);
+        const bool latent = L.y_var > 0;
+        if (latent && L.dist != B200_IR_L_NORMAL && L.dist != B200_IR_L_STUDENTT)
+            return fail("ir: likelihood %d: a latent factor (y_var > 0) is a normal or studentt prior with a Linear location; dist %d is neither", l, L.dist);
+        if (latent && L.N != vars[L.y_var - 1].size)
+            return fail("ir: likelihood %d: a latent factor's N (%lld) must equal the size of its variable (%d)", l, (long long)L.N, vars[L.y_var - 1].size);
+        if (L.N <= 0 || L.N > 0x7fffffff || (!latent && !L.y)) return fail("ir: likelihood %d: missing observations", l);
         if (L.n_terms <= 0 || !L.terms) return fail("ir: likelihood %d: no linear-predictor terms", l);
         const long long N = L.N;
         max_obs = std::max(max_obs, N);
         IrLikD D{};
         D.dist = L.dist; D.n_terms = L.n_terms; D.term0 = (int)terms.size(); D.sigma_kind = L.sigma_kind; D.N = N; D.nu = L.nu;
-        if (upload_raw(m, L.y, (size_t)N, &D.y)) return -1;
+        D.yoff = latent ? vars[L.y_var - 1].offset : -1;
+        if (!latent && upload_raw(m, L.y, (size_t)N, &D.y)) return -1;
         if (ir_param(L.sigma, n, &D.sigma, "likelihood sigma")) return -1;
         if (L.sigma_kind == B200_IR_S_REF && L.sigma.kind != 1) return fail("ir: likelihood %d: sigma_kind REF needs a reference", l);
         b200_ir_param slot = L.sigma;  // the parameter slot as the device reads it: x[ref] for REF, else the value
@@ -1559,6 +1567,7 @@ extern "C" int b200_pointwise_loglik(b200_model* m, int32_t lik, const double* d
     // the IR tables live on the device: read the number of observations of this factor back
     IrLikD L;
     CU(cudaMemcpy(&L, m->ir.liks + lik, sizeof L, cudaMemcpyDeviceToHost));
+    if (L.yoff >= 0) return fail("b200_pointwise_loglik: factor %d is a latent factor (a prior with a Linear location), not a likelihood", lik);
     const double* d_draws = nullptr;
     double* d_out = nullptr;
     Staging sg(m, mem, st);

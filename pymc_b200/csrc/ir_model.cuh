@@ -87,8 +87,10 @@ __device__ __forceinline__ void ir_design_grad(const IrTermD& Tm, const double* 
 // c0: sum of the constant parts over i.  Random dispersion (sigma_kind REF): Gamma keeps sum_i log y_i in sum_log_y;
 // NegativeBinomial keeps the distinct nonzero y values u[k] with their counts cnt[k] (n_tab of them), over which the
 // alpha-dependent normalising terms sum_i lgamma(y_i + a) - lgamma(a) and their digamma gradient are evaluated.
+// yoff >= 0: a latent factor (a Normal / StudentT prior whose location is a linear predictor): y_i = x[yoff + i], the
+// constrained values of a variable of size N, which also receives d logp / d y_i = -r_i; y is null.  -1: y is data.
 struct IrLikD { int dist, n_terms, term0, sigma_kind; long long N; const double* y; const double* sigma_obs; IrParamD sigma;
-                double nu, c0, sum_log_y; const double* tab_u; const double* tab_cnt; int n_tab, pad; };
+                double nu, c0, sum_log_y; const double* tab_u; const double* tab_cnt; int n_tab, yoff; };
 struct IrAr1D { int offset, size; IrParamD phi, sigma; double init_sigma; };
 
 struct IrModel {
@@ -229,7 +231,7 @@ struct IrModel {
                     }
                     eta += pr;
                 }
-                const double yi = L.y[i];
+                const double yi = L.yoff >= 0 ? x[L.yoff + i] : L.y[i];
                 double ri = 0.0;
                 switch (L.dist) {
                     case IRL_NORMAL: {  // continuous.py:526-527
@@ -288,6 +290,7 @@ struct IrModel {
                     default: break;
                 }
                 r[i] = ri;
+                if (L.yoff >= 0) g_s[L.yoff + i] -= ri;  // this thread owns element i of the latent variable
             }
             if (disp && L.sigma_kind == IRS_REF) {  // uniform branch: the alpha-dependent normalising terms
                 const double a = sg_s;

@@ -6,7 +6,8 @@ The reference hands a model to the sampler as one compiled callable over the rav
 each RV's owner node (the representation ``fgraph_from_model`` freezes into ``ModelFreeRV`` / ``ModelObservedRV`` nodes,
 pymc/model/fgraph.py:76-81, :139) -- and pattern-matches them onto the closed factor set of the IR:
 
-    free RV      ->  ir.Var (transform from rvs_to_transforms) + ir.Prior (parameters: constants or scalar free RVs),
+    free RV      ->  ir.Var (transform from rvs_to_transforms) + ir.Prior (parameters: constants or scalar free RVs;
+                     a Normal / StudentT location may be any linear predictor -> ir.Linear, its sigma a constant vector),
                      AR(1) / GaussianRandomWalk -> ir.AR1
     observed RV  ->  ir.Likelihood; its location parameter is parsed into linear-predictor terms
                      (Add / Sub / Neg / Mul / division by a constant / indexing by constant integer arrays / Dot with a
@@ -47,6 +48,11 @@ def _op_name(rv) -> str:
         if name.endswith(suffix):
             name = name[: -len(suffix)]
     return name
+
+
+def _is_copy(node) -> bool:
+    """A copy op of one input (what ``pm.Deterministic`` wraps its expression in, under some PyTensor versions)."""
+    return type(node.op).__name__ in ("Identity", "Copy", "DeepCopyOp", "ViewOp") and len(node.inputs) == 1
 
 
 def _dist_params(rv):
@@ -132,43 +138,7 @@ def from_pymc(model) -> _ir.ModelIR:
             raise NotImplementedError(f"{what}: parameter is neither a constant scalar nor a scalar free RV")
         return float(v.reshape(()))
 
-    priors, ar1 = [], []
-    for rv in free:
-        op = _op_name(rv)
-        ps = _dist_params(rv)
-        vn = name_of[rv]
-        if op in ("autoregressive", "ar"):
-            rhos, sigma = ps[0], ps[1]
-            if int(getattr(rv.owner.op, "ar_order", 1)) != 1 or getattr(rv.owner.op, "constant_term", False):
-                raise NotImplementedError(f"{rv.name}: only AR(1) without a constant term is in the closed set")
-            init = ps[2]
-            if _op_name(init) != "normal":
-                raise NotImplementedError(f"{rv.name}: AR init_dist must be Normal(0, s)")
-            ipar = _dist_params(init)
-            if float(_const_value(ipar[0])) != 0.0:
-                raise NotImplementedError(f"{rv.name}: AR init_dist must be centred at 0")
-            rho = rhos.owner.inputs[0] if (rhos.owner is not None and not isinstance(rhos.owner.op, type(None)) and rhos not in name_of
-                                           and _const_value(rhos) is None and len(rhos.owner.inputs) == 1) else rhos
-            ar1.append(_ir.AR1(vn, param(rho, rv.name + ".rho"), param(sigma, rv.name + ".sigma"), float(_const_value(ipar[1]))))
-            continue
-        if op in ("gaussianrandomwalk", "randomwalk"):
-            raise NotImplementedError(f"{rv.name}: write the random walk as pm.AR(rho=[1.0], ...) for this front-end")
-        if op not in _PRIOR_BY_OP:
-            raise NotImplementedError(f"{rv.name}: distribution {type(rv.owner.op).__name__} is outside the closed set "
-                                      f"{sorted(_ir.PRIOR_DISTS)}")
-        dist, idx = _PRIOR_BY_OP[op]
-        args = [param(ps[i], f"{rv.name}.param{i}") for i in idx]
-        if op in ("halfnormal", "halfcauchy") and float(_const_value(ps[0])) != 0.0:
-            raise NotImplementedError(f"{rv.name}: {op} with a non-zero location")
-        if op == "exponential":  # PyTensor parametrises by scale = 1 / lam
-            if isinstance(args[0], _ir.Ref):
-                raise NotImplementedError(f"{rv.name}: Exponential with a random rate")
-            args[0] = 1.0 / args[0]
-        if op == "gamma":
-            args[1] = 1.0 / args[1]
-        priors.append(_ir.Prior(dist, vn, tuple(args)))
-
-    # ---- observed RVs: likelihoods with a linear predictor ------------------------------------------------------------
+    # ---- linear predictors: likelihood locations, Linear prior locations, Deterministics ------------------------------
     def scalar_op_name(node):
         return type(node.op.scalar_op).__name__.lower() if isinstance(node.op, Elemwise) else ""
 
@@ -183,6 +153,8 @@ def from_pymc(model) -> _ir.ModelIR:
         node = x.owner
         if node is None:
             raise NotImplementedError(f"linear predictor: free input {x} is not a model variable")
+        if _is_copy(node) or scalar_op_name(node) == "identity":  # e.g. the named copy pm.Deterministic makes
+            return terms_of(node.inputs[0], N)
         if isinstance(node.op, DimShuffle):
             return terms_of(node.inputs[0], N)
         if isinstance(node.op, (AdvancedSubtensor1, AdvancedSubtensor, Subtensor)):
@@ -236,6 +208,59 @@ def from_pymc(model) -> _ir.ModelIR:
             out.append(_ir.Term(list(f), coef))
         return out
 
+    priors, ar1 = [], []
+    for rv in free:
+        op = _op_name(rv)
+        ps = _dist_params(rv)
+        vn = name_of[rv]
+        if op in ("autoregressive", "ar"):
+            rhos, sigma = ps[0], ps[1]
+            if int(getattr(rv.owner.op, "ar_order", 1)) != 1 or getattr(rv.owner.op, "constant_term", False):
+                raise NotImplementedError(f"{rv.name}: only AR(1) without a constant term is in the closed set")
+            init = ps[2]
+            if _op_name(init) != "normal":
+                raise NotImplementedError(f"{rv.name}: AR init_dist must be Normal(0, s)")
+            ipar = _dist_params(init)
+            if float(_const_value(ipar[0])) != 0.0:
+                raise NotImplementedError(f"{rv.name}: AR init_dist must be centred at 0")
+            rho = rhos.owner.inputs[0] if (rhos.owner is not None and not isinstance(rhos.owner.op, type(None)) and rhos not in name_of
+                                           and _const_value(rhos) is None and len(rhos.owner.inputs) == 1) else rhos
+            ar1.append(_ir.AR1(vn, param(rho, rv.name + ".rho"), param(sigma, rv.name + ".sigma"), float(_const_value(ipar[1]))))
+            continue
+        if op in ("gaussianrandomwalk", "randomwalk"):
+            raise NotImplementedError(f"{rv.name}: write the random walk as pm.AR(rho=[1.0], ...) for this front-end")
+        if op not in _PRIOR_BY_OP:
+            raise NotImplementedError(f"{rv.name}: distribution {type(rv.owner.op).__name__} is outside the closed set "
+                                      f"{sorted(_ir.PRIOR_DISTS)}")
+        dist, idx = _PRIOR_BY_OP[op]
+        loc, scale = _ir.LINEAR_PRIORS.get(dist, (None, None))
+
+        def prior_arg(i):
+            what = f"{rv.name}.param{i}"
+            if i == loc:
+                try:  # a constant or a scalar free RV; anything else is a linear predictor of the RV's size
+                    return param(ps[i], what)
+                except NotImplementedError:
+                    return _ir.Linear(make_terms(ps[i], size_of[vn]))
+            c = _const_value(ps[i]) if i == scale else None
+            if c is not None and c.size > 1:  # one constant scale per element
+                return np.ravel(np.broadcast_to(c, np.shape(ip[by_rv[rv].name]))).astype(np.float64)
+            return param(ps[i], what)
+
+        args = [prior_arg(i) for i in idx]
+        if op in ("halfnormal", "halfcauchy"):
+            c = _const_value(ps[0])
+            if c is None or np.any(c != 0.0):
+                raise NotImplementedError(f"{rv.name}: {op} with a non-zero location")
+        if op == "exponential":  # PyTensor parametrises by scale = 1 / lam
+            if isinstance(args[0], _ir.Ref):
+                raise NotImplementedError(f"{rv.name}: Exponential with a random rate")
+            args[0] = 1.0 / args[0]
+        if op == "gamma":
+            args[1] = 1.0 / args[1]
+        priors.append(_ir.Prior(dist, vn, tuple(args)))
+
+    # ---- observed RVs: likelihoods with a linear predictor ------------------------------------------------------------
     def strip(x, want):
         """peel one Elemwise layer named `want` (sigmoid / exp) off x, or return None"""
         if x.owner is not None and scalar_op_name(x.owner) == want:
@@ -362,8 +387,7 @@ def from_pymc(model) -> _ir.ModelIR:
         if size is None:
             raise NotImplementedError(f"{dv.name}: the size of this Deterministic is not known statically")
         expr = dv
-        if expr.owner is not None and type(expr.owner.op).__name__ in ("Identity", "Copy", "DeepCopyOp", "ViewOp") and \
-                len(expr.owner.inputs) == 1:
+        if expr.owner is not None and _is_copy(expr.owner):
             expr = expr.owner.inputs[0]  # pm.Deterministic wraps its expression in a named copy
         terms = []
         for c, f in terms_of(expr, size):

@@ -6,7 +6,8 @@ their Jacobians pymc/logprob/transforms.py:880-891, :1026-1073).  The IR keeps e
 
     value variables   ordered, each with a size and a transform (None | "log" | "interval"(lo, hi))
     factors           a closed set, each contributing logp(x) where x are the CONSTRAINED values
-        Prior         elementwise density of one variable; parameters are constants or scalar variables (hierarchies)
+        Prior         elementwise density of one variable; parameters are constants or scalar variables (hierarchies);
+                      a Normal / StudentT location may be a Linear predictor (group-level predictors, nested groups)
         Likelihood    observed y_i with a linear predictor  eta_i = sum_t coef_t[i] * prod_f x_f[idx_f[i]]
                       (affine / indexed / bilinear links: intercepts, slopes x data, group effects, scale * offset ...)
         AR1           h_0 ~ Normal(0, init_sigma), h_t - phi h_{t-1} ~ Normal(0, sigma)   (phi = 1: Gaussian random walk)
@@ -62,6 +63,9 @@ POSITIVE_SUPPORT = "a scalar variable with positive support (a log transform, or
 NEGBIN_POISSON_ALPHA = 1e10  # above: the NegativeBinomial density is its Poisson(mu) limit (discrete.py:727-735)
 SIGMA_NONE, SIGMA_CONST, SIGMA_REF, SIGMA_OBS = 0, 1, 2, 3
 MAX_TERM_FACTORS = 3
+# priors whose location may be a Linear predictor: name -> (location slot, scale slot).  Such a prior is lowered to a
+# latent factor (see ``lower``), which also takes one constant scale per element.
+LINEAR_PRIORS = {"normal": (0, 1), "studentt": (1, 2)}
 
 
 def _positive_support(v) -> bool:
@@ -71,6 +75,14 @@ def _positive_support(v) -> bool:
 def is_design(t) -> bool:
     """A design term: its coef is a 2-D X [N][K] (see ``Term``)."""
     return t.coef is not None and np.ndim(t.coef) == 2
+
+
+def is_latent(p) -> bool:
+    """A Normal / StudentT prior with a Linear location or one scale per element: ``lower`` makes it a latent factor."""
+    if p.dist not in LINEAR_PRIORS or len(p.params) != PRIOR_DISTS[p.dist][1]:
+        return False
+    loc, scale = LINEAR_PRIORS[p.dist]
+    return isinstance(p.params[loc], Linear) or (not isinstance(p.params[scale], Ref) and np.ndim(p.params[scale]) == 1)
 
 
 @dataclass(frozen=True)
@@ -107,6 +119,16 @@ class Term:
 
     factors: list  # [(var_name, idx or None), ...]
     coef: np.ndarray | float | None = None
+
+
+@dataclass
+class Linear:
+    """The location of a Normal / StudentT prior as a linear predictor of the CONSTRAINED variables, in the closed form of a
+    likelihood's location: mu_j = sum_t coef_t[j] * prod_f x_f[idx_f[j]] with j over the elements of the prior's variable
+    (``Term``s, design terms included).  ``a ~ Normal(g0 + g1 * u + r[region], sigma_a)`` is
+    ``Prior("normal", "a", (Linear([Term([("g0", None)]), Term([("g1", None)], coef=u), Term([("r", region)])]), Ref(...)))``."""
+
+    terms: list
 
 
 @dataclass
@@ -192,33 +214,34 @@ class ModelIR:
             if len(p.params) != PRIOR_DISTS[p.dist][1]:
                 raise ValueError(f"prior {p.dist} on {p.var}: expected {PRIOR_DISTS[p.dist][1]} parameters")
             v = self.var(p.var)
+            loc, scale = LINEAR_PRIORS.get(p.dist, (None, None))
             for k, a in enumerate(p.params):
+                what = f"prior {p.dist} on {v.name}"
+                if isinstance(a, Linear):
+                    if k != loc:
+                        raise ValueError(f"{what}: parameter {k} cannot be a Linear predictor (only the location of a "
+                                         f"normal or studentt prior can)")
+                    self._check_terms(a.terms, v.size, f"{what}: location", "its variable's size")
+                    continue
                 if isinstance(a, Ref):
                     if self.var(a.var).size != 1:
                         raise ValueError(f"prior on {p.var}: parameter {a.var} must be a scalar variable")
                     if p.dist in ("uniform", "gamma", "beta") or (p.dist == "studentt" and k == 0):
                         raise ValueError(f"prior {p.dist} on {p.var}: parameter {k} must be a constant")
+                if k == scale and not isinstance(a, Ref) and np.ndim(a) == 1:  # one scale per element
+                    s = np.asarray(a, dtype=np.float64)
+                    if len(s) != v.size or not (np.all(np.isfinite(s)) and np.all(s > 0)):
+                        raise ValueError(f"{what}: sigma per element must be a finite constant > 0 for each of the "
+                                         f"{v.size} elements")
+                    continue
                 if k in SCALE_PARAMS.get(p.dist, {}):
-                    self._check_scale(a, f"prior {p.dist} on {v.name}: {SCALE_PARAMS[p.dist][k]}")
+                    self._check_scale(a, f"{what}: {SCALE_PARAMS[p.dist][k]}")
             self._check_prior_support(p, v)
         for L in self.likelihoods:
             if L.dist not in LIK_DISTS:
                 raise ValueError(f"likelihood {L.dist!r} is not in the closed set {sorted(LIK_DISTS)}")
             N = len(L.y)
-            for t in L.terms:
-                if is_design(t):
-                    self._check_design(t, N, f"likelihood {L.name}")
-                    continue
-                if len(t.factors) > MAX_TERM_FACTORS:  # no factor: a constant offset coef[i]
-                    raise ValueError(f"a term has at most {MAX_TERM_FACTORS} variable factors")
-                for vn, idx in t.factors:
-                    v = self.var(vn)
-                    if idx is None and v.size not in (1, N):
-                        raise ValueError(f"{vn} (size {v.size}) needs an index array to enter a likelihood of length {N}")
-                    if idx is not None and (len(idx) != N or np.min(idx) < 0 or np.max(idx) >= v.size):
-                        raise ValueError(f"index of {vn} out of range")
-                if t.coef is not None and np.ndim(t.coef) == 1 and len(t.coef) != N:
-                    raise ValueError("coef length differs from the number of observations")
+            self._check_terms(L.terms, N, f"likelihood {L.name}", "the number of observations")
             if L.dist in ("normal", "studentt") and L.sigma is None:
                 raise ValueError(f"{L.dist} likelihood needs sigma")
             if isinstance(L.sigma, Ref) and self.var(L.sigma.var).size != 1:
@@ -249,6 +272,25 @@ class ModelIR:
             self._check_scale(a.sigma, f"AR1 on {a.var}: sigma")
             if not (np.isfinite(a.init_sigma) and a.init_sigma > 0):
                 raise ValueError(f"AR1 on {a.var}: init_sigma must be > 0")
+
+    def _check_terms(self, terms, N: int, where: str, length: str) -> None:
+        """Terms of a predictor of length N (a likelihood's observations, or the elements of a prior's variable)."""
+        for t in terms:
+            if is_design(t):
+                self._check_design(t, N, where)
+                continue
+            if len(t.factors) > MAX_TERM_FACTORS:  # no factor: a constant offset coef[i]
+                raise ValueError(f"{where}: a term has at most {MAX_TERM_FACTORS} variable factors")
+            for vn, idx in t.factors:
+                v = self.var(vn)
+                if idx is None and v.size not in (1, N):
+                    raise ValueError(f"{where}: {vn} (size {v.size}) needs an index array to enter a predictor of length {N}")
+                if idx is not None and len(idx) != N:
+                    raise ValueError(f"{where}: the index of {vn} has length {len(idx)}, not {length} {N}")
+                if idx is not None and (np.min(idx) < 0 or np.max(idx) >= v.size):
+                    raise ValueError(f"{where}: index of {vn} out of range")
+            if t.coef is not None and np.ndim(t.coef) == 1 and len(t.coef) != N:
+                raise ValueError(f"{where}: coef length {len(t.coef)} differs from {length} {N}")
 
     def _check_design(self, t, N: int, where: str) -> None:
         """A design term: X [N][K] of finite values, one factor on a variable of size K, no index (the checks prepare_ir
@@ -427,6 +469,34 @@ def radon_ir(n_obs: int = 919, n_counties: int = 85, seed: int = 123) -> ModelIR
     )
 
 
+def radon_centred_ir(n_obs: int = 800, n_counties: int = 32, n_regions: int = 4, seed: int = 41) -> ModelIR:
+    """Centred varying-intercept Radon-shaped model on simulated data, with a group-level predictor and nested groups:
+    a_j ~ Normal(g0 + g1 u_j + r[region_j], sigma_a) over counties j, r_k ~ Normal(0, 1) over regions,
+    y_i ~ Normal(a[county_i] + b floor_i, sigma_y); g0, g1, b ~ Normal(0, 5), sigma_a, sigma_y ~ HalfNormal(1).
+    Every county holds observations (enough of them that the centred form samples without divergences)."""
+    rng = np.random.default_rng(seed)
+    J = n_counties
+    region = (np.arange(J) % n_regions).astype(np.int32)
+    u = rng.standard_normal(J)
+    county = np.concatenate([np.arange(J), rng.integers(0, J, n_obs - J)]).astype(np.int32)
+    floor = (rng.random(n_obs) < 0.3).astype(np.float64)
+    r = rng.normal(0.0, 0.5, n_regions)
+    a = 1.3 + 0.7 * u + r[region] + 0.3 * rng.standard_normal(J)
+    y = a[county] - 0.6 * floor + 0.7 * rng.standard_normal(n_obs)
+    return ModelIR(
+        name="radon_centred",
+        vars=[Var("g0", "g0", 1), Var("g1", "g1", 1), Var("r", "r", n_regions), Var("sigma_a_log__", "sigma_a", 1, "log"),
+              Var("a", "a", J), Var("b", "b", 1), Var("sigma_y_log__", "sigma_y", 1, "log")],
+        priors=[Prior("normal", "g0", (0.0, 5.0)), Prior("normal", "g1", (0.0, 5.0)), Prior("normal", "r", (0.0, 1.0)),
+                Prior("halfnormal", "sigma_a_log__", (1.0,)),
+                Prior("normal", "a", (Linear([Term([("g0", None)]), Term([("g1", None)], coef=u), Term([("r", region)])]),
+                                      Ref("sigma_a_log__"))),
+                Prior("normal", "b", (0.0, 5.0)), Prior("halfnormal", "sigma_y_log__", (1.0,))],
+        likelihoods=[Likelihood("normal", y, [Term([("a", county)]), Term([("b", None)], coef=floor)],
+                                sigma=Ref("sigma_y_log__"))],
+    )
+
+
 def stochvol_ir(T: int = 3000, seed: int = 4) -> ModelIR:
     from .models import stochvol
 
@@ -538,8 +608,9 @@ class LoweredIR:
     vars: np.ndarray        # [n_vars] (offset, size, transform) int32 x3 ; bounds in var_bounds
     var_bounds: np.ndarray  # [n_vars][2]
     priors: list            # [(dist, var, [(kind, value, ref_offset)] * 3)]
-    liks: list              # [dict(dist, N, y, terms=[dict(coef, factors=[(offset, size, idx)])], sigma_kind, sigma_value, sigma_ref, sigma_obs, nu)]
+    liks: list              # [dict(dist, N, y, terms=[dict(coef, factors=[(offset, size, idx)])], sigma_kind, sigma_value, sigma_ref, sigma_obs, nu, y_var)]
                             # a design term's dict also has n_cols = K, with coef = X [N][K]
+                            # y_var 0: y is observed data; v + 1: a latent factor, y is None and its values are variable v's
     ar1: list               # [(var, phi(kind, value, ref), sigma(kind, value, ref), init_sigma)]
 
 
@@ -548,6 +619,43 @@ def _param(ir: ModelIR, a, off):
         v = ir.var(a.var)
         return (1, 0.0, off[v.name])
     return (0, float(a), -1)
+
+
+def _lower_terms(ir: ModelIR, terms: list, N: int, off: dict) -> list:
+    out = []
+    for t in terms:
+        if is_design(t):  # one ABI design term: coef = X row-major, n_cols = K
+            v = ir.var(t.factors[0][0])
+            out.append(dict(coef=np.ascontiguousarray(t.coef, dtype=np.float64), factors=[(off[v.name], v.size, None)],
+                            n_cols=v.size))
+            continue
+        coef = None
+        scale = 1.0
+        if t.coef is not None:
+            if np.ndim(t.coef) == 0:
+                scale = float(t.coef)
+            else:
+                coef = np.ascontiguousarray(t.coef, dtype=np.float64)
+        if scale != 1.0:
+            coef = np.full(N, scale) if coef is None else coef * scale
+        fs = []
+        for vn, idx in t.factors:
+            v = ir.var(vn)
+            fs.append((off[v.name], v.size, None if idx is None else np.ascontiguousarray(idx, dtype=np.int32)))
+        out.append(dict(coef=coef, factors=fs))
+    return out
+
+
+def _lower_slot(ir: ModelIR, par, off: dict) -> dict:
+    """A factor's parameter slot: none, a constant, a scalar variable or one constant per element."""
+    sk, sv, sr, so = SIGMA_NONE, 0.0, -1, None
+    if isinstance(par, Ref):
+        sk, sr = SIGMA_REF, off[ir.var(par.var).name]
+    elif par is not None and np.ndim(par) == 1:
+        sk, so = SIGMA_OBS, np.ascontiguousarray(par, dtype=np.float64)
+    elif par is not None:
+        sk, sv = SIGMA_CONST, float(par)
+    return dict(sigma_kind=sk, sigma_value=sv, sigma_ref=sr, sigma_obs=so)
 
 
 def lower(ir: ModelIR) -> LoweredIR:
@@ -562,46 +670,30 @@ def lower(ir: ModelIR) -> LoweredIR:
         if v.bounds:
             bounds[k] = v.bounds
         index[v.name] = k
-    priors = []
+    priors, latent = [], []
     for p in ir.priors:
+        if is_latent(p):
+            latent.append(p)
+            continue
         pars = [_param(ir, a, off) for a in p.params] + [(0, 0.0, -1)] * (3 - len(p.params))
         priors.append((PRIOR_DISTS[p.dist][0], index[ir.var(p.var).name], pars))
     liks = []
     for L in ir.likelihoods:
-        N = len(L.y)
-        terms = []
-        for t in L.terms:
-            if is_design(t):  # one ABI design term: coef = X row-major, n_cols = K
-                v = ir.var(t.factors[0][0])
-                terms.append(dict(coef=np.ascontiguousarray(t.coef, dtype=np.float64), factors=[(off[v.name], v.size, None)],
-                                  n_cols=v.size))
-                continue
-            coef = None
-            scale = 1.0
-            if t.coef is not None:
-                if np.ndim(t.coef) == 0:
-                    scale = float(t.coef)
-                else:
-                    coef = np.ascontiguousarray(t.coef, dtype=np.float64)
-            if scale != 1.0:
-                coef = np.full(N, scale) if coef is None else coef * scale
-            fs = []
-            for vn, idx in t.factors:
-                v = ir.var(vn)
-                fs.append((off[v.name], v.size, None if idx is None else np.ascontiguousarray(idx, dtype=np.int32)))
-            terms.append(dict(coef=coef, factors=fs))
         # the likelihood's one parameter slot: sigma, or the trials / alpha of the count and positive families
         par = L.trials if L.dist == "binomial_logit" else (L.alpha if L.dist in DISPERSION_LIKS else L.sigma)
-        sk, sv, sr, so = SIGMA_NONE, 0.0, -1, None
-        if isinstance(par, Ref):
-            sk, sr = SIGMA_REF, off[ir.var(par.var).name]
-        elif par is not None and np.ndim(par) == 1:
-            sk, so = SIGMA_OBS, np.ascontiguousarray(par, dtype=np.float64)
-        elif par is not None:
-            sk, sv = SIGMA_CONST, float(par)
-        liks.append(dict(dist=LIK_DISTS[L.dist], N=N, y=np.ascontiguousarray(L.y, dtype=np.float64), terms=terms,
-                         sigma_kind=sk, sigma_value=sv, sigma_ref=sr, sigma_obs=so, nu=float(L.nu)))
-    ar1 = [(index[ir.var(a.var).name], _param(ir, a.phi, off), _param(ir, a.sigma, off), float(a.init_sigma)) for a in ir.ar1]
+        liks.append(dict(dist=LIK_DISTS[L.dist], N=len(L.y), y=np.ascontiguousarray(L.y, dtype=np.float64),
+                         terms=_lower_terms(ir, L.terms, len(L.y), off), nu=float(L.nu), y_var=0,
+                         **_lower_slot(ir, par, off)))
+    # latent factors after the observed likelihoods, so that observed likelihood i keeps index i
+    for p in latent:
+        v = ir.var(p.var)
+        loc, scale = LINEAR_PRIORS[p.dist]
+        mu = p.params[loc]
+        terms = mu.terms if isinstance(mu, Linear) else [Term([(mu.var, None)]) if isinstance(mu, Ref) else Term([], coef=float(mu))]
+        liks.append(dict(dist=LIK_DISTS[p.dist], N=v.size, y=None, terms=_lower_terms(ir, terms, v.size, off),
+                         nu=float(p.params[0]) if p.dist == "studentt" else 0.0, y_var=index[v.name] + 1,
+                         **_lower_slot(ir, p.params[scale], off)))
+    ar1 =[(index[ir.var(a.var).name], _param(ir, a.phi, off), _param(ir, a.sigma, off), float(a.init_sigma)) for a in ir.ar1]
     return LoweredIR(ir.n, vars_, bounds, priors, liks, ar1)
 
 
@@ -624,33 +716,41 @@ def _column_of(t, N: int, ir: ModelIR):
 
 
 def fuse_design_columns(model: ModelIR) -> ModelIR:
-    """A copy of ``model`` in which, per likelihood, each complete run of column terms -- one term per column k = 0..K-1 of
-    the same vector variable of size K, as ``from_pymc`` lowers ``pm.math.dot(X, beta)`` -- is one design term with
-    X[:, k] = the column's coefficient, placed where the run's first term was.  Partial or duplicated runs, indexed group
-    effects, multi-factor terms and Deterministics stay as written; ``model`` itself is not changed."""
+    """A copy of ``model`` in which, per likelihood and per ``Linear`` prior location, each complete run of column terms --
+    one term per column k = 0..K-1 of the same vector variable of size K, as ``from_pymc`` lowers ``pm.math.dot(X, beta)``
+    -- is one design term with X[:, k] = the column's coefficient, placed where the run's first term was.  Partial or
+    duplicated runs, indexed group effects, multi-factor terms and Deterministics stay as written; ``model`` itself is
+    not changed."""
     out = copy.deepcopy(model)
     for L in out.likelihoods:
-        N = len(L.y)
-        runs = {}  # variable -> [(term position, k)]
-        for j, t in enumerate(L.terms):
-            ck = _column_of(t, N, out)
-            if ck is not None:
-                runs.setdefault(ck[0], []).append((j, ck[1]))
-        fused, drop = {}, set()
-        for vn, cols in runs.items():
-            K = out.var(vn).size
-            if sorted(k for _, k in cols) != list(range(K)):
-                continue
-            X = np.empty((N, K))
-            for j, k in cols:
-                c = L.terms[j].coef
-                X[:, k] = 1.0 if c is None else np.asarray(c, dtype=np.float64)
-            first = min(j for j, _ in cols)
-            fused[first] = Term([(vn, None)], coef=X)
-            drop.update(j for j, _ in cols)
-        if fused:
-            L.terms = [fused[j] if j in fused else t for j, t in enumerate(L.terms) if j in fused or j not in drop]
+        L.terms = _fuse_terms(out, L.terms, len(L.y))
+    for p in out.priors:
+        p.params = tuple(Linear(_fuse_terms(out, a.terms, out.var(p.var).size)) if isinstance(a, Linear) else a
+                         for a in p.params)
     return out
+
+
+def _fuse_terms(model: ModelIR, terms: list, N: int) -> list:
+    runs = {}  # variable -> [(term position, k)]
+    for j, t in enumerate(terms):
+        ck = _column_of(t, N, model)
+        if ck is not None:
+            runs.setdefault(ck[0], []).append((j, ck[1]))
+    fused, drop = {}, set()
+    for vn, cols in runs.items():
+        K = model.var(vn).size
+        if sorted(k for _, k in cols) != list(range(K)):
+            continue
+        X = np.empty((N, K))
+        for j, k in cols:
+            c = terms[j].coef
+            X[:, k] = 1.0 if c is None else np.asarray(c, dtype=np.float64)
+        first = min(j for j, _ in cols)
+        fused[first] = Term([(vn, None)], coef=X)
+        drop.update(j for j, _ in cols)
+    if not fused:
+        return terms
+    return [fused[j] if j in fused else t for j, t in enumerate(terms) if j in fused or j not in drop]
 
 
 # ------------------------------------------------------------------------------------------------------------------------
@@ -672,6 +772,8 @@ def specialise(ir: ModelIR, extended: bool = False):
 
     pri = {ir.var(p.var).name: p for p in ir.priors}
     if len(pri) != len(ir.priors) or len(ir.likelihoods) != 1:
+        return None
+    if any(isinstance(a, Linear) or (not isinstance(a, Ref) and np.ndim(a) > 0) for p in ir.priors for a in p.params):
         return None
     L = ir.likelihoods[0]
     names = [v.name for v in ir.vars]

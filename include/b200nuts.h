@@ -10,7 +10,8 @@
  * Conventions
  *   - extern "C", plain pointers and sizes; no C++/torch types cross the boundary.
  *   - every function returns 0 on success, <0 on failure; b200_last_error() gives the message
- *     (thread-local).  No exception crosses the ABI.
+ *     (thread-local).  No exception crosses the ABI.  B200_E_SHAPE (below) marks one refusal that
+ *     a caller may route around.
  *   - NUMERICAL failures are not errors: a non-finite energy inside a trajectory is a divergence
  *     recorded per chain/draw in the stats (reference: IntegrationError -> divergence,
  *     hmc/integration.py:95-107, hmc/nuts.py:399-440); a non-finite energy at the START of a draw
@@ -35,6 +36,12 @@ extern "C" {
 
 #define B200NUTS_VERSION 300 /* 0.3.0: B200_MASS_DENSE_ADAPT (b200_nuts_cfg.mass_update_window / .adaptation_window_multiplier,
                               * b200_chain_summary.final_cov); 0.2.0: b200_model_desc.ir (ModelSpec IR) */
+
+/* b200_model_create: the hand-written kernel of the model kind cannot run this size or data layout (EIGHT_SCHOOLS and
+ * RADON: n > 256, the chain-per-warp limit; RADON: padded observation rows that do not fit 227 KB of shared memory in the
+ * logp launch or in the NUTS launch with no tree level in shared memory).  The same model written as B200_MODEL_IR runs on
+ * the generic device function.  Every other failure returns -1. */
+#define B200_E_SHAPE (-2)
 
 /* memory space of caller-provided buffers */
 #define B200_MEM_HOST 0

@@ -34,6 +34,12 @@ def _sigmoid(x):
     return np.where(x >= 0, 1.0 / (1.0 + e), e / (1.0 + e))
 
 
+def _dsigmoid(x):
+    """sigmoid(x) (1 - sigmoid(x)) as e / (1 + e)^2, e = exp(-|x|): no cancellation in 1 - sigmoid(x) at large |x|."""
+    e = np.exp(-np.abs(x))
+    return e / ((1.0 + e) * (1.0 + e))
+
+
 class IrLogp:
     def __init__(self, ir: ModelIR):
         ir.validate()
@@ -69,7 +75,7 @@ class IrLogp:
                 lo, hi = v.bounds
                 sg = _sigmoid(q[s])
                 x[s] = lo + (hi - lo) * sg
-                dxdq[s] = (hi - lo) * sg * (1.0 - sg)
+                dxdq[s] = (hi - lo) * _dsigmoid(q[s])
                 djdq[s] = 1.0 - 2.0 * sg
                 lp += np.sum(np.log(hi - lo) - _softplus(-q[s]) - _softplus(q[s]))
             else:

@@ -192,7 +192,8 @@ class StochVolLogp:
         gh[:-1] += phi * es
         gh[0] -= h[0]
         g[0] = -mu / 25.0 + np.sum(dh)
-        g[1] = (1.0 - 2.0 * s) + 2.0 * s * (1.0 - s) * np.sum(es * h[:-1])
+        ez = np.exp(-abs(zphi))  # s (1 - s) = e / (1 + e)^2: no cancellation in 1 - s at large |zphi|
+        g[1] = (1.0 - 2.0 * s) + 2.0 * (ez / ((1.0 + ez) * (1.0 + ez))) * np.sum(es * h[:-1])
         g[2] = 1.0 - 10.0 * sig + np.sum(e * e) / sig**2 - (T - 1)
         g[3:] = gh
         return float(logp), g

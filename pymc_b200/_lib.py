@@ -24,6 +24,14 @@ class B200Error(RuntimeError):
     pass
 
 
+class B200ShapeError(B200Error):
+    """b200_model_create returned B200_E_SHAPE: the model kind's hand-written kernel cannot run this size or data layout;
+    the same model as IR runs on the generic device function."""
+
+
+E_SHAPE = -2
+
+
 class ModelDesc(C.Structure):
     _fields_ = [
         ("kind", C.c_int32),
@@ -275,7 +283,7 @@ def load() -> C.CDLL:
 
 def check(rc: int) -> None:
     if rc != 0:
-        raise B200Error(load().b200_last_error().decode())
+        raise (B200ShapeError if rc == E_SHAPE else B200Error)(load().b200_last_error().decode())
 
 
 def require_gpu() -> None:

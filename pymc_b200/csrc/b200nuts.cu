@@ -34,14 +34,26 @@ static thread_local std::string g_err;
 static thread_local double g_last_ms = 0.0;
 static thread_local int g_last_launches = 0;
 
-static int fail(const char* fmt, ...) {
+static int vfail(int rc, const char* fmt, va_list ap) {
     char buf[1024];
+    vsnprintf(buf, sizeof buf, fmt, ap);
+    g_err = buf;
+    return rc;
+}
+static int fail(const char* fmt, ...) {
     va_list ap;
     va_start(ap, fmt);
-    vsnprintf(buf, sizeof buf, fmt, ap);
+    const int rc = vfail(-1, fmt, ap);
     va_end(ap);
-    g_err = buf;
-    return -1;
+    return rc;
+}
+// the model kind's hand-written kernel cannot run this size or layout; the generic IR function can (B200_E_SHAPE)
+static int fail_shape(const char* fmt, ...) {
+    va_list ap;
+    va_start(ap, fmt);
+    const int rc = vfail(B200_E_SHAPE, fmt, ap);
+    va_end(ap);
+    return rc;
 }
 #define CU(call)                                                                                  \
     do {                                                                                          \
@@ -66,6 +78,24 @@ static int current_sm_count() {
     cudaGetDevice(&dev);
     return sm_count(dev);
 }
+
+// Dynamic shared memory of the chain-per-warp / chain-per-CTA launches: the model's staged data (padded to 16 bytes) and
+// one slice per chain of the CTA.  b200_model_create checks a hand-written kind's layout with the same functions, so a
+// model it accepts is one every launch can run.
+static constexpr size_t kMaxDynSmem = 227 * 1024;  // opt-in limit per CTA on sm_90
+static size_t staged_bytes(size_t model_shared) { return (model_shared + 15) & ~(size_t)15; }
+// one-point-per-team kernels (logp_grad_warp_kernel, leapfrog_warp_kernel): 8 chains per CTA at chain = warp, one at chain =
+// CTA; q, g and the team's reduction pad per chain
+static size_t point_smem_bytes(size_t model_shared, int NP, int W) {
+    const int wpb = (W == 1) ? 8 : 1;
+    return staged_bytes(model_shared) + (size_t)wpb * (2 * NP + (W > 1 ? 8 * W : 0)) * sizeof(double);
+}
+// the persistent NUTS kernel with `hot` tree levels in shared memory
+static size_t nuts_smem_bytes(size_t model_shared, int NP, int hot, int W) {
+    const int wpb = (W == 1) ? kNutsWarpChains : 1;
+    return staged_bytes(model_shared) + (size_t)wpb * nuts_warp_smem_bytes(NP, hot, W);
+}
+static int npl_warp(int n);
 
 struct DevBuf {  // owning, grow-only device allocation
     void* p = nullptr;
@@ -198,7 +228,7 @@ static int prepare_radon(b200_model* m, const b200_model_desc* d) {
     const long long N = d->n_obs;
     if (J <= 0 || N <= 0 || !d->x || !d->y || !d->idx) return fail("radon: missing data");
     if (d->n != 2 * J + 5) return fail("radon: n=%d but 2*n_groups+5=%d", d->n, 2 * J + 5);
-    if (J > 0xffff) return fail("radon: n_groups > 65535 unsupported");
+    if (!npl_warp(d->n)) return fail_shape("radon: n=%d exceeds the chain-per-warp limit (256)", d->n);
     std::vector<std::vector<int>> members(J);
     for (long long i = 0; i < N; ++i) {
         const int c = d->idx[i];
@@ -237,6 +267,13 @@ static int prepare_radon(b200_model* m, const b200_model_desc* d) {
     }
     RadonModel::Params& P = m->radon;
     P.K = K; P.M = M; P.J = J; P.n_obs = (int)N; P.E = (int)empty.size();
+    // every CTA stages the whole ELL array: it must fit beside the chains' slices in the logp / leapfrog launch and in the
+    // NUTS launch once its hot window has shrunk to no tree level
+    const int NP = 32 * npl_warp(d->n);
+    const size_t need = std::max(point_smem_bytes(RadonModel::shared_bytes(P), NP, 1), nuts_smem_bytes(RadonModel::shared_bytes(P), NP, 0, 1));
+    if (need > kMaxDynSmem)
+        return fail_shape("radon: the padded observation rows (K=%d, the largest county padded to %d observations) need %zu B "
+                          "of shared memory per CTA, over the 227 KB limit", K, row_len[0], need);
     if (upload(m, xy, &P.xy)) return -1;
     if (upload(m, seg, &P.seg)) return -1;
     if (upload(m, empty, &P.empty)) return -1;
@@ -247,6 +284,7 @@ static int prepare_eight(b200_model* m, const b200_model_desc* d) {
     const int J = (int)d->n_obs;
     if (J <= 0 || !d->y || !d->aux) return fail("eight_schools: missing data");
     if (d->n != J + 2) return fail("eight_schools: n=%d but J+2=%d", d->n, J + 2);
+    if (!npl_warp(d->n)) return fail_shape("eight_schools: n=%d exceeds the chain-per-warp limit (256)", d->n);
     std::vector<double> y(d->y, d->y + J), is2(J), ls(J);
     for (int j = 0; j < J; ++j) {
         if (!(d->aux[j] > 0)) return fail("eight_schools: sigma[%d] must be > 0", j);
@@ -850,8 +888,7 @@ template <class Model, int NPL, int W, class Kern, class... Args>
 static int launch_point_kernel(Kern kern, const b200_model* m, const typename Model::Params& MP, int C, cudaStream_t st,
                                Args... args) {
     const int wpb = (W == 1) ? 8 : 1;  // chains per CTA
-    const size_t data = (Model::shared_bytes(MP) + 15) & ~(size_t)15;
-    const size_t smem = data + (size_t)wpb * (2 * 32 * W * NPL + (W > 1 ? 8 * W : 0)) * sizeof(double);
+    const size_t smem = point_smem_bytes(Model::shared_bytes(MP), 32 * W * NPL, W);
     CU(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
     const int blocks = std::max(1, std::min((C + wpb - 1) / wpb, sm_count(m->device) * 8));
     typename Model::Params MPl;
@@ -1357,13 +1394,13 @@ struct NutsLaunch {
         constexpr int NP = 32 * W * NPL;
         constexpr int wpb = (W == 1) ? kNutsWarpChains : 1;  // chains per CTA (see seg below)
         int hot = std::min((W == 1) ? 2 : 1, P.max_td);      // tree levels whose vectors live in shared memory
-        const size_t data = (Model::shared_bytes(MP) + 15) & ~(size_t)15;
-        size_t smem = data + (size_t)wpb * nuts_warp_smem_bytes(NP, hot, W);
-        while (smem > 227 * 1024 && hot > 0) {  // shrink the hot window until the CTA fits
+        const size_t shared = Model::shared_bytes(MP);
+        size_t smem = nuts_smem_bytes(shared, NP, hot, W);
+        while (smem > kMaxDynSmem && hot > 0) {  // shrink the hot window until the CTA fits
             --hot;
-            smem = data + (size_t)wpb * nuts_warp_smem_bytes(NP, hot, W);
+            smem = nuts_smem_bytes(shared, NP, hot, W);
         }
-        if (smem > 227 * 1024) return fail("nuts: shared memory request %zu B exceeds 227 KB", smem);
+        if (smem > kMaxDynSmem) return fail("nuts: shared memory request %zu B exceeds 227 KB", smem);
         P.hot_levels = hot;
         P.scratch_stride = nuts_scratch_doubles(NP, P.max_td);
         // tree scratch [C][stride] | ChainCtx [C] | done [C] | ticket

@@ -55,6 +55,9 @@ class CompiledModel:
     ``spec`` is either a ``pymc_b200.ir.ModelIR`` (the general interface: any model of the closed factor set; routed to
     a hand-specialised kernel when ``ir.specialise`` recognises its shape, otherwise evaluated by the generic IR device
     function) or a ``models.ModelSpec`` naming one of the hand-written kernels directly (the GEMM-shaped configs).
+    A recognised model whose size or data layout its hand-written kernel cannot run (``b200_model_create`` refuses it with
+    B200_E_SHAPE: Eight Schools or Radon with n > 256, Radon rows too long for shared memory) runs on the generic function;
+    a ``ModelSpec`` of such a model raises ``B200ShapeError``.
 
     On the generic function, ``specialise`` (the default) also evaluates ``ir.fuse_design_columns(spec)``: a design matrix
     written one column per term runs as one team-parallel design term.  ``specialise=False`` evaluates the IR exactly as
@@ -64,13 +67,25 @@ class CompiledModel:
         from . import ir as _ir
 
         self.ir = None
-        lowered = None  # the IR the generic device function evaluates
         if isinstance(spec, _ir.ModelIR):
-            self.ir = lowered = spec
+            self.ir = spec
             fast = _ir.specialise(spec, extended=(specialise == "all")) if specialise else None
-            if fast is None and specialise:  # X beta written one column per term runs as one design term
-                lowered = _ir.fuse_design_columns(spec)
-            spec = fast if fast is not None else _ir_spec(spec)
+            if fast is not None:
+                try:
+                    self._create(fast, None, device)
+                    return
+                except _lib.B200ShapeError:
+                    pass
+            # X beta written one column per term runs as one design term
+            lowered = _ir.fuse_design_columns(spec) if specialise else spec
+            self._create(_ir_spec(spec), lowered, device)
+        else:
+            self._create(spec, None, device)
+
+    def _create(self, spec, lowered, device):
+        """b200_model_create for ``spec``; ``lowered``: the IR the generic device function evaluates (KIND_IR only)."""
+        from . import ir as _ir
+
         self.spec = spec
         self.n = spec.n
         self._lib = _lib.load()

@@ -83,7 +83,7 @@ class LatentLogp:
                 lo, hi = v.bounds
                 sg = ir_numpy._sigmoid(q[s])
                 x[s] = lo + (hi - lo) * sg
-                dxdq[s] = (hi - lo) * sg * (1.0 - sg)
+                dxdq[s] = (hi - lo) * ir_numpy._dsigmoid(q[s])
             else:
                 x[s] = q[s]
         gx = np.zeros(self.n)

@@ -92,11 +92,21 @@ extern "C" {
 #define B200_IR_L_BINOMIAL_LOGIT 5  /* y ~ Binomial(n, logit_p = eta)            discrete.py:141-152    */
 #define B200_IR_L_NEGBINOMIAL_LOG 6 /* y ~ NegativeBinomial(mu = exp(eta), alpha) discrete.py:700-745   */
 #define B200_IR_L_GAMMA_LOG 7       /* y ~ Gamma(alpha, beta = alpha exp(-eta))  continuous.py:2478-2521 */
+/* Normal observations measured with bounds.  For these two dists `y` points at a [3][N] block: row 0 is y, row 1 the lower
+ * bound, row 2 the upper bound of each observation, -inf / +inf where that side is open.  sigma as for NORMAL (CONST, REF
+ * or OBS).
+ *   CENSORED_NORMAL   pm.Censored(Normal(eta, sigma), lower, upper): log Phi(z) where y_i == lower_i, log(1 - Phi(z)) where
+ *                     y_i == upper_i, the Normal density elsewhere, z = (y_i - eta_i) / sigma
+ *   TRUNCATED_NORMAL  pm.TruncatedNormal(eta, sigma, lower, upper): the Normal density minus log(Phi(b) - Phi(a)) of the
+ *                     standardised bounds (a one-sided form where one side is open) */
+#define B200_IR_L_CENSORED_NORMAL 8  /* logprob/censoring.py:213-248 over Normal; dist_math.py:126-142 */
+#define B200_IR_L_TRUNCATED_NORMAL 9 /* TruncatedNormal.logp continuous.py:720-747; dist_math.py:126-182 */
 /* The support rule b200_model_create enforces (as ModelIR.validate does): HalfNormal, HalfCauchy, Exponential, Gamma and
  * LogNormal priors sit on a LOG variable or an INTERVAL with lo >= 0, Beta on an INTERVAL inside [0, 1], Uniform(a, b) on an
  * INTERVAL inside [a, b]; every scale (a prior's sigma / beta / lam, Normal and StudentT sigma including each sigma_obs, an
  * AR(1) sigma, alpha) is a finite constant > 0 or a REF to a scalar of positive support; Poisson y are integers >= 0,
- * Bernoulli y are 0 or 1. */
+ * Bernoulli y are 0 or 1.  Censored and truncated Normal observations: y finite, lower_i < upper_i, lower never +inf and
+ * upper never -inf, lower_i <= y_i <= upper_i; a truncated Normal factor has at least one finite bound. */
 #define B200_IR_S_NONE 0
 #define B200_IR_S_CONST 1 /* sigma.value               */
 #define B200_IR_S_REF 2   /* sigma = x[sigma.ref]      */
@@ -136,7 +146,7 @@ typedef struct b200_ir_term {
 typedef struct b200_ir_lik {
     int32_t dist, n_terms;
     int64_t N;
-    const double* y; /* [N]; NULL allowed when y_var > 0 */
+    const double* y; /* [N]; [3][N] (y, lower, upper) for CENSORED_NORMAL / TRUNCATED_NORMAL; NULL allowed when y_var > 0 */
     const b200_ir_term* terms;
     int32_t sigma_kind, y_var;
     b200_ir_param sigma;

@@ -129,6 +129,7 @@ struct b200_model {
     const double* tr_hi = nullptr;
     IrModel::Params ir{};
     long long ir_max_obs = 0;
+    bool ir_bounded = false;  // a censored / truncated Normal likelihood: the kernels run IrBoundedModel
     DevBuf ir_scratch;  // per-team scratch of the generic IR device function: [teams][n_pad + max N] doubles
     // lock-step (GEMM-shaped) models; every matrix is row-major with rows `ld` doubles apart (n rounded up to 4, zero pad)
     long long ld = 0;
@@ -372,6 +373,11 @@ static bool ir_scale_ok(const b200_ir_param& p, const std::vector<IrVarD>& vars)
     return false;
 }
 #define B200_IR_SCALE_RULE "must be a finite constant > 0 or a scalar variable with positive support (a log transform, or an interval with lo >= 0)"
+// The bounds of censored / truncated Normal observations (ModelIR._validate_bounds, same wording)
+#define B200_IR_BOUND_SIDES "lower must not be +inf or NaN and upper must not be -inf or NaN"
+#define B200_IR_BOUND_ORDER "lower < upper must hold for every observation"
+#define B200_IR_BOUND_Y "y must be finite and lie in [lower, upper] for every observation"
+#define B200_IR_TRUNC_OPEN "truncated_normal needs a finite lower or upper bound; with neither side bounded, write the likelihood as normal"
 
 static int prepare_ir(b200_model* m, const b200_model_desc* d) {
     const b200_ir* R = d->ir;
@@ -542,11 +548,38 @@ static int prepare_ir(b200_model* m, const b200_model_desc* d) {
                     D.sum_log_y = sly;
                 }
             } break;
+            case B200_IR_L_CENSORED_NORMAL: case B200_IR_L_TRUNCATED_NORMAL: {  // y is the [3][N] block (y, lower, upper)
+                const bool cens = L.dist == B200_IR_L_CENSORED_NORMAL;
+                const char* what = cens ? "censored_normal" : "truncated_normal";
+                const double *y = L.y, *lo = L.y + N, *hi = L.y + 2 * N;
+                std::vector<signed char> code(cens ? (size_t)N : 0);
+                long long n_observed = 0;
+                bool bounded = false;
+                for (long long i = 0; i < N; ++i) {
+                    if (std::isnan(lo[i]) || std::isnan(hi[i]) || lo[i] == INFINITY || hi[i] == -INFINITY)
+                        return fail("ir: likelihood %d: %s: " B200_IR_BOUND_SIDES " (at %lld)", l, what, i);
+                    if (!(lo[i] < hi[i])) return fail("ir: likelihood %d: %s: " B200_IR_BOUND_ORDER " (at %lld)", l, what, i);
+                    if (!(std::isfinite(y[i]) && lo[i] <= y[i] && y[i] <= hi[i]))
+                        return fail("ir: likelihood %d: %s: " B200_IR_BOUND_Y " (at %lld)", l, what, i);
+                    bounded = bounded || std::isfinite(lo[i]) || std::isfinite(hi[i]);
+                    if (cens) {
+                        code[i] = y[i] == lo[i] ? 1 : (y[i] == hi[i] ? 2 : 0);
+                        n_observed += code[i] == 0;
+                    }
+                }
+                if (!cens && !bounded) return fail("ir: likelihood %d: " B200_IR_TRUNC_OPEN, l);
+                // -log(2 pi) / 2 of every Normal density term: each uncensored observation, every truncated one
+                D.c0 = -(double)(cens ? n_observed : N) * B200_HALF_LOG_2PI;
+                if (cens ? upload(m, code, &D.cens) : upload_raw(m, lo, 2 * (size_t)N, &D.bnd)) return -1;
+                m->ir_bounded = true;
+            } break;
             default: return fail("ir: likelihood %d: density %d is not in the closed set", l, L.dist);
         }
-        if ((L.dist == B200_IR_L_NORMAL || L.dist == B200_IR_L_STUDENTT) && L.sigma_kind == B200_IR_S_NONE)
+        const bool has_sigma = L.dist == B200_IR_L_NORMAL || L.dist == B200_IR_L_STUDENTT || L.dist == B200_IR_L_CENSORED_NORMAL ||
+                               L.dist == B200_IR_L_TRUNCATED_NORMAL;
+        if (has_sigma && L.sigma_kind == B200_IR_S_NONE)
             return fail("ir: likelihood %d needs sigma", l);
-        if (L.dist == B200_IR_L_NORMAL || L.dist == B200_IR_L_STUDENTT) {
+        if (has_sigma) {
             if (L.sigma_kind == B200_IR_S_OBS) {
                 for (long long i = 0; i < N; ++i)
                     if (!(std::isfinite(L.sigma_obs[i]) && L.sigma_obs[i] > 0))
@@ -745,8 +778,13 @@ static int dispatch(const b200_model* m, F&& f) {
             B200_TEAM(StochVolModel, m->stochvol)
             return fail("stochvol: n=%d exceeds 4096", m->n);
         case B200_MODEL_IR:
-            if (m->n <= 256 && !env_flag("B200_FORCE_TEAM")) { B200_WARP(IrModel, m->ir) }
-            B200_TEAM(IrModel, m->ir)
+            if (m->ir_bounded) {  // a censored / truncated Normal likelihood: the kernels that can evaluate it
+                if (m->n <= 256 && !env_flag("B200_FORCE_TEAM")) { B200_WARP(IrBoundedModel, m->ir) }
+                B200_TEAM(IrBoundedModel, m->ir)
+            } else {
+                if (m->n <= 256 && !env_flag("B200_FORCE_TEAM")) { B200_WARP(IrModel, m->ir) }
+                B200_TEAM(IrModel, m->ir)
+            }
             return fail("ir: n=%d exceeds the chain-per-CTA limit (4096)", m->n);
     }
 #undef B200_WARP
@@ -761,7 +799,7 @@ static int dispatch(const b200_model* m, F&& f) {
 template <class Model>
 static int launch_params(const b200_model* m, const typename Model::Params& MP, long long teams, typename Model::Params* out) {
     *out = MP;
-    if constexpr (std::is_same_v<Model, IrModel>) {
+    if constexpr (std::is_base_of_v<IrModel, Model>) {
         b200_model* mm = const_cast<b200_model*>(m);
         CU(mm->ir_scratch.reserve((size_t)teams * (size_t)mm->ir.stride * sizeof(double)));
         mm->ir.scratch = mm->ir_scratch.as<double>();
@@ -1616,7 +1654,10 @@ extern "C" int b200_pointwise_loglik(b200_model* m, int32_t lik, const double* d
     CU(m->ir_scratch.reserve((size_t)blocks * wpb * (size_t)m->ir.stride * sizeof(double)));
     m->ir.scratch = m->ir_scratch.as<double>();
     Timer t(st);
-    ir_pointwise_kernel<<<blocks, wpb * 32, 0, st>>>(m->ir, lik, D, d_draws, d_out);
+    if (m->ir_bounded)
+        ir_pointwise_kernel<true><<<blocks, wpb * 32, 0, st>>>(m->ir, lik, D, d_draws, d_out);
+    else
+        ir_pointwise_kernel<false><<<blocks, wpb * 32, 0, st>>>(m->ir, lik, D, d_draws, d_out);
     CU(cudaGetLastError());
     t.stop(1);
     return sg.finish();

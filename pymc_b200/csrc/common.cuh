@@ -52,6 +52,66 @@ __device__ __forceinline__ double digamma(double x) {
     return acc + log(x) - 0.5 * r - ser;
 }
 
+// ---------------------------------------------------------------------------------------------
+// Standard normal tails (dist_math.py:126-182, the same region switches), for censored and truncated Normal observations.
+// Phi is the standard normal CDF, phi its density.  The Mills ratio phi(z) / Phi(z) comes from the same erfcx() as the
+// log-CDF where Phi is small, so neither underflows or cancels.
+// ---------------------------------------------------------------------------------------------
+constexpr double kSqrtHalf = 0.70710678118654752440;   // 1 / sqrt(2)
+constexpr double kSqrt2OverPi = 0.79788456080286535588; // sqrt(2 / pi)
+constexpr double kLog2 = 0.69314718055994530942;
+
+// log Phi(z): normal_lcdf, dist_math.py:126-133.  log(1 - Phi(z)) (normal_lccdf, :136-142) is normal_lcdf(-z), the same
+// expression term for term.
+__device__ __forceinline__ double normal_lcdf(double z) {
+    return z < -1.0 ? log(0.5 * erfcx(-z * kSqrtHalf)) - 0.5 * z * z : log1p(-0.5 * erfc(z * kSqrtHalf));
+}
+
+// phi(z) / Phi(z); for z < -1 as sqrt(2/pi) / erfcx(-z / sqrt 2), the two exp(-z^2 / 2) cancelled
+__device__ __forceinline__ double normal_mills(double z) {
+    return z < -1.0 ? kSqrt2OverPi / erfcx(-z * kSqrtHalf) : kSqrt2OverPi * exp(-0.5 * z * z) / erfc(-z * kSqrtHalf);
+}
+
+// (log Phi(z), phi(z) / Phi(z)) of one censored observation
+struct NormalTail { double log_cdf, mills; };
+__device__ __forceinline__ NormalTail normal_tail(double z) {
+    if (z < -1.0) {
+        const double e = erfcx(-z * kSqrtHalf);
+        return {log(0.5 * e) - 0.5 * z * z, kSqrt2OverPi / e};
+    }
+    return {log1p(-0.5 * erfc(z * kSqrtHalf)), kSqrt2OverPi * exp(-0.5 * z * z) / erfc(-z * kSqrtHalf)};
+}
+
+// log(Phi(b) - Phi(a)) for a < b: log_diff_normal_cdf, dist_math.py:145-182, and ra = phi(a) / Z, rb = phi(b) / Z with
+// Z = Phi(b) - Phi(a).  With x = b / sqrt 2, y = a / sqrt 2: both in the upper tail (y > 0), Z = e^(-y^2) D / 2 with
+// D = erfcx(y) - e^(y^2 - x^2) erfcx(x); both in the lower tail (x < 0) the mirror image; else (erf(x) - erf(y)) / 2.
+// y^2 - x^2 is formed as (y - x)(y + x): a narrow window far in a tail keeps its width to rounding.  An open side
+// (a = -inf or b = +inf) takes the one-sided form, which is what the two-sided one reduces to there.  Only the kernels
+// of csrc/ir_model.cuh's IrBoundedModel reach these helpers (DESIGN.md 6).
+struct NormalMass { double log_z, ra, rb; };
+__device__ __forceinline__ NormalMass normal_log_mass(double a, double b) {
+    if (a == -INFINITY) {
+        if (b == INFINITY) return {0.0, 0.0, 0.0};
+        return {normal_lcdf(b), 0.0, normal_mills(b)};
+    }
+    if (b == INFINITY) return {normal_lcdf(-a), normal_mills(-a), 0.0};
+    const double x = b * kSqrtHalf, y = a * kSqrtHalf;
+    if (y > 0.0) {
+        const double e = exp((y - x) * (y + x));
+        const double d = erfcx(y) - e * erfcx(x);
+        const double ra = kSqrt2OverPi / d;
+        return {-kLog2 - y * y + log(d), ra, ra * e};
+    }
+    if (x < 0.0) {
+        const double e = exp((x - y) * (x + y));
+        const double d = erfcx(-x) - e * erfcx(-y);
+        const double rb = kSqrt2OverPi / d;
+        return {-kLog2 - x * x + log(d), rb * e, rb};
+    }
+    const double w = erf(x) - erf(y);  // 2 Z
+    return {-kLog2 + log(w), kSqrt2OverPi * exp(-y * y) / w, kSqrt2OverPi * exp(-x * x) / w};
+}
+
 // Normal(0,1) log-density constant part is added by callers; this is the HalfCauchy(beta) density of
 // x = exp(z) plus the log-transform Jacobian (+z), and its derivative in z.
 // Reference: Cauchy.logp continuous.py:2287-2288, HalfCauchy.logp :2383-2385, LogTransform

@@ -26,7 +26,7 @@ enum { IRT_NONE = 0, IRT_LOG = 1, IRT_INTERVAL = 2 };
 enum { IRP_FLAT = 0, IRP_NORMAL, IRP_HALFNORMAL, IRP_CAUCHY, IRP_HALFCAUCHY, IRP_EXPONENTIAL, IRP_STUDENTT, IRP_UNIFORM,
        IRP_GAMMA, IRP_BETA, IRP_LOGNORMAL };
 enum { IRL_NORMAL = 0, IRL_BERNOULLI_LOGIT, IRL_POISSON_LOG, IRL_STUDENTT, IRL_NORMAL_LOGVAR, IRL_BINOMIAL_LOGIT,
-       IRL_NEGBINOMIAL_LOG, IRL_GAMMA_LOG };
+       IRL_NEGBINOMIAL_LOG, IRL_GAMMA_LOG, IRL_CENSORED_NORMAL, IRL_TRUNCATED_NORMAL };
 enum { IRS_NONE = 0, IRS_CONST, IRS_REF, IRS_OBS };
 constexpr double kNegBinPoissonAlpha = 1e10;  // above: NegativeBinomial -> Poisson(mu) limit (discrete.py:727-735)
 
@@ -87,12 +87,86 @@ __device__ __forceinline__ void ir_design_grad(const IrTermD& Tm, const double* 
 // c0: sum of the constant parts over i.  Random dispersion (sigma_kind REF): Gamma keeps sum_i log y_i in sum_log_y;
 // NegativeBinomial keeps the distinct nonzero y values u[k] with their counts cnt[k] (n_tab of them), over which the
 // alpha-dependent normalising terms sum_i lgamma(y_i + a) - lgamma(a) and their digamma gradient are evaluated.
+// Censored Normal: cens[i] = 0 (observed), 1 (y_i at its lower bound), 2 (at its upper bound); the censoring point is y_i
+// itself.  Truncated Normal: bnd = [2][N], the lower and upper bound of each observation, -inf / +inf where open.
 // yoff >= 0: a latent factor (a Normal / StudentT prior whose location is a linear predictor): y_i = x[yoff + i], the
 // constrained values of a variable of size N, which also receives d logp / d y_i = -r_i; y is null.  -1: y is data.
 struct IrLikD { int dist, n_terms, term0, sigma_kind; long long N; const double* y; const double* sigma_obs; IrParamD sigma;
-                double nu, c0, sum_log_y; const double* tab_u; const double* tab_cnt; int n_tab, yoff; };
+                double nu, c0, sum_log_y; const double* tab_u; const double* tab_cnt; int n_tab, yoff;
+                const signed char* cens; const double* bnd; };
 struct IrAr1D { int offset, size; IrParamD phi, sigma; double init_sigma; };
 
+// eta_i = sum_t coef_t[i] prod_f x_f[idx_f[i]] over the likelihood's terms, t ascending (as eval's observation loop)
+__device__ __forceinline__ double ir_eta(const IrTermD* terms, int n_terms, const double* x, int i, int N) {
+    double eta = 0.0;
+    for (int t = 0; t < n_terms; ++t) {
+        const IrTermD& Tm = terms[t];
+        if (Tm.n_cols) {
+            eta += ir_design_row(Tm, x + Tm.f[0].offset, i, N);
+            continue;
+        }
+        double pr = Tm.coef ? Tm.coef[i] : 1.0;
+        for (int f = 0; f < Tm.n_factors; ++f) {
+            const IrFactorD& Fc = Tm.f[f];
+            pr *= x[Fc.offset + (Fc.idx ? Fc.idx[i] : (Fc.size == 1 ? 0 : i))];
+        }
+        eta += pr;
+    }
+    return eta;
+}
+
+// log p(y_i | eta) of one censored / truncated Normal observation without its constant -log(2 pi) / 2 (in c0), with
+// r = d / d eta and s = d / d sigma.  Censored (logprob/censoring.py:213-248 over Normal): the Normal density where y_i is
+// observed, log Phi(zc) at a bound, zc = z at the lower one and -z at the upper one (normal_lccdf(z) = normal_lcdf(-z)).
+// Truncated (continuous.py:720-747): the Normal density minus log(Phi(b) - Phi(a)) of the standardised bounds.
+struct IrBoundedTerm { double lp, r, s; };
+__device__ __forceinline__ IrBoundedTerm ir_bounded_term(const IrLikD& L, int i, double eta, double sg) {
+    const double z = (L.y[i] - eta) / sg;
+    if (L.dist == IRL_CENSORED_NORMAL) {
+        const int c = L.cens[i];
+        if (c == 0) return {-0.5 * z * z - log(sg), z / sg, (z * z - 1.0) / sg};
+        const double zc = c == 1 ? z : -z;
+        const NormalTail t = normal_tail(zc);
+        return {t.log_cdf, (c == 1 ? -t.mills : t.mills) / sg, -t.mills * zc / sg};
+    }
+    const int N = (int)L.N;
+    const double a = (L.bnd[i] - eta) / sg, b = (L.bnd[N + i] - eta) / sg;  // an open side stays infinite
+    const NormalMass M = normal_log_mass(a, b);
+    const double ta = M.ra == 0.0 ? 0.0 : a * M.ra, tb = M.rb == 0.0 ? 0.0 : b * M.rb;  // inf * 0 = 0
+    return {-0.5 * z * z - log(sg) - M.log_z, (z + M.rb - M.ra) / sg, (z * z - 1.0 + tb - ta) / sg};
+}
+
+// The observation loop of a censored / truncated Normal likelihood, out of line: IrBoundedModel::eval calls it once per
+// such likelihood, so the erfcx() tail math stays out of eval's own observation loop.  Writes r_i = d logp / d eta_i;
+// returns this thread's partial sums of logp and d logp / d sigma.
+struct IrPartials { double lp, s_sig; };
+template <int W>
+__device__ __noinline__ IrPartials ir_bounded_pass(const IrLikD* Lp, const IrTermD* terms, const double* x, double* r,
+                                                   double sg_s, int tid) {
+    constexpr int TS = 32 * W;
+    const IrLikD& L = *Lp;
+    const int N = (int)L.N;
+    double lp = 0.0, s_sig = 0.0;
+    for (int i = tid; i < N; i += TS) {
+        const double eta = ir_eta(terms + L.term0, L.n_terms, x, i, N);
+        const IrBoundedTerm b = ir_bounded_term(L, i, eta, (L.sigma_kind == IRS_OBS) ? L.sigma_obs[i] : sg_s);
+        lp += b.lp;
+        s_sig += b.s;
+        r[i] = b.r;
+    }
+    return {lp, s_sig};
+}
+
+// the pointwise pass's share of the same: log p(y_i | eta) with every constant (a censored value at its bound has none)
+__device__ __noinline__ double ir_bounded_loglik(const IrLikD& L, int i, double eta, double sg) {
+    const bool at_bound = L.dist == IRL_CENSORED_NORMAL && L.cens[i] != 0;
+    return ir_bounded_term(L, i, eta, sg).lp - (at_bound ? 0.0 : B200_HALF_LOG_2PI);
+}
+
+// IrModel evaluates every factor of the closed set except the censored / truncated Normal likelihoods; IrBoundedModel (below)
+// is the same function with those two added.  A kernel's register allocation covers every function it can reach, and the
+// tail math takes about 128 registers, so the engine instantiates its kernels twice and runs a model on IrBoundedModel only
+// when it has such a likelihood (b200_model.ir_bounded): every other IR model keeps the kernels it had before.
 struct IrModel {
     struct Params {
         const IrVarD* vars; const IrPriorD* priors; const IrLikD* liks; const IrTermD* terms; const IrAr1D* ar1;
@@ -107,7 +181,13 @@ struct IrModel {
     __device__ static __forceinline__ double par(const IrParamD& p, const double* x) { return p.kind ? x[p.ref] : p.value; }
 
     template <int NPL, int W, bool SMALL = false>
-    __device__ __noinline__ static double eval(const Params& P, const char*, const double* q_s, double* g_s, int tid, double* red) {
+    __device__ __noinline__ static double eval(const Params& P, const char* s, const double* q_s, double* g_s, int tid, double* red) {
+        return eval_impl<NPL, W, false>(P, s, q_s, g_s, tid, red);
+    }
+
+    template <int NPL, int W, bool BOUNDED>
+    __device__ __forceinline__ static double eval_impl(const Params& P, const char*, const double* q_s, double* g_s, int tid,
+                                                       double* red) {
         constexpr int TS = 32 * W;
         const int slot = (W == 1) ? (int)(blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) : (int)blockIdx.x;
         double* x = P.scratch + (long long)slot * P.stride;
@@ -216,7 +296,15 @@ struct IrModel {
             const bool disp = L.dist == IRL_NEGBINOMIAL_LOG || L.dist == IRL_GAMMA_LOG;  // sg_s is the dispersion alpha
             const double la = disp ? log(sg_s) : 0.0;
             double s_sig = 0.0;
-            for (int i = tid; i < N; i += TS) {
+            const bool bounded = BOUNDED && (L.dist == IRL_CENSORED_NORMAL || L.dist == IRL_TRUNCATED_NORMAL);
+            if constexpr (BOUNDED) {
+                if (bounded) {  // uniform branch: out of line
+                    const IrPartials b = ir_bounded_pass<W>(P.liks + l, P.terms, x, r, sg_s, tid);
+                    lp += b.lp;
+                    s_sig = b.s_sig;
+                }
+            }
+            if (!bounded) for (int i = tid; i < N; i += TS) {
                 double eta = 0.0;
                 for (int t = 0; t < L.n_terms; ++t) {
                     const IrTermD& Tm = P.terms[L.term0 + t];
@@ -419,6 +507,13 @@ struct IrModel {
     }
 };
 
+struct IrBoundedModel : IrModel {
+    template <int NPL, int W, bool SMALL = false>
+    __device__ __noinline__ static double eval(const Params& P, const char* s, const double* q_s, double* g_s, int tid, double* red) {
+        return eval_impl<NPL, W, true>(P, s, q_s, g_s, tid, red);
+    }
+};
+
 // ---------------------------------------------------------------------------------------------------------------------
 // Pointwise log-likelihood of one likelihood factor for a batch of (unconstrained) draws: out[d][i] = log p(y_i | draw d).
 // What pm.compute_log_likelihood evaluates per draw through a compiled function (pymc/stats/log_density.py:31-77,
@@ -426,6 +521,7 @@ struct IrModel {
 // team scratch slice like in eval().  Elementwise constants (log 2pi, lgamma) are included, unlike in eval() where they are
 // folded into one constant per factor.
 // ---------------------------------------------------------------------------------------------------------------------
+template <bool BOUNDED>  // as IrModel / IrBoundedModel
 __global__ void __launch_bounds__(256) ir_pointwise_kernel(const IrModel::Params P, int lik, long long D,
                                                            const double* __restrict__ draws /*[D][n]*/,
                                                            double* __restrict__ out /*[D][N]*/) {
@@ -490,6 +586,9 @@ __global__ void __launch_bounds__(256) ir_pointwise_kernel(const IrModel::Params
                     }
                     break;
                 case IRL_GAMMA_LOG: lp = sg_s * (la - eta) - lgamma(sg_s) + (sg_s - 1.0) * log(yi) - sg_s * yi * exp(-eta); break;
+                case IRL_CENSORED_NORMAL: case IRL_TRUNCATED_NORMAL:
+                    if constexpr (BOUNDED) lp = ir_bounded_loglik(L, i, eta, (L.sigma_kind == IRS_OBS) ? L.sigma_obs[i] : sg_s);
+                    break;
                 default: break;
             }
             out[d * N + i] = lp;

@@ -13,7 +13,9 @@ pymc/model/fgraph.py:76-81, :139) -- and pattern-matches them onto the closed fa
                      (Add / Sub / Neg / Mul / division by a constant / indexing by constant integer arrays / Dot with a
                      constant matrix / broadcasts); Normal(0, exp(eta / 2)) with a linear eta -> the log-variance likelihood;
                      Binomial(n, logit_p = eta) with constant trials, NegativeBinomial(mu = exp(eta), alpha) and
-                     Gamma(alpha, beta = alpha / exp(eta) | alpha * exp(-eta)), alpha a constant or a scalar free RV
+                     Gamma(alpha, beta = alpha / exp(eta) | alpha * exp(-eta)), alpha a constant or a scalar free RV;
+                     pm.Censored(pm.Normal.dist(eta, sigma), lower, upper), pm.TruncatedNormal(eta, sigma, lower, upper)
+                     and pm.Truncated(pm.Normal.dist(eta, sigma), lower, upper) with constant bounds
 
 Anything outside the closed set raises ``NotImplementedError`` naming the offending op, so a model either lowers exactly
 or not at all.  PyMC and PyTensor are NOT importable in the build image (SURVEY 8c); this module imports them lazily and
@@ -354,6 +356,38 @@ def from_pymc(model) -> _ir.ModelIR:
             if eta is None:
                 raise NotImplementedError(f"{rv.name}: write the likelihood as {form}")
             liks.append(_ir.Likelihood("negative_binomial_log", y, make_terms(eta, N), alpha=alpha, name=rv.name))
+        elif op == "truncated":
+            # TruncatedRV (truncated.py:53-130): the base RV's own inputs followed by lower and upper, its op in base_rv_op.
+            # A Normal base never arrives here: pm.Truncated dispatches it to TruncatedNormal (truncated.py:499-505).
+            base_op = getattr(rv.owner.op, "base_rv_op", None)
+            what = type(base_op).__name__ if base_op is not None else type(rv.owner.op).__name__
+            raise NotImplementedError(f"{rv.name}: pm.Truncated of {what} is outside the closed set (only a Normal base "
+                                      "distribution can be truncated)")
+        elif op in ("censored", "truncatednormal"):
+            # CensoredRV: dist params (base, lower, upper) (censored.py:45-76); TruncatedNormalRV: (mu, sigma, lower, upper)
+            # (continuous.py:558-583), which pm.Truncated of a Normal also becomes (truncated.py:499-505)
+            def bound(x, open_value):
+                v = _const_value(x)
+                if v is None:
+                    raise NotImplementedError(f"{rv.name}: censoring / truncation bounds must be constants (random bounds are "
+                                              "outside the closed set)")
+                v = np.asarray(v, dtype=np.float64)
+                if v.size == 1:
+                    return None if float(v.reshape(())) == open_value else float(v.reshape(()))
+                return np.ravel(np.broadcast_to(v, (N,))).astype(np.float64)
+
+            if op == "truncatednormal":
+                mu, s, lo, hi = ps[:4]
+            else:
+                base, lo, hi = ps[:3]
+                if base.owner is None or _op_name(base) != "normal":
+                    what = type(base.owner.op).__name__ if base.owner is not None else str(base)
+                    raise NotImplementedError(f"{rv.name}: pm.Censored of {what} is outside the closed set (only a Normal "
+                                              "base distribution can be censored)")
+                mu, s = _dist_params(base)[:2]
+            dist = "censored_normal" if op == "censored" else "truncated_normal"
+            liks.append(_ir.Likelihood(dist, y, make_terms(mu, N), sigma=sigma_of(s), lower=bound(lo, -np.inf),
+                                       upper=bound(hi, np.inf), name=rv.name))
         elif op == "gamma":  # RV parameters (alpha, scale = reciprocal(beta)), continuous.py:2478-2510
             form = ("pm.Gamma(alpha=a, beta=a / pm.math.exp(linear predictor)) or beta=a * pm.math.exp(-linear predictor), "
                     "a a constant or scalar free RV")

@@ -52,7 +52,18 @@ LIK_DISTS = {
     "binomial_logit": 5,     # y_i ~ Binomial(trials, logit_p = eta_i)                  discrete.py:141-152 (stabilised forms)
     "negative_binomial_log": 6,  # y_i ~ NegativeBinomial(mu = exp(eta_i), alpha)       discrete.py:700-745
     "gamma_log": 7,          # y_i ~ Gamma(alpha, beta = alpha exp(-eta_i))             continuous.py:2478-2521
+    "censored_normal": 8,    # y_i ~ Censored(Normal(eta_i, sigma), lower, upper)       logprob/censoring.py:213-248
+    "truncated_normal": 9,   # y_i ~ TruncatedNormal(eta_i, sigma, lower, upper)        continuous.py:720-747
 }
+# Normal observations with bounds: ``Likelihood.lower`` / ``.upper`` (None, a constant or one value per observation, -inf /
+# +inf where that side is open); lowered as the [3][N] block (y, lower, upper) of include/b200nuts.h
+BOUNDED_LIKS = ("censored_normal", "truncated_normal")
+SIGMA_LIKS = ("normal", "studentt") + BOUNDED_LIKS  # likelihoods whose parameter slot is sigma
+# the support rule of bounded observations (csrc/b200nuts.cu: prepare_ir, same words)
+BOUND_SIDES = "lower must not be +inf or NaN and upper must not be -inf or NaN"
+BOUND_ORDER = "lower < upper must hold for every observation"
+BOUND_Y = "y must be finite and lie in [lower, upper] for every observation"
+TRUNC_OPEN = "truncated_normal needs a finite lower or upper bound; with neither side bounded, write the likelihood as normal"
 DISPERSION_LIKS = ("negative_binomial_log", "gamma_log")  # their `alpha` is a constant or a Ref
 # The support rule.  The device evaluates a density's formula wherever it is asked to, so every variable must be kept
 # inside its prior's support by its transform, and every scale parameter must be positive:
@@ -141,6 +152,15 @@ class Likelihood:
     name: str = "y"
     alpha: float | Ref | None = None           # negative_binomial_log / gamma_log: dispersion (shape)
     trials: float | np.ndarray | None = None   # binomial_logit: number of trials, one for all or one per observation
+    lower: float | np.ndarray | None = None    # censored_normal / truncated_normal: None (open), a constant or one per
+    upper: float | np.ndarray | None = None    # observation, -inf / +inf where that observation's side is open
+
+    def bounds(self) -> tuple[np.ndarray, np.ndarray]:
+        """(lower, upper) of every observation as float arrays, -inf / +inf where open."""
+        N = len(self.y)
+        lo = np.full(N, -np.inf) if self.lower is None else np.broadcast_to(np.asarray(self.lower, dtype=np.float64), (N,))
+        hi = np.full(N, np.inf) if self.upper is None else np.broadcast_to(np.asarray(self.upper, dtype=np.float64), (N,))
+        return np.array(lo), np.array(hi)
 
 
 @dataclass
@@ -242,11 +262,11 @@ class ModelIR:
                 raise ValueError(f"likelihood {L.dist!r} is not in the closed set {sorted(LIK_DISTS)}")
             N = len(L.y)
             self._check_terms(L.terms, N, f"likelihood {L.name}", "the number of observations")
-            if L.dist in ("normal", "studentt") and L.sigma is None:
+            if L.dist in SIGMA_LIKS and L.sigma is None:
                 raise ValueError(f"{L.dist} likelihood needs sigma")
             if isinstance(L.sigma, Ref) and self.var(L.sigma.var).size != 1:
                 raise ValueError("likelihood sigma must be a scalar variable")
-            if L.dist in ("normal", "studentt"):
+            if L.dist in SIGMA_LIKS:
                 if not isinstance(L.sigma, Ref) and np.ndim(L.sigma) == 1:
                     s = np.asarray(L.sigma, dtype=np.float64)
                     if len(s) != N:
@@ -263,6 +283,7 @@ class ModelIR:
             if L.dist == "bernoulli_logit" and not np.all((y == 0.0) | (y == 1.0)):
                 raise ValueError("bernoulli_logit: y must be 0 or 1")
             self._validate_family(L)
+            self._validate_bounds(L)
         for a in self.ar1:
             if self.var(a.var).size < 2:
                 raise ValueError("AR1 needs at least two steps")
@@ -368,6 +389,30 @@ class ModelIR:
         if L.dist in ("binomial_logit",) + DISPERSION_LIKS and L.sigma is not None:
             raise ValueError(f"{L.dist} has no sigma (its parameter is {'trials' if L.dist == 'binomial_logit' else 'alpha'})")
 
+    def _validate_bounds(self, L) -> None:
+        """Bounds of censored / truncated Normal observations (the checks prepare_ir makes, in the same words)."""
+        what = f"{L.dist} likelihood {L.name}"
+        if L.dist not in BOUNDED_LIKS:
+            if L.lower is not None or L.upper is not None:
+                raise ValueError(f"{what}: lower / upper belong to the censored_normal / truncated_normal likelihoods")
+            return
+        N = len(L.y)
+        for side in (L.lower, L.upper):
+            if isinstance(side, Ref):
+                raise ValueError(f"{what}: lower and upper are data (None, a constant or one per observation), not variables")
+            if side is not None and not (np.ndim(side) == 0 or (np.ndim(side) == 1 and len(side) == N)):
+                raise ValueError(f"{what}: lower and upper must be None, a constant or one value per observation (N = {N})")
+        lo, hi = L.bounds()
+        y = np.asarray(L.y, dtype=np.float64)
+        if np.any(np.isnan(lo) | np.isnan(hi) | (lo == np.inf) | (hi == -np.inf)):
+            raise ValueError(f"{what}: {BOUND_SIDES}")
+        if not np.all(lo < hi):
+            raise ValueError(f"{what}: {BOUND_ORDER}")
+        if not (np.all(np.isfinite(y)) and np.all((lo <= y) & (y <= hi))):
+            raise ValueError(f"{what}: {BOUND_Y}")
+        if L.dist == "truncated_normal" and not np.any(np.isfinite(lo) | np.isfinite(hi)):
+            raise ValueError(f"{what}: {TRUNC_OPEN}")
+
     # ---- host-side post-processing (f1): unconstrained draws -> named constrained RVs --------------------------------
     def constrain(self, q: np.ndarray) -> dict:
         out, off = {}, self.offsets()
@@ -426,6 +471,9 @@ class ModelIR:
                         out[f"{L.name}_{vn}_idx"] = np.asarray(idx)
             if L.trials is not None and np.ndim(L.trials) == 1:
                 out[f"{L.name}_trials"] = np.asarray(L.trials)
+            for side in ("lower", "upper"):  # per-observation bounds of censored / truncated observations
+                if np.ndim(getattr(L, side)) == 1:
+                    out[f"{L.name}_{side}"] = np.asarray(getattr(L, side))
         return out
 
 
@@ -597,6 +645,55 @@ def gamma_regression_ir(n_obs: int = 200, n_features: int = 3, seed: int = 37, a
                    likelihoods=[Likelihood("gamma_log", y, terms, alpha=Ref("alpha_log__") if alpha is None else float(alpha))])
 
 
+def censored_regression_ir(n_obs: int = 400, n_groups: int = 8, n_features: int = 3, seed: int = 43) -> ModelIR:
+    """Tobit-style regression on simulated data: a_g ~ Normal(mu_a, sigma_a) (centred), beta ~ Normal(0, 1)^K as a design
+    term, sigma ~ HalfNormal(1), y*_i = a[g_i] + x_i . beta + sigma e_i recorded as y_i = clip(y*_i, lower, upper_i):
+    left-censored at one detection limit for all observations and right-censored at each observation's own follow-up limit."""
+    rng = np.random.default_rng(seed)
+    g = rng.integers(0, n_groups, n_obs).astype(np.int32)
+    X = rng.standard_normal((n_obs, n_features))
+    a = rng.normal(0.5, 0.6, n_groups)
+    ystar = a[g] + X @ rng.normal(0.0, 0.7, n_features) + 0.8 * rng.standard_normal(n_obs)
+    lower = float(np.quantile(ystar, 0.2))  # the detection limit
+    upper = lower + rng.uniform(1.2, 4.0, n_obs)  # follow-up limits
+    y = np.clip(ystar, lower, upper)
+    return ModelIR(
+        name="censored_regression",
+        vars=[Var("mu_a", "mu_a", 1), Var("sigma_a_log__", "sigma_a", 1, "log"), Var("a", "a", n_groups),
+              Var("beta", "beta", n_features), Var("sigma_log__", "sigma", 1, "log")],
+        priors=[Prior("normal", "mu_a", (0.0, 2.0)), Prior("halfnormal", "sigma_a_log__", (1.0,)),
+                Prior("normal", "a", (Ref("mu_a"), Ref("sigma_a_log__"))), Prior("normal", "beta", (0.0, 1.0)),
+                Prior("halfnormal", "sigma_log__", (1.0,))],
+        likelihoods=[Likelihood("censored_normal", y, [Term([("a", g)]), Term([("beta", None)], coef=X)],
+                                sigma=Ref("sigma_log__"), lower=lower, upper=upper)],
+    )
+
+
+def truncated_regression_ir(n_obs: int = 300, n_features: int = 2, seed: int = 47) -> ModelIR:
+    """Regression on data recorded only above a threshold: b0 ~ Normal(0, 5), beta ~ Normal(0, 1)^K as a design term,
+    sigma ~ HalfNormal(1), y_i ~ TruncatedNormal(b0 + x_i . beta, sigma, lower=threshold, upper=upper_i), where a third of the
+    observations also carry an upper bound of their own (+inf for the rest)."""
+    rng = np.random.default_rng(seed)
+    X = rng.standard_normal((n_obs, n_features))
+    eta = 0.4 + X @ (rng.normal(0.0, 0.8, n_features) * np.sqrt(2.0 / max(n_features, 2)))  # sd of eta ~ 0.8 for any K
+    lower = 0.0
+    upper = np.where(rng.random(n_obs) < 1 / 3, rng.uniform(0.5, 2.5, n_obs), np.inf)
+    y = np.empty(n_obs)
+    for i in range(n_obs):  # rejection sampling from each observation's truncated Normal
+        while True:
+            v = eta[i] + 1.1 * rng.standard_normal()
+            if lower < v < upper[i]:
+                y[i] = v
+                break
+    return ModelIR(
+        name="truncated_regression",
+        vars=[Var("b0", "b0", 1), Var("beta", "beta", n_features), Var("sigma_log__", "sigma", 1, "log")],
+        priors=[Prior("normal", "b0", (0.0, 5.0)), Prior("normal", "beta", (0.0, 1.0)), Prior("halfnormal", "sigma_log__", (1.0,))],
+        likelihoods=[Likelihood("truncated_normal", y, [Term([("b0", None)]), Term([("beta", None)], coef=X)],
+                                sigma=Ref("sigma_log__"), lower=lower, upper=upper)],
+    )
+
+
 # ------------------------------------------------------------------------------------------------------------------------
 # lowering: ModelIR -> flat arrays of the C ABI (include/b200nuts.h: b200_ir)
 # ------------------------------------------------------------------------------------------------------------------------
@@ -610,6 +707,7 @@ class LoweredIR:
     priors: list            # [(dist, var, [(kind, value, ref_offset)] * 3)]
     liks: list              # [dict(dist, N, y, terms=[dict(coef, factors=[(offset, size, idx)])], sigma_kind, sigma_value, sigma_ref, sigma_obs, nu, y_var)]
                             # a design term's dict also has n_cols = K, with coef = X [N][K]
+                            # censored_normal / truncated_normal: y is the [3][N] block (y, lower, upper)
                             # y_var 0: y is observed data; v + 1: a latent factor, y is None and its values are variable v's
     ar1: list               # [(var, phi(kind, value, ref), sigma(kind, value, ref), init_sigma)]
 
@@ -681,7 +779,10 @@ def lower(ir: ModelIR) -> LoweredIR:
     for L in ir.likelihoods:
         # the likelihood's one parameter slot: sigma, or the trials / alpha of the count and positive families
         par = L.trials if L.dist == "binomial_logit" else (L.alpha if L.dist in DISPERSION_LIKS else L.sigma)
-        liks.append(dict(dist=LIK_DISTS[L.dist], N=len(L.y), y=np.ascontiguousarray(L.y, dtype=np.float64),
+        y = np.ascontiguousarray(L.y, dtype=np.float64)
+        if L.dist in BOUNDED_LIKS:  # the [3][N] block: y, lower, upper
+            y = np.ascontiguousarray(np.stack([y, *L.bounds()]))
+        liks.append(dict(dist=LIK_DISTS[L.dist], N=len(L.y), y=y,
                          terms=_lower_terms(ir, L.terms, len(L.y), off), nu=float(L.nu), y_var=0,
                          **_lower_slot(ir, par, off)))
     # latent factors after the observed likelihoods, so that observed likelihood i keeps index i

@@ -66,6 +66,12 @@ extern "C" {
 #define B200_IR_T_NONE 0
 #define B200_IR_T_LOG 1
 #define B200_IR_T_INTERVAL 2
+/* Ordered (transforms.py:79-120), ascending: x_0 = z_0 (ORDERED_POSITIVE: exp z_0), x_k = x_{k-1} + exp z_k; log|J| =
+ * sum_{k>=1} z_k (ORDERED_POSITIVE: sum_k z_k).  Not elementwise: the draws of a model with such a variable are constrained
+ * on the host.  An ordered variable takes only real-line priors (flat, normal, studentt, cauchy, or a latent normal /
+ * studentt); ORDERED_POSITIVE also counts as positive support. */
+#define B200_IR_T_ORDERED 3
+#define B200_IR_T_ORDERED_POSITIVE 4
 /* prior densities (pymc/distributions/continuous.py): parameters in p[0..2] */
 #define B200_IR_P_FLAT 0        /*                       :364-419   */
 #define B200_IR_P_NORMAL 1      /* mu, sigma             :526-527   */
@@ -101,6 +107,14 @@ extern "C" {
  *                     standardised bounds (a one-sided form where one side is open) */
 #define B200_IR_L_CENSORED_NORMAL 8  /* logprob/censoring.py:213-248 over Normal; dist_math.py:126-142 */
 #define B200_IR_L_TRUNCATED_NORMAL 9 /* TruncatedNormal.logp continuous.py:720-747; dist_math.py:126-182 */
+/* Ordinal observations y_i in 0..K-1 with K - 1 cutpoints c: log(F(b) - F(a)), a = (c_{y-1} - eta) / s,
+ * b = (c_y - eta) / s, c_{-1} = -inf, c_{K-1} = +inf; F the logistic CDF (s = 1) or the standard Normal one.
+ *   nu             K >= 2
+ *   terms[n_terms] the cutpoint term, one past the predictor's: one unindexed factor on a variable of size K - 1 (ordered
+ *                  unless K = 2), or n_factors = 0 and coef = the K - 1 constants, finite and strictly increasing
+ *   sigma          ORDERED_LOGISTIC: NONE; ORDERED_PROBIT: as for NORMAL (CONST, REF or OBS) */
+#define B200_IR_L_ORDERED_LOGISTIC 10 /* pm.OrderedLogistic discrete.py:1231-1326 as Categorical.logp :1190-1206 */
+#define B200_IR_L_ORDERED_PROBIT 11   /* pm.OrderedProbit discrete.py:1329-1432 as Categorical.logp :1190-1206   */
 /* The support rule b200_model_create enforces (as ModelIR.validate does): HalfNormal, HalfCauchy, Exponential, Gamma and
  * LogNormal priors sit on a LOG variable or an INTERVAL with lo >= 0, Beta on an INTERVAL inside [0, 1], Uniform(a, b) on an
  * INTERVAL inside [a, b]; every scale (a prior's sigma / beta / lam, Normal and StudentT sigma including each sigma_obs, an

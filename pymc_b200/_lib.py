@@ -116,8 +116,9 @@ def build_ir(low):
             pri[k].p[a] = param(pars[a])
     liks = (IrLik * max(1, len(low.liks)))()
     for k, L in enumerate(low.liks):
-        terms = (IrTerm * len(L["terms"]))()
-        for t, T in enumerate(L["terms"]):
+        all_terms = L["terms"] + ([L["cut"]] if "cut" in L else [])  # an ordinal likelihood's cutpoint term goes last
+        terms = (IrTerm * len(all_terms))()
+        for t, T in enumerate(all_terms):
             terms[t].coef = addr(T["coef"])
             terms[t].n_factors = len(T["factors"])
             terms[t].n_cols = int(T.get("n_cols", 0))  # > 0: a design term, coef = X [N][n_cols]

@@ -129,7 +129,8 @@ struct b200_model {
     const double* tr_hi = nullptr;
     IrModel::Params ir{};
     long long ir_max_obs = 0;
-    bool ir_bounded = false;  // a censored / truncated Normal likelihood: the kernels run IrBoundedModel
+    bool ir_extended = false;  // a censored / truncated Normal or ordinal likelihood, or an ordered variable: the kernels
+                               // run IrExtendedModel
     DevBuf ir_scratch;  // per-team scratch of the generic IR device function: [teams][n_pad + max N] doubles
     // lock-step (GEMM-shaped) models; every matrix is row-major with rows `ld` doubles apart (n rounded up to 4, zero pad)
     long long ld = 0;
@@ -362,7 +363,9 @@ static int ir_param(const b200_ir_param& p, int n, IrParamD* out, const char* wh
 // The support rule (pymc_b200/ir.py: ModelIR.validate, same wording): the device evaluates a density's formula wherever
 // it is asked to, so a variable must be kept inside its prior's support by its transform, and every scale parameter must
 // be positive.  A variable has positive support under a log transform or an interval with lo >= 0.
-static bool ir_positive_support(const IrVarD& V) { return V.transform == IRT_LOG || (V.transform == IRT_INTERVAL && V.lo >= 0); }
+static bool ir_positive_support(const IrVarD& V) {
+    return V.transform == IRT_LOG || V.transform == IRT_ORDERED_POSITIVE || (V.transform == IRT_INTERVAL && V.lo >= 0);
+}
 
 // A scale slot (a prior's sigma / beta / lam, a likelihood's sigma, an AR(1) sigma, a dispersion alpha): a finite constant
 // > 0, or a reference to a scalar variable with positive support.
@@ -378,6 +381,14 @@ static bool ir_scale_ok(const b200_ir_param& p, const std::vector<IrVarD>& vars)
 #define B200_IR_BOUND_ORDER "lower < upper must hold for every observation"
 #define B200_IR_BOUND_Y "y must be finite and lie in [lower, upper] for every observation"
 #define B200_IR_TRUNC_OPEN "truncated_normal needs a finite lower or upper bound; with neither side bounded, write the likelihood as normal"
+// Ordered variables and ordinal observations (ModelIR.validate, same wording)
+#define B200_IR_ORDERED_PRIOR "an ordered variable takes only real-line priors (flat, normal, studentt, cauchy, or a latent normal / studentt); ordered_positive also admits the positive priors"
+#define B200_IR_ORD_K "an ordinal likelihood needs K >= 2 categories"
+#define B200_IR_ORD_Y "y must be integers in [0, K - 1]"
+#define B200_IR_CUT_SIZE "the cutpoint variable must have size K - 1"
+#define B200_IR_CUT_ORDERED "a cutpoint variable of size > 1 needs an ordered transform"
+#define B200_IR_CUT_CONST "constant cutpoints must be finite and strictly increasing"
+#define B200_IR_LOGISTIC_SIGMA "ordered_logistic has no sigma"
 
 static int prepare_ir(b200_model* m, const b200_model_desc* d) {
     const b200_ir* R = d->ir;
@@ -389,7 +400,8 @@ static int prepare_ir(b200_model* m, const b200_model_desc* d) {
     for (int v = 0; v < R->n_vars; ++v) {
         const b200_ir_var& V = R->vars[v];
         if (V.offset != off || V.size <= 0) return fail("ir: variable %d: offsets must be contiguous in registration order", v);
-        if (V.transform < B200_IR_T_NONE || V.transform > B200_IR_T_INTERVAL) return fail("ir: variable %d: transform %d", v, V.transform);
+        if (V.transform < B200_IR_T_NONE || V.transform > B200_IR_T_ORDERED_POSITIVE) return fail("ir: variable %d: transform %d", v, V.transform);
+        m->ir_extended = m->ir_extended || V.transform >= B200_IR_T_ORDERED;
         if (V.transform == B200_IR_T_INTERVAL && !(V.lo < V.hi)) return fail("ir: variable %d: interval needs lo < hi", v);
         vars[v] = IrVarD{V.offset, V.size, V.transform, 0, V.lo, V.hi};
         off += V.size;
@@ -416,6 +428,10 @@ static int prepare_ir(b200_model* m, const b200_model_desc* d) {
         if (scale >= 0 && !ir_scale_ok(F.p[scale], vars)) return fail("ir: prior %d: parameter %d (the scale) " B200_IR_SCALE_RULE, k, scale);
         const bool positive = F.dist == B200_IR_P_HALFNORMAL || F.dist == B200_IR_P_HALFCAUCHY || F.dist == B200_IR_P_EXPONENTIAL ||
                               F.dist == B200_IR_P_GAMMA || F.dist == B200_IR_P_LOGNORMAL;
+        const bool real_line = F.dist == B200_IR_P_FLAT || F.dist == B200_IR_P_NORMAL || F.dist == B200_IR_P_STUDENTT ||
+                               F.dist == B200_IR_P_CAUCHY;
+        if (PV.transform >= IRT_ORDERED && !(real_line || (positive && PV.transform == IRT_ORDERED_POSITIVE)))
+            return fail("ir: prior %d: " B200_IR_ORDERED_PRIOR, k);
         if (positive && !ir_positive_support(PV))
             return fail("ir: prior %d: the variable needs a log transform or an interval with lo >= 0 (positive support)", k);
         switch (F.dist) {
@@ -451,7 +467,7 @@ static int prepare_ir(b200_model* m, const b200_model_desc* d) {
     }
     std::vector<IrLikD> liks(std::max(R->n_liks, 0));
     std::vector<IrTermD> terms;
-    long long max_obs = 0;
+    long long max_obs = 0, ord_obs = 0;  // ord_obs: the largest N of an ordinal likelihood (its w row)
     bool has_design = false;
     for (int l = 0; l < R->n_liks; ++l) {
         const b200_ir_lik& L = R->liks[l];
@@ -571,12 +587,24 @@ static int prepare_ir(b200_model* m, const b200_model_desc* d) {
                 // -log(2 pi) / 2 of every Normal density term: each uncensored observation, every truncated one
                 D.c0 = -(double)(cens ? n_observed : N) * B200_HALF_LOG_2PI;
                 if (cens ? upload(m, code, &D.cens) : upload_raw(m, lo, 2 * (size_t)N, &D.bnd)) return -1;
-                m->ir_bounded = true;
+                m->ir_extended = true;
+            } break;
+            case B200_IR_L_ORDERED_LOGISTIC: case B200_IR_L_ORDERED_PROBIT: {  // nu = K; the cutpoint term at terms[n_terms]
+                const double K = L.nu;
+                if (!(K >= 2 && K == std::floor(K) && K <= 0x7fffffff)) return fail("ir: likelihood %d: " B200_IR_ORD_K, l);
+                for (long long i = 0; i < N; ++i)
+                    if (!(L.y[i] >= 0 && L.y[i] <= K - 1) || L.y[i] != std::floor(L.y[i]))
+                        return fail("ir: likelihood %d: " B200_IR_ORD_Y " (at %lld)", l, i);
+                if (L.dist == B200_IR_L_ORDERED_LOGISTIC && L.sigma_kind != B200_IR_S_NONE)
+                    return fail("ir: likelihood %d: " B200_IR_LOGISTIC_SIGMA, l);
+                ord_obs = std::max(ord_obs, N);
+                m->ir_extended = true;
             } break;
             default: return fail("ir: likelihood %d: density %d is not in the closed set", l, L.dist);
         }
+        const bool ordinal = L.dist == B200_IR_L_ORDERED_LOGISTIC || L.dist == B200_IR_L_ORDERED_PROBIT;
         const bool has_sigma = L.dist == B200_IR_L_NORMAL || L.dist == B200_IR_L_STUDENTT || L.dist == B200_IR_L_CENSORED_NORMAL ||
-                               L.dist == B200_IR_L_TRUNCATED_NORMAL;
+                               L.dist == B200_IR_L_TRUNCATED_NORMAL || L.dist == B200_IR_L_ORDERED_PROBIT;
         if (has_sigma && L.sigma_kind == B200_IR_S_NONE)
             return fail("ir: likelihood %d needs sigma", l);
         if (has_sigma) {
@@ -637,6 +665,39 @@ static int prepare_ir(b200_model* m, const b200_model_desc* d) {
             }
             terms.push_back(TD);
         }
+        if (ordinal) {  // the cutpoint term: one unindexed factor on a variable of size K - 1, or K - 1 constants in coef
+            const int K = (int)L.nu;
+            const b200_ir_term& T = L.terms[L.n_terms];
+            IrTermD TD{};
+            if (T.n_cols != 0 || T.n_factors < 0 || T.n_factors > 1)
+                return fail("ir: likelihood %d: the cutpoint term is one variable or K - 1 constants", l);
+            if (T.n_factors == 1) {
+                const b200_ir_factor& F = T.f[0];
+                const IrVarD* V = nullptr;
+                for (const IrVarD& U : vars)
+                    if (U.offset == F.offset) V = &U;
+                if (F.idx || !V || V->size != F.size) return fail("ir: likelihood %d: the cutpoint factor must be a whole variable, unindexed", l);
+                if (F.size != K - 1) return fail("ir: likelihood %d: " B200_IR_CUT_SIZE " (%d, K = %d)", l, F.size, K);
+                if (F.size > 1 && V->transform != IRT_ORDERED && V->transform != IRT_ORDERED_POSITIVE)
+                    return fail("ir: likelihood %d: " B200_IR_CUT_ORDERED, l);
+                // the observations of each category, ascending: category k's are rowobs[rowptr[k] .. rowptr[k + 1])
+                std::vector<int> rowptr(K + 1, 0), rowobs((size_t)N);
+                for (long long i = 0; i < N; ++i) ++rowptr[(int)L.y[i] + 1];
+                for (int k = 0; k < K; ++k) rowptr[k + 1] += rowptr[k];
+                std::vector<int> fill(rowptr.begin(), rowptr.end() - 1);
+                for (long long i = 0; i < N; ++i) rowobs[fill[(int)L.y[i]]++] = (int)i;
+                TD.n_factors = 1;
+                TD.f[0] = IrFactorD{F.offset, F.size, nullptr, nullptr, nullptr};
+                if (upload(m, rowptr, &TD.f[0].rowptr) || upload(m, rowobs, &TD.f[0].rowobs)) return -1;
+            } else {
+                if (!T.coef) return fail("ir: likelihood %d: " B200_IR_CUT_CONST, l);
+                for (int k = 0; k < K - 1; ++k)
+                    if (!std::isfinite(T.coef[k]) || (k > 0 && !(T.coef[k] > T.coef[k - 1])))
+                        return fail("ir: likelihood %d: " B200_IR_CUT_CONST " (at %d)", l, k);
+                if (upload_raw(m, T.coef, (size_t)K - 1, &TD.coef)) return -1;
+            }
+            terms.push_back(TD);
+        }
         liks[l] = D;
     }
     std::vector<IrAr1D> ars(std::max(R->n_ar1, 0));
@@ -656,7 +717,8 @@ static int prepare_ir(b200_model* m, const b200_model_desc* d) {
         upload(m, ars, &P.ar1))
         return -1;
     P.n_pad = (n + 3) & ~3;
-    P.stride = P.n_pad + ((max_obs + 3) & ~3LL) + (has_design ? kIrPartDoubles : 0);
+    P.ord_row = ord_obs ? (int)(P.n_pad + ((max_obs + 3) & ~3LL)) : 0;  // after r, before the design partials
+    P.stride = P.n_pad + ((max_obs + 3) & ~3LL) + ((ord_obs + 3) & ~3LL) + (has_design ? kIrPartDoubles : 0);
     m->ir_max_obs = max_obs;
     return 0;
 }
@@ -778,9 +840,9 @@ static int dispatch(const b200_model* m, F&& f) {
             B200_TEAM(StochVolModel, m->stochvol)
             return fail("stochvol: n=%d exceeds 4096", m->n);
         case B200_MODEL_IR:
-            if (m->ir_bounded) {  // a censored / truncated Normal likelihood: the kernels that can evaluate it
-                if (m->n <= 256 && !env_flag("B200_FORCE_TEAM")) { B200_WARP(IrBoundedModel, m->ir) }
-                B200_TEAM(IrBoundedModel, m->ir)
+            if (m->ir_extended) {  // a censored / truncated Normal likelihood: the kernels that can evaluate it
+                if (m->n <= 256 && !env_flag("B200_FORCE_TEAM")) { B200_WARP(IrExtendedModel, m->ir) }
+                B200_TEAM(IrExtendedModel, m->ir)
             } else {
                 if (m->n <= 256 && !env_flag("B200_FORCE_TEAM")) { B200_WARP(IrModel, m->ir) }
                 B200_TEAM(IrModel, m->ir)
@@ -1654,7 +1716,7 @@ extern "C" int b200_pointwise_loglik(b200_model* m, int32_t lik, const double* d
     CU(m->ir_scratch.reserve((size_t)blocks * wpb * (size_t)m->ir.stride * sizeof(double)));
     m->ir.scratch = m->ir_scratch.as<double>();
     Timer t(st);
-    if (m->ir_bounded)
+    if (m->ir_extended)
         ir_pointwise_kernel<true><<<blocks, wpb * 32, 0, st>>>(m->ir, lik, D, d_draws, d_out);
     else
         ir_pointwise_kernel<false><<<blocks, wpb * 32, 0, st>>>(m->ir, lik, D, d_draws, d_out);

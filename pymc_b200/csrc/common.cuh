@@ -87,7 +87,7 @@ __device__ __forceinline__ NormalTail normal_tail(double z) {
 // D = erfcx(y) - e^(y^2 - x^2) erfcx(x); both in the lower tail (x < 0) the mirror image; else (erf(x) - erf(y)) / 2.
 // y^2 - x^2 is formed as (y - x)(y + x): a narrow window far in a tail keeps its width to rounding.  An open side
 // (a = -inf or b = +inf) takes the one-sided form, which is what the two-sided one reduces to there.  Only the kernels
-// of csrc/ir_model.cuh's IrBoundedModel reach these helpers (DESIGN.md 6).
+// of csrc/ir_model.cuh's IrExtendedModel reach these helpers (DESIGN.md 6).
 struct NormalMass { double log_z, ra, rb; };
 __device__ __forceinline__ NormalMass normal_log_mass(double a, double b) {
     if (a == -INFINITY) {

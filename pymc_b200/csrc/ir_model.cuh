@@ -22,11 +22,12 @@
 
 namespace b200 {
 
-enum { IRT_NONE = 0, IRT_LOG = 1, IRT_INTERVAL = 2 };
+enum { IRT_NONE = 0, IRT_LOG = 1, IRT_INTERVAL = 2, IRT_ORDERED = 3, IRT_ORDERED_POSITIVE = 4 };
 enum { IRP_FLAT = 0, IRP_NORMAL, IRP_HALFNORMAL, IRP_CAUCHY, IRP_HALFCAUCHY, IRP_EXPONENTIAL, IRP_STUDENTT, IRP_UNIFORM,
        IRP_GAMMA, IRP_BETA, IRP_LOGNORMAL };
 enum { IRL_NORMAL = 0, IRL_BERNOULLI_LOGIT, IRL_POISSON_LOG, IRL_STUDENTT, IRL_NORMAL_LOGVAR, IRL_BINOMIAL_LOGIT,
-       IRL_NEGBINOMIAL_LOG, IRL_GAMMA_LOG, IRL_CENSORED_NORMAL, IRL_TRUNCATED_NORMAL };
+       IRL_NEGBINOMIAL_LOG, IRL_GAMMA_LOG, IRL_CENSORED_NORMAL, IRL_TRUNCATED_NORMAL, IRL_ORDERED_LOGISTIC,
+       IRL_ORDERED_PROBIT };
 enum { IRS_NONE = 0, IRS_CONST, IRS_REF, IRS_OBS };
 constexpr double kNegBinPoissonAlpha = 1e10;  // above: NegativeBinomial -> Poisson(mu) limit (discrete.py:727-735)
 
@@ -136,7 +137,7 @@ __device__ __forceinline__ IrBoundedTerm ir_bounded_term(const IrLikD& L, int i,
     return {-0.5 * z * z - log(sg) - M.log_z, (z + M.rb - M.ra) / sg, (z * z - 1.0 + tb - ta) / sg};
 }
 
-// The observation loop of a censored / truncated Normal likelihood, out of line: IrBoundedModel::eval calls it once per
+// The observation loop of a censored / truncated Normal likelihood, out of line: IrExtendedModel::eval calls it once per
 // such likelihood, so the erfcx() tail math stays out of eval's own observation loop.  Writes r_i = d logp / d eta_i;
 // returns this thread's partial sums of logp and d logp / d sigma.
 struct IrPartials { double lp, s_sig; };
@@ -163,17 +164,129 @@ __device__ __noinline__ double ir_bounded_loglik(const IrLikD& L, int i, double 
     return ir_bounded_term(L, i, eta, sg).lp - (at_bound ? 0.0 : B200_HALF_LOG_2PI);
 }
 
-// IrModel evaluates every factor of the closed set except the censored / truncated Normal likelihoods; IrBoundedModel (below)
-// is the same function with those two added.  A kernel's register allocation covers every function it can reach, and the
-// tail math takes about 128 registers, so the engine instantiates its kernels twice and runs a model on IrBoundedModel only
-// when it has such a likelihood (b200_model.ir_bounded): every other IR model keeps the kernels it had before.
+// ---- ordinal observations: OrderedLogistic / OrderedProbit (discrete.py:1231-1432) as the Categorical they build
+// (Categorical.logp, :1190-1206).  K = L.nu categories, y_i in 0..K-1; the K-1 cutpoints c are terms[term0 + n_terms]:
+// one unindexed factor on a variable of size K-1 (f[0].rowptr / rowobs: the observations of each category, ascending), or
+// no factor and coef = the constants.  With a = (c_{y-1} - eta) / s, b = (c_y - eta) / s (c_{-1} = -inf, c_{K-1} = +inf;
+// s = 1 for the logistic link), log p = log(F(b) - F(a)):
+//   logistic  -softplus(-b) - softplus(a) + log1mexp(a - b), the gap b - a taken from the cutpoints themselves, and the
+//             one-sided form at an end category;
+//   probit    normal_log_mass(a, b).
+// The reference forms p in probability space (compute_p, :1312-1326 / :1416-1432) and takes its log, so it returns -inf
+// where F(b) - F(a) underflows or cancels; this stays finite for every finite eta.
+// Returns lp, rs = s d lp / d eta, w = d lp / d c_y (so d lp / d c_{y-1} = -rs / s - w) and ds = d lp / d s.
+struct IrOrdinalTerm { double lp, rs, w, ds; };
+__device__ __forceinline__ IrOrdinalTerm ir_ordinal_term(const IrLikD& L, const IrTermD& C, const double* x, int i, double eta,
+                                                         double s) {
+    const int K = (int)L.nu, y = (int)L.y[i];
+    const double* c = C.n_factors ? x + C.f[0].offset : C.coef;
+    const bool lo_open = y == 0, hi_open = y == K - 1;
+    const double a = lo_open ? -INFINITY : (c[y - 1] - eta) / s, b = hi_open ? INFINITY : (c[y] - eta) / s;
+    if (L.dist == IRL_ORDERED_PROBIT) {
+        const NormalMass M = normal_log_mass(a, b);
+        const double ta = M.ra == 0.0 ? 0.0 : a * M.ra, tb = M.rb == 0.0 ? 0.0 : b * M.rb;  // inf * 0 = 0
+        return {M.log_z, M.ra - M.rb, M.rb / s, (ta - tb) / s};
+    }
+    const double sa = lo_open ? 0.0 : sigmoid(a), sb = hi_open ? 0.0 : sigmoid(-b);  // F(a), 1 - F(b)
+    double lp = (lo_open ? 0.0 : -softplus(a)) + (hi_open ? 0.0 : -softplus(-b)), w = sb;
+    if (!lo_open && !hi_open) {
+        const double gap = (c[y] - c[y - 1]) / s;  // b - a without the cancellation of forming it from a and b
+        lp += log(-expm1(-gap));
+        w += 1.0 / expm1(gap);
+    }
+    return {lp, sa - sb, w, 0.0};
+}
+
+// The observation loop of an ordinal likelihood, out of line like ir_bounded_pass.  Writes r_i = d logp / d eta_i and
+// w_i = d logp / d c_{y_i}; returns this thread's partial sums of logp and d logp / d sigma.
+template <int W>
+__device__ __noinline__ IrPartials ir_ordinal_pass(const IrLikD* Lp, const IrTermD* terms, const double* x, double* r,
+                                                   double* w, double sg_s, int tid) {
+    constexpr int TS = 32 * W;
+    const IrLikD& L = *Lp;
+    const int N = (int)L.N;
+    const IrTermD& C = terms[L.term0 + L.n_terms];
+    double lp = 0.0, s_sig = 0.0;
+    for (int i = tid; i < N; i += TS) {
+        const double eta = ir_eta(terms + L.term0, L.n_terms, x, i, N);
+        const double s = L.sigma_kind == IRS_OBS ? L.sigma_obs[i] : (L.sigma_kind == IRS_NONE ? 1.0 : sg_s);
+        const IrOrdinalTerm o = ir_ordinal_term(L, C, x, i, eta, s);
+        lp += o.lp;
+        s_sig += o.ds;
+        r[i] = o.rs / s;
+        w[i] = o.w;
+    }
+    return {lp, s_sig};
+}
+
+// d logp / d c_k = sum of w_i over category k + sum of (-r_i - w_i) over category k + 1, each over the category's
+// observations in ascending order (the CSR of the cutpoint term), one thread per cutpoint: no atomics, a fixed order.
+template <int W>
+__device__ __noinline__ void ir_cutpoint_grad(const IrLikD* Lp, const IrTermD* terms, const double* r, const double* w,
+                                              double* g, int tid) {
+    constexpr int TS = 32 * W;
+    const IrLikD& L = *Lp;
+    const IrFactorD& F = terms[L.term0 + L.n_terms].f[0];
+    for (int k = tid; k < F.size; k += TS) {
+        double a = 0.0;
+        for (int e = F.rowptr[k]; e < F.rowptr[k + 1]; ++e) a += w[F.rowobs[e]];
+        for (int e = F.rowptr[k + 1]; e < F.rowptr[k + 2]; ++e) {
+            const int i = F.rowobs[e];
+            a -= r[i] + w[i];
+        }
+        g[F.offset + k] += a;
+    }
+}
+
+// the pointwise pass's share: log p(y_i | eta), which has no constant
+__device__ __noinline__ double ir_ordinal_loglik(const IrLikD& L, const IrTermD* terms, const double* x, int i, double eta) {
+    const double s = L.sigma_kind == IRS_NONE ? 1.0 : (L.sigma_kind == IRS_OBS ? L.sigma_obs[i] : (L.sigma_kind == IRS_REF ? x[L.sigma.ref] : L.sigma.value));
+    return ir_ordinal_term(L, terms[L.term0 + L.n_terms], x, i, eta, s).lp;
+}
+
+// ---- the ordered transform (transforms.py:79-120): x_0 = z_0 (positive: e^{z_0}), x_k = x_{k-1} + e^{z_k}; log|J| =
+// sum_{k>=1} z_k (positive: sum_k z_k).  Not elementwise, so one thread of the team runs it, k ascending (np.cumsum's
+// order): O(size) serial work per evaluation, for vectors as short as cutpoints are.
+__device__ __noinline__ double ir_ordered_forward(const IrVarD* Vp, const double* q, double* x) {
+    const int o = Vp->offset, n = Vp->size;
+    const bool pos = Vp->transform == IRT_ORDERED_POSITIVE;
+    double acc = pos ? exp(q[o]) : q[o], lj = pos ? q[o] : 0.0;
+    x[o] = acc;
+    for (int k = 1; k < n; ++k) {
+        const double z = q[o + k];
+        acc += exp(z);
+        lj += z;
+        x[o + k] = acc;
+    }
+    return lj;
+}
+
+// The chain rule through it, in place on g: d/dz_j = e^{z_j} sum_{k>=j} g_k + 1 for j >= 1 (and j = 0 when positive), and
+// d/dz_0 = sum_k g_k otherwise.  The reverse cumulative sum runs k descending, on one thread.
+__device__ __noinline__ void ir_ordered_chain(const IrVarD* Vp, const double* q, double* g) {
+    const int o = Vp->offset, n = Vp->size;
+    const bool pos = Vp->transform == IRT_ORDERED_POSITIVE;
+    double s = 0.0;
+    for (int k = n - 1; k >= 0; --k) {
+        s += g[o + k];
+        g[o + k] = (k == 0 && !pos) ? s : fma(exp(q[o + k]), s, 1.0);
+    }
+}
+
+// IrModel evaluates every factor of the closed set except the censored / truncated Normal and the ordinal likelihoods and
+// the ordered transform; IrExtendedModel (below) is the same function with those added, each out of line.  A kernel's
+// register allocation covers every function it can reach, and the tail math takes about 128 registers, so the engine
+// instantiates its kernels twice and runs a model on IrExtendedModel only when it has one of them (b200_model.ir_extended):
+// every other IR model keeps the kernels it had before.
 struct IrModel {
     struct Params {
         const IrVarD* vars; const IrPriorD* priors; const IrLikD* liks; const IrTermD* terms; const IrAr1D* ar1;
         int n_vars, n_priors, n_liks, n_ar1, n;
         double* scratch;            // [slots][stride]
-        long long stride;           // doubles per team: n_pad + max N (+ kIrPartDoubles with a design term)
+        long long stride;           // doubles per team: n_pad + max N (+ max N with an ordinal likelihood)
+                                    // (+ kIrPartDoubles with a design term)
         int n_pad;
+        int ord_row;                // offset of an ordinal likelihood's w row in the team slice (0: none)
     };
     __host__ __device__ static size_t shared_bytes(const Params&) { return 0; }
     __device__ static void stage(const Params&, char*, uint64_t*) {}
@@ -185,7 +298,7 @@ struct IrModel {
         return eval_impl<NPL, W, false>(P, s, q_s, g_s, tid, red);
     }
 
-    template <int NPL, int W, bool BOUNDED>
+    template <int NPL, int W, bool EXTENDED>
     __device__ __forceinline__ static double eval_impl(const Params& P, const char*, const double* q_s, double* g_s, int tid,
                                                        double* red) {
         constexpr int TS = 32 * W;
@@ -198,6 +311,13 @@ struct IrModel {
         // ---- 1. constrain (+ log-Jacobians); gx accumulates in g_s -----------------------------------------------------
         for (int v = 0; v < P.n_vars; ++v) {
             const IrVarD V = P.vars[v];
+            if constexpr (EXTENDED) {
+                if (V.transform >= IRT_ORDERED) {  // uniform branch: a prefix sum, on one thread
+                    if (tid == 0) lp += ir_ordered_forward(P.vars + v, q_s, x);
+                    for (int j = tid; j < V.size; j += TS) g_s[V.offset + j] = 0.0;
+                    continue;
+                }
+            }
             for (int j = tid; j < V.size; j += TS) {
                 const int i = V.offset + j;
                 const double z = q_s[i];
@@ -296,10 +416,12 @@ struct IrModel {
             const bool disp = L.dist == IRL_NEGBINOMIAL_LOG || L.dist == IRL_GAMMA_LOG;  // sg_s is the dispersion alpha
             const double la = disp ? log(sg_s) : 0.0;
             double s_sig = 0.0;
-            const bool bounded = BOUNDED && (L.dist == IRL_CENSORED_NORMAL || L.dist == IRL_TRUNCATED_NORMAL);
-            if constexpr (BOUNDED) {
+            const bool ordinal = EXTENDED && (L.dist == IRL_ORDERED_LOGISTIC || L.dist == IRL_ORDERED_PROBIT);
+            const bool bounded = EXTENDED && (ordinal || L.dist == IRL_CENSORED_NORMAL || L.dist == IRL_TRUNCATED_NORMAL);
+            if constexpr (EXTENDED) {
                 if (bounded) {  // uniform branch: out of line
-                    const IrPartials b = ir_bounded_pass<W>(P.liks + l, P.terms, x, r, sg_s, tid);
+                    const IrPartials b = ordinal ? ir_ordinal_pass<W>(P.liks + l, P.terms, x, r, x + P.ord_row, sg_s, tid)
+                                                 : ir_bounded_pass<W>(P.liks + l, P.terms, x, r, sg_s, tid);
                     lp += b.lp;
                     s_sig = b.s_sig;
                 }
@@ -404,6 +526,12 @@ struct IrModel {
             }
             if (tid == 0) lp += L.c0;
             team_sync<W>();
+            if constexpr (EXTENDED) {
+                if (ordinal && P.terms[L.term0 + L.n_terms].n_factors) {  // uniform branch: variable cutpoints
+                    ir_cutpoint_grad<W>(P.liks + l, P.terms, r, x + P.ord_row, g_s, tid);
+                    team_sync<W>();
+                }
+            }
             if (L.sigma_kind == IRS_REF) {
                 const double tot = team_sum<W>(s_sig, tid, red);
                 if (tid == 0) g_s[L.sigma.ref] += tot;
@@ -487,6 +615,12 @@ struct IrModel {
         for (int v = 0; v < P.n_vars; ++v) {
             const IrVarD V = P.vars[v];
             if (V.transform == IRT_NONE) continue;
+            if constexpr (EXTENDED) {
+                if (V.transform >= IRT_ORDERED) {  // uniform branch: a reverse prefix sum, on one thread
+                    if (tid == 0) ir_ordered_chain(P.vars + v, q_s, g_s);
+                    continue;
+                }
+            }
             for (int j = tid; j < V.size; j += TS) {
                 const int i = V.offset + j;
                 const double xv = x[i];
@@ -507,7 +641,7 @@ struct IrModel {
     }
 };
 
-struct IrBoundedModel : IrModel {
+struct IrExtendedModel : IrModel {
     template <int NPL, int W, bool SMALL = false>
     __device__ __noinline__ static double eval(const Params& P, const char* s, const double* q_s, double* g_s, int tid, double* red) {
         return eval_impl<NPL, W, true>(P, s, q_s, g_s, tid, red);
@@ -521,7 +655,7 @@ struct IrBoundedModel : IrModel {
 // team scratch slice like in eval().  Elementwise constants (log 2pi, lgamma) are included, unlike in eval() where they are
 // folded into one constant per factor.
 // ---------------------------------------------------------------------------------------------------------------------
-template <bool BOUNDED>  // as IrModel / IrBoundedModel
+template <bool EXTENDED>  // as IrModel / IrExtendedModel
 __global__ void __launch_bounds__(256) ir_pointwise_kernel(const IrModel::Params P, int lik, long long D,
                                                            const double* __restrict__ draws /*[D][n]*/,
                                                            double* __restrict__ out /*[D][N]*/) {
@@ -535,6 +669,12 @@ __global__ void __launch_bounds__(256) ir_pointwise_kernel(const IrModel::Params
         const double* q = draws + d * n;
         for (int v = 0; v < P.n_vars; ++v) {
             const IrVarD V = P.vars[v];
+            if constexpr (EXTENDED) {
+                if (V.transform >= IRT_ORDERED) {
+                    if (lane == 0) ir_ordered_forward(P.vars + v, q, x);
+                    continue;
+                }
+            }
             for (int j = lane; j < V.size; j += 32) {
                 const double z = q[V.offset + j];
                 x[V.offset + j] = V.transform == IRT_LOG ? exp(z) : (V.transform == IRT_INTERVAL ? V.lo + (V.hi - V.lo) * sigmoid(z) : z);
@@ -587,9 +727,11 @@ __global__ void __launch_bounds__(256) ir_pointwise_kernel(const IrModel::Params
                     break;
                 case IRL_GAMMA_LOG: lp = sg_s * (la - eta) - lgamma(sg_s) + (sg_s - 1.0) * log(yi) - sg_s * yi * exp(-eta); break;
                 case IRL_CENSORED_NORMAL: case IRL_TRUNCATED_NORMAL:
-                    if constexpr (BOUNDED) lp = ir_bounded_loglik(L, i, eta, (L.sigma_kind == IRS_OBS) ? L.sigma_obs[i] : sg_s);
+                    if constexpr (EXTENDED) lp = ir_bounded_loglik(L, i, eta, (L.sigma_kind == IRS_OBS) ? L.sigma_obs[i] : sg_s);
                     break;
-                default: break;
+                default:  // the ordinal likelihoods
+                    if constexpr (EXTENDED) lp = ir_ordinal_loglik(L, P.terms, x, i, eta);
+                    break;
             }
             out[d * N + i] = lp;
         }

@@ -15,7 +15,10 @@ pymc/model/fgraph.py:76-81, :139) -- and pattern-matches them onto the closed fa
                      Binomial(n, logit_p = eta) with constant trials, NegativeBinomial(mu = exp(eta), alpha) and
                      Gamma(alpha, beta = alpha / exp(eta) | alpha * exp(-eta)), alpha a constant or a scalar free RV;
                      pm.Censored(pm.Normal.dist(eta, sigma), lower, upper), pm.TruncatedNormal(eta, sigma, lower, upper)
-                     and pm.Truncated(pm.Normal.dist(eta, sigma), lower, upper) with constant bounds
+                     and pm.Truncated(pm.Normal.dist(eta, sigma), lower, upper) with constant bounds;
+                     pm.OrderedLogistic / pm.OrderedProbit: the Categorical whose p is their compute_p graph, with or
+                     without the {name}_probs Deterministic (recorded, evaluated from the draws)
+    transform    ->  None, log, interval, and Ordered() / Ordered(positive=True) -> "ordered" / "ordered_positive"
 
 Anything outside the closed set raises ``NotImplementedError`` naming the offending op, so a model either lowers exactly
 or not at all.  PyMC and PyTensor are NOT importable in the build image (SURVEY 8c); this module imports them lazily and
@@ -109,6 +112,14 @@ def from_pymc(model) -> _ir.ModelIR:
         transform, bounds = None, None
         if tr is None:
             pass
+        elif tname == "chain":
+            raise NotImplementedError(f"{rv.name}: Chain([...]) transforms are outside the closed set (None, log, interval, "
+                                      "ordered)")
+        elif tname == "ordered":  # Ordered(positive, ascending), transforms.py:79-120
+            if not getattr(tr, "ascending", True):
+                raise NotImplementedError(f"{rv.name}: Ordered(ascending=False) is outside the closed set (only ascending "
+                                          "ordered transforms)")
+            transform = "ordered_positive" if getattr(tr, "positive", False) else "ordered"
         elif "log" in tname and "odds" not in tname and "interval" not in tname:
             transform = "log"
         elif "interval" in tname or "logodds" in tname:
@@ -286,6 +297,75 @@ def from_pymc(model) -> _ir.ModelIR:
         except NotImplementedError:
             return False
 
+    def graph_nodes(x):
+        """every variable with an owner in the graph under x"""
+        out, seen, stack = [], set(), [x]
+        while stack:
+            v = stack.pop()
+            if v.owner is None or id(v) in seen:
+                continue
+            seen.add(id(v))
+            out.append(v)
+            stack.extend(v.owner.inputs)
+        return out
+
+    def cutpoints_of(x):
+        """a vector free RV (-> Ref) or a constant 1-D array of cutpoints under DimShuffle layers, else None"""
+        while x.owner is not None and isinstance(x.owner.op, DimShuffle):
+            x = x.owner.inputs[0]
+        if x in name_of:
+            return _ir.Ref(name_of[x])
+        c = _const_value(x)
+        return np.asarray(c, dtype=np.float64) if c is not None and c.ndim == 1 else None
+
+    def ordinal_of(p):
+        """(dist, eta, cutpoints, sigma) of a Categorical p built by OrderedLogistic.compute_p (discrete.py:1312-1326:
+        differences of a concatenation around sigmoid(cutpoints - eta[:, None])) or OrderedProbit.compute_p (:1416-1432:
+        exp of a concatenation of normal_lccdf / log_diff_normal_cdf / normal_lcdf of eta[:, None] - cutpoints, each
+        standardising as (x - 0) / sigma, dist_math.py:126-182), else None"""
+        while p.owner is not None and _is_copy(p.owner):  # the {name}_probs Deterministic (compute_p=True)
+            p = p.owner.inputs[0]
+        if p.owner is None:
+            return None
+        nodes = graph_nodes(p)
+        ops = {scalar_op_name(v.owner) for v in nodes}
+        top = scalar_op_name(p.owner)
+        if top == "sub" and "sigmoid" in ops:
+            for v in nodes:
+                if scalar_op_name(v.owner) == "sigmoid":
+                    inner = v.owner.inputs[0]
+                    if inner.owner is not None and scalar_op_name(inner.owner) == "sub":
+                        c = cutpoints_of(inner.owner.inputs[0])
+                        if c is not None:
+                            return "ordered_logistic", inner.owner.inputs[1], c, None
+            return None
+        if top != "exp" or not ops & {"erfc", "erfcx", "erf"}:
+            return None
+        probits = None
+        for v in nodes:
+            if scalar_op_name(v.owner) == "sub":
+                c = cutpoints_of(v.owner.inputs[1])
+                if c is not None and (isinstance(c, _ir.Ref) or c.size >= 1):
+                    probits = v
+                    break
+        if probits is None:
+            return None
+        sigmas = []
+        for v in nodes:  # (x - mu) / sigma with x a slice of the probits
+            if scalar_op_name(v.owner) in ("truediv", "true_div"):
+                num, den = v.owner.inputs
+                if num.owner is not None and scalar_op_name(num.owner) == "sub" and \
+                        any(w is probits for w in graph_nodes(num.owner.inputs[0])):
+                    sigmas.append(den)
+        if not sigmas:
+            return None
+        s = [param(d.owner.inputs[0] if d.owner is not None and isinstance(d.owner.op, DimShuffle) else d, "sigma")
+             for d in sigmas]
+        if any(t != s[0] for t in s):
+            return None
+        return "ordered_probit", probits.owner.inputs[0], cutpoints_of(probits.owner.inputs[1]), s[0]
+
+    probs_of = {}  # id of a {name}_probs Deterministic's expression -> the ordinal likelihood's name
     liks = []
     for rv in model.observed_RVs:
         y = _const_value(model.rvs_to_values[rv])
@@ -411,12 +491,30 @@ def from_pymc(model) -> _ir.ModelIR:
             if eta is None:
                 raise NotImplementedError(f"{rv.name}: write the likelihood as {form}")
             liks.append(_ir.Likelihood("gamma_log", y, make_terms(eta, N), alpha=alpha, name=rv.name))
+        elif op == "categorical":  # pm.OrderedLogistic / pm.OrderedProbit build Categorical(p = compute_p(eta, cutpoints))
+            form = ("pm.OrderedLogistic(eta, cutpoints) or pm.OrderedProbit(eta, cutpoints, sigma): a Categorical with a "
+                    "free p, logit_p / softmax, or a p of another form is outside the closed set")
+            found = ordinal_of(ps[0])
+            if found is None:
+                raise NotImplementedError(f"{rv.name}: Categorical: only {form}")
+            dist, eta, cut, s = found
+            if isinstance(cut, _ir.Ref) and size_of[cut.var] > 1 and \
+                    next(v for v in vars_ if v.name == cut.var).transform not in _ir.ORDERED_TRANSFORMS:
+                raise NotImplementedError(f"{rv.name}: the cutpoints {cut.var} need transform=pm.distributions.transforms."
+                                          "ordered (unordered vector cutpoints)")
+            liks.append(_ir.Likelihood(dist, y, make_terms(eta, N), sigma=s, cutpoints=cut, name=rv.name))
+            probs_of[id(ps[0])] = rv.name
         else:
             raise NotImplementedError(f"{rv.name}: likelihood {type(rv.owner.op).__name__} is outside the closed set "
                                       f"{sorted(_ir.LIK_DISTS)}")
     # ---- pm.Deterministic: recorded in the posterior, never part of logp -------------------------------------------------
     dets = []
     for dv in getattr(model, "deterministics", []) or []:
+        if id(dv) in probs_of:  # {name}_probs of an ordinal likelihood: evaluated from its own factor
+            L = next(L for L in liks if L.name == probs_of[id(dv)])
+            K = (size_of[L.cutpoints.var] if isinstance(L.cutpoints, _ir.Ref) else len(L.cutpoints)) + 1
+            dets.append(_ir.Deterministic(dv.name, len(L.y) * K, [], probs_of=L.name))
+            continue
         size = _static_size(dv)
         if size is None:
             raise NotImplementedError(f"{dv.name}: the size of this Deterministic is not known statically")

@@ -22,12 +22,20 @@ needs no new CUDA.  Models whose IR matches a hand-specialised kernel (Eight Sch
 from __future__ import annotations
 
 import copy
+import dataclasses
 from dataclasses import dataclass, field
 
 import numpy as np
 
 # ids shared with include/b200nuts.h ------------------------------------------------------------------------------------
-TRANSFORMS = {None: 0, "log": 1, "interval": 2}
+TRANSFORMS = {None: 0, "log": 1, "interval": 2,
+              "ordered": 3, "ordered_positive": 4}  # Ordered() / Ordered(positive=True), transforms.py:79-120
+ORDERED_TRANSFORMS = ("ordered", "ordered_positive")
+# An ordered variable is not constrained elementwise (a cumulative sum): it takes only real-line priors, and
+# ordered_positive also counts as positive support (csrc/b200nuts.cu: prepare_ir, same words)
+REAL_LINE_PRIORS = ("flat", "normal", "studentt", "cauchy")
+ORDERED_PRIOR = ("an ordered variable takes only real-line priors (flat, normal, studentt, cauchy, or a latent normal / "
+                 "studentt); ordered_positive also admits the positive priors")
 # priors: name -> (id, number of parameters)
 PRIOR_DISTS = {
     "flat": (0, 0),          # Flat / HalfFlat: logp 0                                  continuous.py:364-383, :400-419
@@ -54,11 +62,23 @@ LIK_DISTS = {
     "gamma_log": 7,          # y_i ~ Gamma(alpha, beta = alpha exp(-eta_i))             continuous.py:2478-2521
     "censored_normal": 8,    # y_i ~ Censored(Normal(eta_i, sigma), lower, upper)       logprob/censoring.py:213-248
     "truncated_normal": 9,   # y_i ~ TruncatedNormal(eta_i, sigma, lower, upper)        continuous.py:720-747
+    "ordered_logistic": 10,  # y_i ~ OrderedLogistic(eta_i, cutpoints)                  discrete.py:1231-1326, :1190-1206
+    "ordered_probit": 11,    # y_i ~ OrderedProbit(eta_i, cutpoints, sigma)             discrete.py:1329-1432, :1190-1206
 }
+# Ordinal observations: y_i in 0..K-1 and ``Likelihood.cutpoints``, a Ref to a variable of size K - 1 (ordered unless
+# K = 2) or K - 1 constants, finite and strictly increasing; lowered with nu = K and the cutpoint term one past the
+# predictor's terms (include/b200nuts.h)
+ORDINAL_LIKS = ("ordered_logistic", "ordered_probit")
+ORD_K = "an ordinal likelihood needs K >= 2 categories"
+ORD_Y = "y must be integers in [0, K - 1]"
+CUT_SIZE = "the cutpoint variable must have size K - 1"
+CUT_ORDERED = "a cutpoint variable of size > 1 needs an ordered transform"
+CUT_CONST = "constant cutpoints must be finite and strictly increasing"
+LOGISTIC_SIGMA = "ordered_logistic has no sigma"
 # Normal observations with bounds: ``Likelihood.lower`` / ``.upper`` (None, a constant or one value per observation, -inf /
 # +inf where that side is open); lowered as the [3][N] block (y, lower, upper) of include/b200nuts.h
 BOUNDED_LIKS = ("censored_normal", "truncated_normal")
-SIGMA_LIKS = ("normal", "studentt") + BOUNDED_LIKS  # likelihoods whose parameter slot is sigma
+SIGMA_LIKS = ("normal", "studentt") + BOUNDED_LIKS + ("ordered_probit",)  # likelihoods whose parameter slot is sigma
 # the support rule of bounded observations (csrc/b200nuts.cu: prepare_ir, same words)
 BOUND_SIDES = "lower must not be +inf or NaN and upper must not be -inf or NaN"
 BOUND_ORDER = "lower < upper must hold for every observation"
@@ -80,7 +100,16 @@ LINEAR_PRIORS = {"normal": (0, 1), "studentt": (1, 2)}
 
 
 def _positive_support(v) -> bool:
-    return v.transform == "log" or (v.transform == "interval" and v.bounds[0] >= 0.0)
+    return v.transform in ("log", "ordered_positive") or (v.transform == "interval" and v.bounds[0] >= 0.0)
+
+
+def ordered_backward(z: np.ndarray, positive: bool) -> np.ndarray:
+    """Ordered.backward (transforms.py:96-106) along the last axis: x_0 = z_0 (positive: exp z_0), x_k = x_{k-1} + exp z_k,
+    summed in np.cumsum's order (k ascending), as the device does."""
+    d = np.exp(z)
+    if not positive:
+        d[..., 0] = z[..., 0]
+    return np.cumsum(d, axis=-1)
 
 
 def is_design(t) -> bool:
@@ -154,6 +183,13 @@ class Likelihood:
     trials: float | np.ndarray | None = None   # binomial_logit: number of trials, one for all or one per observation
     lower: float | np.ndarray | None = None    # censored_normal / truncated_normal: None (open), a constant or one per
     upper: float | np.ndarray | None = None    # observation, -inf / +inf where that observation's side is open
+    cutpoints: Ref | np.ndarray | None = None  # ordered_logistic / ordered_probit: K - 1 cutpoints (see ORDINAL_LIKS)
+
+    def n_categories(self, model: "ModelIR") -> int:
+        """K of an ordinal likelihood: one more than its number of cutpoints."""
+        if isinstance(self.cutpoints, Ref):
+            return model.var(self.cutpoints.var).size + 1
+        return int(np.size(self.cutpoints)) + 1
 
     def bounds(self) -> tuple[np.ndarray, np.ndarray]:
         """(lower, upper) of every observation as float arrays, -inf / +inf where open."""
@@ -172,6 +208,25 @@ class Deterministic:
     name: str
     size: int
     terms: list
+    probs_of: str | None = None  # the {name}_probs of ordinal likelihood `probs_of`: [N, K] category probabilities, from
+                                 # that likelihood's eta, cutpoints and sigma (terms unused)
+
+
+def ordinal_log_probs(dist: str, eta, cutpoints, sigma=1.0) -> np.ndarray:
+    """log P(y = k | eta) for k = 0..K-1 along a new last axis: OrderedLogistic / OrderedProbit.compute_p
+    (discrete.py:1312-1326, :1416-1432) in log space, as the difference of upper tails above the mode and of lower ones below."""
+    from scipy.special import log_ndtr
+
+    c = np.asarray(cutpoints, dtype=np.float64)
+    eta, s = np.asarray(eta, dtype=np.float64)[..., None], np.asarray(sigma, dtype=np.float64)[..., None]
+    inf = np.full(c.shape[:-1] + (1,), np.inf)
+    a = (np.concatenate([-inf, c], axis=-1) - eta) / s  # [..., N, K]
+    b = (np.concatenate([c, inf], axis=-1) - eta) / s
+    log_cdf = (lambda t: -np.logaddexp(0.0, -t)) if dist == "ordered_logistic" else log_ndtr
+    with np.errstate(divide="ignore", invalid="ignore"):
+        upper = log_cdf(-a) + np.log1p(-np.exp(log_cdf(-b) - log_cdf(-a)))
+        lower = log_cdf(b) + np.log1p(-np.exp(log_cdf(a) - log_cdf(b)))
+    return np.where(a > 0, upper, lower)
 
 
 @dataclass
@@ -284,6 +339,7 @@ class ModelIR:
                 raise ValueError("bernoulli_logit: y must be 0 or 1")
             self._validate_family(L)
             self._validate_bounds(L)
+            self._validate_ordinal(L)
         for a in self.ar1:
             if self.var(a.var).size < 2:
                 raise ValueError("AR1 needs at least two steps")
@@ -342,6 +398,9 @@ class ModelIR:
     def _check_prior_support(self, p, v) -> None:
         """The variable's transform keeps it inside the prior's support; the constant parameters are in their domain."""
         lo, hi = v.bounds if v.transform == "interval" else (None, None)
+        if v.transform in ORDERED_TRANSFORMS and not (
+                p.dist in REAL_LINE_PRIORS or (p.dist in POSITIVE_PRIORS and v.transform == "ordered_positive")):
+            raise ValueError(f"prior {p.dist} on {v.name}: {ORDERED_PRIOR}")
         if p.dist in POSITIVE_PRIORS and not _positive_support(v):
             raise ValueError(f"prior {p.dist} on {v.name}: the variable needs a log transform or an interval with lo >= 0 "
                              "(positive support)")
@@ -413,6 +472,32 @@ class ModelIR:
         if L.dist == "truncated_normal" and not np.any(np.isfinite(lo) | np.isfinite(hi)):
             raise ValueError(f"{what}: {TRUNC_OPEN}")
 
+    def _validate_ordinal(self, L) -> None:
+        """Cutpoints and categories of ordinal observations (the checks prepare_ir makes, in the same words)."""
+        what = f"{L.dist} likelihood {L.name}"
+        if L.dist not in ORDINAL_LIKS:
+            if L.cutpoints is not None:
+                raise ValueError(f"{what}: cutpoints belong to the ordered_logistic / ordered_probit likelihoods")
+            return
+        if L.dist == "ordered_logistic" and L.sigma is not None:
+            raise ValueError(f"{what}: {LOGISTIC_SIGMA}")
+        if L.cutpoints is None:
+            raise ValueError(f"{what}: needs cutpoints")
+        if isinstance(L.cutpoints, Ref):
+            v = self.var(L.cutpoints.var)
+            if v.size > 1 and v.transform not in ORDERED_TRANSFORMS:
+                raise ValueError(f"{what}: {CUT_ORDERED}")
+        else:
+            c = np.asarray(L.cutpoints, dtype=np.float64)
+            if c.ndim != 1 or not (np.all(np.isfinite(c)) and np.all(np.diff(c) > 0)):
+                raise ValueError(f"{what}: {CUT_CONST}")
+        K = L.n_categories(self)
+        if K < 2:
+            raise ValueError(f"{what}: {ORD_K}")
+        y = np.asarray(L.y, dtype=np.float64)
+        if not (np.all(np.isfinite(y)) and np.all(y == np.floor(y)) and np.all((y >= 0) & (y <= K - 1))):
+            raise ValueError(f"{what}: {ORD_Y}")
+
     # ---- host-side post-processing (f1): unconstrained draws -> named constrained RVs --------------------------------
     def constrain(self, q: np.ndarray) -> dict:
         out, off = {}, self.offsets()
@@ -424,6 +509,8 @@ class ModelIR:
                 lo, hi = v.bounds
                 s = 1.0 / (1.0 + np.exp(-x))
                 x = s * hi + (1.0 - s) * lo
+            elif v.transform in ORDERED_TRANSFORMS:
+                x = ordered_backward(np.array(x, dtype=np.float64), v.transform == "ordered_positive")
             out[v.rv_name] = x[..., 0] if v.size == 1 else x
         return out
 
@@ -432,6 +519,18 @@ class ModelIR:
         returns them): value_i = sum_t coef_t[i] * prod_f x_f[idx_f[i]]."""
         out = {}
         for d in self.deterministics:
+            if d.probs_of is not None:  # an ordinal likelihood's category probabilities, [..., N, K]
+                L = next(L for L in self.likelihoods if L.name == d.probs_of)
+                eta = np.asarray(dataclasses.replace(self, deterministics=[Deterministic("eta", len(L.y), L.terms)])
+                                 .eval_deterministics(posterior)["eta"])
+                c = posterior[self.var(L.cutpoints.var).rv_name] if isinstance(L.cutpoints, Ref) else L.cutpoints
+                c = np.asarray(c, dtype=np.float64)
+                c = c[..., None] if isinstance(L.cutpoints, Ref) and self.var(L.cutpoints.var).size == 1 else c
+                s = 1.0 if L.dist == "ordered_logistic" else (
+                    np.asarray(posterior[self.var(L.sigma.var).rv_name])[..., None] if isinstance(L.sigma, Ref) else L.sigma)
+                lead = eta.shape[:-1]
+                out[d.name] = np.exp(ordinal_log_probs(L.dist, eta, np.broadcast_to(c[..., None, :], lead + (1, c.shape[-1])), s))
+                continue
             lead = None
             total = 0.0
             for t in d.terms:
@@ -474,6 +573,8 @@ class ModelIR:
             for side in ("lower", "upper"):  # per-observation bounds of censored / truncated observations
                 if np.ndim(getattr(L, side)) == 1:
                     out[f"{L.name}_{side}"] = np.asarray(getattr(L, side))
+            if L.cutpoints is not None and not isinstance(L.cutpoints, Ref):  # constant cutpoints of ordinal observations
+                out[f"{L.name}_cutpoints"] = np.asarray(L.cutpoints)
         return out
 
 
@@ -694,6 +795,38 @@ def truncated_regression_ir(n_obs: int = 300, n_features: int = 2, seed: int = 4
     )
 
 
+def ordinal_regression_ir(link: str = "logistic", n_obs: int = 300, n_groups: int = 6, n_features: int = 2, K: int = 5,
+                          sigma: str | None = None, seed: int = 53) -> ModelIR:
+    """Ordinal regression on simulated ratings: z_g ~ Normal(0, 1), sigma_a ~ HalfNormal(1) (non-centred group intercepts
+    sigma_a z[g_i]), beta ~ Normal(0, 1)^F as a design term, cutpoints ~ Normal(linspace(-2, 2, K - 1), 5) with the
+    ordered transform, y_i ~ OrderedLogistic(eta_i, cutpoints) or OrderedProbit(eta_i, cutpoints, sigma) with sigma the
+    constant 1 (``sigma=None`` or "const") or sigma ~ HalfNormal(1) (``sigma="var"``)."""
+    if link not in ("logistic", "probit"):
+        raise ValueError("link must be 'logistic' or 'probit'")
+    rng = np.random.default_rng(seed)
+    g = rng.integers(0, n_groups, n_obs).astype(np.int32)
+    X = rng.standard_normal((n_obs, n_features))
+    eta = rng.normal(0.0, 0.7, n_groups)[g] + X @ rng.normal(0.0, 0.8, n_features)
+    mu_c = np.linspace(-2.0, 2.0, K - 1)
+    noise = rng.logistic(size=n_obs) if link == "logistic" else rng.standard_normal(n_obs)
+    y = np.searchsorted(mu_c + rng.normal(0.0, 0.2, K - 1).cumsum() * 0.3, eta + noise).astype(np.float64)
+    z0 = np.concatenate([[mu_c[0]], np.log(np.diff(mu_c))])  # the support point linspace(-2, 2) in the ordered space
+    vars_ = [Var("z", "z", n_groups), Var("sigma_a_log__", "sigma_a", 1, "log"), Var("beta", "beta", n_features),
+             Var("cutpoints_ordered__", "cutpoints", K - 1, "ordered", initial=z0)]
+    priors = [Prior("normal", "z", (0.0, 1.0)), Prior("halfnormal", "sigma_a_log__", (1.0,)), Prior("normal", "beta", (0.0, 1.0)),
+              Prior("normal", "cutpoints_ordered__", (Linear([Term([], coef=mu_c)]), 5.0))]
+    s = None
+    if link == "probit":
+        s = 1.0
+        if sigma == "var":
+            vars_.append(Var("sigma_log__", "sigma", 1, "log"))
+            priors.append(Prior("halfnormal", "sigma_log__", (1.0,)))
+            s = Ref("sigma_log__")
+    terms = [Term([("sigma_a_log__", None), ("z", g)]), Term([("beta", None)], coef=X)]
+    return ModelIR(name=f"ordinal_{link}", vars=vars_, priors=priors,
+                   likelihoods=[Likelihood(f"ordered_{link}", y, terms, sigma=s, cutpoints=Ref("cutpoints_ordered__"))])
+
+
 # ------------------------------------------------------------------------------------------------------------------------
 # lowering: ModelIR -> flat arrays of the C ABI (include/b200nuts.h: b200_ir)
 # ------------------------------------------------------------------------------------------------------------------------
@@ -708,6 +841,7 @@ class LoweredIR:
     liks: list              # [dict(dist, N, y, terms=[dict(coef, factors=[(offset, size, idx)])], sigma_kind, sigma_value, sigma_ref, sigma_obs, nu, y_var)]
                             # a design term's dict also has n_cols = K, with coef = X [N][K]
                             # censored_normal / truncated_normal: y is the [3][N] block (y, lower, upper)
+                            # ordered_logistic / ordered_probit: nu = K, and cut = the cutpoint term (a term dict)
                             # y_var 0: y is observed data; v + 1: a latent factor, y is None and its values are variable v's
     ar1: list               # [(var, phi(kind, value, ref), sigma(kind, value, ref), init_sigma)]
 
@@ -782,9 +916,15 @@ def lower(ir: ModelIR) -> LoweredIR:
         y = np.ascontiguousarray(L.y, dtype=np.float64)
         if L.dist in BOUNDED_LIKS:  # the [3][N] block: y, lower, upper
             y = np.ascontiguousarray(np.stack([y, *L.bounds()]))
-        liks.append(dict(dist=LIK_DISTS[L.dist], N=len(L.y), y=y,
-                         terms=_lower_terms(ir, L.terms, len(L.y), off), nu=float(L.nu), y_var=0,
-                         **_lower_slot(ir, par, off)))
+        extra = {}
+        if L.dist in ORDINAL_LIKS:  # nu = K; the cutpoint term goes one past the predictor's terms
+            c = L.cutpoints
+            extra = dict(nu=float(L.n_categories(ir)),
+                         cut=dict(coef=None, factors=[(off[ir.var(c.var).name], ir.var(c.var).size, None)])
+                         if isinstance(c, Ref) else dict(coef=np.ascontiguousarray(c, dtype=np.float64), factors=[]))
+        liks.append(dict(dict(dist=LIK_DISTS[L.dist], N=len(L.y), y=y,
+                              terms=_lower_terms(ir, L.terms, len(L.y), off), nu=float(L.nu), y_var=0,
+                              **_lower_slot(ir, par, off)), **extra))
     # latent factors after the observed likelihoods, so that observed likelihood i keeps index i
     for p in latent:
         v = ir.var(p.var)

@@ -45,7 +45,7 @@ class VarInfo:
     rv_name: str  # random-variable name, e.g. "tau"
     offset: int
     size: int
-    transform: str | None = None  # None | "log" | "interval"
+    transform: str | None = None  # None | "log" | "interval" | "ordered" | "ordered_positive"
     bounds: tuple[float, float] | None = None  # for "interval"
 
 
@@ -81,6 +81,11 @@ class ModelSpec:
                 a, b = v.bounds
                 s = 1.0 / (1.0 + np.exp(-x))
                 x = s * b + (1.0 - s) * a
+            elif v.transform in ("ordered", "ordered_positive"):  # Ordered.backward, transforms.py:96-106
+                d = np.exp(x)
+                if v.transform == "ordered":
+                    d[..., 0] = x[..., 0]
+                x = np.cumsum(d, axis=-1)
             if v.size == 1:
                 x = x[..., 0]
             out[v.rv_name] = x

@@ -115,6 +115,22 @@ extern "C" {
  *   sigma          ORDERED_LOGISTIC: NONE; ORDERED_PROBIT: as for NORMAL (CONST, REF or OBS) */
 #define B200_IR_L_ORDERED_LOGISTIC 10 /* pm.OrderedLogistic discrete.py:1231-1326 as Categorical.logp :1190-1206 */
 #define B200_IR_L_ORDERED_PROBIT 11   /* pm.OrderedProbit discrete.py:1329-1432 as Categorical.logp :1190-1206   */
+/* Zero-inflated and hurdle observations with mixing probability psi, the probability of the count / positive component f
+ * (the family of the same name above at eta; P0 = f(0)):
+ *   ZERO_INFLATED_*  y = 0: log((1 - psi) + psi P0);  y > 0: log psi + log f(y)
+ *   HURDLE_*         y = 0: log(1 - psi);             y > 0: log psi + log f(y) - log(1 - P0)  (HURDLE_GAMMA: no division)
+ *   terms[n_terms ..] the psi block, one past the predictor's terms; nu says its form:
+ *                  nu = 0      one term, psi itself: n_factors = 0 and coef = the one constant, 0 < psi < 1; or one unindexed
+ *                              factor on a scalar variable with an INTERVAL inside [0, 1] and coef = NULL
+ *                  nu = m >= 1 psi_i = sigmoid(zeta_i), zeta_i the sum of the m terms terms[n_terms .. n_terms + m), of any kind
+ *   sigma          the family's slot: NONE (Poisson), trials as for BINOMIAL_LOGIT, alpha as for NEGBINOMIAL_LOG / GAMMA_LOG
+ *   y              integers >= 0 (ZERO_INFLATED_BINOMIAL: <= n); HURDLE_GAMMA: finite and >= 0.  y_var must be 0. */
+#define B200_IR_L_ZERO_INFLATED_POISSON 12           /* pm.ZeroInflatedPoisson mixture.py:577-638           */
+#define B200_IR_L_ZERO_INFLATED_BINOMIAL 13          /* pm.ZeroInflatedBinomial mixture.py:641-702          */
+#define B200_IR_L_ZERO_INFLATED_NEGATIVE_BINOMIAL 14 /* pm.ZeroInflatedNegativeBinomial mixture.py:705-802  */
+#define B200_IR_L_HURDLE_POISSON 15                  /* pm.HurdlePoisson mixture.py:873-922                 */
+#define B200_IR_L_HURDLE_NEGATIVE_BINOMIAL 16        /* pm.HurdleNegativeBinomial mixture.py:925-978        */
+#define B200_IR_L_HURDLE_GAMMA 17                    /* pm.HurdleGamma mixture.py:981-1034                  */
 /* The support rule b200_model_create enforces (as ModelIR.validate does): HalfNormal, HalfCauchy, Exponential, Gamma and
  * LogNormal priors sit on a LOG variable or an INTERVAL with lo >= 0, Beta on an INTERVAL inside [0, 1], Uniform(a, b) on an
  * INTERVAL inside [a, b]; every scale (a prior's sigma / beta / lam, Normal and StudentT sigma including each sigma_obs, an

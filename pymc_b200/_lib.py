@@ -116,7 +116,8 @@ def build_ir(low):
             pri[k].p[a] = param(pars[a])
     liks = (IrLik * max(1, len(low.liks)))()
     for k, L in enumerate(low.liks):
-        all_terms = L["terms"] + ([L["cut"]] if "cut" in L else [])  # an ordinal likelihood's cutpoint term goes last
+        # an ordinal likelihood's cutpoint term, or a zero-inflated / hurdle likelihood's psi block, goes last
+        all_terms = L["terms"] + ([L["cut"]] if "cut" in L else []) + L.get("psi", [])
         terms = (IrTerm * len(all_terms))()
         for t, T in enumerate(all_terms):
             terms[t].coef = addr(T["coef"])

@@ -389,6 +389,16 @@ static bool ir_scale_ok(const b200_ir_param& p, const std::vector<IrVarD>& vars)
 #define B200_IR_CUT_ORDERED "a cutpoint variable of size > 1 needs an ordered transform"
 #define B200_IR_CUT_CONST "constant cutpoints must be finite and strictly increasing"
 #define B200_IR_LOGISTIC_SIGMA "ordered_logistic has no sigma"
+// Zero-inflated and hurdle observations (ModelIR.validate, same wording)
+#define B200_IR_PSI_NU "nu must be an integer >= 0: 0 for psi itself, m >= 1 for the m terms of logit(psi)"
+#define B200_IR_PSI_BLOCK "the psi block is one constant or one unindexed scalar variable (nu = 0), or the terms of logit(psi) (nu >= 1)"
+#define B200_IR_PSI_CONST "a constant psi must be finite and lie in (0, 1)"
+#define B200_IR_PSI_ONE "psi = 1 leaves no zero component: write the plain likelihood (poisson_log, binomial_logit, negative_binomial_log or gamma_log)"
+#define B200_IR_PSI_VAR "a psi variable must be scalar with an interval transform inside [0, 1] (0 <= lo < hi <= 1)"
+#define B200_IR_ZI_Y "y must be integers >= 0"
+#define B200_IR_ZIB_Y "y must be integers with 0 <= y <= trials"
+#define B200_IR_HG_Y "y must be finite and >= 0"
+#define B200_IR_ZIP_SLOT "zero_inflated_poisson and hurdle_poisson take no sigma, trials or alpha"
 
 static int prepare_ir(b200_model* m, const b200_model_desc* d) {
     const b200_ir* R = d->ir;
@@ -467,7 +477,8 @@ static int prepare_ir(b200_model* m, const b200_model_desc* d) {
     }
     std::vector<IrLikD> liks(std::max(R->n_liks, 0));
     std::vector<IrTermD> terms;
-    long long max_obs = 0, ord_obs = 0;  // ord_obs: the largest N of an ordinal likelihood (its w row)
+    // ord_obs / zeta_obs: the largest N of an ordinal likelihood (its w row) / of a logit psi (its zeta row); one row serves both
+    long long max_obs = 0, ord_obs = 0, zeta_obs = 0;
     bool has_design = false;
     for (int l = 0; l < R->n_liks; ++l) {
         const b200_ir_lik& L = R->liks[l];
@@ -600,9 +611,61 @@ static int prepare_ir(b200_model* m, const b200_model_desc* d) {
                 ord_obs = std::max(ord_obs, N);
                 m->ir_extended = true;
             } break;
+            case B200_IR_L_ZERO_INFLATED_POISSON: case B200_IR_L_ZERO_INFLATED_BINOMIAL:
+            case B200_IR_L_ZERO_INFLATED_NEGATIVE_BINOMIAL: case B200_IR_L_HURDLE_POISSON:
+            case B200_IR_L_HURDLE_NEGATIVE_BINOMIAL: case B200_IR_L_HURDLE_GAMMA: {  // nu: the form of the psi block
+                if (!(L.nu >= 0 && L.nu == std::floor(L.nu) && L.nu <= 0x7fff)) return fail("ir: likelihood %d: " B200_IR_PSI_NU, l);
+                const bool bin = L.dist == B200_IR_L_ZERO_INFLATED_BINOMIAL, gam = L.dist == B200_IR_L_HURDLE_GAMMA;
+                const bool nb = L.dist == B200_IR_L_ZERO_INFLATED_NEGATIVE_BINOMIAL || L.dist == B200_IR_L_HURDLE_NEGATIVE_BINOMIAL;
+                if (bin && L.sigma_kind != B200_IR_S_CONST && L.sigma_kind != B200_IR_S_OBS)
+                    return fail("ir: likelihood %d: Binomial trials must be a constant or one per observation", l);
+                if ((nb || gam) && L.sigma_kind != B200_IR_S_CONST && L.sigma_kind != B200_IR_S_REF)
+                    return fail("ir: likelihood %d: %s alpha must be a constant or a scalar variable", l, gam ? "Gamma" : "NegativeBinomial");
+                if ((nb || gam) && !ir_scale_ok(slot, vars))
+                    return fail("ir: likelihood %d: %s alpha " B200_IR_SCALE_RULE, l, gam ? "Gamma" : "NegativeBinomial");
+                if (!bin && !nb && !gam && L.sigma_kind != B200_IR_S_NONE) return fail("ir: likelihood %d: " B200_IR_ZIP_SLOT, l);
+                const double a = L.sigma.value;
+                const bool fold = nb && L.sigma_kind == B200_IR_S_CONST && a <= kNegBinPoissonAlpha;
+                double c = 0, sly = 0;
+                long long n_pos = 0;
+                std::map<double, double> count;  // distinct nonzero y -> multiplicity, ascending
+                for (long long i = 0; i < N; ++i) {
+                    const double y = L.y[i];
+                    if (gam) {  // the Gamma's normaliser covers the y > 0 only
+                        if (!(std::isfinite(y) && y >= 0)) return fail("ir: likelihood %d: " B200_IR_HG_Y " (at %lld)", l, i);
+                        if (y > 0) { sly += std::log(y); ++n_pos; }
+                        continue;
+                    }
+                    if (!(y >= 0) || y != std::floor(y) || std::isinf(y)) return fail("ir: likelihood %d: " B200_IR_ZI_Y " (at %lld)", l, i);
+                    c -= std::lgamma(y + 1.0);  // 0 at y = 0, as every constant below
+                    if (bin) {
+                        const double nt = L.sigma_kind == B200_IR_S_OBS ? L.sigma_obs[i] : L.sigma.value;
+                        if (!std::isfinite(nt) || !(nt >= 0) || nt != std::floor(nt)) return fail("ir: likelihood %d: Binomial trials must be integers >= 0 (at %lld)", l, i);
+                        if (y > nt) return fail("ir: likelihood %d: " B200_IR_ZIB_Y " (at %lld)", l, i);
+                        c += std::lgamma(nt + 1.0) - std::lgamma(nt - y + 1.0);
+                    }
+                    if (fold) c += std::lgamma(y + a) - std::lgamma(a);
+                    if (nb && y > 0) count[y] += 1.0;
+                }
+                if (gam && L.sigma_kind == B200_IR_S_CONST) {
+                    c = (double)n_pos * (a * std::log(a) - std::lgamma(a)) + (a - 1.0) * sly;
+                } else if (gam) {
+                    D.sum_log_y = sly;
+                    D.n_tab = (int)n_pos;  // N+
+                }
+                D.c0 = c;
+                if (nb && L.sigma_kind == B200_IR_S_REF) {
+                    std::vector<double> u, cnt;
+                    for (const auto& kv : count) { u.push_back(kv.first); cnt.push_back(kv.second); }
+                    D.n_tab = (int)u.size();
+                    if (upload(m, u, &D.tab_u) || upload(m, cnt, &D.tab_cnt)) return -1;
+                }
+                m->ir_extended = true;
+            } break;
             default: return fail("ir: likelihood %d: density %d is not in the closed set", l, L.dist);
         }
         const bool ordinal = L.dist == B200_IR_L_ORDERED_LOGISTIC || L.dist == B200_IR_L_ORDERED_PROBIT;
+        const bool zi = L.dist >= B200_IR_L_ZERO_INFLATED_POISSON && L.dist <= B200_IR_L_HURDLE_GAMMA;
         const bool has_sigma = L.dist == B200_IR_L_NORMAL || L.dist == B200_IR_L_STUDENTT || L.dist == B200_IR_L_CENSORED_NORMAL ||
                                L.dist == B200_IR_L_TRUNCATED_NORMAL || L.dist == B200_IR_L_ORDERED_PROBIT;
         if (has_sigma && L.sigma_kind == B200_IR_S_NONE)
@@ -616,54 +679,87 @@ static int prepare_ir(b200_model* m, const b200_model_desc* d) {
                 return fail("ir: likelihood %d: sigma " B200_IR_SCALE_RULE, l);
             }
         }
-        for (int t = 0; t < L.n_terms; ++t) {
-            const b200_ir_term& T = L.terms[t];
-            if (T.n_factors < 0 || T.n_factors > 3) return fail("ir: likelihood %d term %d: 0..3 variable factors", l, t);
-            IrTermD TD{};
-            TD.n_factors = T.n_factors;
-            if (T.n_cols != 0) {  // design term: coef is X [N][n_cols]; the same checks and words as ModelIR.validate()
-                const int K = T.n_cols;
-                if (T.n_factors != 1) return fail("ir: likelihood %d term %d: a design term has exactly one factor", l, t);
-                if (T.f[0].idx) return fail("ir: likelihood %d term %d: a design term's factor takes no index", l, t);
-                if (K < 0 || T.f[0].size != K || !T.coef)
-                    return fail("ir: likelihood %d term %d: X must have shape (N, size of the variable)", l, t);
-                if (T.f[0].offset < 0 || T.f[0].offset + K > n) return fail("ir: likelihood %d term %d: factor slice outside q", l, t);
-                std::vector<double> xt((size_t)N * K);
-                for (long long i = 0; i < N; ++i)
-                    for (int k = 0; k < K; ++k) {
-                        const double v = T.coef[i * K + k];
-                        if (!std::isfinite(v)) return fail("ir: likelihood %d term %d: X must be finite (at row %lld, column %d)", l, t, i, k);
-                        xt[(size_t)k * N + i] = v;
-                    }
-                TD.n_cols = K;
-                TD.f[0] = IrFactorD{T.f[0].offset, K, nullptr, nullptr, nullptr};
-                if (upload_raw(m, T.coef, (size_t)N * K, &TD.coef) || upload(m, xt, &TD.xt)) return -1;
-                has_design = true;
-                terms.push_back(TD);
-                continue;
-            }
-            if (T.coef && upload_raw(m, T.coef, (size_t)N, &TD.coef)) return -1;
-            for (int f = 0; f < T.n_factors; ++f) {
-                const b200_ir_factor& F = T.f[f];
-                if (F.offset < 0 || F.size <= 0 || F.offset + F.size > n) return fail("ir: likelihood %d term %d: factor slice outside q", l, t);
-                IrFactorD FD{};
-                FD.offset = F.offset; FD.size = F.size;
-                if (F.idx) {
-                    std::vector<int> rowptr(F.size + 1, 0), rowobs((size_t)N);
-                    for (long long i = 0; i < N; ++i) {
-                        if (F.idx[i] < 0 || F.idx[i] >= F.size) return fail("ir: likelihood %d term %d: index %d out of range at %lld", l, t, F.idx[i], i);
-                        ++rowptr[F.idx[i] + 1];
-                    }
-                    for (int j = 0; j < F.size; ++j) rowptr[j + 1] += rowptr[j];
-                    std::vector<int> fill(rowptr.begin(), rowptr.end() - 1);
-                    for (long long i = 0; i < N; ++i) rowobs[fill[F.idx[i]]++] = (int)i;  // ascending i inside a row: fixed order
-                    if (upload_raw(m, F.idx, (size_t)N, &FD.idx) || upload(m, rowptr, &FD.rowptr) || upload(m, rowobs, &FD.rowobs)) return -1;
-                } else if (F.size != 1 && F.size != N) {
-                    return fail("ir: likelihood %d term %d: a variable of size %d needs an index to enter %lld observations", l, t, F.size, N);
+        // the checks and uploads of terms[t0 .. t1): the predictor's, and those of the logit of a zero-inflated / hurdle psi
+        auto add_terms = [&](int t0, int t1) -> int {
+            for (int t = t0; t < t1; ++t) {
+                const b200_ir_term& T = L.terms[t];
+                if (T.n_factors < 0 || T.n_factors > 3) return fail("ir: likelihood %d term %d: 0..3 variable factors", l, t);
+                IrTermD TD{};
+                TD.n_factors = T.n_factors;
+                if (T.n_cols != 0) {  // design term: coef is X [N][n_cols]; the same checks and words as ModelIR.validate()
+                    const int K = T.n_cols;
+                    if (T.n_factors != 1) return fail("ir: likelihood %d term %d: a design term has exactly one factor", l, t);
+                    if (T.f[0].idx) return fail("ir: likelihood %d term %d: a design term's factor takes no index", l, t);
+                    if (K < 0 || T.f[0].size != K || !T.coef)
+                        return fail("ir: likelihood %d term %d: X must have shape (N, size of the variable)", l, t);
+                    if (T.f[0].offset < 0 || T.f[0].offset + K > n) return fail("ir: likelihood %d term %d: factor slice outside q", l, t);
+                    std::vector<double> xt((size_t)N * K);
+                    for (long long i = 0; i < N; ++i)
+                        for (int k = 0; k < K; ++k) {
+                            const double v = T.coef[i * K + k];
+                            if (!std::isfinite(v)) return fail("ir: likelihood %d term %d: X must be finite (at row %lld, column %d)", l, t, i, k);
+                            xt[(size_t)k * N + i] = v;
+                        }
+                    TD.n_cols = K;
+                    TD.f[0] = IrFactorD{T.f[0].offset, K, nullptr, nullptr, nullptr};
+                    if (upload_raw(m, T.coef, (size_t)N * K, &TD.coef) || upload(m, xt, &TD.xt)) return -1;
+                    has_design = true;
+                    terms.push_back(TD);
+                    continue;
                 }
-                TD.f[f] = FD;
+                if (T.coef && upload_raw(m, T.coef, (size_t)N, &TD.coef)) return -1;
+                for (int f = 0; f < T.n_factors; ++f) {
+                    const b200_ir_factor& F = T.f[f];
+                    if (F.offset < 0 || F.size <= 0 || F.offset + F.size > n) return fail("ir: likelihood %d term %d: factor slice outside q", l, t);
+                    IrFactorD FD{};
+                    FD.offset = F.offset; FD.size = F.size;
+                    if (F.idx) {
+                        std::vector<int> rowptr(F.size + 1, 0), rowobs((size_t)N);
+                        for (long long i = 0; i < N; ++i) {
+                            if (F.idx[i] < 0 || F.idx[i] >= F.size) return fail("ir: likelihood %d term %d: index %d out of range at %lld", l, t, F.idx[i], i);
+                            ++rowptr[F.idx[i] + 1];
+                        }
+                        for (int j = 0; j < F.size; ++j) rowptr[j + 1] += rowptr[j];
+                        std::vector<int> fill(rowptr.begin(), rowptr.end() - 1);
+                        for (long long i = 0; i < N; ++i) rowobs[fill[F.idx[i]]++] = (int)i;  // ascending i inside a row: fixed order
+                        if (upload_raw(m, F.idx, (size_t)N, &FD.idx) || upload(m, rowptr, &FD.rowptr) || upload(m, rowobs, &FD.rowobs)) return -1;
+                    } else if (F.size != 1 && F.size != N) {
+                        return fail("ir: likelihood %d term %d: a variable of size %d needs an index to enter %lld observations", l, t, F.size, N);
+                    }
+                    TD.f[f] = FD;
+                }
+                terms.push_back(TD);
             }
-            terms.push_back(TD);
+            return 0;
+        };
+        if (add_terms(0, L.n_terms)) return -1;
+        if (zi) {  // the psi block at terms[n_terms ..]: nu = 0, psi itself; nu = m >= 1, the m terms of logit(psi)
+            const int mt = (int)L.nu;
+            if (mt > 0) {
+                if (add_terms(L.n_terms, L.n_terms + mt)) return -1;
+                zeta_obs = std::max(zeta_obs, N);
+            } else {
+                const b200_ir_term& T = L.terms[L.n_terms];
+                IrTermD TD{};
+                if (T.n_cols != 0 || (T.n_factors == 0) != (T.coef != nullptr) || T.n_factors > 1 || T.n_factors < 0)
+                    return fail("ir: likelihood %d: " B200_IR_PSI_BLOCK, l);
+                if (T.n_factors == 0) {
+                    const double psi = T.coef[0];
+                    if (psi == 1.0) return fail("ir: likelihood %d: " B200_IR_PSI_ONE, l);
+                    if (!(std::isfinite(psi) && psi > 0.0 && psi < 1.0)) return fail("ir: likelihood %d: " B200_IR_PSI_CONST, l);
+                    if (upload_raw(m, T.coef, 1, &TD.coef)) return -1;
+                } else {
+                    const b200_ir_factor& F = T.f[0];
+                    const IrVarD* V = nullptr;
+                    for (const IrVarD& U : vars)
+                        if (U.offset == F.offset) V = &U;
+                    if (F.idx || !V || V->size != 1 || F.size != 1 || V->transform != IRT_INTERVAL || !(V->lo >= 0.0 && V->hi <= 1.0))
+                        return fail("ir: likelihood %d: " B200_IR_PSI_VAR, l);
+                    TD.n_factors = 1;
+                    TD.f[0] = IrFactorD{F.offset, 1, nullptr, nullptr, nullptr};
+                }
+                terms.push_back(TD);
+            }
         }
         if (ordinal) {  // the cutpoint term: one unindexed factor on a variable of size K - 1, or K - 1 constants in coef
             const int K = (int)L.nu;
@@ -717,8 +813,9 @@ static int prepare_ir(b200_model* m, const b200_model_desc* d) {
         upload(m, ars, &P.ar1))
         return -1;
     P.n_pad = (n + 3) & ~3;
-    P.ord_row = ord_obs ? (int)(P.n_pad + ((max_obs + 3) & ~3LL)) : 0;  // after r, before the design partials
-    P.stride = P.n_pad + ((max_obs + 3) & ~3LL) + ((ord_obs + 3) & ~3LL) + (has_design ? kIrPartDoubles : 0);
+    const long long row2 = std::max(ord_obs, zeta_obs);  // likelihoods are evaluated one after another: they share the row
+    P.ord_row = row2 ? (int)(P.n_pad + ((max_obs + 3) & ~3LL)) : 0;  // after r, before the design partials
+    P.stride = P.n_pad + ((max_obs + 3) & ~3LL) + ((row2 + 3) & ~3LL) + (has_design ? kIrPartDoubles : 0);
     m->ir_max_obs = max_obs;
     return 0;
 }

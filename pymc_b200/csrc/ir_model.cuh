@@ -27,7 +27,8 @@ enum { IRP_FLAT = 0, IRP_NORMAL, IRP_HALFNORMAL, IRP_CAUCHY, IRP_HALFCAUCHY, IRP
        IRP_GAMMA, IRP_BETA, IRP_LOGNORMAL };
 enum { IRL_NORMAL = 0, IRL_BERNOULLI_LOGIT, IRL_POISSON_LOG, IRL_STUDENTT, IRL_NORMAL_LOGVAR, IRL_BINOMIAL_LOGIT,
        IRL_NEGBINOMIAL_LOG, IRL_GAMMA_LOG, IRL_CENSORED_NORMAL, IRL_TRUNCATED_NORMAL, IRL_ORDERED_LOGISTIC,
-       IRL_ORDERED_PROBIT };
+       IRL_ORDERED_PROBIT, IRL_ZI_POISSON, IRL_ZI_BINOMIAL, IRL_ZI_NEGBINOMIAL, IRL_HURDLE_POISSON, IRL_HURDLE_NEGBINOMIAL,
+       IRL_HURDLE_GAMMA };
 enum { IRS_NONE = 0, IRS_CONST, IRS_REF, IRS_OBS };
 constexpr double kNegBinPoissonAlpha = 1e10;  // above: NegativeBinomial -> Poisson(mu) limit (discrete.py:727-735)
 
@@ -87,7 +88,9 @@ __device__ __forceinline__ void ir_design_grad(const IrTermD& Tm, const double* 
 }
 // c0: sum of the constant parts over i.  Random dispersion (sigma_kind REF): Gamma keeps sum_i log y_i in sum_log_y;
 // NegativeBinomial keeps the distinct nonzero y values u[k] with their counts cnt[k] (n_tab of them), over which the
-// alpha-dependent normalising terms sum_i lgamma(y_i + a) - lgamma(a) and their digamma gradient are evaluated.
+// alpha-dependent normalising terms sum_i lgamma(y_i + a) - lgamma(a) and their digamma gradient are evaluated; the
+// zero-inflated and hurdle NegativeBinomial use the same table.  hurdle_gamma: sum_log_y = sum of log y_i over y_i > 0
+// and n_tab = N+, the number of such y_i.
 // Censored Normal: cens[i] = 0 (observed), 1 (y_i at its lower bound), 2 (at its upper bound); the censoring point is y_i
 // itself.  Truncated Normal: bnd = [2][N], the lower and upper bound of each observation, -inf / +inf where open.
 // yoff >= 0: a latent factor (a Normal / StudentT prior whose location is a linear predictor): y_i = x[yoff + i], the
@@ -244,6 +247,144 @@ __device__ __noinline__ double ir_ordinal_loglik(const IrLikD& L, const IrTermD*
     return ir_ordinal_term(L, terms[L.term0 + L.n_terms], x, i, eta, s).lp;
 }
 
+// ---- zero-inflated and hurdle observations (mixture.py:560-1035).  psi is the probability of the count / positive
+// component f, the family at mu = exp(eta) (Binomial: p = sigmoid(eta)), P0 = f(0):
+//   zero-inflated (mixture_logprob, :469-494)  y = 0: logaddexp(log(1 - psi), log psi + log P0);  y > 0: log psi + log f(y)
+//   hurdle (marginal_hurdle_logprob, :846-870) y = 0: log(1 - psi);  y > 0: log psi + log f(y) - log(1 - P0), the discrete
+//                                              component being Truncated(f, lower=1) (:826-829); Gamma has P0 = 0
+// log P0 is -e^eta (Poisson), -n softplus(eta) (Binomial), -a softplus(eta - log a) (NegativeBinomial, whose a > 1e10
+// Poisson limit is kept).  log(1 - P0) = log1mexp(log P0), and log m (m = -log P0) where m is below 1e-304, so the density
+// stays finite for every finite eta.  The psi block is terms[term0 + n_terms ..]: nu = 0, psi itself, one constant
+// (coef[0]) or one scalar variable; nu = m >= 1, psi = sigmoid(zeta), zeta the sum of the m terms, with log psi =
+// -softplus(-zeta) and log(1 - psi) = -softplus(zeta).  The constants of f (-lgamma(y + 1), binomln(n, y), and the
+// NegativeBinomial's lgamma(y + a) - lgamma(a), the Gamma normaliser over the y > 0) are in c0 / the alpha terms of eval.
+// Returns lp, r = d lp / d eta, dz = d lp / d zeta, dpsi = d lp / d psi, da = d lp / d alpha.
+struct IrZiTerm { double lp, r, dz, dpsi, da; };
+__device__ __forceinline__ IrZiTerm ir_zi_term(int dist, double y, double eta, double nt, double a, double la, double lpsi,
+                                               double l1psi, double psi) {
+    // the family: lf = log f(y) less its constants, rf / af = its eta / alpha derivatives; lP0 = log P0 with r0 / a0;
+    // lm = log(-lP0)
+    double lf, rf, af = 0.0, lP0 = -INFINITY, r0 = 0.0, a0 = 0.0, lm = INFINITY;
+    if (dist == IRL_HURDLE_GAMMA) {  // continuous.py:2512-2521, beta = a exp(-eta)
+        const double w = y * exp(-eta);
+        lf = -a * (eta + w);
+        rf = a * (w - 1.0);
+        af = -(eta + w);
+    } else if (dist == IRL_ZI_BINOMIAL) {  // discrete.py:141-152 in PyTensor's stabilised forms
+        lP0 = -nt * softplus(eta);
+        r0 = -nt * sigmoid(eta);
+        lf = y * eta + lP0;
+        rf = y + r0;
+    } else if (dist != IRL_ZI_POISSON && dist != IRL_HURDLE_POISSON && a <= kNegBinPoissonAlpha) {  // discrete.py:700-745
+        const double d = eta - la, e = exp(-fabs(d)), l1 = log1p(e), h = 1.0 / (1.0 + e);
+        const double s = d >= 0 ? h : e * h, sc = d >= 0 ? e * h : h;
+        const double sp = fmax(d, 0.0) + l1;  // softplus(d)
+        lP0 = -a * sp;
+        r0 = -a * s;
+        a0 = s - sp;
+        lf = lP0 - y * (fmax(-d, 0.0) + l1);
+        rf = y * sc + r0;
+        af = 1.0 - sp - sc * (1.0 + y / a);
+        lm = la + (d < -30.0 ? d - 0.5 * e : log(sp));  // log softplus(d) = d - e^d / 2 to rounding below -30
+    } else {  // discrete.py:581-586, and the NegativeBinomial's Poisson limit (:727-735)
+        const double mu = exp(eta);
+        lP0 = -mu;
+        r0 = -mu;
+        lf = y * eta - mu;
+        rf = y - mu;
+        lm = eta;
+    }
+    const bool hurdle = dist >= IRL_HURDLE_POISSON;
+    if (y == 0.0) {
+        if (hurdle) return {l1psi, 0.0, -psi, -exp(-l1psi), 0.0};
+        const double t = lpsi + lP0, u = t - l1psi;  // u: the log-odds of the count component at a zero
+        const double lp = fmax(t, l1psi) + log1p(exp(-fabs(u)));
+        const double w = sigmoid(u);
+        // d/dpsi = -(1 - P0) / ((1 - psi) + psi P0): one quotient, finite as psi -> 1
+        return {lp, w * r0, w - psi, expm1(lP0) * exp(-lp), w * a0};
+    }
+    IrZiTerm o{lpsi + lf, rf, 1.0 - psi, exp(-lpsi), af};
+    if (hurdle && dist != IRL_HURDLE_GAMMA) {  // - log(1 - P0)
+        if (lm < -700.0) {  // m = -log P0 < 1e-304: log(1 - e^-m) = log m, d log m / d eta = 1, d log m / d a = 0
+            o.lp -= lm;
+            o.r -= 1.0;
+        } else {
+            const double q = 1.0 / expm1(-lP0);
+            o.lp -= lP0 > -0.6931471805599453 ? log(-expm1(lP0)) : log1p(-exp(lP0));
+            o.r += r0 * q;
+            o.da += a0 * q;
+        }
+    }
+    return o;
+}
+
+// The observation loop of a zero-inflated / hurdle likelihood, out of line like ir_bounded_pass.  Writes r_i = d logp /
+// d eta_i and, for a logit psi, z_i = d logp / d zeta_i; returns this thread's partial sums of logp, d logp / d alpha and
+// d logp / d psi.
+struct IrZiPartials { double lp, s_a, s_psi; };
+__device__ __forceinline__ void ir_zi_psi(const IrTermD& T, const double* x, double* psi, double* lpsi, double* l1psi) {
+    *psi = T.n_factors ? x[T.f[0].offset] : T.coef[0];  // nu = 0: one constant or one scalar variable
+    *lpsi = log(*psi);
+    *l1psi = log1p(-*psi);
+}
+template <int W>
+__device__ __noinline__ IrZiPartials ir_zi_pass(const IrLikD* Lp, const IrTermD* terms, const double* x, double* r,
+                                                double* zr, double sg_s, double la, int tid) {
+    constexpr int TS = 32 * W;
+    const IrLikD& L = *Lp;
+    const int N = (int)L.N, m = (int)L.nu;
+    const IrTermD* pt = terms + L.term0 + L.n_terms;  // the psi block
+    double psi = 0.0, lpsi = 0.0, l1psi = 0.0;
+    if (m == 0) ir_zi_psi(*pt, x, &psi, &lpsi, &l1psi);
+    double lp = 0.0, s_a = 0.0, s_psi = 0.0;
+    for (int i = tid; i < N; i += TS) {
+        const double eta = ir_eta(terms + L.term0, L.n_terms, x, i, N);
+        if (m > 0) {
+            const double z = ir_eta(pt, m, x, i, N);
+            psi = sigmoid(z);
+            lpsi = -softplus(-z);
+            l1psi = -softplus(z);
+        }
+        const double nt = L.sigma_kind == IRS_OBS ? L.sigma_obs[i] : sg_s;
+        const IrZiTerm o = ir_zi_term(L.dist, L.y[i], eta, nt, sg_s, la, lpsi, l1psi, psi);
+        lp += o.lp;
+        s_a += o.da;
+        s_psi += o.dpsi;
+        r[i] = o.r;
+        if (m > 0) zr[i] = o.dz;
+    }
+    return {lp, s_a, s_psi};
+}
+
+// the pointwise pass's share: log p(y_i | eta, psi) with every constant of f
+__device__ __noinline__ double ir_zi_loglik(const IrLikD& L, const IrTermD* terms, const double* x, int i, double eta,
+                                            double sg_s) {
+    const int N = (int)L.N, m = (int)L.nu;
+    const IrTermD* pt = terms + L.term0 + L.n_terms;
+    double psi, lpsi, l1psi;
+    if (m == 0) {
+        ir_zi_psi(*pt, x, &psi, &lpsi, &l1psi);
+    } else {
+        const double z = ir_eta(pt, m, x, i, N);
+        psi = sigmoid(z);
+        lpsi = -softplus(-z);
+        l1psi = -softplus(z);
+    }
+    const double y = L.y[i], nt = L.sigma_kind == IRS_OBS ? L.sigma_obs[i] : sg_s, la = log(sg_s);
+    double lp = ir_zi_term(L.dist, y, eta, nt, sg_s, la, lpsi, l1psi, psi).lp;
+    if (y > 0.0) {
+        if (L.dist == IRL_HURDLE_GAMMA)
+            lp += sg_s * la - lgamma(sg_s) + (sg_s - 1.0) * log(y);
+        else if (L.dist == IRL_ZI_BINOMIAL)
+            lp += lgamma(nt + 1.0) - lgamma(y + 1.0) - lgamma(nt - y + 1.0);
+        else if (L.dist == IRL_ZI_POISSON || L.dist == IRL_HURDLE_POISSON || sg_s > kNegBinPoissonAlpha)
+            lp -= lgamma(y + 1.0);
+        else
+            lp += lgamma(y + sg_s) - lgamma(sg_s) - lgamma(y + 1.0);
+    }
+    return lp;
+}
+
 // ---- the ordered transform (transforms.py:79-120): x_0 = z_0 (positive: e^{z_0}), x_k = x_{k-1} + e^{z_k}; log|J| =
 // sum_{k>=1} z_k (positive: sum_k z_k).  Not elementwise, so one thread of the team runs it, k ascending (np.cumsum's
 // order): O(size) serial work per evaluation, for vectors as short as cutpoints are.
@@ -273,8 +414,9 @@ __device__ __noinline__ void ir_ordered_chain(const IrVarD* Vp, const double* q,
     }
 }
 
-// IrModel evaluates every factor of the closed set except the censored / truncated Normal and the ordinal likelihoods and
-// the ordered transform; IrExtendedModel (below) is the same function with those added, each out of line.  A kernel's
+// IrModel evaluates every factor of the closed set except the censored / truncated Normal, the ordinal, the zero-inflated
+// and the hurdle likelihoods and the ordered transform; IrExtendedModel (below) is the same function with those added,
+// each out of line.  A kernel's
 // register allocation covers every function it can reach, and the tail math takes about 128 registers, so the engine
 // instantiates its kernels twice and runs a model on IrExtendedModel only when it has one of them (b200_model.ir_extended):
 // every other IR model keeps the kernels it had before.
@@ -283,15 +425,63 @@ struct IrModel {
         const IrVarD* vars; const IrPriorD* priors; const IrLikD* liks; const IrTermD* terms; const IrAr1D* ar1;
         int n_vars, n_priors, n_liks, n_ar1, n;
         double* scratch;            // [slots][stride]
-        long long stride;           // doubles per team: n_pad + max N (+ max N with an ordinal likelihood)
+        long long stride;           // doubles per team: n_pad + max N (+ max N of the ordinal and logit-psi likelihoods)
                                     // (+ kIrPartDoubles with a design term)
         int n_pad;
-        int ord_row;                // offset of an ordinal likelihood's w row in the team slice (0: none)
+        int ord_row;                // offset of the second per-observation row in the team slice (0: none): an ordinal
+                                    // likelihood's w, or the d logp / d zeta of a logit psi; likelihoods take turns
     };
     __host__ __device__ static size_t shared_bytes(const Params&) { return 0; }
     __device__ static void stage(const Params&, char*, uint64_t*) {}
 
     __device__ static __forceinline__ double par(const IrParamD& p, const double* x) { return p.kind ? x[p.ref] : p.value; }
+
+    // The gradient of every (term, factor) of the block terms[term0 .. term0 + n_terms) of length N, given r_i = d logp /
+    // d (the block's sum)_i: d sum_i / d x_f = coef * (other factors).  A likelihood's predictor runs it with its r row,
+    // the logit of a zero-inflated / hurdle psi with its zeta row.  The caller has synchronised the team after writing r.
+    template <int W>
+    __device__ __forceinline__ static void term_grad(const Params& P, int term0, int n_terms, const double* r, int N,
+                                                     double* x, double* g_s, int tid, double* red) {
+        constexpr int TS = 32 * W;
+        for (int t = 0; t < n_terms; ++t) {
+            const IrTermD& Tm = P.terms[term0 + t];
+            if (Tm.n_cols) {  // uniform branch: the residuals r are complete after the caller's barrier
+                ir_design_grad<W>(Tm, r, N, g_s + Tm.f[0].offset, x + P.stride - kIrPartDoubles, tid);
+                team_sync<W>();
+                continue;
+            }
+            for (int f = 0; f < Tm.n_factors; ++f) {
+                const IrFactorD& Fc = Tm.f[f];
+                auto others = [&](int i) -> double {
+                    double pr = Tm.coef ? Tm.coef[i] : 1.0;
+                    for (int f2 = 0; f2 < Tm.n_factors; ++f2) {
+                        if (f2 == f) continue;
+                        const IrFactorD& F2 = Tm.f[f2];
+                        pr *= x[F2.offset + (F2.idx ? F2.idx[i] : (F2.size == 1 ? 0 : i))];
+                    }
+                    return pr;
+                };
+                if (!Fc.idx && Fc.size == 1) {  // scalar target: team reduction over the observations
+                    double a = 0.0;
+                    for (int i = tid; i < N; i += TS) a = fma(r[i], others(i), a);
+                    a = team_sum<W>(a, tid, red);
+                    if (tid == 0) g_s[Fc.offset] += a;
+                } else if (!Fc.idx) {  // elementwise target (vector variable of the block's length)
+                    for (int i = tid; i < N; i += TS) g_s[Fc.offset + i] += r[i] * others(i);
+                } else {  // indexed target: pull through the CSR transpose of idx (fixed order)
+                    for (int j = tid; j < Fc.size; j += TS) {
+                        double a = 0.0;
+                        for (int e = Fc.rowptr[j]; e < Fc.rowptr[j + 1]; ++e) {
+                            const int i = Fc.rowobs[e];
+                            a = fma(r[i], others(i), a);
+                        }
+                        g_s[Fc.offset + j] += a;
+                    }
+                }
+                team_sync<W>();
+            }
+        }
+    }
 
     template <int NPL, int W, bool SMALL = false>
     __device__ __noinline__ static double eval(const Params& P, const char* s, const double* q_s, double* g_s, int tid, double* red) {
@@ -413,13 +603,21 @@ struct IrModel {
             const IrLikD L = P.liks[l];
             const int N = (int)L.N;
             const double sg_s = (L.sigma_kind == IRS_REF) ? x[L.sigma.ref] : L.sigma.value;
-            const bool disp = L.dist == IRL_NEGBINOMIAL_LOG || L.dist == IRL_GAMMA_LOG;  // sg_s is the dispersion alpha
+            const bool zi = EXTENDED && L.dist >= IRL_ZI_POISSON;  // zero-inflated / hurdle
+            const bool gamma = L.dist == IRL_GAMMA_LOG || (EXTENDED && L.dist == IRL_HURDLE_GAMMA);
+            const bool disp = L.dist == IRL_NEGBINOMIAL_LOG || gamma ||  // sg_s is the dispersion alpha
+                              (EXTENDED && (L.dist == IRL_ZI_NEGBINOMIAL || L.dist == IRL_HURDLE_NEGBINOMIAL));
             const double la = disp ? log(sg_s) : 0.0;
-            double s_sig = 0.0;
+            double s_sig = 0.0, s_psi = 0.0;
             const bool ordinal = EXTENDED && (L.dist == IRL_ORDERED_LOGISTIC || L.dist == IRL_ORDERED_PROBIT);
-            const bool bounded = EXTENDED && (ordinal || L.dist == IRL_CENSORED_NORMAL || L.dist == IRL_TRUNCATED_NORMAL);
+            const bool bounded = EXTENDED && (ordinal || zi || L.dist == IRL_CENSORED_NORMAL || L.dist == IRL_TRUNCATED_NORMAL);
             if constexpr (EXTENDED) {
-                if (bounded) {  // uniform branch: out of line
+                if (zi) {  // uniform branch: out of line
+                    const IrZiPartials b = ir_zi_pass<W>(P.liks + l, P.terms, x, r, x + P.ord_row, sg_s, la, tid);
+                    lp += b.lp;
+                    s_sig = b.s_a;
+                    s_psi = b.s_psi;
+                } else if (bounded) {  // uniform branch: out of line
                     const IrPartials b = ordinal ? ir_ordinal_pass<W>(P.liks + l, P.terms, x, r, x + P.ord_row, sg_s, tid)
                                                  : ir_bounded_pass<W>(P.liks + l, P.terms, x, r, sg_s, tid);
                     lp += b.lp;
@@ -505,11 +703,12 @@ struct IrModel {
             if (disp && L.sigma_kind == IRS_REF) {  // uniform branch: the alpha-dependent normalising terms
                 const double a = sg_s;
                 const IrLikD& Lt = P.liks[l];  // read here, not kept live through the observation loop
-                if (L.dist == IRL_GAMMA_LOG) {
+                if (gamma) {
                     if (tid == 0) {
                         const double sly = Lt.sum_log_y;
-                        lp += (double)N * (a * la - lgamma(a)) + (a - 1.0) * sly;
-                        s_sig += (double)N * (la + 1.0 - digamma(a)) + sly;
+                        const double Ny = (EXTENDED && L.dist == IRL_HURDLE_GAMMA) ? (double)Lt.n_tab : (double)N;  // N+
+                        lp += Ny * (a * la - lgamma(a)) + (a - 1.0) * sly;
+                        s_sig += Ny * (la + 1.0 - digamma(a)) + sly;
                     }
                 } else if (a <= kNegBinPoissonAlpha) {
                     // sum_i lgamma(y_i + a) - lgamma(a) over the distinct values: team-strided, fixed order
@@ -531,51 +730,24 @@ struct IrModel {
                     ir_cutpoint_grad<W>(P.liks + l, P.terms, r, x + P.ord_row, g_s, tid);
                     team_sync<W>();
                 }
+                if (zi) {  // uniform branch: the psi block's gradient
+                    const IrTermD* pt = P.terms + L.term0 + L.n_terms;
+                    if (L.nu > 0.0) {  // the terms of logit(psi), fed the zeta row
+                        term_grad<W>(P, L.term0 + L.n_terms, (int)L.nu, x + P.ord_row, N, x, g_s, tid, red);
+                    } else if (pt->n_factors) {  // a psi variable: one team reduction
+                        const double tot = team_sum<W>(s_psi, tid, red);
+                        if (tid == 0) g_s[pt->f[0].offset] += tot;
+                        team_sync<W>();
+                    }
+                }
             }
             if (L.sigma_kind == IRS_REF) {
                 const double tot = team_sum<W>(s_sig, tid, red);
                 if (tid == 0) g_s[L.sigma.ref] += tot;
                 team_sync<W>();
             }
-            // gradient of every (term, factor): d eta_i / d x_f = coef * (other factors)
-            for (int t = 0; t < L.n_terms; ++t) {
-                const IrTermD& Tm = P.terms[L.term0 + t];
-                if (Tm.n_cols) {  // uniform branch: the residuals r are complete after the barrier above
-                    ir_design_grad<W>(Tm, r, N, g_s + Tm.f[0].offset, x + P.stride - kIrPartDoubles, tid);
-                    team_sync<W>();
-                    continue;
-                }
-                for (int f = 0; f < Tm.n_factors; ++f) {
-                    const IrFactorD& Fc = Tm.f[f];
-                    auto others = [&](int i) -> double {
-                        double pr = Tm.coef ? Tm.coef[i] : 1.0;
-                        for (int f2 = 0; f2 < Tm.n_factors; ++f2) {
-                            if (f2 == f) continue;
-                            const IrFactorD& F2 = Tm.f[f2];
-                            pr *= x[F2.offset + (F2.idx ? F2.idx[i] : (F2.size == 1 ? 0 : i))];
-                        }
-                        return pr;
-                    };
-                    if (!Fc.idx && Fc.size == 1) {  // scalar target: team reduction over the observations
-                        double a = 0.0;
-                        for (int i = tid; i < N; i += TS) a = fma(r[i], others(i), a);
-                        a = team_sum<W>(a, tid, red);
-                        if (tid == 0) g_s[Fc.offset] += a;
-                    } else if (!Fc.idx) {  // elementwise target (vector variable of the likelihood's length)
-                        for (int i = tid; i < N; i += TS) g_s[Fc.offset + i] += r[i] * others(i);
-                    } else {  // indexed target: pull through the CSR transpose of idx (fixed order)
-                        for (int j = tid; j < Fc.size; j += TS) {
-                            double a = 0.0;
-                            for (int e = Fc.rowptr[j]; e < Fc.rowptr[j + 1]; ++e) {
-                                const int i = Fc.rowobs[e];
-                                a = fma(r[i], others(i), a);
-                            }
-                            g_s[Fc.offset + j] += a;
-                        }
-                    }
-                    team_sync<W>();
-                }
-            }
+            // gradient of every (term, factor) of the predictor: d eta_i / d x_f = coef * (other factors)
+            term_grad<W>(P, L.term0, L.n_terms, r, N, x, g_s, tid, red);
         }
 
         // ---- 2c. AR(1): h_0 ~ Normal(0, init_sigma), h_t - phi h_{t-1} ~ Normal(0, sigma)  (timeseries.py:646-676) ------
@@ -729,8 +901,10 @@ __global__ void __launch_bounds__(256) ir_pointwise_kernel(const IrModel::Params
                 case IRL_CENSORED_NORMAL: case IRL_TRUNCATED_NORMAL:
                     if constexpr (EXTENDED) lp = ir_bounded_loglik(L, i, eta, (L.sigma_kind == IRS_OBS) ? L.sigma_obs[i] : sg_s);
                     break;
-                default:  // the ordinal likelihoods
-                    if constexpr (EXTENDED) lp = ir_ordinal_loglik(L, P.terms, x, i, eta);
+                default:  // the ordinal, zero-inflated and hurdle likelihoods
+                    if constexpr (EXTENDED)
+                        lp = L.dist >= IRL_ZI_POISSON ? ir_zi_loglik(L, P.terms, x, i, eta, sg_s)
+                                                      : ir_ordinal_loglik(L, P.terms, x, i, eta);
                     break;
             }
             out[d * N + i] = lp;

@@ -17,7 +17,10 @@ pymc/model/fgraph.py:76-81, :139) -- and pattern-matches them onto the closed fa
                      pm.Censored(pm.Normal.dist(eta, sigma), lower, upper), pm.TruncatedNormal(eta, sigma, lower, upper)
                      and pm.Truncated(pm.Normal.dist(eta, sigma), lower, upper) with constant bounds;
                      pm.OrderedLogistic / pm.OrderedProbit: the Categorical whose p is their compute_p graph, with or
-                     without the {name}_probs Deterministic (recorded, evaluated from the draws)
+                     without the {name}_probs Deterministic (recorded, evaluated from the draws);
+                     pm.ZeroInflatedPoisson / Binomial / NegativeBinomial and pm.HurdlePoisson / NegativeBinomial / Gamma:
+                     the mixture of DiracDelta(0) and the family above with weights stack([1 - psi, psi]), psi a
+                     constant, a scalar free RV or pm.math.invlogit(linear predictor)
     transform    ->  None, log, interval, and Ordered() / Ordered(positive=True) -> "ordered" / "ordered_positive"
 
 Anything outside the closed set raises ``NotImplementedError`` naming the offending op, so a model either lowers exactly
@@ -47,7 +50,10 @@ _PRIOR_BY_OP = {  # RV op class name (lower-cased, "rv" stripped) -> (ir dist, p
 
 
 def _op_name(rv) -> str:
-    op = rv.owner.op
+    return _op_class_name(rv.owner.op)
+
+
+def _op_class_name(op) -> str:
     name = type(op).__name__.lower()
     for suffix in ("rv",):
         if name.endswith(suffix):
@@ -365,6 +371,147 @@ def from_pymc(model) -> _ir.ModelIR:
             return None
         return "ordered_probit", probits.owner.inputs[0], cutpoints_of(probits.owner.inputs[1]), s[0]
 
+    def family_of(op, ps, name, N):
+        """(dist, eta, parameter slot) of a count / positive family RV (op, its dist params ps): pm.Poisson(mu=exp(eta)),
+        pm.Binomial(n, logit_p=eta), pm.NegativeBinomial(mu=exp(eta), alpha), pm.Gamma(alpha, beta=alpha / exp(eta));
+        observed likelihoods and the components of zero-inflated / hurdle mixtures share it."""
+        if op == "poisson":
+            eta = strip(ps[0], "exp")
+            if eta is None:
+                raise NotImplementedError(f"{name}: write the rate as pm.math.exp(linear predictor)")
+            return "poisson_log", eta, {}
+        if op == "binomial":  # RV parameters (n, p); logit_p= and p=invlogit(eta) both give p = sigmoid(eta)
+            form = "pm.Binomial(n=trials, logit_p=linear predictor) with constant trials"
+            nt = _const_value(ps[0])
+            eta = inputs_of(ps[1], "sigmoid")
+            if nt is None or eta is None:
+                raise NotImplementedError(f"{name}: write the likelihood as {form}")
+            trials = float(nt.reshape(())) if nt.size == 1 else np.ravel(np.broadcast_to(nt, (N,))).astype(np.float64)
+            return "binomial_logit", eta[0], {"trials": trials}
+        if op in ("negbinomial", "nbinom"):  # RV parameters (n = alpha, p = alpha / (mu + alpha)), discrete.py:700-723
+            form = "pm.NegativeBinomial(mu=pm.math.exp(linear predictor), alpha=constant or scalar free RV)"
+            try:
+                alpha = param(ps[0], name + ".alpha")
+            except NotImplementedError:
+                raise NotImplementedError(f"{name}: write the likelihood as {form}") from None
+            div, eta = inputs_of(ps[1], "truediv"), None
+            den = inputs_of(div[1], "add") if div is not None and same_param(div[0], alpha) else None
+            if den is not None and len(den) == 2:
+                for mu_, a_ in (den, den[::-1]):
+                    e = inputs_of(mu_, "exp")
+                    if e is not None and same_param(a_, alpha):
+                        eta = e[0]
+                        break
+            if eta is None:
+                raise NotImplementedError(f"{name}: write the likelihood as {form}")
+            return "negative_binomial_log", eta, {"alpha": alpha}
+        # op == "gamma": RV parameters (alpha, scale = reciprocal(beta)), continuous.py:2478-2510
+        form = ("pm.Gamma(alpha=a, beta=a / pm.math.exp(linear predictor)) or beta=a * pm.math.exp(-linear predictor), "
+                "a a constant or scalar free RV")
+        try:
+            alpha = param(ps[0], name + ".alpha")
+        except NotImplementedError:
+            raise NotImplementedError(f"{name}: write the likelihood as {form}") from None
+        beta, eta = inputs_of(ps[1], "reciprocal"), None
+        if beta is not None:
+            div, mul = inputs_of(beta[0], "truediv"), inputs_of(beta[0], "mul")
+            if div is not None and same_param(div[0], alpha):  # a / exp(eta)
+                e = inputs_of(div[1], "exp")
+                eta = e[0] if e is not None else None
+            elif mul is not None and len(mul) == 2:  # a * exp(-eta), either order
+                for a_, e_ in (mul, mul[::-1]):
+                    e = inputs_of(e_, "exp")
+                    ng = inputs_of(e[0], "neg") if e is not None else None
+                    if ng is not None and same_param(a_, alpha):
+                        eta = ng[0]
+                        break
+        if eta is None:
+            raise NotImplementedError(f"{name}: write the likelihood as {form}")
+        return "gamma_log", eta, {"alpha": alpha}
+
+    def stack_of(w):
+        """the entries of a stack / join / make_vector of scalars or vectors along the last axis, under DimShuffle layers"""
+        while w.owner is not None and isinstance(w.owner.op, DimShuffle):
+            w = w.owner.inputs[0]
+        if w.owner is None or type(w.owner.op).__name__ not in ("Join", "MakeVector", "Stack"):
+            return None
+        ins = list(w.owner.inputs)
+        if type(w.owner.op).__name__ == "Join":
+            ins = ins[1:]  # the axis
+        out = []
+        for x in ins:
+            while x.owner is not None and isinstance(x.owner.op, DimShuffle):
+                x = x.owner.inputs[0]
+            out.append(x)
+        return out
+
+    def psi_of(w, name, N):
+        """psi of mixture weights stack([1 - psi, psi], axis=-1): a constant, a scalar free RV (-> Ref), or
+        invlogit / sigmoid of a linear predictor (-> Linear, the logit of psi)"""
+        form = ("the weights of a zero-inflated / hurdle mixture are stack([1 - psi, psi]) with psi a constant, a scalar "
+                "free RV or pm.math.invlogit(linear predictor)")
+        ent = stack_of(w)
+        if ent is None or len(ent) != 2:
+            raise NotImplementedError(f"{name}: {form}")
+        one_minus, p = ent
+        sub = inputs_of(one_minus, "sub")
+        if sub is None or len(sub) != 2 or _const_value(sub[0]) is None or np.any(_const_value(sub[0]) != 1.0):
+            raise NotImplementedError(f"{name}: {form}")
+        q = sub[1]
+        while q.owner is not None and isinstance(q.owner.op, DimShuffle):
+            q = q.owner.inputs[0]
+        if q is not p:
+            raise NotImplementedError(f"{name}: {form}")
+        z = inputs_of(p, "sigmoid")
+        if z is not None:
+            return _ir.Linear(make_terms(z[0], N))
+        if p in name_of and size_of[name_of[p]] != 1:
+            raise NotImplementedError(f"{name}: a vector psi variable is outside the closed set (psi is a constant, a "
+                                      "scalar free RV or pm.math.invlogit(linear predictor))")
+        c = _const_value(p)
+        if c is not None and c.size != 1:
+            raise NotImplementedError(f"{name}: a per-observation constant psi is outside the closed set (psi is a "
+                                      "constant, a scalar free RV or pm.math.invlogit(linear predictor))")
+        try:
+            return param(p, name + ".psi")
+        except NotImplementedError:
+            raise NotImplementedError(f"{name}: {form}") from None
+
+    def zero_inflated_of(rv, ps, N):
+        """(dist, eta, parameter slot, psi) of pm.ZeroInflated* (a Mixture of [DiracDelta(0), f], mixture.py:560-574) or
+        pm.Hurdle* (a _Hurdle of [DiracDelta(0), Truncated(f, lower=1) | Gamma], :812-844)"""
+        hurdle = "hurdle" in _op_name(rv)
+        w, comps = ps[0], ps[1:]
+        zero = comps[0] if comps else None
+        if len(comps) != 2 or zero.owner is None or _op_name(zero) != "diracdelta" or \
+                _const_value(_dist_params(zero)[0]) is None or np.any(_const_value(_dist_params(zero)[0]) != 0):
+            raise NotImplementedError(f"{rv.name}: pm.Mixture / pm.NormalMixture is outside the closed set (only the "
+                                      "zero-inflated Poisson, Binomial and NegativeBinomial mixtures)")
+        comp = comps[1]
+        cop = _op_name(comp)
+        if hurdle and cop == "lognormal":
+            raise NotImplementedError(f"{rv.name}: pm.HurdleLogNormal is outside the closed set (there is no LogNormal "
+                                      "likelihood)")
+        cps = _dist_params(comp)
+        truncated = cop == "truncated"
+        if hurdle and truncated:  # Truncated(f, lower=1): f's own parameters, then lower and upper
+            cop = _op_class_name(comp.owner.op.base_rv_op)
+            lo, hi = _const_value(cps[-2]), _const_value(cps[-1])
+            if lo is None or hi is None or np.any(lo != 1) or np.any(hi != np.inf):
+                raise NotImplementedError(f"{rv.name}: a hurdle's count component is Truncated(f, lower=1)")
+            cps = cps[: -2][-({"poisson": 1}.get(cop, 2)):]
+        # a hurdle's count component is Truncated(f, lower=1), its Gamma component the Gamma itself
+        ok = (truncated and cop in ("poisson", "negbinomial", "nbinom")) or (not truncated and cop == "gamma") if hurdle else \
+            cop in ("poisson", "binomial", "negbinomial", "nbinom")
+        if not ok:
+            what = "pm.HurdlePoisson / HurdleNegativeBinomial / HurdleGamma" if hurdle else \
+                "pm.ZeroInflatedPoisson / ZeroInflatedBinomial / ZeroInflatedNegativeBinomial"
+            raise NotImplementedError(f"{rv.name}: a mixture with a {type(comp.owner.op).__name__} component is outside "
+                                      f"the closed set (only {what})")
+        fam, eta, slot = family_of(cop, cps, rv.name, N)
+        dist = next(d for d, f in _ir.ZI_FAMILY.items() if f == fam and d.startswith("hurdle" if hurdle else "zero"))
+        return dist, eta, slot, psi_of(w, rv.name, N)
+
     probs_of = {}  # id of a {name}_probs Deterministic's expression -> the ordinal likelihood's name
     liks = []
     for rv in model.observed_RVs:
@@ -406,36 +553,12 @@ def from_pymc(model) -> _ir.ModelIR:
             if eta is None:
                 raise NotImplementedError(f"{rv.name}: write the likelihood as pm.Bernoulli(logit_p=...)")
             liks.append(_ir.Likelihood("bernoulli_logit", y, make_terms(eta, N), name=rv.name))
-        elif op == "poisson":
-            eta = strip(ps[0], "exp")
-            if eta is None:
-                raise NotImplementedError(f"{rv.name}: write the rate as pm.math.exp(linear predictor)")
-            liks.append(_ir.Likelihood("poisson_log", y, make_terms(eta, N), name=rv.name))
-        elif op == "binomial":  # RV parameters (n, p); logit_p= and p=invlogit(eta) both give p = sigmoid(eta)
-            form = "pm.Binomial(n=trials, logit_p=linear predictor) with constant trials"
-            nt = _const_value(ps[0])
-            eta = inputs_of(ps[1], "sigmoid")
-            if nt is None or eta is None:
-                raise NotImplementedError(f"{rv.name}: write the likelihood as {form}")
-            trials = float(nt.reshape(())) if nt.size == 1 else np.ravel(np.broadcast_to(nt, (N,))).astype(np.float64)
-            liks.append(_ir.Likelihood("binomial_logit", y, make_terms(eta[0], N), trials=trials, name=rv.name))
-        elif op in ("negbinomial", "nbinom"):  # RV parameters (n = alpha, p = alpha / (mu + alpha)), discrete.py:700-723
-            form = "pm.NegativeBinomial(mu=pm.math.exp(linear predictor), alpha=constant or scalar free RV)"
-            try:
-                alpha = param(ps[0], rv.name + ".alpha")
-            except NotImplementedError:
-                raise NotImplementedError(f"{rv.name}: write the likelihood as {form}") from None
-            div, eta = inputs_of(ps[1], "truediv"), None
-            den = inputs_of(div[1], "add") if div is not None and same_param(div[0], alpha) else None
-            if den is not None and len(den) == 2:
-                for mu_, a_ in (den, den[::-1]):
-                    e = inputs_of(mu_, "exp")
-                    if e is not None and same_param(a_, alpha):
-                        eta = e[0]
-                        break
-            if eta is None:
-                raise NotImplementedError(f"{rv.name}: write the likelihood as {form}")
-            liks.append(_ir.Likelihood("negative_binomial_log", y, make_terms(eta, N), alpha=alpha, name=rv.name))
+        elif op in ("poisson", "binomial", "negbinomial", "nbinom", "gamma"):
+            dist, eta, slot = family_of(op, ps, rv.name, N)
+            liks.append(_ir.Likelihood(dist, y, make_terms(eta, N), name=rv.name, **slot))
+        elif op in ("mixture", "_hurdle", "hurdle"):  # pm.ZeroInflated* / pm.Hurdle*
+            dist, eta, slot, psi = zero_inflated_of(rv, ps, N)
+            liks.append(_ir.Likelihood(dist, y, make_terms(eta, N), name=rv.name, psi=psi, **slot))
         elif op == "truncated":
             # TruncatedRV (truncated.py:53-130): the base RV's own inputs followed by lower and upper, its op in base_rv_op.
             # A Normal base never arrives here: pm.Truncated dispatches it to TruncatedNormal (truncated.py:499-505).
@@ -468,29 +591,6 @@ def from_pymc(model) -> _ir.ModelIR:
             dist = "censored_normal" if op == "censored" else "truncated_normal"
             liks.append(_ir.Likelihood(dist, y, make_terms(mu, N), sigma=sigma_of(s), lower=bound(lo, -np.inf),
                                        upper=bound(hi, np.inf), name=rv.name))
-        elif op == "gamma":  # RV parameters (alpha, scale = reciprocal(beta)), continuous.py:2478-2510
-            form = ("pm.Gamma(alpha=a, beta=a / pm.math.exp(linear predictor)) or beta=a * pm.math.exp(-linear predictor), "
-                    "a a constant or scalar free RV")
-            try:
-                alpha = param(ps[0], rv.name + ".alpha")
-            except NotImplementedError:
-                raise NotImplementedError(f"{rv.name}: write the likelihood as {form}") from None
-            beta, eta = inputs_of(ps[1], "reciprocal"), None
-            if beta is not None:
-                div, mul = inputs_of(beta[0], "truediv"), inputs_of(beta[0], "mul")
-                if div is not None and same_param(div[0], alpha):  # a / exp(eta)
-                    e = inputs_of(div[1], "exp")
-                    eta = e[0] if e is not None else None
-                elif mul is not None and len(mul) == 2:  # a * exp(-eta), either order
-                    for a_, e_ in (mul, mul[::-1]):
-                        e = inputs_of(e_, "exp")
-                        ng = inputs_of(e[0], "neg") if e is not None else None
-                        if ng is not None and same_param(a_, alpha):
-                            eta = ng[0]
-                            break
-            if eta is None:
-                raise NotImplementedError(f"{rv.name}: write the likelihood as {form}")
-            liks.append(_ir.Likelihood("gamma_log", y, make_terms(eta, N), alpha=alpha, name=rv.name))
         elif op == "categorical":  # pm.OrderedLogistic / pm.OrderedProbit build Categorical(p = compute_p(eta, cutpoints))
             form = ("pm.OrderedLogistic(eta, cutpoints) or pm.OrderedProbit(eta, cutpoints, sigma): a Categorical with a "
                     "free p, logit_p / softmax, or a p of another form is outside the closed set")

@@ -64,7 +64,33 @@ LIK_DISTS = {
     "truncated_normal": 9,   # y_i ~ TruncatedNormal(eta_i, sigma, lower, upper)        continuous.py:720-747
     "ordered_logistic": 10,  # y_i ~ OrderedLogistic(eta_i, cutpoints)                  discrete.py:1231-1326, :1190-1206
     "ordered_probit": 11,    # y_i ~ OrderedProbit(eta_i, cutpoints, sigma)             discrete.py:1329-1432, :1190-1206
+    "zero_inflated_poisson": 12,            # ZeroInflatedPoisson(psi, mu = exp(eta_i))            mixture.py:577-638
+    "zero_inflated_binomial": 13,           # ZeroInflatedBinomial(psi, trials, logit_p = eta_i)   mixture.py:641-702
+    "zero_inflated_negative_binomial": 14,  # ZeroInflatedNegativeBinomial(psi, exp(eta_i), alpha) mixture.py:705-802
+    "hurdle_poisson": 15,                   # HurdlePoisson(psi, mu = exp(eta_i))                  mixture.py:873-922
+    "hurdle_negative_binomial": 16,         # HurdleNegativeBinomial(psi, exp(eta_i), alpha)       mixture.py:925-978
+    "hurdle_gamma": 17,                     # HurdleGamma(psi, alpha, beta = alpha / exp(eta_i))   mixture.py:981-1034
 }
+# Zero-inflated and hurdle observations: ``Likelihood.psi`` is the probability of the count / positive component, a
+# constant in (0, 1), a Ref to a scalar variable with an interval transform inside [0, 1], or a Linear: the logit of psi.
+# Each is its family (ZI_FAMILY) with the family's parameter slot (trials, alpha).  Lowered with the psi block one past the
+# predictor's terms and nu = 0 (psi itself) or the number of terms of logit(psi) (include/b200nuts.h).
+ZI_FAMILY = {"zero_inflated_poisson": "poisson_log", "zero_inflated_binomial": "binomial_logit",
+             "zero_inflated_negative_binomial": "negative_binomial_log", "hurdle_poisson": "poisson_log",
+             "hurdle_negative_binomial": "negative_binomial_log", "hurdle_gamma": "gamma_log"}
+ZI_LIKS = tuple(ZI_FAMILY)
+# the refusals (csrc/b200nuts.cu: prepare_ir, same words)
+PSI_NU = "nu must be an integer >= 0: 0 for psi itself, m >= 1 for the m terms of logit(psi)"
+PSI_BLOCK = ("the psi block is one constant or one unindexed scalar variable (nu = 0), or the terms of logit(psi) "
+             "(nu >= 1)")
+PSI_CONST = "a constant psi must be finite and lie in (0, 1)"
+PSI_ONE = ("psi = 1 leaves no zero component: write the plain likelihood (poisson_log, binomial_logit, "
+           "negative_binomial_log or gamma_log)")
+PSI_VAR = "a psi variable must be scalar with an interval transform inside [0, 1] (0 <= lo < hi <= 1)"
+ZI_Y = "y must be integers >= 0"
+ZIB_Y = "y must be integers with 0 <= y <= trials"
+HG_Y = "y must be finite and >= 0"
+ZIP_SLOT = "zero_inflated_poisson and hurdle_poisson take no sigma, trials or alpha"
 # Ordinal observations: y_i in 0..K-1 and ``Likelihood.cutpoints``, a Ref to a variable of size K - 1 (ordered unless
 # K = 2) or K - 1 constants, finite and strictly increasing; lowered with nu = K and the cutpoint term one past the
 # predictor's terms (include/b200nuts.h)
@@ -184,6 +210,7 @@ class Likelihood:
     lower: float | np.ndarray | None = None    # censored_normal / truncated_normal: None (open), a constant or one per
     upper: float | np.ndarray | None = None    # observation, -inf / +inf where that observation's side is open
     cutpoints: Ref | np.ndarray | None = None  # ordered_logistic / ordered_probit: K - 1 cutpoints (see ORDINAL_LIKS)
+    psi: float | Ref | Linear | None = None    # the zero-inflated / hurdle likelihoods (ZI_LIKS): a Linear is logit(psi)
 
     def n_categories(self, model: "ModelIR") -> int:
         """K of an ordinal likelihood: one more than its number of cutpoints."""
@@ -340,6 +367,7 @@ class ModelIR:
             self._validate_family(L)
             self._validate_bounds(L)
             self._validate_ordinal(L)
+            self._validate_psi(L)
         for a in self.ar1:
             if self.var(a.var).size < 2:
                 raise ValueError("AR1 needs at least two steps")
@@ -421,7 +449,13 @@ class ModelIR:
         """Support and parameter rules of the count / positive families (the same checks prepare_ir makes)."""
         y = np.asarray(L.y, dtype=np.float64)
         integer = lambda a: bool(np.all(np.isfinite(a)) and np.all(a == np.floor(a)))  # noqa: E731
-        if L.dist == "binomial_logit":
+        fam = ZI_FAMILY.get(L.dist, L.dist)  # a zero-inflated / hurdle likelihood follows its family's rules
+        if L.dist in ("zero_inflated_poisson", "hurdle_poisson"):
+            if not integer(y) or np.any(y < 0):
+                raise ValueError(f"{L.dist}: {ZI_Y}")
+            if L.sigma is not None:
+                raise ValueError(f"{L.dist}: {ZIP_SLOT}")
+        if fam == "binomial_logit":
             if L.trials is None or isinstance(L.trials, Ref):
                 raise ValueError("binomial_logit: trials must be a constant scalar or a constant array")
             n = np.asarray(L.trials, dtype=np.float64)
@@ -430,22 +464,24 @@ class ModelIR:
             if not integer(n) or np.any(n < 0):
                 raise ValueError("binomial_logit: trials must be integers >= 0")
             if not integer(y) or np.any(y < 0) or np.any(y > n):
-                raise ValueError("binomial_logit: y must be integers with 0 <= y <= trials")
+                raise ValueError(f"{L.dist}: {ZIB_Y}")
         elif L.trials is not None:
             raise ValueError(f"{L.dist}: trials belong to binomial_logit")
-        if L.dist in DISPERSION_LIKS:
+        if fam in DISPERSION_LIKS:
             if L.alpha is None:
                 raise ValueError(f"{L.dist} needs alpha")
             if isinstance(L.alpha, Ref) and self.var(L.alpha.var).size != 1:
                 raise ValueError(f"{L.dist}: alpha must be a scalar variable")
             self._check_scale(L.alpha, f"{L.dist}: alpha")
-            if L.dist == "negative_binomial_log" and (not integer(y) or np.any(y < 0)):
-                raise ValueError("negative_binomial_log: y must be integers >= 0")
+            if fam == "negative_binomial_log" and (not integer(y) or np.any(y < 0)):
+                raise ValueError(f"{L.dist}: {ZI_Y}")
             if L.dist == "gamma_log" and not (np.all(np.isfinite(y)) and np.all(y > 0)):
                 raise ValueError("gamma_log: y must be > 0")
+            if L.dist == "hurdle_gamma" and not (np.all(np.isfinite(y)) and np.all(y >= 0)):
+                raise ValueError(f"hurdle_gamma: {HG_Y}")
         elif L.alpha is not None:
             raise ValueError(f"{L.dist}: alpha belongs to the negative_binomial_log / gamma_log likelihoods")
-        if L.dist in ("binomial_logit",) + DISPERSION_LIKS and L.sigma is not None:
+        if fam in ("binomial_logit",) + DISPERSION_LIKS and L.sigma is not None:
             raise ValueError(f"{L.dist} has no sigma (its parameter is {'trials' if L.dist == 'binomial_logit' else 'alpha'})")
 
     def _validate_bounds(self, L) -> None:
@@ -497,6 +533,32 @@ class ModelIR:
         y = np.asarray(L.y, dtype=np.float64)
         if not (np.all(np.isfinite(y)) and np.all(y == np.floor(y)) and np.all((y >= 0) & (y <= K - 1))):
             raise ValueError(f"{what}: {ORD_Y}")
+
+    def _validate_psi(self, L) -> None:
+        """psi of zero-inflated / hurdle observations (the checks prepare_ir makes, in the same words)."""
+        what = f"{L.dist} likelihood {L.name}"
+        if L.dist not in ZI_LIKS:
+            if L.psi is not None:
+                raise ValueError(f"{what}: psi belongs to the zero-inflated and hurdle likelihoods")
+            return
+        psi = L.psi
+        if psi is None:
+            raise ValueError(f"{what}: needs psi")
+        if isinstance(psi, Linear):
+            if not psi.terms:
+                raise ValueError(f"{what}: {PSI_BLOCK}")
+            self._check_terms(psi.terms, len(L.y), f"{what}: logit(psi)", "the number of observations")
+        elif isinstance(psi, Ref):
+            v = self.var(psi.var)
+            if not (v.size == 1 and v.transform == "interval" and v.bounds[0] >= 0.0 and v.bounds[1] <= 1.0):
+                raise ValueError(f"{what}: {PSI_VAR}")
+        else:
+            if np.ndim(psi) != 0:  # one constant per observation is not provided
+                raise ValueError(f"{what}: {PSI_BLOCK}")
+            if float(psi) == 1.0:
+                raise ValueError(f"{what}: {PSI_ONE}")
+            if not (np.isfinite(float(psi)) and 0.0 < float(psi) < 1.0):
+                raise ValueError(f"{what}: {PSI_CONST}")
 
     # ---- host-side post-processing (f1): unconstrained draws -> named constrained RVs --------------------------------
     def constrain(self, q: np.ndarray) -> dict:
@@ -575,6 +637,15 @@ class ModelIR:
                     out[f"{L.name}_{side}"] = np.asarray(getattr(L, side))
             if L.cutpoints is not None and not isinstance(L.cutpoints, Ref):  # constant cutpoints of ordinal observations
                 out[f"{L.name}_cutpoints"] = np.asarray(L.cutpoints)
+            if isinstance(L.psi, Linear):  # the data of logit(psi) of zero-inflated / hurdle observations
+                for k, t in enumerate(L.psi.terms):
+                    if t.coef is not None and np.ndim(t.coef) in (1, 2):
+                        out[f"{L.name}_psi_coef{k}"] = np.asarray(t.coef)
+                    for vn, idx in t.factors:
+                        if idx is not None:
+                            out[f"{L.name}_psi_{vn}_idx"] = np.asarray(idx)
+            elif L.psi is not None and not isinstance(L.psi, Ref):  # a constant psi
+                out[f"{L.name}_psi"] = np.asarray(float(L.psi))
         return out
 
 
@@ -827,6 +898,70 @@ def ordinal_regression_ir(link: str = "logistic", n_obs: int = 300, n_groups: in
                    likelihoods=[Likelihood(f"ordered_{link}", y, terms, sigma=s, cutpoints=Ref("cutpoints_ordered__"))])
 
 
+def zero_inflated_ir(dist: str = "zero_inflated_poisson", psi: str = "const", n_obs: int = 300, n_groups: int = 6,
+                     n_features: int = 2, seed: int = 59) -> ModelIR:
+    """A zero-inflated or hurdle regression (``dist`` in ZI_LIKS) on simulated data with real excess zeros:
+    b0 ~ Normal(0, 2), z_g ~ Normal(0, 1) and sigma_a ~ HalfNormal(1) (non-centred group intercepts sigma_a z[g_i]),
+    beta ~ Normal(0, 1)^F as a design term, eta_i = b0 + sigma_a z[g_i] + x_i . beta; the family's alpha ~ Exponential(1)
+    (NegativeBinomial) or HalfNormal(2) (Gamma), and trials 0..11 per observation (Binomial).  psi: "const" (0.65),
+    "var" (psi ~ Beta(2, 2) on interval(0, 1)) or "logit" (logit psi_i = g0 + w_i . gamma with g0 ~ Normal(0, 1.5) and
+    gamma ~ Normal(0, 1)^2 as a design term)."""
+    if dist not in ZI_FAMILY:
+        raise ValueError(f"dist must be one of {ZI_LIKS}")
+    if psi not in ("const", "var", "logit"):
+        raise ValueError("psi must be 'const', 'var' or 'logit'")
+    rng = np.random.default_rng(seed)
+    fam = ZI_FAMILY[dist]
+    g = rng.integers(0, n_groups, n_obs).astype(np.int32)
+    X = rng.standard_normal((n_obs, n_features))
+    Zp = rng.standard_normal((n_obs, 2))
+    eta = 0.8 + rng.normal(0.0, 0.5, n_groups)[g] + X @ rng.normal(0.0, 0.4, n_features)
+    psi_true = {"const": np.full(n_obs, 0.65), "var": np.full(n_obs, 0.6),
+                "logit": 1.0 / (1.0 + np.exp(-(0.4 + Zp @ np.array([0.8, -0.6]))))}[psi]
+    mu, a_true = np.exp(eta), 2.0
+    trials = rng.integers(0, 12, n_obs).astype(np.float64) if fam == "binomial_logit" else None
+
+    def draw(i):
+        if fam == "poisson_log":
+            return rng.poisson(mu[i])
+        if fam == "binomial_logit":
+            return rng.binomial(int(trials[i]), 1.0 / (1.0 + np.exp(-eta[i])))
+        if fam == "negative_binomial_log":
+            return rng.negative_binomial(a_true, a_true / (mu[i] + a_true))
+        return rng.gamma(a_true, mu[i] / a_true)
+
+    y = np.zeros(n_obs)
+    for i in range(n_obs):
+        if rng.random() < psi_true[i]:
+            v = draw(i)
+            while dist.startswith("hurdle") and fam != "gamma_log" and v == 0:  # Truncated(f, lower=1)
+                v = draw(i)
+            y[i] = v
+    vars_ = [Var("b0", "b0", 1), Var("z", "z", n_groups), Var("sigma_a_log__", "sigma_a", 1, "log"),
+             Var("beta", "beta", n_features)]
+    priors = [Prior("normal", "b0", (0.0, 2.0)), Prior("normal", "z", (0.0, 1.0)), Prior("halfnormal", "sigma_a_log__", (1.0,)),
+              Prior("normal", "beta", (0.0, 1.0))]
+    alpha = None
+    if fam in DISPERSION_LIKS:
+        vars_.append(Var("alpha_log__", "alpha", 1, "log"))
+        priors.append(Prior("exponential" if fam == "negative_binomial_log" else "halfnormal", "alpha_log__",
+                            (1.0,) if fam == "negative_binomial_log" else (2.0,)))
+        alpha = Ref("alpha_log__")
+    if psi == "const":
+        p = 0.65
+    elif psi == "var":
+        vars_.append(Var("psi_logodds__", "psi", 1, "interval", bounds=(0.0, 1.0)))
+        priors.append(Prior("beta", "psi_logodds__", (2.0, 2.0)))
+        p = Ref("psi_logodds__")
+    else:
+        vars_ += [Var("g0", "g0", 1), Var("gamma", "gamma", 2)]
+        priors += [Prior("normal", "g0", (0.0, 1.5)), Prior("normal", "gamma", (0.0, 1.0))]
+        p = Linear([Term([("g0", None)]), Term([("gamma", None)], coef=Zp)])
+    terms = [Term([("b0", None)]), Term([("sigma_a_log__", None), ("z", g)]), Term([("beta", None)], coef=X)]
+    return ModelIR(name=f"{dist}_{psi}", vars=vars_, priors=priors,
+                   likelihoods=[Likelihood(dist, y, terms, alpha=alpha, trials=trials, psi=p)])
+
+
 # ------------------------------------------------------------------------------------------------------------------------
 # lowering: ModelIR -> flat arrays of the C ABI (include/b200nuts.h: b200_ir)
 # ------------------------------------------------------------------------------------------------------------------------
@@ -842,6 +977,7 @@ class LoweredIR:
                             # a design term's dict also has n_cols = K, with coef = X [N][K]
                             # censored_normal / truncated_normal: y is the [3][N] block (y, lower, upper)
                             # ordered_logistic / ordered_probit: nu = K, and cut = the cutpoint term (a term dict)
+                            # zero-inflated / hurdle: nu = 0 or m, and psi = the psi block (a list of term dicts)
                             # y_var 0: y is observed data; v + 1: a latent factor, y is None and its values are variable v's
     ar1: list               # [(var, phi(kind, value, ref), sigma(kind, value, ref), init_sigma)]
 
@@ -912,7 +1048,8 @@ def lower(ir: ModelIR) -> LoweredIR:
     liks = []
     for L in ir.likelihoods:
         # the likelihood's one parameter slot: sigma, or the trials / alpha of the count and positive families
-        par = L.trials if L.dist == "binomial_logit" else (L.alpha if L.dist in DISPERSION_LIKS else L.sigma)
+        fam = ZI_FAMILY.get(L.dist, L.dist)
+        par = L.trials if fam == "binomial_logit" else (L.alpha if fam in DISPERSION_LIKS else L.sigma)
         y = np.ascontiguousarray(L.y, dtype=np.float64)
         if L.dist in BOUNDED_LIKS:  # the [3][N] block: y, lower, upper
             y = np.ascontiguousarray(np.stack([y, *L.bounds()]))
@@ -922,6 +1059,14 @@ def lower(ir: ModelIR) -> LoweredIR:
             extra = dict(nu=float(L.n_categories(ir)),
                          cut=dict(coef=None, factors=[(off[ir.var(c.var).name], ir.var(c.var).size, None)])
                          if isinstance(c, Ref) else dict(coef=np.ascontiguousarray(c, dtype=np.float64), factors=[]))
+        if L.dist in ZI_LIKS:  # the psi block goes one past the predictor's terms; nu = 0 (psi) or its number of terms
+            psi = L.psi
+            if isinstance(psi, Linear):
+                extra = dict(nu=float(len(psi.terms)), psi=_lower_terms(ir, psi.terms, len(L.y), off))
+            elif isinstance(psi, Ref):
+                extra = dict(nu=0.0, psi=[dict(coef=None, factors=[(off[ir.var(psi.var).name], 1, None)])])
+            else:
+                extra = dict(nu=0.0, psi=[dict(coef=np.array([float(psi)]), factors=[])])
         liks.append(dict(dict(dist=LIK_DISTS[L.dist], N=len(L.y), y=y,
                               terms=_lower_terms(ir, L.terms, len(L.y), off), nu=float(L.nu), y_var=0,
                               **_lower_slot(ir, par, off)), **extra))
@@ -961,10 +1106,12 @@ def fuse_design_columns(model: ModelIR) -> ModelIR:
     one term per column k = 0..K-1 of the same vector variable of size K, as ``from_pymc`` lowers ``pm.math.dot(X, beta)``
     -- is one design term with X[:, k] = the column's coefficient, placed where the run's first term was.  Partial or
     duplicated runs, indexed group effects, multi-factor terms and Deterministics stay as written; ``model`` itself is
-    not changed."""
+    not changed.  The terms of a likelihood's logit(psi) are fused the same way."""
     out = copy.deepcopy(model)
     for L in out.likelihoods:
         L.terms = _fuse_terms(out, L.terms, len(L.y))
+        if isinstance(L.psi, Linear):  # logit(psi) of a zero-inflated / hurdle likelihood
+            L.psi = Linear(_fuse_terms(out, L.psi.terms, len(L.y)))
     for p in out.priors:
         p.params = tuple(Linear(_fuse_terms(out, a.terms, out.var(p.var).size)) if isinstance(a, Linear) else a
                          for a in p.params)
@@ -1012,7 +1159,7 @@ def specialise(ir: ModelIR, extended: bool = False):
         return not isinstance(p.params[k], Ref) and (want is None or float(p.params[k]) == want)
 
     pri = {ir.var(p.var).name: p for p in ir.priors}
-    if len(pri) != len(ir.priors) or len(ir.likelihoods) != 1:
+    if len(pri) != len(ir.priors) or len(ir.likelihoods) != 1 or ir.likelihoods[0].dist in ZI_LIKS:
         return None
     if any(isinstance(a, Linear) or (not isinstance(a, Ref) and np.ndim(a) > 0) for p in ir.priors for a in p.params):
         return None

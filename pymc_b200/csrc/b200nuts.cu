@@ -128,9 +128,10 @@ struct b200_model {
     const double* tr_lo = nullptr;
     const double* tr_hi = nullptr;
     IrModel::Params ir{};
-    long long ir_max_obs = 0;
-    bool ir_extended = false;  // a censored / truncated Normal or ordinal likelihood, or an ordered variable: the kernels
-                               // run IrExtendedModel
+    std::vector<IrLikD> ir_liks;  // the host copy of ir.liks
+    DevBuf ir_tables;             // the data arrays ir's tables point into (prepare_ir)
+    bool ir_extended = false;  // a censored / truncated Normal, ordinal, zero-inflated or hurdle likelihood, or an ordered
+                               // variable: the kernels run IrExtendedModel
     DevBuf ir_scratch;  // per-team scratch of the generic IR device function: [teams][n_pad + max N] doubles
     // lock-step (GEMM-shaped) models; every matrix is row-major with rows `ld` doubles apart (n rounded up to 4, zero pad)
     long long ld = 0;
@@ -186,6 +187,89 @@ static int upload_raw(b200_model* m, const T* h, size_t count, const T** out) {
 template <class T>
 static int upload(b200_model* m, const std::vector<T>& h, const T** out) { return upload_raw(m, h.data(), h.size(), out); }
 
+// The array arguments of one C-ABI call.  With B200_MEM_DEVICE the kernels use the caller's pointers; with B200_MEM_HOST
+// every non-null array gets a device copy.  Those copies are lent from ONE arena in the model handle (stage_arena unless
+// another is given), sized in commit() from the requests themselves, so a steady-state call makes no cudaMalloc / cudaFree
+// at all (per-call allocations synchronise the device and make a public-API call take far longer than its kernel).
+//   DIRECT: an OUTPUT in page-locked host memory (cudaHostAlloc / cudaHostRegister, e.g. a torch pinned tensor) is written
+//           by the kernel itself through its device alias (UVA), so the device->host transfer overlaps the run instead of
+//           following it (2.9 GB of draws per Radon bench step).
+//   OWN:    a per-call allocation instead of arena space, for arrays the arena must not grow to (the draws).
+// Usage: add() every array, commit() before the launch, finish() after it.
+class Staging {
+  public:
+    enum Dir { IN = 1, OUT = 2, INOUT = 3 };
+    enum Flag { DIRECT = 1, OWN = 2 };
+    Staging(b200_model* m, int mem, cudaStream_t st, DevBuf* arena = nullptr)
+        : arena_(arena ? *arena : m->stage_arena), host_(mem == B200_MEM_HOST), st_(st) {}
+    // `count` elements at `user`, no CUDA call; commit() stores the pointer the kernels use in *dst
+    template <class T>
+    void add(T** dst, T* user, size_t count, Dir dir, int flags = 0) {
+        reqs_.push_back(Req{dst, &put<T>, const_cast<void*>(static_cast<const void*>(user)), count * sizeof(T), dir, flags});
+    }
+    int commit() {
+        size_t lent = 0;
+        for (Req& r : reqs_) {
+            r.copy = host_ && r.user;
+            if (r.copy && (r.flags & DIRECT) && r.dir == OUT) {
+                cudaPointerAttributes at{};
+                if (cudaPointerGetAttributes(&at, r.user) == cudaSuccess && at.type == cudaMemoryTypeHost && at.devicePointer) {
+                    r.dev = at.devicePointer;
+                    r.copy = false;
+                } else {
+                    cudaGetLastError();  // pageable memory: not an error, fall back to a device copy
+                }
+            }
+            if (r.copy && !(r.flags & OWN)) {
+                r.off = lent;
+                lent += (r.bytes + 255) & ~(size_t)255;
+            }
+        }
+        if (lent) CU(arena_.reserve(lent));
+        for (Req& r : reqs_) {
+            if (r.copy) {
+                if (r.flags & OWN) {
+                    own_.emplace_back();
+                    CU(own_.back().reserve(r.bytes));
+                    r.dev = own_.back().p;
+                } else {
+                    r.dev = arena_.as<char>() + r.off;
+                }
+                if (r.dir & IN) CU(cudaMemcpyAsync(r.dev, r.user, r.bytes, cudaMemcpyHostToDevice, st_));
+            } else if (!r.dev) {
+                r.dev = r.user;
+            }
+            r.put(r.dst, r.dev);
+        }
+        return 0;
+    }
+    // device->host copies of the outputs, then wait for the stream
+    int finish() {
+        for (const Req& r : reqs_)
+            if (r.copy && (r.dir & OUT)) CU(cudaMemcpyAsync(r.user, r.dev, r.bytes, cudaMemcpyDeviceToHost, st_));
+        CU(cudaStreamSynchronize(st_));
+        return 0;
+    }
+
+  private:
+    struct Req {
+        void* dst;
+        void (*put)(void* dst, void* dev);
+        void* user;
+        size_t bytes;
+        int dir, flags;
+        bool copy = false;  // a device copy of a host array
+        size_t off = 0;     // its place in the arena
+        void* dev = nullptr;
+    };
+    template <class T> static void put(void* dst, void* dev) { *static_cast<T**>(dst) = static_cast<T*>(dev); }
+    DevBuf& arena_;
+    bool host_;
+    cudaStream_t st_;
+    std::vector<Req> reqs_;
+    std::deque<DevBuf> own_;
+};
+
 extern "C" int b200_version(void) { return B200NUTS_VERSION; }
 extern "C" const char* b200_last_error(void) { return g_err.c_str(); }
 extern "C" int b200_struct_size(int which) {
@@ -219,6 +303,12 @@ extern "C" int b200_device_count(void) {
 
 extern "C" int b200_set_device(int device) {
     CU(cudaSetDevice(device));
+    return 0;
+}
+
+static int use_current_device(b200_model* m) {  // a new handle's tables go to the caller's current device
+    if (b200_device_count() == 0) return fail("b200_model_create: no CUDA device visible");
+    cudaGetDevice(&m->device);
     return 0;
 }
 
@@ -347,11 +437,12 @@ static int prepare_logistic(b200_model* m, const b200_model_desc* d) {
     return 0;
 }
 
-
 // ------------------------------------------------------------------------------------------------
 // ModelSpec IR -> device tables (csrc/ir_model.cuh).  Validates the closed set, precomputes the constant parts of the
 // densities on the host (lgamma, log 2pi ...) and builds, for every indexed factor, the CSR transpose of its gather index
-// (element -> observations) that the gradient is pulled through (deterministic, no atomics).
+// (element -> observations) that the gradient is pulled through (deterministic, no atomics).  All of it is one host pass
+// that makes no CUDA call, so a description is refused in the same words with or without a device; prepare_ir uploads the
+// tables once it is accepted.
 // ------------------------------------------------------------------------------------------------
 static int ir_param(const b200_ir_param& p, int n, IrParamD* out, const char* what) {
     if (p.kind != 0 && p.kind != 1) return fail("ir: %s: parameter kind %d", what, p.kind);
@@ -399,445 +490,437 @@ static bool ir_scale_ok(const b200_ir_param& p, const std::vector<IrVarD>& vars)
 #define B200_IR_ZIB_Y "y must be integers with 0 <= y <= trials"
 #define B200_IR_HG_Y "y must be finite and >= 0"
 #define B200_IR_ZIP_SLOT "zero_inflated_poisson and hurdle_poisson take no sigma, trials or alpha"
+static constexpr double LOG_PI = 1.1447298858494001741, LOG_2 = 0.69314718055994530942;
+
+// The pass over a b200_ir.  Its steps return 0 or fail(...); the arrays they record in `sg` stay put until the upload.
+struct IrPass {
+    Staging& sg;
+    int n;  // elements of q
+    std::vector<IrVarD> vars;
+    std::deque<IrTermD> terms;
+    std::deque<std::vector<int>> ints;  // the CSR tables
+    std::deque<std::vector<double>> reals;  // Xt, the distinct-count tables
+    std::deque<std::vector<signed char>> codes;  // the censoring codes
+    // the largest N of any likelihood / of an ordinal one (its w row) / of a logit psi (its zeta row)
+    long long max_obs = 0, ord_obs = 0, zeta_obs = 0;
+    bool has_design = false;
+    template <class T> void add(const T** dst, const T* host, size_t count) { sg.add(dst, host, count, Staging::IN); }
+};
+
+static const IrVarD* ir_var_at(const std::vector<IrVarD>& vars, int offset) {
+    for (const IrVarD& V : vars)
+        if (V.offset == offset) return &V;
+    return nullptr;
+}
+
+// CSR transpose of key[0 .. N) in [0, K): rowobs[rowptr[k] .. rowptr[k + 1]) are the i with key[i] = k, ascending
+template <class Key>
+static void ir_csr(IrPass& c, const Key* key, long long N, int K, IrFactorD& F) {
+    std::vector<int>& rowptr = c.ints.emplace_back((size_t)K + 1);
+    std::vector<int>& rowobs = c.ints.emplace_back((size_t)N);
+    for (long long i = 0; i < N; ++i) ++rowptr[(int)key[i] + 1];
+    for (int k = 0; k < K; ++k) rowptr[k + 1] += rowptr[k];
+    std::vector<int> fill(rowptr.begin(), rowptr.end() - 1);
+    for (long long i = 0; i < N; ++i) rowobs[fill[(int)key[i]]++] = (int)i;
+    c.add(&F.rowptr, rowptr.data(), rowptr.size());
+    c.add(&F.rowobs, rowobs.data(), rowobs.size());
+}
+
+static int ir_vars(IrPass& c, const b200_ir& R) {
+    if (R.n_vars <= 0 || !R.vars) return fail("ir: no value variables");
+    int off = 0;
+    for (int v = 0; v < R.n_vars; ++v) {
+        const b200_ir_var& V = R.vars[v];
+        if (V.offset != off || V.size <= 0) return fail("ir: variable %d: offsets must be contiguous in registration order", v);
+        if (V.transform < B200_IR_T_NONE || V.transform > B200_IR_T_ORDERED_POSITIVE) return fail("ir: variable %d: transform %d", v, V.transform);
+        if (V.transform == B200_IR_T_INTERVAL && !(V.lo < V.hi)) return fail("ir: variable %d: interval needs lo < hi", v);
+        c.vars.push_back(IrVarD{V.offset, V.size, V.transform, 0, V.lo, V.hi});
+        off += V.size;
+    }
+    if (off != c.n) return fail("ir: variables cover %d elements but n = %d", off, c.n);
+    return 0;
+}
+
+static int ir_prior(const IrPass& c, const b200_ir_prior& F, int k, IrPriorD& P) {
+    if (F.var < 0 || F.var >= (int)c.vars.size()) return fail("ir: prior %d: variable index %d", k, F.var);
+    const IrVarD& PV = c.vars[F.var];
+    P.dist = F.dist; P.offset = PV.offset; P.size = PV.size;
+    for (int a = 0; a < 3; ++a)
+        if (ir_param(F.p[a], c.n, &P.p[a], "prior")) return -1;
+    auto cst = [&](int a) { return F.p[a].kind == 0; };
+    int scale = -1;  // which parameter is the prior's scale
+    switch (F.dist) {
+        case B200_IR_P_NORMAL: case B200_IR_P_LOGNORMAL: case B200_IR_P_CAUCHY: scale = 1; break;
+        case B200_IR_P_HALFNORMAL: case B200_IR_P_HALFCAUCHY: case B200_IR_P_EXPONENTIAL: scale = 0; break;
+        case B200_IR_P_STUDENTT: scale = 2; break;
+        default: break;
+    }
+    if (scale >= 0 && !ir_scale_ok(F.p[scale], c.vars)) return fail("ir: prior %d: parameter %d (the scale) " B200_IR_SCALE_RULE, k, scale);
+    const bool positive = F.dist == B200_IR_P_HALFNORMAL || F.dist == B200_IR_P_HALFCAUCHY || F.dist == B200_IR_P_EXPONENTIAL ||
+                          F.dist == B200_IR_P_GAMMA || F.dist == B200_IR_P_LOGNORMAL;
+    const bool real_line = F.dist == B200_IR_P_FLAT || F.dist == B200_IR_P_NORMAL || F.dist == B200_IR_P_STUDENTT ||
+                           F.dist == B200_IR_P_CAUCHY;
+    if (PV.transform >= IRT_ORDERED && !(real_line || (positive && PV.transform == IRT_ORDERED_POSITIVE)))
+        return fail("ir: prior %d: " B200_IR_ORDERED_PRIOR, k);
+    if (positive && !ir_positive_support(PV))
+        return fail("ir: prior %d: the variable needs a log transform or an interval with lo >= 0 (positive support)", k);
+    switch (F.dist) {
+        case B200_IR_P_FLAT: case B200_IR_P_EXPONENTIAL: break;
+        case B200_IR_P_NORMAL: case B200_IR_P_LOGNORMAL: P.c0 = -B200_HALF_LOG_2PI; break;
+        case B200_IR_P_HALFNORMAL: P.c0 = 0.5 * (LOG_2 - LOG_PI); break;
+        case B200_IR_P_CAUCHY: P.c0 = -LOG_PI; break;
+        case B200_IR_P_HALFCAUCHY: P.c0 = LOG_2 - LOG_PI; break;
+        case B200_IR_P_STUDENTT: {
+            if (!cst(0) || !(F.p[0].value > 0)) return fail("ir: prior %d: StudentT nu must be a positive constant", k);
+            const double nu = F.p[0].value;
+            P.c0 = std::lgamma(0.5 * (nu + 1.0)) - std::lgamma(0.5 * nu) - 0.5 * std::log(nu) - 0.5 * LOG_PI;
+        } break;
+        case B200_IR_P_UNIFORM:
+            if (!cst(0) || !cst(1) || !(F.p[0].value < F.p[1].value)) return fail("ir: prior %d: Uniform bounds must be constants lo < hi", k);
+            if (!(PV.transform == IRT_INTERVAL && PV.lo >= F.p[0].value && PV.hi <= F.p[1].value))
+                return fail("ir: prior %d: the variable needs an interval inside the Uniform bounds", k);
+            P.c0 = -std::log(F.p[1].value - F.p[0].value);
+            break;
+        case B200_IR_P_GAMMA:
+            if (!cst(0) || !cst(1) || !(F.p[0].value > 0) || !(F.p[1].value > 0)) return fail("ir: prior %d: Gamma needs constant alpha, beta > 0", k);
+            P.c0 = F.p[0].value * std::log(F.p[1].value) - std::lgamma(F.p[0].value);
+            break;
+        case B200_IR_P_BETA:
+            if (!cst(0) || !cst(1) || !(F.p[0].value > 0) || !(F.p[1].value > 0)) return fail("ir: prior %d: Beta needs constant alpha, beta > 0", k);
+            if (!(PV.transform == IRT_INTERVAL && PV.lo >= 0 && PV.hi <= 1)) return fail("ir: prior %d: the variable needs an interval inside [0, 1]", k);
+            P.c0 = -(std::lgamma(F.p[0].value) + std::lgamma(F.p[1].value) - std::lgamma(F.p[0].value + F.p[1].value));
+            break;
+        default: return fail("ir: prior %d: density %d is not in the closed set", k, F.dist);
+    }
+    return 0;
+}
+
+// Family `fam` (Poisson, Binomial, NegativeBinomial, Gamma), plain or inside a zero-inflated / hurdle likelihood (`zeros`:
+// y = 0 is allowed, and the Gamma normaliser covers the N+ y > 0 only): slot rules, y (`ybad`) and trials checks, constants.
+// The plain Binomial checks trials before y and sums binomln(n, y) as one term; the zero-inflated one checks y first.
+static int ir_family(IrPass& c, const b200_ir_lik& L, int l, const b200_ir_param& slot, int fam, const char* ybad, bool zeros,
+                     IrLikD& D) {
+    const bool bin = fam == B200_IR_L_BINOMIAL_LOGIT, nb = fam == B200_IR_L_NEGBINOMIAL_LOG, gam = fam == B200_IR_L_GAMMA_LOG;
+    const char* name = gam ? "Gamma" : "NegativeBinomial";
+    if (bin && L.sigma_kind != B200_IR_S_CONST && L.sigma_kind != B200_IR_S_OBS)
+        return fail("ir: likelihood %d: Binomial trials must be a constant or one per observation", l);
+    if ((nb || gam) && L.sigma_kind != B200_IR_S_CONST && L.sigma_kind != B200_IR_S_REF)
+        return fail("ir: likelihood %d: %s alpha must be a constant or a scalar variable", l, name);
+    if ((nb || gam) && !ir_scale_ok(slot, c.vars)) return fail("ir: likelihood %d: %s alpha " B200_IR_SCALE_RULE, l, name);
+    const double a = L.sigma.value;
+    const bool fold = nb && L.sigma_kind == B200_IR_S_CONST && a <= kNegBinPoissonAlpha;
+    double c0 = 0, sly = 0;
+    long long n_pos = 0;
+    std::map<double, double> count;  // distinct nonzero y -> multiplicity, ascending
+    for (long long i = 0; i < L.N; ++i) {
+        const double y = L.y[i];
+        if (gam) {
+            if (!(std::isfinite(y) && (zeros ? y >= 0 : y > 0))) return fail("ir: likelihood %d: %s (at %lld)", l, ybad, i);
+            if (y > 0) { sly += std::log(y); ++n_pos; }
+            continue;
+        }
+        const bool natural = y >= 0 && y == std::floor(y) && !std::isinf(y);  // an integer >= 0
+        if (!natural && (zeros || !bin)) return fail("ir: likelihood %d: %s (at %lld)", l, ybad, i);
+        const double nt = !bin ? 0.0 : L.sigma_kind == B200_IR_S_OBS ? L.sigma_obs[i] : L.sigma.value;
+        if (bin && !(std::isfinite(nt) && nt >= 0 && nt == std::floor(nt)))
+            return fail("ir: likelihood %d: Binomial trials must be integers >= 0 (at %lld)", l, i);
+        if (bin && (!natural || y > nt)) return fail("ir: likelihood %d: %s (at %lld)", l, zeros ? B200_IR_ZIB_Y : ybad, i);
+        if (bin && !zeros) c0 += std::lgamma(nt + 1.0) - std::lgamma(y + 1.0) - std::lgamma(nt - y + 1.0);
+        else c0 -= std::lgamma(y + 1.0);  // 0 at y = 0, as every constant below
+        if (bin && zeros) c0 += std::lgamma(nt + 1.0) - std::lgamma(nt - y + 1.0);
+        if (fold) c0 += std::lgamma(y + a) - std::lgamma(a);
+        if (nb && y > 0) count[y] += 1.0;
+    }
+    if (gam && L.sigma_kind == B200_IR_S_CONST) {
+        c0 = (double)n_pos * (a * std::log(a) - std::lgamma(a)) + (a - 1.0) * sly;
+    } else if (gam) {
+        D.sum_log_y = sly;
+        if (zeros) D.n_tab = (int)n_pos;  // N+
+    }
+    D.c0 = c0;
+    if (nb && L.sigma_kind == B200_IR_S_REF) {  // a random alpha's normaliser sums over the distinct-count table
+        std::vector<double>& u = c.reals.emplace_back();
+        std::vector<double>& cnt = c.reals.emplace_back();
+        for (const auto& kv : count) { u.push_back(kv.first); cnt.push_back(kv.second); }
+        D.n_tab = (int)u.size();
+        c.add(&D.tab_u, u.data(), u.size());
+        c.add(&D.tab_cnt, cnt.data(), cnt.size());
+    }
+    return 0;
+}
+
+// censored / truncated Normal: y is the [3][N] block (y, lower, upper)
+static int ir_bounds(IrPass& c, const b200_ir_lik& L, int l, IrLikD& D) {
+    const long long N = L.N;
+    const bool cens = L.dist == B200_IR_L_CENSORED_NORMAL;
+    const char* what = cens ? "censored_normal" : "truncated_normal";
+    const double *y = L.y, *lo = L.y + N, *hi = L.y + 2 * N;
+    std::vector<signed char>& code = c.codes.emplace_back(cens ? (size_t)N : 0);
+    long long n_observed = 0;
+    bool bounded = false;
+    for (long long i = 0; i < N; ++i) {
+        if (std::isnan(lo[i]) || std::isnan(hi[i]) || lo[i] == INFINITY || hi[i] == -INFINITY)
+            return fail("ir: likelihood %d: %s: " B200_IR_BOUND_SIDES " (at %lld)", l, what, i);
+        if (!(lo[i] < hi[i])) return fail("ir: likelihood %d: %s: " B200_IR_BOUND_ORDER " (at %lld)", l, what, i);
+        if (!(std::isfinite(y[i]) && lo[i] <= y[i] && y[i] <= hi[i]))
+            return fail("ir: likelihood %d: %s: " B200_IR_BOUND_Y " (at %lld)", l, what, i);
+        bounded = bounded || std::isfinite(lo[i]) || std::isfinite(hi[i]);
+        if (cens) {
+            code[i] = y[i] == lo[i] ? 1 : (y[i] == hi[i] ? 2 : 0);
+            n_observed += code[i] == 0;
+        }
+    }
+    if (!cens && !bounded) return fail("ir: likelihood %d: " B200_IR_TRUNC_OPEN, l);
+    // -log(2 pi) / 2 of every Normal density term: each uncensored observation, every truncated one
+    D.c0 = -(double)(cens ? n_observed : N) * B200_HALF_LOG_2PI;
+    if (cens) c.add(&D.cens, code.data(), code.size());
+    else c.add(&D.bnd, lo, 2 * (size_t)N);
+    return 0;
+}
+
+// ordered logistic / probit: nu = K
+static int ir_ordinal(IrPass& c, const b200_ir_lik& L, int l) {
+    const double K = L.nu;
+    if (!(K >= 2 && K == std::floor(K) && K <= 0x7fffffff)) return fail("ir: likelihood %d: " B200_IR_ORD_K, l);
+    for (long long i = 0; i < L.N; ++i)
+        if (!(L.y[i] >= 0 && L.y[i] <= K - 1) || L.y[i] != std::floor(L.y[i]))
+            return fail("ir: likelihood %d: " B200_IR_ORD_Y " (at %lld)", l, i);
+    if (L.dist == B200_IR_L_ORDERED_LOGISTIC && L.sigma_kind != B200_IR_S_NONE)
+        return fail("ir: likelihood %d: " B200_IR_LOGISTIC_SIGMA, l);
+    c.ord_obs = std::max(c.ord_obs, (long long)L.N);
+    return 0;
+}
+
+// terms[t0 .. t1) of a likelihood: the predictor's, or those of the logit of a zero-inflated / hurdle psi
+static int ir_terms(IrPass& c, const b200_ir_lik& L, int l, int t0, int t1) {
+    const long long N = L.N;
+    for (int t = t0; t < t1; ++t) {
+        const b200_ir_term& T = L.terms[t];
+        if (T.n_factors < 0 || T.n_factors > 3) return fail("ir: likelihood %d term %d: 0..3 variable factors", l, t);
+        IrTermD& TD = c.terms.emplace_back();
+        TD.n_factors = T.n_factors;
+        if (T.n_cols != 0) {  // design term: coef is X [N][n_cols]; the same checks and words as ModelIR.validate()
+            const int K = T.n_cols;
+            if (T.n_factors != 1) return fail("ir: likelihood %d term %d: a design term has exactly one factor", l, t);
+            if (T.f[0].idx) return fail("ir: likelihood %d term %d: a design term's factor takes no index", l, t);
+            if (K < 0 || T.f[0].size != K || !T.coef)
+                return fail("ir: likelihood %d term %d: X must have shape (N, size of the variable)", l, t);
+            if (T.f[0].offset < 0 || T.f[0].offset + K > c.n) return fail("ir: likelihood %d term %d: factor slice outside q", l, t);
+            std::vector<double>& xt = c.reals.emplace_back((size_t)N * K);
+            for (long long i = 0; i < N; ++i)
+                for (int k = 0; k < K; ++k) {
+                    const double v = T.coef[i * K + k];
+                    if (!std::isfinite(v)) return fail("ir: likelihood %d term %d: X must be finite (at row %lld, column %d)", l, t, i, k);
+                    xt[(size_t)k * N + i] = v;
+                }
+            TD.n_cols = K;
+            TD.f[0] = IrFactorD{T.f[0].offset, K, nullptr, nullptr, nullptr};
+            c.add(&TD.coef, T.coef, (size_t)N * K);
+            c.add(&TD.xt, xt.data(), xt.size());
+            c.has_design = true;
+            continue;
+        }
+        if (T.coef) c.add(&TD.coef, T.coef, (size_t)N);
+        for (int f = 0; f < T.n_factors; ++f) {
+            const b200_ir_factor& F = T.f[f];
+            if (F.offset < 0 || F.size <= 0 || F.offset + F.size > c.n) return fail("ir: likelihood %d term %d: factor slice outside q", l, t);
+            IrFactorD& FD = TD.f[f];
+            FD.offset = F.offset; FD.size = F.size;
+            if (F.idx) {
+                for (long long i = 0; i < N; ++i)
+                    if (F.idx[i] < 0 || F.idx[i] >= F.size) return fail("ir: likelihood %d term %d: index %d out of range at %lld", l, t, F.idx[i], i);
+                c.add(&FD.idx, F.idx, (size_t)N);
+                ir_csr(c, F.idx, N, F.size, FD);
+            } else if (F.size != 1 && F.size != N) {
+                return fail("ir: likelihood %d term %d: a variable of size %d needs an index to enter %lld observations", l, t, F.size, N);
+            }
+        }
+    }
+    return 0;
+}
+
+// the psi block at terms[n_terms ..]: nu = 0, psi itself; nu = m >= 1, the m terms of logit(psi)
+static int ir_psi(IrPass& c, const b200_ir_lik& L, int l) {
+    if (L.nu > 0) {
+        c.zeta_obs = std::max(c.zeta_obs, (long long)L.N);
+        return ir_terms(c, L, l, L.n_terms, L.n_terms + (int)L.nu);
+    }
+    const b200_ir_term& T = L.terms[L.n_terms];
+    if (T.n_cols != 0 || (T.n_factors == 0) != (T.coef != nullptr) || T.n_factors > 1 || T.n_factors < 0)
+        return fail("ir: likelihood %d: " B200_IR_PSI_BLOCK, l);
+    IrTermD& TD = c.terms.emplace_back();
+    if (T.n_factors == 0) {
+        const double psi = T.coef[0];
+        if (psi == 1.0) return fail("ir: likelihood %d: " B200_IR_PSI_ONE, l);
+        if (!(std::isfinite(psi) && psi > 0.0 && psi < 1.0)) return fail("ir: likelihood %d: " B200_IR_PSI_CONST, l);
+        c.add(&TD.coef, T.coef, 1);
+    } else {
+        const b200_ir_factor& F = T.f[0];
+        const IrVarD* V = ir_var_at(c.vars, F.offset);
+        if (F.idx || !V || V->size != 1 || F.size != 1 || V->transform != IRT_INTERVAL || !(V->lo >= 0.0 && V->hi <= 1.0))
+            return fail("ir: likelihood %d: " B200_IR_PSI_VAR, l);
+        TD.n_factors = 1;
+        TD.f[0] = IrFactorD{F.offset, 1, nullptr, nullptr, nullptr};
+    }
+    return 0;
+}
+
+// the cutpoint term at terms[n_terms]: one unindexed factor on a variable of size K - 1, or K - 1 constants in coef
+static int ir_cutpoints(IrPass& c, const b200_ir_lik& L, int l) {
+    const int K = (int)L.nu;
+    const b200_ir_term& T = L.terms[L.n_terms];
+    if (T.n_cols != 0 || T.n_factors < 0 || T.n_factors > 1)
+        return fail("ir: likelihood %d: the cutpoint term is one variable or K - 1 constants", l);
+    IrTermD& TD = c.terms.emplace_back();
+    if (T.n_factors == 1) {
+        const b200_ir_factor& F = T.f[0];
+        const IrVarD* V = ir_var_at(c.vars, F.offset);
+        if (F.idx || !V || V->size != F.size) return fail("ir: likelihood %d: the cutpoint factor must be a whole variable, unindexed", l);
+        if (F.size != K - 1) return fail("ir: likelihood %d: " B200_IR_CUT_SIZE " (%d, K = %d)", l, F.size, K);
+        if (F.size > 1 && V->transform != IRT_ORDERED && V->transform != IRT_ORDERED_POSITIVE)
+            return fail("ir: likelihood %d: " B200_IR_CUT_ORDERED, l);
+        TD.n_factors = 1;
+        TD.f[0] = IrFactorD{F.offset, F.size, nullptr, nullptr, nullptr};
+        ir_csr(c, L.y, L.N, K, TD.f[0]);  // the observations of each category
+    } else {
+        if (!T.coef) return fail("ir: likelihood %d: " B200_IR_CUT_CONST, l);
+        for (int k = 0; k < K - 1; ++k)
+            if (!std::isfinite(T.coef[k]) || (k > 0 && !(T.coef[k] > T.coef[k - 1])))
+                return fail("ir: likelihood %d: " B200_IR_CUT_CONST " (at %d)", l, k);
+        c.add(&TD.coef, T.coef, (size_t)K - 1);
+    }
+    return 0;
+}
+
+static int ir_lik(IrPass& c, const b200_ir_lik& L, int l, IrLikD& D) {
+    const int n_vars = (int)c.vars.size();
+    // y_var = v + 1: a latent factor, a Normal / StudentT prior on variable v with a linear-predictor location
+    if (L.y_var < 0 || L.y_var > n_vars) return fail("ir: likelihood %d: y_var %d outside [0, n_vars = %d]", l, L.y_var, n_vars);
+    const bool latent = L.y_var > 0;
+    if (latent && L.dist != B200_IR_L_NORMAL && L.dist != B200_IR_L_STUDENTT)
+        return fail("ir: likelihood %d: a latent factor (y_var > 0) is a normal or studentt prior with a Linear location; dist %d is neither", l, L.dist);
+    if (latent && L.N != c.vars[L.y_var - 1].size)
+        return fail("ir: likelihood %d: a latent factor's N (%lld) must equal the size of its variable (%d)", l, (long long)L.N, c.vars[L.y_var - 1].size);
+    if (L.N <= 0 || L.N > 0x7fffffff || (!latent && !L.y)) return fail("ir: likelihood %d: missing observations", l);
+    if (L.n_terms <= 0 || !L.terms) return fail("ir: likelihood %d: no linear-predictor terms", l);
+    const long long N = L.N;
+    c.max_obs = std::max(c.max_obs, N);
+    D.dist = L.dist; D.n_terms = L.n_terms; D.term0 = (int)c.terms.size(); D.sigma_kind = L.sigma_kind; D.N = N; D.nu = L.nu;
+    D.yoff = latent ? c.vars[L.y_var - 1].offset : -1;
+    if (!latent) c.add(&D.y, L.y, (size_t)N);
+    if (ir_param(L.sigma, c.n, &D.sigma, "likelihood sigma")) return -1;
+    if (L.sigma_kind == B200_IR_S_REF && L.sigma.kind != 1) return fail("ir: likelihood %d: sigma_kind REF needs a reference", l);
+    b200_ir_param slot = L.sigma;  // the parameter slot as the device reads it: x[ref] for REF, else the value
+    slot.kind = L.sigma_kind == B200_IR_S_REF ? 1 : 0;
+    if (L.sigma_kind == B200_IR_S_OBS) {
+        if (!L.sigma_obs) return fail("ir: likelihood %d: sigma_obs missing", l);
+        c.add(&D.sigma_obs, L.sigma_obs, (size_t)N);
+    }
+    int rc = 0;
+    switch (L.dist) {
+        case B200_IR_L_NORMAL: case B200_IR_L_NORMAL_LOGVAR: D.c0 = -(double)N * B200_HALF_LOG_2PI; break;
+        case B200_IR_L_BERNOULLI_LOGIT:
+            for (long long i = 0; i < N; ++i)
+                if (L.y[i] != 0.0 && L.y[i] != 1.0) return fail("ir: likelihood %d: bernoulli_logit: y must be 0 or 1 (at %lld)", l, i);
+            break;
+        case B200_IR_L_STUDENTT:
+            if (!(L.nu > 0)) return fail("ir: likelihood %d: StudentT nu must be > 0", l);
+            D.c0 = (double)N * (std::lgamma(0.5 * (L.nu + 1.0)) - std::lgamma(0.5 * L.nu) - 0.5 * std::log(L.nu) - 0.5 * LOG_PI);
+            break;
+        case B200_IR_L_POISSON_LOG: rc = ir_family(c, L, l, slot, L.dist, "poisson_log: y must be integers >= 0", false, D); break;
+        case B200_IR_L_BINOMIAL_LOGIT: rc = ir_family(c, L, l, slot, L.dist, "Binomial y must be an integer in [0, n]", false, D); break;
+        case B200_IR_L_NEGBINOMIAL_LOG: rc = ir_family(c, L, l, slot, L.dist, "NegativeBinomial y must be an integer >= 0", false, D); break;
+        case B200_IR_L_GAMMA_LOG: rc = ir_family(c, L, l, slot, L.dist, "Gamma y must be > 0", false, D); break;
+        case B200_IR_L_CENSORED_NORMAL: case B200_IR_L_TRUNCATED_NORMAL: rc = ir_bounds(c, L, l, D); break;
+        case B200_IR_L_ORDERED_LOGISTIC: case B200_IR_L_ORDERED_PROBIT: rc = ir_ordinal(c, L, l); break;
+        case B200_IR_L_ZERO_INFLATED_POISSON: case B200_IR_L_ZERO_INFLATED_BINOMIAL:
+        case B200_IR_L_ZERO_INFLATED_NEGATIVE_BINOMIAL: case B200_IR_L_HURDLE_POISSON:
+        case B200_IR_L_HURDLE_NEGATIVE_BINOMIAL: case B200_IR_L_HURDLE_GAMMA: {  // nu: the form of the psi block
+            if (!(L.nu >= 0 && L.nu == std::floor(L.nu) && L.nu <= 0x7fff)) return fail("ir: likelihood %d: " B200_IR_PSI_NU, l);
+            static const int family[] = {B200_IR_L_POISSON_LOG, B200_IR_L_BINOMIAL_LOGIT, B200_IR_L_NEGBINOMIAL_LOG,
+                                         B200_IR_L_POISSON_LOG, B200_IR_L_NEGBINOMIAL_LOG, B200_IR_L_GAMMA_LOG};
+            const int fam = family[L.dist - B200_IR_L_ZERO_INFLATED_POISSON];
+            if (fam == B200_IR_L_POISSON_LOG && L.sigma_kind != B200_IR_S_NONE) return fail("ir: likelihood %d: " B200_IR_ZIP_SLOT, l);
+            rc = ir_family(c, L, l, slot, fam, fam == B200_IR_L_GAMMA_LOG ? B200_IR_HG_Y : B200_IR_ZI_Y, true, D);
+        } break;
+        default: return fail("ir: likelihood %d: density %d is not in the closed set", l, L.dist);
+    }
+    if (rc) return rc;
+    const bool has_sigma = L.dist == B200_IR_L_NORMAL || L.dist == B200_IR_L_STUDENTT || L.dist == B200_IR_L_CENSORED_NORMAL ||
+                           L.dist == B200_IR_L_TRUNCATED_NORMAL || L.dist == B200_IR_L_ORDERED_PROBIT;
+    if (has_sigma && L.sigma_kind == B200_IR_S_NONE) return fail("ir: likelihood %d needs sigma", l);
+    if (has_sigma && L.sigma_kind == B200_IR_S_OBS) {
+        for (long long i = 0; i < N; ++i)
+            if (!(std::isfinite(L.sigma_obs[i]) && L.sigma_obs[i] > 0))
+                return fail("ir: likelihood %d: sigma must be a finite constant > 0 for every observation (at %lld)", l, i);
+    } else if (has_sigma && !ir_scale_ok(slot, c.vars)) {
+        return fail("ir: likelihood %d: sigma " B200_IR_SCALE_RULE, l);
+    }
+    if (ir_terms(c, L, l, 0, L.n_terms)) return -1;
+    if (L.dist == B200_IR_L_ORDERED_LOGISTIC || L.dist == B200_IR_L_ORDERED_PROBIT) return ir_cutpoints(c, L, l);
+    return L.dist >= B200_IR_L_ZERO_INFLATED_POISSON ? ir_psi(c, L, l) : 0;
+}
+
+static int ir_ar1(const IrPass& c, const b200_ir_ar1& A, int k, IrAr1D& D) {
+    if (A.var < 0 || A.var >= (int)c.vars.size() || c.vars[A.var].size < 2) return fail("ir: ar1 %d: bad variable", k);
+    if (!(A.init_sigma > 0)) return fail("ir: ar1 %d: init_sigma must be > 0", k);
+    D.offset = c.vars[A.var].offset; D.size = c.vars[A.var].size; D.init_sigma = A.init_sigma;
+    if (ir_param(A.phi, c.n, &D.phi, "ar1 phi") || ir_param(A.sigma, c.n, &D.sigma, "ar1 sigma")) return -1;
+    if (!ir_scale_ok(A.sigma, c.vars)) return fail("ir: ar1 %d: sigma " B200_IR_SCALE_RULE, k);
+    return 0;
+}
 
 static int prepare_ir(b200_model* m, const b200_model_desc* d) {
     const b200_ir* R = d->ir;
     if (!R) return fail("ir: desc.ir is null");
-    if (R->n_vars <= 0 || !R->vars) return fail("ir: no value variables");
-    const int n = d->n;
-    std::vector<IrVarD> vars(R->n_vars);
-    int off = 0;
-    for (int v = 0; v < R->n_vars; ++v) {
-        const b200_ir_var& V = R->vars[v];
-        if (V.offset != off || V.size <= 0) return fail("ir: variable %d: offsets must be contiguous in registration order", v);
-        if (V.transform < B200_IR_T_NONE || V.transform > B200_IR_T_ORDERED_POSITIVE) return fail("ir: variable %d: transform %d", v, V.transform);
-        m->ir_extended = m->ir_extended || V.transform >= B200_IR_T_ORDERED;
-        if (V.transform == B200_IR_T_INTERVAL && !(V.lo < V.hi)) return fail("ir: variable %d: interval needs lo < hi", v);
-        vars[v] = IrVarD{V.offset, V.size, V.transform, 0, V.lo, V.hi};
-        off += V.size;
-    }
-    if (off != n) return fail("ir: variables cover %d elements but n = %d", off, n);
-    const double LOG_PI = 1.1447298858494001741, LOG_2 = 0.69314718055994530942;
+    Staging sg(m, B200_MEM_HOST, nullptr, &m->ir_tables);
+    IrPass c{sg, d->n};
+    if (ir_vars(c, *R)) return -1;
     std::vector<IrPriorD> priors(std::max(R->n_priors, 0));
-    for (int k = 0; k < R->n_priors; ++k) {
-        const b200_ir_prior& F = R->priors[k];
-        if (F.var < 0 || F.var >= R->n_vars) return fail("ir: prior %d: variable index %d", k, F.var);
-        IrPriorD P{};
-        P.dist = F.dist; P.offset = vars[F.var].offset; P.size = vars[F.var].size;
-        for (int a = 0; a < 3; ++a)
-            if (ir_param(F.p[a], n, &P.p[a], "prior")) return -1;
-        auto cst = [&](int a) { return F.p[a].kind == 0; };
-        const IrVarD& PV = vars[F.var];
-        int scale = -1;  // which parameter is the prior's scale
-        switch (F.dist) {
-            case B200_IR_P_NORMAL: case B200_IR_P_LOGNORMAL: case B200_IR_P_CAUCHY: scale = 1; break;
-            case B200_IR_P_HALFNORMAL: case B200_IR_P_HALFCAUCHY: case B200_IR_P_EXPONENTIAL: scale = 0; break;
-            case B200_IR_P_STUDENTT: scale = 2; break;
-            default: break;
-        }
-        if (scale >= 0 && !ir_scale_ok(F.p[scale], vars)) return fail("ir: prior %d: parameter %d (the scale) " B200_IR_SCALE_RULE, k, scale);
-        const bool positive = F.dist == B200_IR_P_HALFNORMAL || F.dist == B200_IR_P_HALFCAUCHY || F.dist == B200_IR_P_EXPONENTIAL ||
-                              F.dist == B200_IR_P_GAMMA || F.dist == B200_IR_P_LOGNORMAL;
-        const bool real_line = F.dist == B200_IR_P_FLAT || F.dist == B200_IR_P_NORMAL || F.dist == B200_IR_P_STUDENTT ||
-                               F.dist == B200_IR_P_CAUCHY;
-        if (PV.transform >= IRT_ORDERED && !(real_line || (positive && PV.transform == IRT_ORDERED_POSITIVE)))
-            return fail("ir: prior %d: " B200_IR_ORDERED_PRIOR, k);
-        if (positive && !ir_positive_support(PV))
-            return fail("ir: prior %d: the variable needs a log transform or an interval with lo >= 0 (positive support)", k);
-        switch (F.dist) {
-            case B200_IR_P_FLAT: break;
-            case B200_IR_P_NORMAL: case B200_IR_P_LOGNORMAL: P.c0 = -B200_HALF_LOG_2PI; break;
-            case B200_IR_P_HALFNORMAL: P.c0 = 0.5 * (LOG_2 - LOG_PI); break;
-            case B200_IR_P_CAUCHY: P.c0 = -LOG_PI; break;
-            case B200_IR_P_HALFCAUCHY: P.c0 = LOG_2 - LOG_PI; break;
-            case B200_IR_P_EXPONENTIAL: break;
-            case B200_IR_P_STUDENTT: {
-                if (!cst(0) || !(F.p[0].value > 0)) return fail("ir: prior %d: StudentT nu must be a positive constant", k);
-                const double nu = F.p[0].value;
-                P.c0 = std::lgamma(0.5 * (nu + 1.0)) - std::lgamma(0.5 * nu) - 0.5 * std::log(nu) - 0.5 * LOG_PI;
-            } break;
-            case B200_IR_P_UNIFORM:
-                if (!cst(0) || !cst(1) || !(F.p[0].value < F.p[1].value)) return fail("ir: prior %d: Uniform bounds must be constants lo < hi", k);
-                if (!(PV.transform == IRT_INTERVAL && PV.lo >= F.p[0].value && PV.hi <= F.p[1].value))
-                    return fail("ir: prior %d: the variable needs an interval inside the Uniform bounds", k);
-                P.c0 = -std::log(F.p[1].value - F.p[0].value);
-                break;
-            case B200_IR_P_GAMMA:
-                if (!cst(0) || !cst(1) || !(F.p[0].value > 0) || !(F.p[1].value > 0)) return fail("ir: prior %d: Gamma needs constant alpha, beta > 0", k);
-                P.c0 = F.p[0].value * std::log(F.p[1].value) - std::lgamma(F.p[0].value);
-                break;
-            case B200_IR_P_BETA:
-                if (!cst(0) || !cst(1) || !(F.p[0].value > 0) || !(F.p[1].value > 0)) return fail("ir: prior %d: Beta needs constant alpha, beta > 0", k);
-                if (!(PV.transform == IRT_INTERVAL && PV.lo >= 0 && PV.hi <= 1)) return fail("ir: prior %d: the variable needs an interval inside [0, 1]", k);
-                P.c0 = -(std::lgamma(F.p[0].value) + std::lgamma(F.p[1].value) - std::lgamma(F.p[0].value + F.p[1].value));
-                break;
-            default: return fail("ir: prior %d: density %d is not in the closed set", k, F.dist);
-        }
-        priors[k] = P;
-    }
-    std::vector<IrLikD> liks(std::max(R->n_liks, 0));
-    std::vector<IrTermD> terms;
-    // ord_obs / zeta_obs: the largest N of an ordinal likelihood (its w row) / of a logit psi (its zeta row); one row serves both
-    long long max_obs = 0, ord_obs = 0, zeta_obs = 0;
-    bool has_design = false;
-    for (int l = 0; l < R->n_liks; ++l) {
-        const b200_ir_lik& L = R->liks[l];
-        // y_var = v + 1: a latent factor, a Normal / StudentT prior on variable v with a linear-predictor location
-        if (L.y_var < 0 || L.y_var > R->n_vars) return fail("ir: likelihood %d: y_var %d outside [0, n_vars = %d]", l, L.y_var, R->n_vars);
-        const bool latent = L.y_var > 0;
-        if (latent && L.dist != B200_IR_L_NORMAL && L.dist != B200_IR_L_STUDENTT)
-            return fail("ir: likelihood %d: a latent factor (y_var > 0) is a normal or studentt prior with a Linear location; dist %d is neither", l, L.dist);
-        if (latent && L.N != vars[L.y_var - 1].size)
-            return fail("ir: likelihood %d: a latent factor's N (%lld) must equal the size of its variable (%d)", l, (long long)L.N, vars[L.y_var - 1].size);
-        if (L.N <= 0 || L.N > 0x7fffffff || (!latent && !L.y)) return fail("ir: likelihood %d: missing observations", l);
-        if (L.n_terms <= 0 || !L.terms) return fail("ir: likelihood %d: no linear-predictor terms", l);
-        const long long N = L.N;
-        max_obs = std::max(max_obs, N);
-        IrLikD D{};
-        D.dist = L.dist; D.n_terms = L.n_terms; D.term0 = (int)terms.size(); D.sigma_kind = L.sigma_kind; D.N = N; D.nu = L.nu;
-        D.yoff = latent ? vars[L.y_var - 1].offset : -1;
-        if (!latent && upload_raw(m, L.y, (size_t)N, &D.y)) return -1;
-        if (ir_param(L.sigma, n, &D.sigma, "likelihood sigma")) return -1;
-        if (L.sigma_kind == B200_IR_S_REF && L.sigma.kind != 1) return fail("ir: likelihood %d: sigma_kind REF needs a reference", l);
-        b200_ir_param slot = L.sigma;  // the parameter slot as the device reads it: x[ref] for REF, else the value
-        slot.kind = L.sigma_kind == B200_IR_S_REF ? 1 : 0;
-        if (L.sigma_kind == B200_IR_S_OBS) {
-            if (!L.sigma_obs) return fail("ir: likelihood %d: sigma_obs missing", l);
-            if (upload_raw(m, L.sigma_obs, (size_t)N, &D.sigma_obs)) return -1;
-        }
-        switch (L.dist) {
-            case B200_IR_L_NORMAL: case B200_IR_L_NORMAL_LOGVAR: D.c0 = -(double)N * B200_HALF_LOG_2PI; break;
-            case B200_IR_L_BERNOULLI_LOGIT:
-                for (long long i = 0; i < N; ++i)
-                    if (L.y[i] != 0.0 && L.y[i] != 1.0) return fail("ir: likelihood %d: bernoulli_logit: y must be 0 or 1 (at %lld)", l, i);
-                break;
-            case B200_IR_L_POISSON_LOG: {
-                double c = 0;
-                for (long long i = 0; i < N; ++i) {
-                    const double y = L.y[i];
-                    if (!(y >= 0) || y != std::floor(y) || std::isinf(y)) return fail("ir: likelihood %d: poisson_log: y must be integers >= 0 (at %lld)", l, i);
-                    c -= std::lgamma(y + 1.0);
-                }
-                D.c0 = c;
-            } break;
-            case B200_IR_L_STUDENTT:
-                if (!(L.nu > 0)) return fail("ir: likelihood %d: StudentT nu must be > 0", l);
-                D.c0 = (double)N * (std::lgamma(0.5 * (L.nu + 1.0)) - std::lgamma(0.5 * L.nu) - 0.5 * std::log(L.nu) - 0.5 * LOG_PI);
-                break;
-            case B200_IR_L_BINOMIAL_LOGIT: {  // c0 = sum_i binomln(n_i, y_i)
-                if (L.sigma_kind != B200_IR_S_CONST && L.sigma_kind != B200_IR_S_OBS)
-                    return fail("ir: likelihood %d: Binomial trials must be a constant or one per observation", l);
-                double c = 0;
-                for (long long i = 0; i < N; ++i) {
-                    const double nt = L.sigma_kind == B200_IR_S_OBS ? L.sigma_obs[i] : L.sigma.value, y = L.y[i];
-                    if (!std::isfinite(nt) || !(nt >= 0) || nt != std::floor(nt)) return fail("ir: likelihood %d: Binomial trials must be integers >= 0 (at %lld)", l, i);
-                    if (!(y >= 0 && y <= nt) || y != std::floor(y)) return fail("ir: likelihood %d: Binomial y must be an integer in [0, n] (at %lld)", l, i);
-                    c += std::lgamma(nt + 1.0) - std::lgamma(y + 1.0) - std::lgamma(nt - y + 1.0);
-                }
-                D.c0 = c;
-            } break;
-            case B200_IR_L_NEGBINOMIAL_LOG: {
-                if (L.sigma_kind != B200_IR_S_CONST && L.sigma_kind != B200_IR_S_REF)
-                    return fail("ir: likelihood %d: NegativeBinomial alpha must be a constant or a scalar variable", l);
-                if (!ir_scale_ok(slot, vars)) return fail("ir: likelihood %d: NegativeBinomial alpha " B200_IR_SCALE_RULE, l);
-                const double a = L.sigma.value;
-                const bool fold = L.sigma_kind == B200_IR_S_CONST && a <= kNegBinPoissonAlpha;
-                double c = 0;
-                std::map<double, double> count;  // distinct nonzero y -> multiplicity, ascending
-                for (long long i = 0; i < N; ++i) {
-                    const double y = L.y[i];
-                    if (!(y >= 0) || y != std::floor(y) || std::isinf(y)) return fail("ir: likelihood %d: NegativeBinomial y must be an integer >= 0 (at %lld)", l, i);
-                    c -= std::lgamma(y + 1.0);
-                    if (fold) c += std::lgamma(y + a) - std::lgamma(a);
-                    if (y > 0) count[y] += 1.0;
-                }
-                D.c0 = c;
-                if (L.sigma_kind == B200_IR_S_REF) {
-                    std::vector<double> u, cnt;
-                    for (const auto& kv : count) { u.push_back(kv.first); cnt.push_back(kv.second); }
-                    D.n_tab = (int)u.size();
-                    if (upload(m, u, &D.tab_u) || upload(m, cnt, &D.tab_cnt)) return -1;
-                }
-            } break;
-            case B200_IR_L_GAMMA_LOG: {
-                if (L.sigma_kind != B200_IR_S_CONST && L.sigma_kind != B200_IR_S_REF)
-                    return fail("ir: likelihood %d: Gamma alpha must be a constant or a scalar variable", l);
-                if (!ir_scale_ok(slot, vars)) return fail("ir: likelihood %d: Gamma alpha " B200_IR_SCALE_RULE, l);
-                double sly = 0;
-                for (long long i = 0; i < N; ++i) {
-                    if (!(L.y[i] > 0) || std::isinf(L.y[i])) return fail("ir: likelihood %d: Gamma y must be > 0 (at %lld)", l, i);
-                    sly += std::log(L.y[i]);
-                }
-                if (L.sigma_kind == B200_IR_S_CONST) {
-                    const double a = L.sigma.value;
-                    D.c0 = (double)N * (a * std::log(a) - std::lgamma(a)) + (a - 1.0) * sly;
-                } else {
-                    D.sum_log_y = sly;
-                }
-            } break;
-            case B200_IR_L_CENSORED_NORMAL: case B200_IR_L_TRUNCATED_NORMAL: {  // y is the [3][N] block (y, lower, upper)
-                const bool cens = L.dist == B200_IR_L_CENSORED_NORMAL;
-                const char* what = cens ? "censored_normal" : "truncated_normal";
-                const double *y = L.y, *lo = L.y + N, *hi = L.y + 2 * N;
-                std::vector<signed char> code(cens ? (size_t)N : 0);
-                long long n_observed = 0;
-                bool bounded = false;
-                for (long long i = 0; i < N; ++i) {
-                    if (std::isnan(lo[i]) || std::isnan(hi[i]) || lo[i] == INFINITY || hi[i] == -INFINITY)
-                        return fail("ir: likelihood %d: %s: " B200_IR_BOUND_SIDES " (at %lld)", l, what, i);
-                    if (!(lo[i] < hi[i])) return fail("ir: likelihood %d: %s: " B200_IR_BOUND_ORDER " (at %lld)", l, what, i);
-                    if (!(std::isfinite(y[i]) && lo[i] <= y[i] && y[i] <= hi[i]))
-                        return fail("ir: likelihood %d: %s: " B200_IR_BOUND_Y " (at %lld)", l, what, i);
-                    bounded = bounded || std::isfinite(lo[i]) || std::isfinite(hi[i]);
-                    if (cens) {
-                        code[i] = y[i] == lo[i] ? 1 : (y[i] == hi[i] ? 2 : 0);
-                        n_observed += code[i] == 0;
-                    }
-                }
-                if (!cens && !bounded) return fail("ir: likelihood %d: " B200_IR_TRUNC_OPEN, l);
-                // -log(2 pi) / 2 of every Normal density term: each uncensored observation, every truncated one
-                D.c0 = -(double)(cens ? n_observed : N) * B200_HALF_LOG_2PI;
-                if (cens ? upload(m, code, &D.cens) : upload_raw(m, lo, 2 * (size_t)N, &D.bnd)) return -1;
-                m->ir_extended = true;
-            } break;
-            case B200_IR_L_ORDERED_LOGISTIC: case B200_IR_L_ORDERED_PROBIT: {  // nu = K; the cutpoint term at terms[n_terms]
-                const double K = L.nu;
-                if (!(K >= 2 && K == std::floor(K) && K <= 0x7fffffff)) return fail("ir: likelihood %d: " B200_IR_ORD_K, l);
-                for (long long i = 0; i < N; ++i)
-                    if (!(L.y[i] >= 0 && L.y[i] <= K - 1) || L.y[i] != std::floor(L.y[i]))
-                        return fail("ir: likelihood %d: " B200_IR_ORD_Y " (at %lld)", l, i);
-                if (L.dist == B200_IR_L_ORDERED_LOGISTIC && L.sigma_kind != B200_IR_S_NONE)
-                    return fail("ir: likelihood %d: " B200_IR_LOGISTIC_SIGMA, l);
-                ord_obs = std::max(ord_obs, N);
-                m->ir_extended = true;
-            } break;
-            case B200_IR_L_ZERO_INFLATED_POISSON: case B200_IR_L_ZERO_INFLATED_BINOMIAL:
-            case B200_IR_L_ZERO_INFLATED_NEGATIVE_BINOMIAL: case B200_IR_L_HURDLE_POISSON:
-            case B200_IR_L_HURDLE_NEGATIVE_BINOMIAL: case B200_IR_L_HURDLE_GAMMA: {  // nu: the form of the psi block
-                if (!(L.nu >= 0 && L.nu == std::floor(L.nu) && L.nu <= 0x7fff)) return fail("ir: likelihood %d: " B200_IR_PSI_NU, l);
-                const bool bin = L.dist == B200_IR_L_ZERO_INFLATED_BINOMIAL, gam = L.dist == B200_IR_L_HURDLE_GAMMA;
-                const bool nb = L.dist == B200_IR_L_ZERO_INFLATED_NEGATIVE_BINOMIAL || L.dist == B200_IR_L_HURDLE_NEGATIVE_BINOMIAL;
-                if (bin && L.sigma_kind != B200_IR_S_CONST && L.sigma_kind != B200_IR_S_OBS)
-                    return fail("ir: likelihood %d: Binomial trials must be a constant or one per observation", l);
-                if ((nb || gam) && L.sigma_kind != B200_IR_S_CONST && L.sigma_kind != B200_IR_S_REF)
-                    return fail("ir: likelihood %d: %s alpha must be a constant or a scalar variable", l, gam ? "Gamma" : "NegativeBinomial");
-                if ((nb || gam) && !ir_scale_ok(slot, vars))
-                    return fail("ir: likelihood %d: %s alpha " B200_IR_SCALE_RULE, l, gam ? "Gamma" : "NegativeBinomial");
-                if (!bin && !nb && !gam && L.sigma_kind != B200_IR_S_NONE) return fail("ir: likelihood %d: " B200_IR_ZIP_SLOT, l);
-                const double a = L.sigma.value;
-                const bool fold = nb && L.sigma_kind == B200_IR_S_CONST && a <= kNegBinPoissonAlpha;
-                double c = 0, sly = 0;
-                long long n_pos = 0;
-                std::map<double, double> count;  // distinct nonzero y -> multiplicity, ascending
-                for (long long i = 0; i < N; ++i) {
-                    const double y = L.y[i];
-                    if (gam) {  // the Gamma's normaliser covers the y > 0 only
-                        if (!(std::isfinite(y) && y >= 0)) return fail("ir: likelihood %d: " B200_IR_HG_Y " (at %lld)", l, i);
-                        if (y > 0) { sly += std::log(y); ++n_pos; }
-                        continue;
-                    }
-                    if (!(y >= 0) || y != std::floor(y) || std::isinf(y)) return fail("ir: likelihood %d: " B200_IR_ZI_Y " (at %lld)", l, i);
-                    c -= std::lgamma(y + 1.0);  // 0 at y = 0, as every constant below
-                    if (bin) {
-                        const double nt = L.sigma_kind == B200_IR_S_OBS ? L.sigma_obs[i] : L.sigma.value;
-                        if (!std::isfinite(nt) || !(nt >= 0) || nt != std::floor(nt)) return fail("ir: likelihood %d: Binomial trials must be integers >= 0 (at %lld)", l, i);
-                        if (y > nt) return fail("ir: likelihood %d: " B200_IR_ZIB_Y " (at %lld)", l, i);
-                        c += std::lgamma(nt + 1.0) - std::lgamma(nt - y + 1.0);
-                    }
-                    if (fold) c += std::lgamma(y + a) - std::lgamma(a);
-                    if (nb && y > 0) count[y] += 1.0;
-                }
-                if (gam && L.sigma_kind == B200_IR_S_CONST) {
-                    c = (double)n_pos * (a * std::log(a) - std::lgamma(a)) + (a - 1.0) * sly;
-                } else if (gam) {
-                    D.sum_log_y = sly;
-                    D.n_tab = (int)n_pos;  // N+
-                }
-                D.c0 = c;
-                if (nb && L.sigma_kind == B200_IR_S_REF) {
-                    std::vector<double> u, cnt;
-                    for (const auto& kv : count) { u.push_back(kv.first); cnt.push_back(kv.second); }
-                    D.n_tab = (int)u.size();
-                    if (upload(m, u, &D.tab_u) || upload(m, cnt, &D.tab_cnt)) return -1;
-                }
-                m->ir_extended = true;
-            } break;
-            default: return fail("ir: likelihood %d: density %d is not in the closed set", l, L.dist);
-        }
-        const bool ordinal = L.dist == B200_IR_L_ORDERED_LOGISTIC || L.dist == B200_IR_L_ORDERED_PROBIT;
-        const bool zi = L.dist >= B200_IR_L_ZERO_INFLATED_POISSON && L.dist <= B200_IR_L_HURDLE_GAMMA;
-        const bool has_sigma = L.dist == B200_IR_L_NORMAL || L.dist == B200_IR_L_STUDENTT || L.dist == B200_IR_L_CENSORED_NORMAL ||
-                               L.dist == B200_IR_L_TRUNCATED_NORMAL || L.dist == B200_IR_L_ORDERED_PROBIT;
-        if (has_sigma && L.sigma_kind == B200_IR_S_NONE)
-            return fail("ir: likelihood %d needs sigma", l);
-        if (has_sigma) {
-            if (L.sigma_kind == B200_IR_S_OBS) {
-                for (long long i = 0; i < N; ++i)
-                    if (!(std::isfinite(L.sigma_obs[i]) && L.sigma_obs[i] > 0))
-                        return fail("ir: likelihood %d: sigma must be a finite constant > 0 for every observation (at %lld)", l, i);
-            } else if (!ir_scale_ok(slot, vars)) {
-                return fail("ir: likelihood %d: sigma " B200_IR_SCALE_RULE, l);
-            }
-        }
-        // the checks and uploads of terms[t0 .. t1): the predictor's, and those of the logit of a zero-inflated / hurdle psi
-        auto add_terms = [&](int t0, int t1) -> int {
-            for (int t = t0; t < t1; ++t) {
-                const b200_ir_term& T = L.terms[t];
-                if (T.n_factors < 0 || T.n_factors > 3) return fail("ir: likelihood %d term %d: 0..3 variable factors", l, t);
-                IrTermD TD{};
-                TD.n_factors = T.n_factors;
-                if (T.n_cols != 0) {  // design term: coef is X [N][n_cols]; the same checks and words as ModelIR.validate()
-                    const int K = T.n_cols;
-                    if (T.n_factors != 1) return fail("ir: likelihood %d term %d: a design term has exactly one factor", l, t);
-                    if (T.f[0].idx) return fail("ir: likelihood %d term %d: a design term's factor takes no index", l, t);
-                    if (K < 0 || T.f[0].size != K || !T.coef)
-                        return fail("ir: likelihood %d term %d: X must have shape (N, size of the variable)", l, t);
-                    if (T.f[0].offset < 0 || T.f[0].offset + K > n) return fail("ir: likelihood %d term %d: factor slice outside q", l, t);
-                    std::vector<double> xt((size_t)N * K);
-                    for (long long i = 0; i < N; ++i)
-                        for (int k = 0; k < K; ++k) {
-                            const double v = T.coef[i * K + k];
-                            if (!std::isfinite(v)) return fail("ir: likelihood %d term %d: X must be finite (at row %lld, column %d)", l, t, i, k);
-                            xt[(size_t)k * N + i] = v;
-                        }
-                    TD.n_cols = K;
-                    TD.f[0] = IrFactorD{T.f[0].offset, K, nullptr, nullptr, nullptr};
-                    if (upload_raw(m, T.coef, (size_t)N * K, &TD.coef) || upload(m, xt, &TD.xt)) return -1;
-                    has_design = true;
-                    terms.push_back(TD);
-                    continue;
-                }
-                if (T.coef && upload_raw(m, T.coef, (size_t)N, &TD.coef)) return -1;
-                for (int f = 0; f < T.n_factors; ++f) {
-                    const b200_ir_factor& F = T.f[f];
-                    if (F.offset < 0 || F.size <= 0 || F.offset + F.size > n) return fail("ir: likelihood %d term %d: factor slice outside q", l, t);
-                    IrFactorD FD{};
-                    FD.offset = F.offset; FD.size = F.size;
-                    if (F.idx) {
-                        std::vector<int> rowptr(F.size + 1, 0), rowobs((size_t)N);
-                        for (long long i = 0; i < N; ++i) {
-                            if (F.idx[i] < 0 || F.idx[i] >= F.size) return fail("ir: likelihood %d term %d: index %d out of range at %lld", l, t, F.idx[i], i);
-                            ++rowptr[F.idx[i] + 1];
-                        }
-                        for (int j = 0; j < F.size; ++j) rowptr[j + 1] += rowptr[j];
-                        std::vector<int> fill(rowptr.begin(), rowptr.end() - 1);
-                        for (long long i = 0; i < N; ++i) rowobs[fill[F.idx[i]]++] = (int)i;  // ascending i inside a row: fixed order
-                        if (upload_raw(m, F.idx, (size_t)N, &FD.idx) || upload(m, rowptr, &FD.rowptr) || upload(m, rowobs, &FD.rowobs)) return -1;
-                    } else if (F.size != 1 && F.size != N) {
-                        return fail("ir: likelihood %d term %d: a variable of size %d needs an index to enter %lld observations", l, t, F.size, N);
-                    }
-                    TD.f[f] = FD;
-                }
-                terms.push_back(TD);
-            }
-            return 0;
-        };
-        if (add_terms(0, L.n_terms)) return -1;
-        if (zi) {  // the psi block at terms[n_terms ..]: nu = 0, psi itself; nu = m >= 1, the m terms of logit(psi)
-            const int mt = (int)L.nu;
-            if (mt > 0) {
-                if (add_terms(L.n_terms, L.n_terms + mt)) return -1;
-                zeta_obs = std::max(zeta_obs, N);
-            } else {
-                const b200_ir_term& T = L.terms[L.n_terms];
-                IrTermD TD{};
-                if (T.n_cols != 0 || (T.n_factors == 0) != (T.coef != nullptr) || T.n_factors > 1 || T.n_factors < 0)
-                    return fail("ir: likelihood %d: " B200_IR_PSI_BLOCK, l);
-                if (T.n_factors == 0) {
-                    const double psi = T.coef[0];
-                    if (psi == 1.0) return fail("ir: likelihood %d: " B200_IR_PSI_ONE, l);
-                    if (!(std::isfinite(psi) && psi > 0.0 && psi < 1.0)) return fail("ir: likelihood %d: " B200_IR_PSI_CONST, l);
-                    if (upload_raw(m, T.coef, 1, &TD.coef)) return -1;
-                } else {
-                    const b200_ir_factor& F = T.f[0];
-                    const IrVarD* V = nullptr;
-                    for (const IrVarD& U : vars)
-                        if (U.offset == F.offset) V = &U;
-                    if (F.idx || !V || V->size != 1 || F.size != 1 || V->transform != IRT_INTERVAL || !(V->lo >= 0.0 && V->hi <= 1.0))
-                        return fail("ir: likelihood %d: " B200_IR_PSI_VAR, l);
-                    TD.n_factors = 1;
-                    TD.f[0] = IrFactorD{F.offset, 1, nullptr, nullptr, nullptr};
-                }
-                terms.push_back(TD);
-            }
-        }
-        if (ordinal) {  // the cutpoint term: one unindexed factor on a variable of size K - 1, or K - 1 constants in coef
-            const int K = (int)L.nu;
-            const b200_ir_term& T = L.terms[L.n_terms];
-            IrTermD TD{};
-            if (T.n_cols != 0 || T.n_factors < 0 || T.n_factors > 1)
-                return fail("ir: likelihood %d: the cutpoint term is one variable or K - 1 constants", l);
-            if (T.n_factors == 1) {
-                const b200_ir_factor& F = T.f[0];
-                const IrVarD* V = nullptr;
-                for (const IrVarD& U : vars)
-                    if (U.offset == F.offset) V = &U;
-                if (F.idx || !V || V->size != F.size) return fail("ir: likelihood %d: the cutpoint factor must be a whole variable, unindexed", l);
-                if (F.size != K - 1) return fail("ir: likelihood %d: " B200_IR_CUT_SIZE " (%d, K = %d)", l, F.size, K);
-                if (F.size > 1 && V->transform != IRT_ORDERED && V->transform != IRT_ORDERED_POSITIVE)
-                    return fail("ir: likelihood %d: " B200_IR_CUT_ORDERED, l);
-                // the observations of each category, ascending: category k's are rowobs[rowptr[k] .. rowptr[k + 1])
-                std::vector<int> rowptr(K + 1, 0), rowobs((size_t)N);
-                for (long long i = 0; i < N; ++i) ++rowptr[(int)L.y[i] + 1];
-                for (int k = 0; k < K; ++k) rowptr[k + 1] += rowptr[k];
-                std::vector<int> fill(rowptr.begin(), rowptr.end() - 1);
-                for (long long i = 0; i < N; ++i) rowobs[fill[(int)L.y[i]]++] = (int)i;
-                TD.n_factors = 1;
-                TD.f[0] = IrFactorD{F.offset, F.size, nullptr, nullptr, nullptr};
-                if (upload(m, rowptr, &TD.f[0].rowptr) || upload(m, rowobs, &TD.f[0].rowobs)) return -1;
-            } else {
-                if (!T.coef) return fail("ir: likelihood %d: " B200_IR_CUT_CONST, l);
-                for (int k = 0; k < K - 1; ++k)
-                    if (!std::isfinite(T.coef[k]) || (k > 0 && !(T.coef[k] > T.coef[k - 1])))
-                        return fail("ir: likelihood %d: " B200_IR_CUT_CONST " (at %d)", l, k);
-                if (upload_raw(m, T.coef, (size_t)K - 1, &TD.coef)) return -1;
-            }
-            terms.push_back(TD);
-        }
-        liks[l] = D;
-    }
+    for (int k = 0; k < R->n_priors; ++k)
+        if (ir_prior(c, R->priors[k], k, priors[k])) return -1;
+    m->ir_liks.assign(std::max(R->n_liks, 0), IrLikD{});  // filled in place: sg holds the addresses of their pointers
+    for (int l = 0; l < R->n_liks; ++l)
+        if (ir_lik(c, R->liks[l], l, m->ir_liks[l])) return -1;
     std::vector<IrAr1D> ars(std::max(R->n_ar1, 0));
-    for (int k = 0; k < R->n_ar1; ++k) {
-        const b200_ir_ar1& A = R->ar1[k];
-        if (A.var < 0 || A.var >= R->n_vars || vars[A.var].size < 2) return fail("ir: ar1 %d: bad variable", k);
-        if (!(A.init_sigma > 0)) return fail("ir: ar1 %d: init_sigma must be > 0", k);
-        IrAr1D D{};
-        D.offset = vars[A.var].offset; D.size = vars[A.var].size; D.init_sigma = A.init_sigma;
-        if (ir_param(A.phi, n, &D.phi, "ar1 phi") || ir_param(A.sigma, n, &D.sigma, "ar1 sigma")) return -1;
-        if (!ir_scale_ok(A.sigma, vars)) return fail("ir: ar1 %d: sigma " B200_IR_SCALE_RULE, k);
-        ars[k] = D;
-    }
+    for (int k = 0; k < R->n_ar1; ++k)
+        if (ir_ar1(c, R->ar1[k], k, ars[k])) return -1;
+    // the description is accepted: upload its data, then the tables that point into it
+    if (use_current_device(m) || sg.commit() || sg.finish()) return -1;
+    const std::vector<IrTermD> terms(c.terms.begin(), c.terms.end());
     IrModel::Params& P = m->ir;
-    P.n_vars = R->n_vars; P.n_priors = (int)priors.size(); P.n_liks = (int)liks.size(); P.n_ar1 = (int)ars.size(); P.n = n;
-    if (upload(m, vars, &P.vars) || upload(m, priors, &P.priors) || upload(m, liks, &P.liks) || upload(m, terms, &P.terms) ||
+    P.n_vars = R->n_vars; P.n_priors = (int)priors.size(); P.n_liks = (int)m->ir_liks.size(); P.n_ar1 = (int)ars.size(); P.n = c.n;
+    if (upload(m, c.vars, &P.vars) || upload(m, priors, &P.priors) || upload(m, m->ir_liks, &P.liks) || upload(m, terms, &P.terms) ||
         upload(m, ars, &P.ar1))
         return -1;
-    P.n_pad = (n + 3) & ~3;
-    const long long row2 = std::max(ord_obs, zeta_obs);  // likelihoods are evaluated one after another: they share the row
-    P.ord_row = row2 ? (int)(P.n_pad + ((max_obs + 3) & ~3LL)) : 0;  // after r, before the design partials
-    P.stride = P.n_pad + ((max_obs + 3) & ~3LL) + ((row2 + 3) & ~3LL) + (has_design ? kIrPartDoubles : 0);
-    m->ir_max_obs = max_obs;
+    P.n_pad = (c.n + 3) & ~3;
+    const long long row2 = std::max(c.ord_obs, c.zeta_obs);  // likelihoods are evaluated one after another: they share the row
+    P.ord_row = row2 ? (int)(P.n_pad + ((c.max_obs + 3) & ~3LL)) : 0;  // after r, before the design partials
+    P.stride = P.n_pad + ((c.max_obs + 3) & ~3LL) + ((row2 + 3) & ~3LL) + (c.has_design ? kIrPartDoubles : 0);
+    m->ir_extended = std::any_of(c.vars.begin(), c.vars.end(), [](const IrVarD& V) { return V.transform >= IRT_ORDERED; }) ||
+                     std::any_of(m->ir_liks.begin(), m->ir_liks.end(), [](const IrLikD& L) { return L.dist >= B200_IR_L_CENSORED_NORMAL; });
     return 0;
 }
 
 extern "C" int b200_model_create(const b200_model_desc* desc, b200_model** out) {
     if (!desc || !out) return fail("b200_model_create: null argument");
     if (desc->n <= 0) return fail("b200_model_create: n must be positive");
-    if (b200_device_count() == 0) return fail("b200_model_create: no CUDA device visible");
     b200_model* m = new b200_model();
     m->kind = desc->kind;
     m->n = desc->n;
-    cudaGetDevice(&m->device);
     int rc = 0;
-    switch (desc->kind) {
-        case B200_MODEL_STD_NORMAL: m->std_normal.n = desc->n; break;
-        case B200_MODEL_EIGHT_SCHOOLS: rc = prepare_eight(m, desc); break;
-        case B200_MODEL_RADON: rc = prepare_radon(m, desc); break;
-        case B200_MODEL_STOCHVOL: rc = prepare_stochvol(m, desc); break;
-        case B200_MODEL_MVGAUSS: rc = prepare_mvgauss(m, desc); break;
-        case B200_MODEL_LOGISTIC: rc = prepare_logistic(m, desc); break;
-        case B200_MODEL_IR: rc = prepare_ir(m, desc); break;
-        default: rc = fail("b200_model_create: model kind %d not implemented", desc->kind);
+    if (desc->kind == B200_MODEL_IR) {
+        rc = prepare_ir(m, desc);  // checks the whole description before it asks for the device
+    } else if (!(rc = use_current_device(m))) {
+        switch (desc->kind) {
+            case B200_MODEL_STD_NORMAL: m->std_normal.n = desc->n; break;
+            case B200_MODEL_EIGHT_SCHOOLS: rc = prepare_eight(m, desc); break;
+            case B200_MODEL_RADON: rc = prepare_radon(m, desc); break;
+            case B200_MODEL_STOCHVOL: rc = prepare_stochvol(m, desc); break;
+            case B200_MODEL_MVGAUSS: rc = prepare_mvgauss(m, desc); break;
+            case B200_MODEL_LOGISTIC: rc = prepare_logistic(m, desc); break;
+            default: rc = fail("b200_model_create: model kind %d not implemented", desc->kind);
+        }
     }
     if (rc) {
         delete m;
@@ -987,88 +1070,6 @@ struct Timer {
         if (a) cudaEventDestroy(a);
         if (b) cudaEventDestroy(b);
     }
-};
-
-// The array arguments of one C-ABI call.  With B200_MEM_DEVICE the kernels use the caller's pointers; with B200_MEM_HOST
-// every non-null array gets a device copy.  Those copies are lent from ONE arena in the model handle, sized in commit() from
-// the requests themselves, so a steady-state call makes no cudaMalloc / cudaFree at all (per-call allocations synchronise
-// the device and make a public-API call take far longer than its kernel).
-//   DIRECT: an OUTPUT in page-locked host memory (cudaHostAlloc / cudaHostRegister, e.g. a torch pinned tensor) is written
-//           by the kernel itself through its device alias (UVA), so the device->host transfer overlaps the run instead of
-//           following it (2.9 GB of draws per Radon bench step).
-//   OWN:    a per-call allocation instead of arena space, for arrays the arena must not grow to (the draws).
-// Usage: add() every array, commit() before the launch, finish() after it.
-class Staging {
-  public:
-    enum Dir { IN = 1, OUT = 2, INOUT = 3 };
-    enum Flag { DIRECT = 1, OWN = 2 };
-    Staging(b200_model* m, int mem, cudaStream_t st) : m_(m), host_(mem == B200_MEM_HOST), st_(st) {}
-    // `count` elements at `user`; commit() stores the pointer the kernels use in *dst
-    template <class T>
-    void add(T** dst, T* user, size_t count, Dir dir, int flags = 0) {
-        reqs_.push_back(Req{dst, &put<T>, const_cast<void*>(static_cast<const void*>(user)), count * sizeof(T), dir, flags});
-    }
-    int commit() {
-        size_t lent = 0;
-        for (Req& r : reqs_) {
-            r.copy = host_ && r.user;
-            if (r.copy && (r.flags & DIRECT) && r.dir == OUT) {
-                cudaPointerAttributes at{};
-                if (cudaPointerGetAttributes(&at, r.user) == cudaSuccess && at.type == cudaMemoryTypeHost && at.devicePointer) {
-                    r.dev = at.devicePointer;
-                    r.copy = false;
-                } else {
-                    cudaGetLastError();  // pageable memory: not an error, fall back to a device copy
-                }
-            }
-            if (r.copy && !(r.flags & OWN)) {
-                r.off = lent;
-                lent += (r.bytes + 255) & ~(size_t)255;
-            }
-        }
-        if (lent) CU(m_->stage_arena.reserve(lent));
-        for (Req& r : reqs_) {
-            if (r.copy) {
-                if (r.flags & OWN) {
-                    own_.emplace_back();
-                    CU(own_.back().reserve(r.bytes));
-                    r.dev = own_.back().p;
-                } else {
-                    r.dev = m_->stage_arena.as<char>() + r.off;
-                }
-                if (r.dir & IN) CU(cudaMemcpyAsync(r.dev, r.user, r.bytes, cudaMemcpyHostToDevice, st_));
-            } else if (!r.dev) {
-                r.dev = r.user;
-            }
-            r.put(r.dst, r.dev);
-        }
-        return 0;
-    }
-    // device->host copies of the outputs, then wait for the stream
-    int finish() {
-        for (const Req& r : reqs_)
-            if (r.copy && (r.dir & OUT)) CU(cudaMemcpyAsync(r.user, r.dev, r.bytes, cudaMemcpyDeviceToHost, st_));
-        CU(cudaStreamSynchronize(st_));
-        return 0;
-    }
-
-  private:
-    struct Req {
-        void* dst;
-        void (*put)(void* dst, void* dev);
-        void* user;
-        size_t bytes;
-        int dir, flags;
-        bool copy = false;  // a device copy of a host array
-        size_t off = 0;     // its place in the arena
-        void* dev = nullptr;
-    };
-    template <class T> static void put(void* dst, void* dev) { *static_cast<T**>(dst) = static_cast<T*>(dev); }
-    b200_model* m_;
-    bool host_;
-    cudaStream_t st_;
-    std::vector<Req> reqs_;
-    std::deque<DevBuf> own_;
 };
 
 static int env_int(const char* name, int dflt) {
@@ -1798,9 +1799,7 @@ extern "C" int b200_pointwise_loglik(b200_model* m, int32_t lik, const double* d
     if (D <= 0) return 0;
     CU(cudaSetDevice(m->device));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
-    // the IR tables live on the device: read the number of observations of this factor back
-    IrLikD L;
-    CU(cudaMemcpy(&L, m->ir.liks + lik, sizeof L, cudaMemcpyDeviceToHost));
+    const IrLikD& L = m->ir_liks[lik];
     if (L.yoff >= 0) return fail("b200_pointwise_loglik: factor %d is a latent factor (a prior with a Linear location), not a likelihood", lik);
     const double* d_draws = nullptr;
     double* d_out = nullptr;

@@ -1,4 +1,7 @@
-"""Shared helpers: model specs per golden file, GPU replay (free-running and single-draw), oracle replay."""
+"""Shared helpers: model specs per golden file, GPU replay (free-running and single-draw), oracle replay, raw C-ABI model
+creation."""
+import ctypes
+
 import numpy as np
 
 from pymc_b200 import _lib, models
@@ -26,6 +29,23 @@ SPEC_OF = {
 TREE_KW = {"radon_small_adapt": dict(max_treedepth=6, early_max_treedepth=4)}
 DISCRETE = ["depth", "tree_size", "index_in_trajectory", "diverging", "reached_max_treedepth"]
 CONTINUOUS = ["step_size", "step_size_bar", "mean_tree_accept", "energy", "energy_error", "max_energy_error", "model_logp"]
+
+
+def create_raw(low):
+    """b200_model_create on lowered tables as given, without ModelIR.validate(): what a direct C-ABI caller gets.  None when
+    the tables are accepted.  prepare_ir asks for a device only after every check of the tables has passed, so on a machine
+    without one, the no-device refusal means the same."""
+    lib = _lib.load()
+    c_ir, keep = _lib.build_ir(low)
+    d = _lib.ModelDesc()
+    d.kind, d.n, d.ir = _lib.MODEL_IR, low.n, ctypes.addressof(c_ir)
+    h = ctypes.c_void_p()
+    rc = lib.b200_model_create(ctypes.byref(d), ctypes.byref(h))
+    if rc == 0:
+        lib.b200_model_destroy(h)
+        return None
+    err = lib.b200_last_error().decode()
+    return None if err == "b200_model_create: no CUDA device visible" else err
 
 
 def relerr(a, b):

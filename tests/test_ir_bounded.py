@@ -685,18 +685,17 @@ def test_pointwise_log_likelihood_and_the_log_likelihood_group_match_scipy():
         assert np.array_equal(res.constant_data["y_upper"], m.likelihoods[0].upper)
 
 
-@pytest.mark.gpu
 def test_model_create_refuses_malformed_bound_tables_through_the_c_abi():
     """prepare_ir makes the checks of validate(), with the same words, for callers of the C ABI; a bounded Normal is not a
     latent factor."""
-    from test_ir_families import _create_raw
+    from b200_helpers import create_raw
 
     def block_edit(builder, row, k, value):
         low = ir.lower(builder())
-        assert _create_raw(low) is None
+        assert create_raw(low) is None
         low.liks[0]["y"] = low.liks[0]["y"].copy()
         low.liks[0]["y"][row, k] = value
-        return _create_raw(low)
+        return create_raw(low)
 
     c, t = ir.censored_regression_ir, ir.truncated_regression_ir
     for builder, row, k, value, msg in [
@@ -710,14 +709,14 @@ def test_model_create_refuses_malformed_bound_tables_through_the_c_abi():
     low.liks[0]["y"] = low.liks[0]["y"].copy()
     low.liks[0]["y"][1] = -np.inf
     low.liks[0]["y"][2] = np.inf
-    err = _create_raw(low)
+    err = create_raw(low)
     assert err is not None and ir.TRUNC_OPEN in err, err
     for builder in (c, t):
         low = ir.lower(builder())
         low.liks[0]["sigma_value"], low.liks[0]["sigma_kind"] = -1.0, ir.SIGMA_CONST
-        err = _create_raw(low)
+        err = create_raw(low)
         assert err is not None and "must be a finite constant > 0" in err, err
         low = ir.lower(builder())
         low.liks[0]["y_var"] = 1  # as a latent factor on its first variable
-        err = _create_raw(low)
+        err = create_raw(low)
         assert err is not None and "latent factor" in err, err

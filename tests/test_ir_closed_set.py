@@ -878,14 +878,13 @@ def test_pointwise_log_likelihood_matches_scipy(cid):
                                        err_msg=f"{cid} likelihood {lik}")
 
 
-@pytest.mark.gpu
 def test_model_create_refuses_tables_outside_the_support_through_the_c_abi():
     """b200_model_create makes the support checks of validate(), with the same words, for callers of the C ABI."""
-    from test_ir_families import _create_raw
+    from b200_helpers import create_raw
 
     def lowered(cid):
         low = ir.lower(build(cid))
-        assert _create_raw(low) is None  # the unedited tables are accepted
+        assert create_raw(low) is None  # the unedited tables are accepted
         return low
 
     def var_index(cid, name):
@@ -974,5 +973,5 @@ def test_model_create_refuses_tables_outside_the_support_through_the_c_abi():
     for cid, edit, msg in edits:
         low = lowered(cid)
         edit(low)
-        err = _create_raw(low)
+        err = create_raw(low)
         assert err is not None and msg in err, (cid, msg, err)

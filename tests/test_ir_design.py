@@ -597,9 +597,8 @@ def test_pointwise_log_likelihood_matches_scipy(K):
                 np.testing.assert_allclose(ll[k], want, rtol=1e-12, atol=1e-12, err_msg=f"{m.name} likelihood {lik}")
 
 
-@pytest.mark.gpu
 def test_model_create_refuses_malformed_design_tables_through_the_c_abi():
-    from test_ir_families import _create_raw
+    from b200_helpers import create_raw
 
     m = design_model("normal", 30, 8, group=3)
 
@@ -608,7 +607,7 @@ def test_model_create_refuses_malformed_design_tables_through_the_c_abi():
         T = low.liks[0]["terms"][1]
         assert T["n_cols"] == 8
         edit(T)
-        return _create_raw(low)
+        return create_raw(low)
 
     assert case(lambda T: None) is None
 

@@ -8,6 +8,8 @@ import numpy as np
 import pytest
 from scipy import stats
 
+from b200_helpers import create_raw
+
 from pymc_b200 import _lib, ir
 
 
@@ -466,28 +468,13 @@ def test_sampler_records_the_log_likelihood_group_for_the_families():
             assert np.array_equal(res.constant_data["y_trials"], m.likelihoods[0].trials)
 
 
-def _create_raw(low):
-    """b200_model_create on lowered tables as given, without ModelIR.validate(): what a direct C-ABI caller gets."""
-    lib = _lib.load()
-    c_ir, keep = _lib.build_ir(low)
-    d = _lib.ModelDesc()
-    d.kind, d.n, d.ir = _lib.MODEL_IR, low.n, ctypes.addressof(c_ir)
-    h = ctypes.c_void_p()
-    rc = lib.b200_model_create(ctypes.byref(d), ctypes.byref(h))
-    if rc == 0:
-        lib.b200_model_destroy(h)
-        return None
-    return lib.b200_last_error().decode()
-
-
-@pytest.mark.gpu
 def test_model_create_rejects_out_of_support_tables_through_the_c_abi():
     """prepare_ir checks what validate() checks, for callers of the C ABI that bypass the Python front end."""
     def case(builder, edit):
         low = ir.lower(builder())
-        assert _create_raw(low) is None  # the unedited tables are accepted
+        assert create_raw(low) is None  # the unedited tables are accepted
         edit(low.liks[0], low)
-        return _create_raw(low)
+        return create_raw(low)
 
     def setter(**kw):
         def f(L, low):

@@ -725,15 +725,14 @@ def test_log_likelihood_group_holds_only_the_observed_likelihood():
     assert lib.b200_pointwise_loglik(cm._h, 0, q.ctypes.data, 2, np.empty((2, len(L.y))).ctypes.data, _lib.MEM_HOST, None) == 0
 
 
-@pytest.mark.gpu
 def test_model_create_refuses_malformed_latent_tables():
-    from test_ir_families import _create_raw
+    from b200_helpers import create_raw
 
     def edited(edit):
         low = ir.lower(nested_ir())
-        assert _create_raw(low) is None
+        assert create_raw(low) is None
         edit(low.liks[2], low)
-        return _create_raw(low)
+        return create_raw(low)
 
     def setter(**kw):
         return lambda L, low: L.update(kw)

@@ -606,15 +606,14 @@ def test_pointwise_log_likelihood_and_the_log_likelihood_group_match_scipy():
         np.testing.assert_allclose(ll, scipy_ll(m, res.unconstrained), rtol=1e-10, atol=1e-10)
 
 
-@pytest.mark.gpu
 def test_model_create_refuses_malformed_psi_and_y_tables_through_the_c_abi():
-    from test_ir_families import _create_raw
+    from b200_helpers import create_raw
 
     def edited(builder, edit):
         low = ir.lower(builder())
-        assert _create_raw(low) is None
+        assert create_raw(low) is None
         edit(low)
-        return _create_raw(low)
+        return create_raw(low)
 
     def set_y(low, v, i=0):
         low.liks[0]["y"] = low.liks[0]["y"].copy()

@@ -1,6 +1,7 @@
 """Shared helpers: model specs per golden file, GPU replay (free-running and single-draw), oracle replay, raw C-ABI model
-creation."""
+creation and refusal, central differences, and the device-against-oracle checks every IR likelihood family runs."""
 import ctypes
+import os
 
 import numpy as np
 
@@ -46,6 +47,115 @@ def create_raw(low):
         return None
     err = lib.b200_last_error().decode()
     return None if err == "b200_model_create: no CUDA device visible" else err
+
+
+def refusal_after_edit(build, edit):
+    """create_raw on the lowered tables of build() after edit(low) changed them in place; the unedited tables must be
+    accepted, so that the refusal is the edit's."""
+    from pymc_b200 import ir
+
+    low = ir.lower(build())
+    assert create_raw(low) is None  # the unedited tables are accepted
+    edit(low)
+    return create_raw(low)
+
+
+def fd_grad(f, q, h=1e-6):
+    """Central differences of the log-density f(q)[0] in every coordinate."""
+    g = np.empty_like(q)
+    for i in range(len(q)):
+        e = np.zeros_like(q)
+        e[i] = h
+        g[i] = (f(q + e)[0] - f(q - e)[0]) / (2 * h)
+    return g
+
+
+def random_dense_cov(n, rank, diag, scale, seed):
+    """diag * I + U U^T with U an n x rank standard-normal draw times scale, symmetrised: a fixed dense mass matrix."""
+    U = np.random.default_rng(seed).standard_normal((n, rank)) * scale
+    cov = np.diag(np.full(n, diag)) + U @ U.T
+    return 0.5 * (cov + cov.T)
+
+
+def logp_at_both_team_shapes(cm, Q):
+    """cm.logp_dlogp(Q) with the default dispatch (chain = warp up to 256 coordinates), then with chain = CTA forced by
+    B200_FORCE_TEAM=1.  Each shape runs twice and must repeat bit for bit; the environment is restored.  Returns
+    {"warp": (lp, g), "cta": (lp, g)}."""
+    old = os.environ.pop("B200_FORCE_TEAM", None)
+    out = {}
+    try:
+        for team in ("warp", "cta"):
+            if team == "cta":
+                os.environ["B200_FORCE_TEAM"] = "1"
+            lp, g = cm.logp_dlogp(Q)
+            lp2, g2 = cm.logp_dlogp(Q)
+            assert np.array_equal(lp, lp2) and np.array_equal(g, g2), team
+            out[team] = lp, g
+    finally:
+        os.environ.pop("B200_FORCE_TEAM", None)
+        if old is not None:
+            os.environ["B200_FORCE_TEAM"] = old
+    return out
+
+
+def fixed_step_against_oracle(m, f, eps, *, specialise=False, dense_cov=None, C=3, T=12, seed=9, q0_seed=None):
+    """Fixed-step NUTS on the generic device function against the oracle sampler on the NumPy density f, chain by chain:
+    equal tree sizes and divergences at every draw, positions within 1e-9.  The C starts are the initial point plus
+    U(-0.3, 0.3) from q0_seed (default: seed); seed also makes the chains' streams.  The mass matrix is the identity, or
+    dense_cov.  specialise is CompiledModel's choice of path."""
+    from oracle import nuts_numpy
+    from pymc_b200 import engine
+    from pymc_b200 import rng as brng
+
+    cm = engine.CompiledModel(m, specialise=specialise)
+    assert cm.spec.name == "ir"
+    q0 = m.initial_point() + np.random.default_rng(seed if q0_seed is None else q0_seed).uniform(-0.3, 0.3, (C, m.n))
+    step_rngs, pot_rngs, _ = brng.chain_generators(seed, C)
+    z = brng.momentum_noise(pot_rngs, T, m.n)
+    if dense_cov is not None:
+        cm.set_dense_mass(dense_cov)
+    res = cm.nuts_run(q0, brng.pack_pcg64(step_rngs), tune=0, draws=T, z=z, mass="diag" if dense_cov is None else "dense",
+                      adapt_step_size=False, eps0=np.full(C, eps))
+    for c in range(C):
+        mass = nuts_numpy.DiagMass(np.ones(m.n)) if dense_cov is None else nuts_numpy.DenseMass(dense_cov)
+        o = nuts_numpy.Oracle(f, mass, adapt_step_size=False)
+        o.da = nuts_numpy.DualAveraging(eps)
+        o.rng, o.tune = step_rngs[c], False
+        qs, st = o.run(q0[c], 0, T, z=z[c])
+        for k in ("tree_size", "diverging"):
+            assert np.array_equal(np.asarray(st[k]).astype(float), np.asarray(res.stats[k][c]).astype(float)), (m.name, c, k)
+        assert np.max(np.abs(qs - res.draws[c])) <= 1e-9, (m.name, c)
+
+
+def adaptive_against_oracle(m, f, *, specialise=False, chain_seed, spread, philox_seed, oracle_seed, se_bound,
+                            max_divergence=None):
+    """64 device chains against 8 oracle chains on the NumPy density f, both NUTS with diagonal mass adaptation, 400 tuning
+    and 300 kept draws from starts spread U(-spread, spread) around the initial point.  Posterior means must agree within
+    se_bound standard errors (pooled draws, effective sizes taken generously), standard deviations within 25 %, and with
+    max_divergence, the device's share of divergent draws must stay below it.  Returns the device run."""
+    from oracle import nuts_numpy
+    from pymc_b200 import engine
+    from pymc_b200 import rng as brng
+
+    cm = engine.CompiledModel(m, specialise=specialise)
+    assert cm.spec.name == "ir"
+    C = 64
+    sr, _, js = brng.chain_generators(chain_seed, C)
+    q0 = np.stack([m.initial_point() + np.random.default_rng(s).uniform(-spread, spread, m.n) for s in js])
+    run = cm.nuts_run(q0, brng.pack_pcg64(sr), tune=400, draws=300, mean0=np.broadcast_to(q0.mean(0), q0.shape).copy(),
+                      store_warmup=False, philox_seed=philox_seed)
+    xs = []
+    for c in range(8):
+        o = nuts_numpy.Oracle(f, nuts_numpy.DiagMass(np.ones(m.n), adapt=True, initial_mean=q0[c].copy(), initial_weight=10))
+        o.setup_chain(np.random.default_rng(oracle_seed + c))
+        xs.append(o.run(q0[c], 400, 300)[0][400:])
+    xo, xg = np.concatenate(xs), run.draws.reshape(-1, m.n)
+    se = np.sqrt(xo.var(0) / 300 + xg.var(0) / 2000)
+    assert np.max(np.abs(xo.mean(0) - xg.mean(0)) / se) < se_bound
+    assert np.all(np.abs(np.log(xo.std(0) / xg.std(0))) < 0.25)
+    if max_divergence is not None:
+        assert run.stats["diverging"].mean() < max_divergence
+    return run
 
 
 def relerr(a, b):

@@ -6,21 +6,10 @@ lower and upper, its op in ``base_rv_op``), and random bounds are refused by nam
 import numpy as np
 import pytest
 from test_frontend_mock import Constant, FakeModel, LogTransform, Variable, apply, bcast, elem, fake_pytensor, rv  # noqa: F401
+from test_frontend_mock import same_density
 
+from oracle.ir_numpy_bounded import make_logp
 from pymc_b200 import ir
-
-
-def _same_density(m, ref, seed=0):
-    from oracle import ir_numpy_bounded
-
-    f, g = ir_numpy_bounded.make_logp(m), ir_numpy_bounded.make_logp(ref)
-    assert m.n == ref.n and [v.name for v in m.vars] == [v.name for v in ref.vars]
-    rng = np.random.default_rng(seed)
-    for _ in range(4):
-        q = ref.initial_point() + rng.uniform(-0.7, 0.7, ref.n)
-        (a, ga), (b, gb) = f(q), g(q)
-        assert abs(a - b) <= 1e-12 * abs(b)
-        np.testing.assert_allclose(ga, gb, rtol=1e-12, atol=1e-12)
 
 
 def _model(rng, N, obs):
@@ -76,7 +65,7 @@ def test_bounded_graphs_lower_to_the_bounded_likelihoods(fake_pytensor, spelling
         assert (got is None and exp is None) or np.array_equal(got, exp), (got, exp)
     ref = ir.ModelIR(vars=vars_, priors=priors, likelihoods=[ir.Likelihood(dist, y, terms, sigma=ir.Ref("sigma_log__"),
                                                                            lower=want[0], upper=want[1])])
-    _same_density(m, ref)
+    same_density(make_logp(m), make_logp(ref), m, ref, spread=0.7)
 
 
 def truncated_rv(name, base_op, *base_params, lower, upper):

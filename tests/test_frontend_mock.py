@@ -54,6 +54,10 @@ class Dot:
     pass
 
 
+class Join:
+    pass
+
+
 class Subtensor:
     pass
 
@@ -96,8 +100,9 @@ class FakeModel:
         self.name, self.free_RVs, self.observed_RVs = name, [], []
         self.rvs_to_values, self.rvs_to_transforms, self._ip = {}, {}, {}
 
-    def free(self, r, size, transform=None, initial=None):
-        vname = r.name + ("_log__" if transform is not None else "")
+    def free(self, r, size, transform=None, initial=None, suffix=None):
+        """suffix: what PyMC appends to the value variable's name; "_log__" under a transform unless given."""
+        vname = r.name + (suffix if suffix is not None else "_log__" if transform is not None else "")
         self.free_RVs.append(r)
         self.rvs_to_values[r] = Variable(vname)
         self.rvs_to_transforms[r] = transform
@@ -148,6 +153,19 @@ def _same_density(m, f_ref, n, seed=0):
         lp_ref, dlp_ref = f_ref(q)
         assert abs(lp - lp_ref) <= 1e-11 * max(1.0, abs(lp_ref))
         np.testing.assert_allclose(dlp, dlp_ref, rtol=1e-10, atol=1e-10)
+
+
+def same_density(f, g, m, ref, *, spread, seed=0):
+    """m, which from_pymc made, against the hand-built IR ref: the same value variables and transforms, and the same
+    log-density and gradient (f of m, g of ref, the caller's oracle) at four points around ref's initial point."""
+    assert m.n == ref.n and [v.name for v in m.vars] == [v.name for v in ref.vars]
+    assert [v.transform for v in m.vars] == [v.transform for v in ref.vars]
+    rng = np.random.default_rng(seed)
+    for _ in range(4):
+        q = ref.initial_point() + rng.uniform(-spread, spread, ref.n)
+        (a, ga), (b, gb) = f(q), g(q)
+        assert abs(a - b) <= 1e-12 * abs(b)
+        np.testing.assert_allclose(ga, gb, rtol=1e-12, atol=1e-12)
 
 
 def test_eight_schools_graph_lowers_to_the_reference_density(fake_pytensor):
@@ -256,9 +274,7 @@ def test_stochastic_volatility_graph_ar1_interval_and_log_variance_likelihood(fa
     mu = M.free(rv("NormalRV", "mu", Constant(0.0), Constant(5.0)), 1)
     lo, hi = Constant(-1.0), Constant(1.0)
     phi = rv("UniformRV", "phi", lo, hi)
-    M.free(phi, 1, IntervalTransform(lo, hi))
-    M.rvs_to_values[phi].name = "phi_interval__"
-    M._ip["phi_interval__"] = M._ip.pop("phi_log__")
+    M.free(phi, 1, IntervalTransform(lo, hi), suffix="_interval__")
     sigma = M.free(rv("ExponentialRV", "sigma", Constant(0.1)), 1, LogTransform(), initial=[np.log(0.1)])
     init = rv("NormalRV", "init", Constant(0.0), Constant(1.0))
     ar_op = type("AutoRegressiveRV", (), {"ar_order": 1, "constant_term": False,

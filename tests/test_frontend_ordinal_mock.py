@@ -10,14 +10,11 @@ chained transforms and unordered vector cutpoints are refused by name.  A real-P
 import numpy as np
 import pytest
 from scipy import special, stats
-from test_frontend_mock import Constant, FakeModel, LogTransform, SharedVariable, Variable, apply, bcast, elem, fake_pytensor, rv  # noqa: F401
-from test_frontend_mock import AdvancedSubtensor1, Dot, Subtensor
+from test_frontend_mock import Constant, FakeModel, LogTransform, SharedVariable, apply, bcast, elem, fake_pytensor, rv  # noqa: F401
+from test_frontend_mock import AdvancedSubtensor1, Dot, Join, Subtensor, same_density
+from test_ir_ordinal import oracle
 
 from pymc_b200 import ir
-
-
-class Join:
-    pass
 
 
 def _op(name):
@@ -26,16 +23,6 @@ def _op(name):
 
 def ordered(positive=False, ascending=True):
     return type("Ordered", (), {"positive": positive, "ascending": ascending})()
-
-
-def _free(M, r, size, transform, initial=None):
-    """M.free under the value name PyMC gives a transformed vector: {name}_{transform}__"""
-    M.free(r, size, transform, initial)
-    old = M.rvs_to_values[r].name
-    suffix = "_ordered__" if type(transform).__name__ == "Ordered" else ("_log__" if transform is not None else "")
-    M.rvs_to_values[r] = Variable(r.name + suffix)
-    M._ip[r.name + suffix] = M._ip.pop(old)
-    return r
 
 
 def _sub(x):
@@ -72,7 +59,8 @@ def _model(link, compute_p=True, sigma="const", positive=False, seed=3, N=40, K=
     beta = M.free(rv("NormalRV", "beta", Constant(0.0), Constant(1.0)), 2)
     tr = ordered(positive) if cut_transform == "ordered" else cut_transform
     z0 = np.concatenate([[0.0 if positive else -2.0], np.log(np.diff(mu_c))])
-    cut = _free(M, rv("NormalRV", "cutpoints", Constant(mu_c), Constant(5.0)), K - 1, tr, initial=z0)
+    cut = M.free(rv("NormalRV", "cutpoints", Constant(mu_c), Constant(5.0)), K - 1, tr, initial=z0,
+                 suffix="_ordered__" if type(tr).__name__ == "Ordered" else None)
     vars_ = [ir.Var("a", "a", 4), ir.Var("beta", "beta", 2),
              ir.Var("cutpoints_ordered__", "cutpoints", K - 1, "ordered_positive" if positive else "ordered")]
     priors = [ir.Prior("normal", "a", (0.0, 1.0)), ir.Prior("normal", "beta", (0.0, 1.0)),
@@ -100,19 +88,6 @@ def _model(link, compute_p=True, sigma="const", positive=False, seed=3, N=40, K=
     return M, ref
 
 
-def _same_density(m, ref, seed=0):
-    from test_ir_ordinal import _oracle
-
-    f, g = _oracle(m), _oracle(ref)
-    assert [v.name for v in m.vars] == [v.name for v in ref.vars] and [v.transform for v in m.vars] == [v.transform for v in ref.vars]
-    rng = np.random.default_rng(seed)
-    for _ in range(4):
-        q = ref.initial_point() + rng.uniform(-0.5, 0.5, ref.n)
-        (a, ga), (b, gb) = f(q), g(q)
-        assert abs(a - b) <= 1e-12 * abs(b)
-        np.testing.assert_allclose(ga, gb, rtol=1e-12, atol=1e-12)
-
-
 def _numpy_probs(link, eta, c, s=1.0):
     """compute_p restated in probability space (discrete.py:1312-1326, :1416-1432)"""
     cc = np.concatenate([[-np.inf], c, [np.inf]])
@@ -133,7 +108,7 @@ def test_ordinal_graphs_lower_to_the_ordinal_likelihoods(fake_pytensor, link, si
     L = m.likelihoods[0]
     assert L.dist == f"ordered_{link}" and L.cutpoints == ir.Ref("cutpoints_ordered__")
     assert L.sigma == ref.likelihoods[0].sigma
-    _same_density(m, ref)
+    same_density(oracle(m), oracle(ref), m, ref, spread=0.5)
     if not compute_p:
         assert m.deterministics == []
         return
@@ -144,9 +119,7 @@ def test_ordinal_graphs_lower_to_the_ordinal_likelihoods(fake_pytensor, link, si
     probs = m.eval_deterministics(post)["y_probs"]
     assert probs.shape == (3, 2, 40, 5)
     np.testing.assert_allclose(probs.sum(-1), 1.0, rtol=1e-13)
-    from test_ir_ordinal import _oracle
-
-    f = _oracle(m)
+    f = oracle(m)
     for ix in np.ndindex(3, 2):
         x, _ = f.constrained(q[ix])
         s = 1.0 if link == "logistic" else f.scale(L, x)[0]
@@ -160,7 +133,7 @@ def test_ordered_positive_transform_maps_to_ordered_positive(fake_pytensor):
     M, ref = _model("logistic", positive=True)
     m = from_pymc(M)
     assert m.var("cutpoints").transform == "ordered_positive"
-    _same_density(m, ref)
+    same_density(oracle(m), oracle(ref), m, ref, spread=0.5)
 
 
 def test_other_categoricals_and_transforms_are_refused_by_name(fake_pytensor):
@@ -209,9 +182,7 @@ def test_real_pymc_ordered_logistic_and_probit_lower_to_the_oracle_density():
                 pm.OrderedProbit("y", eta=eta, cutpoints=cut, sigma=1.0, observed=y)
         m = from_pymc(model)
         assert m.likelihoods[0].dist == f"ordered_{link}" and m.var("cutpoints").transform == "ordered"
-        from test_ir_ordinal import _oracle
-
-        f = _oracle(m)
+        f = oracle(m)
         lp_fn = model.compile_logp()
         q = m.initial_point()
         ip = model.initial_point()

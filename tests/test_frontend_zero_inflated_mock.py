@@ -8,27 +8,15 @@ HurdleLogNormal, other mixtures and other forms of psi are refused by name."""
 import numpy as np
 import pytest
 from test_frontend_bounded_mock import truncated_rv
-from test_frontend_mock import Constant, FakeModel, LogTransform, SharedVariable, Variable, apply, bcast, elem, fake_pytensor, rv  # noqa: F401
-from test_frontend_mock import AdvancedSubtensor1, Dot
+from test_frontend_mock import Constant, FakeModel, LogTransform, SharedVariable, apply, bcast, elem, fake_pytensor, rv  # noqa: F401
+from test_frontend_mock import AdvancedSubtensor1, Dot, Join, same_density
+from test_ir_zero_inflated import oracle
 
 from pymc_b200 import ir
 
 
-class Join:
-    pass
-
-
 class LogOddsTransform:
     pass
-
-
-def _free(M, r, size, transform, suffix, initial=None):
-    """M.free under the value name PyMC gives a transformed variable: {name}_{suffix}__"""
-    M.free(r, size, transform, initial)
-    old = M.rvs_to_values[r].name
-    M.rvs_to_values[r] = Variable(r.name + suffix)
-    M._ip[r.name + suffix] = M._ip.pop(old)
-    return r
 
 
 def weights(psi):
@@ -81,7 +69,7 @@ def _model(dist, psi_kind, seed=3, N=40):
     if psi_kind == "const":
         psi, p_ir = Constant(0.7), 0.7
     elif psi_kind == "var":
-        psi = _free(M, rv("BetaRV", "psi", Constant(2.0), Constant(2.0)), 1, LogOddsTransform(), "_logodds__")
+        psi = M.free(rv("BetaRV", "psi", Constant(2.0), Constant(2.0)), 1, LogOddsTransform(), suffix="_logodds__")
         vars_.append(ir.Var("psi_logodds__", "psi", 1, "interval", bounds=(0.0, 1.0)))
         priors.append(ir.Prior("beta", "psi_logodds__", (2.0, 2.0)))
         p_ir = ir.Ref("psi_logodds__")
@@ -101,19 +89,6 @@ def _model(dist, psi_kind, seed=3, N=40):
     return M, ref
 
 
-def _same_density(m, ref, seed=0):
-    from test_ir_zero_inflated import _oracle
-
-    f, g = _oracle(m), _oracle(ref)
-    assert [v.name for v in m.vars] == [v.name for v in ref.vars] and [v.transform for v in m.vars] == [v.transform for v in ref.vars]
-    rng = np.random.default_rng(seed)
-    for _ in range(4):
-        q = ref.initial_point() + rng.uniform(-0.5, 0.5, ref.n)
-        (a, ga), (b, gb) = f(q), g(q)
-        assert abs(a - b) <= 1e-12 * abs(b)
-        np.testing.assert_allclose(ga, gb, rtol=1e-12, atol=1e-12)
-
-
 @pytest.mark.parametrize("psi_kind", ["const", "var", "logit"])
 @pytest.mark.parametrize("dist", ir.ZI_LIKS)
 def test_each_spelling_lowers_to_the_hand_built_density(fake_pytensor, dist, psi_kind):
@@ -123,7 +98,7 @@ def test_each_spelling_lowers_to_the_hand_built_density(fake_pytensor, dist, psi
     m = from_pymc(M)
     L = m.likelihoods[0]
     assert L.dist == dist and type(L.psi) is type(ref.likelihoods[0].psi)
-    _same_density(m, ref)
+    same_density(oracle(m), oracle(ref), m, ref, spread=0.5)
     # and it lowers: psi block one past the predictor's terms
     low = ir.lower(ir.fuse_design_columns(m))
     assert low.liks[0]["nu"] == (2.0 if psi_kind == "logit" else 0.0) and len(low.liks[0]["psi"]) == (2 if psi_kind == "logit" else 1)
@@ -187,7 +162,7 @@ def test_other_mixtures_and_forms_of_psi_are_refused_by_name(fake_pytensor):
 
     def vector_psi():
         M, eta, y, N = _base()
-        p = _free(M, rv("BetaRV", "p", Constant(2.0), Constant(2.0)), N, LogOddsTransform(), "_logodds__")
+        p = M.free(rv("BetaRV", "p", Constant(2.0), Constant(2.0)), N, LogOddsTransform(), suffix="_logodds__")
         M.observe(rv("MixtureRV", "y", weights(p), dirac(), rv("PoissonRV", None, elem("Exp", eta))), y)
         return M
 

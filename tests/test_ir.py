@@ -7,16 +7,9 @@ import numpy as np
 import pytest
 from scipy import stats
 
+from b200_helpers import adaptive_against_oracle, fd_grad, fixed_step_against_oracle
+
 from pymc_b200 import _lib, ir, models
-
-
-def fd_grad(f, q, h=1e-6):
-    g = np.empty_like(q)
-    for i in range(len(q)):
-        e = np.zeros_like(q)
-        e[i] = h
-        g[i] = (f(q + e)[0] - f(q - e)[0]) / (2 * h)
-    return g
 
 
 @pytest.mark.parametrize("name", ["eight_schools", "radon", "stochvol"])
@@ -249,44 +242,13 @@ def test_ir_models_reproduce_the_reference_goldens_without_model_specific_cuda(g
 def test_new_model_runs_with_no_new_cuda_and_matches_the_oracle_sampler():
     """A model no kernel was written for (centred varying-intercept logistic regression): fixed-step NUTS on the device
     equals the oracle NUTS on the IR's NumPy logp draw by draw; an adaptive run recovers the oracle's posterior."""
-    from oracle import ir_numpy, nuts_numpy
-    from pymc_b200 import engine
-    from pymc_b200 import rng as brng
+    from oracle import ir_numpy
 
     m = ir.varying_intercept_logistic_ir()
-    cm = engine.CompiledModel(m)
-    assert cm.spec.name == "ir"
     f = ir_numpy.make_logp(m)
-    C, T, eps = 3, 12, 0.05
-    rs = np.random.default_rng(5)
-    q0 = m.initial_point() + rs.uniform(-0.3, 0.3, (C, m.n))
-    step_rngs, pot_rngs, _ = brng.chain_generators(9, C)
-    z = brng.momentum_noise(pot_rngs, T, m.n)
-    res = cm.nuts_run(q0, brng.pack_pcg64(step_rngs), tune=0, draws=T, z=z, mass="diag", adapt_step_size=False,
-                      eps0=np.full(C, eps))
-    for c in range(C):
-        o = nuts_numpy.Oracle(f, nuts_numpy.DiagMass(np.ones(m.n)), adapt_step_size=False)
-        o.da = nuts_numpy.DualAveraging(eps)
-        o.rng, o.tune = step_rngs[c], False
-        qs, st = o.run(q0[c], 0, T, z=z[c])
-        assert np.array_equal(st["tree_size"], res.stats["tree_size"][c])
-        assert np.max(np.abs(qs - res.draws[c])) <= 1e-9
-    # adaptive run, device momentum: posterior of 64 chains vs 8 oracle chains
-    C = 64
-    sr, _, js = brng.chain_generators(21, C)
-    q0 = np.stack([m.initial_point() + np.random.default_rng(s).uniform(-1, 1, m.n) for s in js])
-    run = cm.nuts_run(q0, brng.pack_pcg64(sr), tune=400, draws=300, mean0=np.broadcast_to(q0.mean(0), q0.shape).copy(),
-                      store_warmup=False, philox_seed=3)
-    xs = []
-    for c in range(8):
-        o = nuts_numpy.Oracle(f, nuts_numpy.DiagMass(np.ones(m.n), adapt=True, initial_mean=q0[c].copy(), initial_weight=10))
-        o.setup_chain(np.random.default_rng(100 + c))
-        xs.append(o.run(q0[c], 400, 300)[0][400:])
-    xo, xg = np.concatenate(xs), run.draws.reshape(-1, m.n)
-    se = np.sqrt(xo.var(0) / 300 + xg.var(0) / 2000)  # generous effective sample sizes
-    assert np.max(np.abs(xo.mean(0) - xg.mean(0)) / se) < 5.0
-    assert np.all(np.abs(np.log(xo.std(0) / xg.std(0))) < 0.25)
-    assert run.stats["diverging"].mean() < 0.02
+    fixed_step_against_oracle(m, f, 0.05, specialise=True, q0_seed=5)
+    adaptive_against_oracle(m, f, specialise=True, chain_seed=21, spread=1, philox_seed=3, oracle_seed=100, se_bound=5.0,
+                            max_divergence=0.02)
 
 
 @pytest.mark.gpu

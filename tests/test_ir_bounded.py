@@ -20,6 +20,8 @@ import numpy as np
 import pytest
 from mpmath import mp, mpf
 from scipy import stats
+from b200_helpers import (adaptive_against_oracle, fixed_step_against_oracle, logp_at_both_team_shapes, random_dense_cov,
+                          refusal_after_edit)
 from test_ir_closed_set import GRAD_TOL, LP_TOL, MP_DPS
 
 from pymc_b200 import _lib, ir
@@ -542,7 +544,7 @@ BUILDERS = {
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("cid", CASE_IDS)
-def test_device_logp_matches_the_mp_reference_and_the_oracle(cid, monkeypatch):
+def test_device_logp_matches_the_mp_reference_and_the_oracle(cid):
     """Chain = warp, then chain = CTA forced: each against the mp reference and the oracle, bit-identical when repeated."""
     from oracle import ir_numpy_bounded
     from pymc_b200 import engine
@@ -554,16 +556,10 @@ def test_device_logp_matches_the_mp_reference_and_the_oracle(cid, monkeypatch):
     Q, lp_mp, S, g_mp, G = mp_reference(cid)
     go = np.array([f(q)[1] for q in Q])
     lo = np.array([f(q)[0] for q in Q])
-    for team in ("warp", "cta"):
-        if team == "cta":
-            monkeypatch.setenv("B200_FORCE_TEAM", "1")
-        lp, g = cm.logp_dlogp(Q)
-        lp2, g2 = cm.logp_dlogp(Q)
-        assert np.array_equal(lp, lp2) and np.array_equal(g, g2), (cid, team)
+    for team, (lp, g) in logp_at_both_team_shapes(cm, Q).items():
         assert np.all(np.isfinite(lp)) and np.all(np.isfinite(g)), (cid, team)
         assert_close_to_reference(lp, g, lp_mp, S, g_mp, G, (cid, team))
         assert_close_to_reference(lp, g, lo, S, go, G, (cid, team, "oracle"))
-    monkeypatch.delenv("B200_FORCE_TEAM")
 
 
 @pytest.mark.gpu
@@ -585,71 +581,33 @@ def test_device_function_matches_the_oracle_on_the_builders(name):
     assert np.array_equal(lp, lp2) and np.array_equal(g, g2)
 
 
-def _fixed_step_against_oracle(m, eps, *, dense_cov=None, C=3, T=12, seed=9):
-    from oracle import ir_numpy_bounded, nuts_numpy
-    from pymc_b200 import engine
-    from pymc_b200 import rng as brng
-
-    cm = engine.CompiledModel(m, specialise=False)
-    f = ir_numpy_bounded.make_logp(m)
-    q0 = m.initial_point() + np.random.default_rng(seed).uniform(-0.3, 0.3, (C, m.n))
-    step_rngs, pot_rngs, _ = brng.chain_generators(seed, C)
-    z = brng.momentum_noise(pot_rngs, T, m.n)
-    if dense_cov is not None:
-        cm.set_dense_mass(dense_cov)
-    res = cm.nuts_run(q0, brng.pack_pcg64(step_rngs), tune=0, draws=T, z=z, mass="diag" if dense_cov is None else "dense",
-                      adapt_step_size=False, eps0=np.full(C, eps))
-    for c in range(C):
-        mass = nuts_numpy.DiagMass(np.ones(m.n)) if dense_cov is None else nuts_numpy.DenseMass(dense_cov)
-        o = nuts_numpy.Oracle(f, mass, adapt_step_size=False)
-        o.da = nuts_numpy.DualAveraging(eps)
-        o.rng, o.tune = step_rngs[c], False
-        qs, st = o.run(q0[c], 0, T, z=z[c])
-        assert np.array_equal(st["tree_size"], res.stats["tree_size"][c]), (m.name, c)
-        assert np.max(np.abs(qs - res.draws[c])) <= 1e-9, (m.name, c)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("name,eps", [("censored", 0.05), ("truncated", 0.05), ("censored_cta", 0.01)])
 def test_fixed_step_nuts_matches_the_oracle_sampler(name, eps):
-    _fixed_step_against_oracle(BUILDERS[name](), eps)
+    from oracle import ir_numpy_bounded
+
+    m = BUILDERS[name]()
+    fixed_step_against_oracle(m, ir_numpy_bounded.make_logp(m), eps)
 
 
 @pytest.mark.gpu
 def test_lockstep_dense_mass_run_matches_the_oracle():
+    from oracle import ir_numpy_bounded
+
     m = ir.truncated_regression_ir()
-    rng = np.random.default_rng(12)
-    U = rng.standard_normal((m.n, 2)) * 0.05
-    cov = np.diag(np.full(m.n, 0.02)) + U @ U.T
-    _fixed_step_against_oracle(m, 0.3, dense_cov=0.5 * (cov + cov.T), C=2, T=10)
+    fixed_step_against_oracle(m, ir_numpy_bounded.make_logp(m), 0.3, dense_cov=random_dense_cov(m.n, 2, 0.02, 0.05, 12),
+                              C=2, T=10)
 
 
 @pytest.mark.gpu
 def test_adaptive_censored_run_matches_the_oracle_posterior():
     """64 device chains against 8 oracle chains (NUTS with diagonal mass adaptation) on the censored regression: posterior
     means within 5 SE, standard deviations within 25 %, divergences below 2 %."""
-    from oracle import ir_numpy_bounded, nuts_numpy
-    from pymc_b200 import engine
-    from pymc_b200 import rng as brng
+    from oracle import ir_numpy_bounded
 
     m = ir.censored_regression_ir()
-    cm = engine.CompiledModel(m)
-    f = ir_numpy_bounded.make_logp(m)
-    C = 64
-    sr, _, js = brng.chain_generators(23, C)
-    q0 = np.stack([m.initial_point() + np.random.default_rng(s).uniform(-1, 1, m.n) for s in js])
-    run = cm.nuts_run(q0, brng.pack_pcg64(sr), tune=400, draws=300, mean0=np.broadcast_to(q0.mean(0), q0.shape).copy(),
-                      store_warmup=False, philox_seed=5)
-    xs = []
-    for c in range(8):
-        o = nuts_numpy.Oracle(f, nuts_numpy.DiagMass(np.ones(m.n), adapt=True, initial_mean=q0[c].copy(), initial_weight=10))
-        o.setup_chain(np.random.default_rng(200 + c))
-        xs.append(o.run(q0[c], 400, 300)[0][400:])
-    xo, xg = np.concatenate(xs), run.draws.reshape(-1, m.n)
-    se = np.sqrt(xo.var(0) / 300 + xg.var(0) / 2000)
-    assert np.max(np.abs(xo.mean(0) - xg.mean(0)) / se) < 5.0
-    assert np.all(np.abs(np.log(xo.std(0) / xg.std(0))) < 0.25)
-    assert run.stats["diverging"].mean() < 0.02
+    adaptive_against_oracle(m, ir_numpy_bounded.make_logp(m), specialise=True, chain_seed=23, spread=1, philox_seed=5,
+                            oracle_seed=200, se_bound=5.0, max_divergence=0.02)
 
 
 def _scipy_on_draws(m, q):
@@ -688,35 +646,28 @@ def test_pointwise_log_likelihood_and_the_log_likelihood_group_match_scipy():
 def test_model_create_refuses_malformed_bound_tables_through_the_c_abi():
     """prepare_ir makes the checks of validate(), with the same words, for callers of the C ABI; a bounded Normal is not a
     latent factor."""
-    from b200_helpers import create_raw
+    def set_y(row, k, value):
+        def edit(low):
+            low.liks[0]["y"] = low.liks[0]["y"].copy()
+            low.liks[0]["y"][row, k] = value
+        return edit
 
-    def block_edit(builder, row, k, value):
-        low = ir.lower(builder())
-        assert create_raw(low) is None
+    def both_open(low):
         low.liks[0]["y"] = low.liks[0]["y"].copy()
-        low.liks[0]["y"][row, k] = value
-        return create_raw(low)
+        low.liks[0]["y"][1] = -np.inf
+        low.liks[0]["y"][2] = np.inf
 
     c, t = ir.censored_regression_ir, ir.truncated_regression_ir
-    for builder, row, k, value, msg in [
-        (c, 1, 0, np.inf, ir.BOUND_SIDES), (t, 2, 0, -np.inf, ir.BOUND_SIDES), (c, 2, 3, np.nan, ir.BOUND_SIDES),
-        (c, 2, 0, -100.0, ir.BOUND_ORDER), (t, 2, 0, -1.0, ir.BOUND_ORDER),
-        (c, 0, 0, -100.0, ir.BOUND_Y), (t, 0, 0, -1.0, ir.BOUND_Y), (c, 0, 1, np.nan, ir.BOUND_Y),
-    ]:
-        err = block_edit(builder, row, k, value)
+    bad_sigma = lambda low: low.liks[0].update(sigma_value=-1.0, sigma_kind=ir.SIGMA_CONST)  # noqa: E731
+    as_latent = lambda low: low.liks[0].update(y_var=1)  # noqa: E731  (a latent factor on its first variable)
+    cases = [
+        (c, set_y(1, 0, np.inf), ir.BOUND_SIDES), (t, set_y(2, 0, -np.inf), ir.BOUND_SIDES),
+        (c, set_y(2, 3, np.nan), ir.BOUND_SIDES), (c, set_y(2, 0, -100.0), ir.BOUND_ORDER), (t, set_y(2, 0, -1.0), ir.BOUND_ORDER),
+        (c, set_y(0, 0, -100.0), ir.BOUND_Y), (t, set_y(0, 0, -1.0), ir.BOUND_Y), (c, set_y(0, 1, np.nan), ir.BOUND_Y),
+        (t, both_open, ir.TRUNC_OPEN),
+        (c, bad_sigma, "must be a finite constant > 0"), (t, bad_sigma, "must be a finite constant > 0"),
+        (c, as_latent, "latent factor"), (t, as_latent, "latent factor"),
+    ]
+    for builder, edit, msg in cases:
+        err = refusal_after_edit(builder, edit)
         assert err is not None and msg in err, (msg, err)
-    low = ir.lower(t())
-    low.liks[0]["y"] = low.liks[0]["y"].copy()
-    low.liks[0]["y"][1] = -np.inf
-    low.liks[0]["y"][2] = np.inf
-    err = create_raw(low)
-    assert err is not None and ir.TRUNC_OPEN in err, err
-    for builder in (c, t):
-        low = ir.lower(builder())
-        low.liks[0]["sigma_value"], low.liks[0]["sigma_kind"] = -1.0, ir.SIGMA_CONST
-        err = create_raw(low)
-        assert err is not None and "must be a finite constant > 0" in err, err
-        low = ir.lower(builder())
-        low.liks[0]["y_var"] = 1  # as a latent factor on its first variable
-        err = create_raw(low)
-        assert err is not None and "latent factor" in err, err

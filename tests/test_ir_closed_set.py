@@ -32,6 +32,7 @@ import pytest
 from mpmath import mp, mpf
 from scipy import stats
 from scipy.special import expit
+from b200_helpers import fixed_step_against_oracle, logp_at_both_team_shapes, random_dense_cov, refusal_after_edit
 from test_frontend_mock import fake_pytensor  # noqa: F401
 
 from pymc_b200 import ir
@@ -721,7 +722,7 @@ def test_from_pymc_refuses_a_positive_variable_without_its_transform(fake_pytens
 # ------------------------------------------------------------------------------------------------------------------------
 @pytest.mark.gpu
 @pytest.mark.parametrize("cid", CASE_IDS)
-def test_device_logp_matches_the_mp_reference_and_the_oracle(cid, monkeypatch):
+def test_device_logp_matches_the_mp_reference_and_the_oracle(cid):
     """Chain = warp, then the same handle with chain = CTA forced: each against the mp reference and the oracle, each
     bit-identical when repeated, the two equal to rounding.  Far-out interval points against the oracle."""
     from oracle import ir_numpy_families
@@ -733,22 +734,16 @@ def test_device_logp_matches_the_mp_reference_and_the_oracle(cid, monkeypatch):
     f = ir_numpy_families.make_logp(m)
     Q, lp_mp, S, g_mp = mp_reference(cid)
     lo, go = np.array([f(q)[0] for q in Q]), np.array([f(q)[1] for q in Q])
-    far = far_interval_points(m)
-    out = {}
-    for team in ("warp", "cta"):
-        if team == "cta":
-            monkeypatch.setenv("B200_FORCE_TEAM", "1")
-        lp, g = cm.logp_dlogp(Q)
-        lp2, g2 = cm.logp_dlogp(Q)
-        assert np.array_equal(lp, lp2) and np.array_equal(g, g2), (cid, team)
+    out = logp_at_both_team_shapes(cm, Q)
+    for team, (lp, g) in out.items():
         assert_close_to_reference(lp, g, lp_mp, S, g_mp, (cid, team))
         assert np.max(np.abs(lp - lo) / np.abs(lo)) <= 1e-12, (cid, team)
         assert np.max(np.abs(g - go) / np.maximum(1.0, np.max(np.abs(go), axis=1, keepdims=True))) <= 1e-12, (cid, team)
-        out[team] = lp, g
-        if far is not None:
-            lpf, gf = cm.logp_dlogp(far)
-            with np.errstate(all="ignore"):
-                ref = [f(q) for q in far]
+    far = far_interval_points(m)
+    if far is not None:
+        with np.errstate(all="ignore"):
+            ref = [f(q) for q in far]
+        for team, (lpf, gf) in logp_at_both_team_shapes(cm, far).items():
             for k, (a, b) in enumerate(ref):
                 assert np.isfinite(lpf[k]) == np.isfinite(a), (cid, team, k)
                 if np.isfinite(a):
@@ -756,7 +751,6 @@ def test_device_logp_matches_the_mp_reference_and_the_oracle(cid, monkeypatch):
                     fin = np.isfinite(b)
                     assert np.array_equal(np.isfinite(gf[k]), fin), (cid, team, k)
                     assert np.max(np.abs(gf[k][fin] - b[fin]), initial=0.0) <= 1e-12 * max(1.0, np.max(np.abs(b[fin]), initial=0.0))
-    monkeypatch.delenv("B200_FORCE_TEAM")
     (lw, gw), (lc, gc) = out["warp"], out["cta"]
     assert np.all(np.abs(lw - lc) <= LP_TOL * S), cid
     assert np.all(np.max(np.abs(gw - gc), axis=1) <= GRAD_TOL * np.maximum(1.0, np.max(np.abs(gw), axis=1))), cid
@@ -823,22 +817,21 @@ NUTS_CASES = [  # one per likelihood kind, two likelihoods, two AR(1) factors; f
 @pytest.mark.parametrize("team", ["warp", "cta"])
 @pytest.mark.parametrize("cid,eps", NUTS_CASES, ids=[c for c, _ in NUTS_CASES])
 def test_fixed_step_nuts_matches_the_oracle_sampler(cid, eps, team, monkeypatch):
-    from test_ir_families import _fixed_step_against_oracle
+    from oracle import ir_numpy_families
 
     if team == "cta":
         monkeypatch.setenv("B200_FORCE_TEAM", "1")
-    _fixed_step_against_oracle(build(cid), eps, C=2, T=10)
+    m = build(cid)
+    fixed_step_against_oracle(m, ir_numpy_families.make_logp(m), eps, C=2, T=10)
 
 
 @pytest.mark.gpu
 def test_lockstep_dense_mass_run_matches_the_oracle_on_two_likelihoods():
-    from test_ir_families import _fixed_step_against_oracle
+    from oracle import ir_numpy_families
 
     m = build("two_likelihoods-normal50-bernoulli20")
-    rng = np.random.default_rng(5)
-    U = rng.standard_normal((m.n, 3)) * 0.05
-    cov = np.diag(np.full(m.n, 0.05)) + U @ U.T
-    _fixed_step_against_oracle(m, 0.25, dense_cov=0.5 * (cov + cov.T), C=2, T=10)
+    fixed_step_against_oracle(m, ir_numpy_families.make_logp(m), 0.25, dense_cov=random_dense_cov(m.n, 3, 0.05, 0.05, 5),
+                              C=2, T=10)
 
 
 def _eta(m, L, q):
@@ -880,13 +873,6 @@ def test_pointwise_log_likelihood_matches_scipy(cid):
 
 def test_model_create_refuses_tables_outside_the_support_through_the_c_abi():
     """b200_model_create makes the support checks of validate(), with the same words, for callers of the C ABI."""
-    from b200_helpers import create_raw
-
-    def lowered(cid):
-        low = ir.lower(build(cid))
-        assert create_raw(low) is None  # the unedited tables are accepted
-        return low
-
     def var_index(cid, name):
         return [v.name for v in build(cid).vars].index(name)
 
@@ -971,7 +957,5 @@ def test_model_create_refuses_tables_outside_the_support_through_the_c_abi():
         low.liks[0]["y"][2] = 2.0
 
     for cid, edit, msg in edits:
-        low = lowered(cid)
-        edit(low)
-        err = create_raw(low)
+        err = refusal_after_edit(lambda: build(cid), edit)
         assert err is not None and msg in err, (cid, msg, err)

@@ -16,6 +16,7 @@ import re
 
 import numpy as np
 import pytest
+from b200_helpers import fixed_step_against_oracle, logp_at_both_team_shapes, random_dense_cov, refusal_after_edit
 from test_frontend_mock import (AdvancedSubtensor1, Constant, Dot, FakeModel, LogTransform, SharedVariable, apply, bcast,
                                 elem, fake_pytensor, rv)  # noqa: F401
 from test_ir_closed_set import GRAD_TOL, LP_TOL, scipy_loglik
@@ -444,22 +445,22 @@ def _sweep():
 
 
 def _check_device(cm, m, Q, what):
+    """Both team shapes, each repeated bit for bit, against the design oracle; returns {team: (lp, g)}."""
     f = design_logp(m)
-    lp, g = cm.logp_dlogp(Q)
-    lp2, g2 = cm.logp_dlogp(Q)
-    assert np.array_equal(lp, lp2) and np.array_equal(g, g2), what
-    for k, q in enumerate(Q):
-        lo, go = f(q)
-        S = pieces_scale(m, q, lo)
-        assert abs(lp[k] - lo) <= LP_TOL * S, (what, k, abs(lp[k] - lo) / S)
-        err = np.max(np.abs(g[k] - go)) / max(1.0, np.max(np.abs(go)))
-        assert err <= GRAD_TOL, (what, k, err)
-    return lp, g
+    out = logp_at_both_team_shapes(cm, Q)
+    for team, (lp, g) in out.items():
+        for k, q in enumerate(Q):
+            lo, go = f(q)
+            S = pieces_scale(m, q, lo)
+            assert abs(lp[k] - lo) <= LP_TOL * S, (what, team, k, abs(lp[k] - lo) / S)
+            err = np.max(np.abs(g[k] - go)) / max(1.0, np.max(np.abs(go)))
+            assert err <= GRAD_TOL, (what, team, k, err)
+    return out
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("dist", FAMILIES)
-def test_device_design_term_matches_the_oracle(dist, monkeypatch):
+def test_device_design_term_matches_the_oracle(dist):
     from pymc_b200 import engine
 
     for d, K, N in _sweep():
@@ -468,12 +469,7 @@ def test_device_design_term_matches_the_oracle(dist, monkeypatch):
         m = design_model(dist, N, K, seed=K + N)
         cm = engine.CompiledModel(m)
         assert cm.spec.name == "ir"
-        Q = _points(m, 3, K)
-        for team in ("warp", "cta"):
-            if team == "cta":
-                monkeypatch.setenv("B200_FORCE_TEAM", "1")
-            _check_device(cm, m, Q, (dist, K, N, team))
-        monkeypatch.delenv("B200_FORCE_TEAM")
+        _check_device(cm, m, _points(m, 3, K), (dist, K, N))
 
 
 SHAPES = {
@@ -487,18 +483,12 @@ SHAPES = {
 @pytest.mark.gpu
 @pytest.mark.parametrize("shape", list(SHAPES))
 @pytest.mark.parametrize("K", [33, 300])
-def test_device_design_term_in_composite_models(shape, K, monkeypatch):
+def test_device_design_term_in_composite_models(shape, K):
     from pymc_b200 import engine
 
     m = SHAPES[shape](K)
-    cm = engine.CompiledModel(m)
     Q = _points(m, 3, 9, spread=0.3)
-    out = {}
-    for team in ("warp", "cta"):
-        if team == "cta":
-            monkeypatch.setenv("B200_FORCE_TEAM", "1")
-        out[team] = _check_device(cm, m, Q, (shape, K, team))
-    monkeypatch.delenv("B200_FORCE_TEAM")
+    out = _check_device(engine.CompiledModel(m), m, Q, (shape, K))
     # the column form on the generic function, as written, agrees
     lc, gc = engine.CompiledModel(as_columns(m), specialise=False).logp_dlogp(Q)
     lp, g = out["warp"]
@@ -534,32 +524,6 @@ def test_fused_and_as_written_agree_on_the_device(builder):
     assert np.all(np.max(np.abs(gf - gw), axis=1) <= GRAD_TOL * np.maximum(1.0, np.max(np.abs(gw), axis=1)))
 
 
-def _fixed_step(m, eps, *, dense_cov=None, C=2, T=10, seed=9):
-    """The device NUTS run with a fixed step against the oracle sampler on the NumPy density: identical trees, positions
-    within 1e-9."""
-    from oracle import nuts_numpy
-    from pymc_b200 import engine
-    from pymc_b200 import rng as brng
-
-    cm = engine.CompiledModel(m)
-    f = design_logp(m)
-    q0 = m.initial_point() + np.random.default_rng(seed).uniform(-0.3, 0.3, (C, m.n))
-    step_rngs, pot_rngs, _ = brng.chain_generators(seed, C)
-    z = brng.momentum_noise(pot_rngs, T, m.n)
-    if dense_cov is not None:
-        cm.set_dense_mass(dense_cov)
-    res = cm.nuts_run(q0, brng.pack_pcg64(step_rngs), tune=0, draws=T, z=z, mass="diag" if dense_cov is None else "dense",
-                      adapt_step_size=False, eps0=np.full(C, eps))
-    for c in range(C):
-        mass = nuts_numpy.DiagMass(np.ones(m.n)) if dense_cov is None else nuts_numpy.DenseMass(dense_cov)
-        o = nuts_numpy.Oracle(f, mass, adapt_step_size=False)
-        o.da = nuts_numpy.DualAveraging(eps)
-        o.rng, o.tune = step_rngs[c], False
-        qs, st = o.run(q0[c], 0, T, z=z[c])
-        assert np.array_equal(st["tree_size"], res.stats["tree_size"][c]), (m.name, c)
-        assert np.max(np.abs(qs - res.draws[c])) <= 1e-9, (m.name, c)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("team", ["warp", "cta"])
 @pytest.mark.parametrize("shape,eps", [("glm", 0.15), ("group", 0.05), ("two_likelihoods", 0.1)])
@@ -567,16 +531,14 @@ def test_fixed_step_nuts_matches_the_oracle_sampler(shape, eps, team, monkeypatc
     if team == "cta":
         monkeypatch.setenv("B200_FORCE_TEAM", "1")
     m = design_model("bernoulli_logit", 200, 40, seed=5) if shape == "glm" else SHAPES[shape](33)
-    _fixed_step(m, eps)
+    fixed_step_against_oracle(m, design_logp(m), eps, specialise=True, C=2, T=10)
 
 
 @pytest.mark.gpu
 def test_lockstep_dense_mass_run_matches_the_oracle():
     m = design_model("negative_binomial_log", 150, 20, seed=6, group=4)
-    rng = np.random.default_rng(5)
-    U = rng.standard_normal((m.n, 3)) * 0.05
-    cov = np.diag(np.full(m.n, 0.05)) + U @ U.T
-    _fixed_step(m, 0.2, dense_cov=0.5 * (cov + cov.T))
+    fixed_step_against_oracle(m, design_logp(m), 0.2, specialise=True, dense_cov=random_dense_cov(m.n, 3, 0.05, 0.05, 5), C=2,
+                              T=10)
 
 
 @pytest.mark.gpu
@@ -598,18 +560,14 @@ def test_pointwise_log_likelihood_matches_scipy(K):
 
 
 def test_model_create_refuses_malformed_design_tables_through_the_c_abi():
-    from b200_helpers import create_raw
-
     m = design_model("normal", 30, 8, group=3)
 
-    def case(edit):
-        low = ir.lower(m)
-        T = low.liks[0]["terms"][1]
-        assert T["n_cols"] == 8
-        edit(T)
-        return create_raw(low)
-
-    assert case(lambda T: None) is None
+    def design_term(edit):
+        def f(low):
+            T = low.liks[0]["terms"][1]
+            assert T["n_cols"] == 8
+            edit(T)
+        return f
 
     def nan(T):
         T["coef"] = T["coef"].copy()
@@ -622,5 +580,5 @@ def test_model_create_refuses_malformed_design_tables_through_the_c_abi():
         (lambda T: T.update(factors=[]), "a design term has exactly one factor"),
         (nan, "X must be finite"),
     ]:
-        err = case(edit)
+        err = refusal_after_edit(lambda: m, design_term(edit))
         assert err is not None and re.search(msg, err), (msg, err)

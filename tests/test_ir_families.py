@@ -8,18 +8,9 @@ import numpy as np
 import pytest
 from scipy import stats
 
-from b200_helpers import create_raw
+from b200_helpers import adaptive_against_oracle, fd_grad, fixed_step_against_oracle, random_dense_cov, refusal_after_edit
 
 from pymc_b200 import _lib, ir
-
-
-def fd_grad(f, q, h=1e-6):
-    g = np.empty_like(q)
-    for i in range(len(q)):
-        e = np.zeros_like(q)
-        e[i] = h
-        g[i] = (f(q + e)[0] - f(q - e)[0]) / (2 * h)
-    return g
 
 
 def _sigmoid(x):
@@ -345,72 +336,33 @@ def test_negative_binomial_reproduces_the_reference_golden_on_the_generic_functi
         assert np.max(np.abs(res.draws[c] - d["draws_q"][c])) <= 1e-9
 
 
-def _fixed_step_against_oracle(m, eps, *, dense_cov=None, C=3, T=12, seed=9):
-    from oracle import ir_numpy_families, nuts_numpy
-    from pymc_b200 import engine
-    from pymc_b200 import rng as brng
-
-    cm = engine.CompiledModel(m, specialise=False)
-    f = ir_numpy_families.make_logp(m)
-    q0 = m.initial_point() + np.random.default_rng(seed).uniform(-0.3, 0.3, (C, m.n))
-    step_rngs, pot_rngs, _ = brng.chain_generators(seed, C)
-    z = brng.momentum_noise(pot_rngs, T, m.n)
-    if dense_cov is not None:
-        cm.set_dense_mass(dense_cov)
-    res = cm.nuts_run(q0, brng.pack_pcg64(step_rngs), tune=0, draws=T, z=z, mass="diag" if dense_cov is None else "dense",
-                      adapt_step_size=False, eps0=np.full(C, eps))
-    for c in range(C):
-        mass = nuts_numpy.DiagMass(np.ones(m.n)) if dense_cov is None else nuts_numpy.DenseMass(dense_cov)
-        o = nuts_numpy.Oracle(f, mass, adapt_step_size=False)
-        o.da = nuts_numpy.DualAveraging(eps)
-        o.rng, o.tune = step_rngs[c], False
-        qs, st = o.run(q0[c], 0, T, z=z[c])
-        assert np.array_equal(st["tree_size"], res.stats["tree_size"][c]), (m.name, c)
-        assert np.max(np.abs(qs - res.draws[c])) <= 1e-9, (m.name, c)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("name,eps", [("binomial", 0.05), ("gamma", 0.05), ("negbin_cta", 0.02)])
 def test_fixed_step_nuts_matches_the_oracle_sampler(name, eps):
-    _fixed_step_against_oracle(FAMILY_MODELS[name](), eps)
+    from oracle import ir_numpy_families
+
+    m = FAMILY_MODELS[name]()
+    fixed_step_against_oracle(m, ir_numpy_families.make_logp(m), eps)
 
 
 @pytest.mark.gpu
 def test_lockstep_dense_mass_run_matches_the_oracle_on_the_negative_binomial_model():
+    from oracle import ir_numpy_families
+
     m = ir.negative_binomial_ir()
-    rng = np.random.default_rng(12)
-    U = rng.standard_normal((m.n, 3)) * 0.05
-    cov = np.diag(np.full(m.n, 0.04)) + U @ U.T
-    _fixed_step_against_oracle(m, 0.3, dense_cov=0.5 * (cov + cov.T), C=2, T=10)
+    fixed_step_against_oracle(m, ir_numpy_families.make_logp(m), 0.3, dense_cov=random_dense_cov(m.n, 3, 0.04, 0.05, 12),
+                              C=2, T=10)
 
 
 @pytest.mark.gpu
 def test_adaptive_negative_binomial_run_matches_the_oracle_posterior():
     """64 device chains against 8 oracle chains (NUTS with diagonal mass adaptation) on the hierarchical negative-binomial
     regression with a random alpha: posterior means within 5 SE, standard deviations within 25 %, few divergences."""
-    from oracle import ir_numpy_families, nuts_numpy
-    from pymc_b200 import engine
-    from pymc_b200 import rng as brng
+    from oracle import ir_numpy_families
 
     m = ir.negative_binomial_ir()
-    cm = engine.CompiledModel(m)
-    assert cm.spec.name == "ir"
-    f = ir_numpy_families.make_logp(m)
-    C = 64
-    sr, _, js = brng.chain_generators(21, C)
-    q0 = np.stack([m.initial_point() + np.random.default_rng(s).uniform(-1, 1, m.n) for s in js])
-    run = cm.nuts_run(q0, brng.pack_pcg64(sr), tune=400, draws=300, mean0=np.broadcast_to(q0.mean(0), q0.shape).copy(),
-                      store_warmup=False, philox_seed=3)
-    xs = []
-    for c in range(8):
-        o = nuts_numpy.Oracle(f, nuts_numpy.DiagMass(np.ones(m.n), adapt=True, initial_mean=q0[c].copy(), initial_weight=10))
-        o.setup_chain(np.random.default_rng(100 + c))
-        xs.append(o.run(q0[c], 400, 300)[0][400:])
-    xo, xg = np.concatenate(xs), run.draws.reshape(-1, m.n)
-    se = np.sqrt(xo.var(0) / 300 + xg.var(0) / 2000)
-    assert np.max(np.abs(xo.mean(0) - xg.mean(0)) / se) < 5.0
-    assert np.all(np.abs(np.log(xo.std(0) / xg.std(0))) < 0.25)
-    assert run.stats["diverging"].mean() < 0.02
+    adaptive_against_oracle(m, ir_numpy_families.make_logp(m), specialise=True, chain_seed=21, spread=1, philox_seed=3,
+                            oracle_seed=100, se_bound=5.0, max_divergence=0.02)
 
 
 def _scipy_pointwise(m, q):
@@ -470,14 +422,9 @@ def test_sampler_records_the_log_likelihood_group_for_the_families():
 
 def test_model_create_rejects_out_of_support_tables_through_the_c_abi():
     """prepare_ir checks what validate() checks, for callers of the C ABI that bypass the Python front end."""
-    def case(builder, edit):
-        low = ir.lower(builder())
-        assert create_raw(low) is None  # the unedited tables are accepted
-        edit(low.liks[0], low)
-        return create_raw(low)
-
     def setter(**kw):
-        def f(L, low):
+        def f(low):
+            L = low.liks[0]
             for k, v in kw.items():
                 if k == "y0":
                     L["y"] = L["y"].copy()
@@ -508,5 +455,5 @@ def test_model_create_rejects_out_of_support_tables_through_the_c_abi():
         (nb_ref, setter(sigma_ref=0), "positive support"),     # alpha pointing at mu_a (no transform)
         (ga_ref, setter(sigma_ref=0), "positive support"),     # alpha pointing at b0
     ]:
-        err = case(builder, edit)
+        err = refusal_after_edit(builder, edit)
         assert err is not None and msg in err, (msg, err)

@@ -24,6 +24,7 @@ import numpy as np
 import pytest
 from mpmath import mp, mpf
 from scipy import stats
+from b200_helpers import fd_grad, fixed_step_against_oracle, logp_at_both_team_shapes, random_dense_cov, refusal_after_edit
 from test_frontend_mock import fake_pytensor  # noqa: F401
 from test_ir_closed_set import (GRAD_TOL, LP_TOL, MP_DPS, SCALE_RULE, _mp_constrain, _mp_factors, _mp_prior_pieces,
                                 assert_close_to_reference, points)
@@ -211,31 +212,6 @@ def oracle(m):
     return ir_latent_oracle.make_logp(m)
 
 
-def _fixed_step_against_oracle(m, eps, *, dense_cov=None, C=2, T=10, seed=9):
-    """Fixed-step NUTS on the device against the oracle sampler on the latent oracle: identical trees, positions 1e-9."""
-    from oracle import nuts_numpy
-    from pymc_b200 import engine
-    from pymc_b200 import rng as brng
-
-    cm = engine.CompiledModel(m, specialise=False)
-    f = oracle(m)
-    q0 = m.initial_point() + np.random.default_rng(seed).uniform(-0.3, 0.3, (C, m.n))
-    step_rngs, pot_rngs, _ = brng.chain_generators(seed, C)
-    z = brng.momentum_noise(pot_rngs, T, m.n)
-    if dense_cov is not None:
-        cm.set_dense_mass(dense_cov)
-    res = cm.nuts_run(q0, brng.pack_pcg64(step_rngs), tune=0, draws=T, z=z, mass="diag" if dense_cov is None else "dense",
-                      adapt_step_size=False, eps0=np.full(C, eps))
-    for c in range(C):
-        mass = nuts_numpy.DiagMass(np.ones(m.n)) if dense_cov is None else nuts_numpy.DenseMass(dense_cov)
-        o = nuts_numpy.Oracle(f, mass, adapt_step_size=False)
-        o.da = nuts_numpy.DualAveraging(eps)
-        o.rng, o.tune = step_rngs[c], False
-        qs, st = o.run(q0[c], 0, T, z=z[c])
-        assert np.array_equal(st["tree_size"], res.stats["tree_size"][c]), (m.name, c)
-        assert np.max(np.abs(qs - res.draws[c])) <= 1e-9, (m.name, c)
-
-
 # ------------------------------------------------------------------------------------------------------------------------
 # CPU: the reference and the oracle
 # ------------------------------------------------------------------------------------------------------------------------
@@ -308,8 +284,7 @@ def test_oracle_gradient_by_central_differences(cid):
     f = oracle(m)
     q = m.initial_point() + np.random.default_rng(7).uniform(-0.8, 0.8, m.n)
     g = f(q)[1]
-    h = 1e-5
-    fd = np.array([(f(q + h * e)[0] - f(q - h * e)[0]) / (2 * h) for e in np.eye(m.n)])
+    fd = fd_grad(f, q, h=1e-5)
     np.testing.assert_allclose(fd, g, rtol=1e-6, atol=1e-6 * max(1.0, np.max(np.abs(g))))
 
 
@@ -617,7 +592,7 @@ def test_real_pymc_centred_models_lower_to_their_own_density():
 # ------------------------------------------------------------------------------------------------------------------------
 @pytest.mark.gpu
 @pytest.mark.parametrize("cid", CASE_IDS)
-def test_device_logp_matches_the_mp_reference_and_the_oracle(cid, monkeypatch):
+def test_device_logp_matches_the_mp_reference_and_the_oracle(cid):
     from pymc_b200 import engine
 
     m = build(cid)
@@ -626,18 +601,11 @@ def test_device_logp_matches_the_mp_reference_and_the_oracle(cid, monkeypatch):
     f = oracle(m)
     Q, lp_mp, S, g_mp = mp_reference(cid)
     lo, go = np.array([f(q)[0] for q in Q]), np.array([f(q)[1] for q in Q])
-    out = {}
-    for team in ("warp", "cta"):
-        if team == "cta":
-            monkeypatch.setenv("B200_FORCE_TEAM", "1")
-        lp, g = cm.logp_dlogp(Q)
-        lp2, g2 = cm.logp_dlogp(Q)
-        assert np.array_equal(lp, lp2) and np.array_equal(g, g2), (cid, team)
+    out = logp_at_both_team_shapes(cm, Q)
+    for team, (lp, g) in out.items():
         assert_close_to_reference(lp, g, lp_mp, S, g_mp, (cid, team))
         assert np.max(np.abs(lp - lo) / np.abs(lo)) <= 1e-12, (cid, team)
         assert np.max(np.abs(g - go) / np.maximum(1.0, np.max(np.abs(go), axis=1, keepdims=True))) <= 1e-12, (cid, team)
-        out[team] = lp, g
-    monkeypatch.delenv("B200_FORCE_TEAM")
     (lw, gw), (lc, gc) = out["warp"], out["cta"]
     assert np.all(np.abs(lw - lc) <= LP_TOL * S), cid
     assert np.all(np.max(np.abs(gw - gc), axis=1) <= GRAD_TOL * np.maximum(1.0, np.max(np.abs(gw), axis=1))), cid
@@ -649,16 +617,14 @@ def test_device_logp_matches_the_mp_reference_and_the_oracle(cid, monkeypatch):
 def test_fixed_step_nuts_matches_the_oracle_sampler(name, eps, team, monkeypatch):
     if team == "cta":
         monkeypatch.setenv("B200_FORCE_TEAM", "1")
-    _fixed_step_against_oracle(ir.radon_centred_ir() if name == "radon_centred" else nested_ir(), eps, C=2, T=10)
+    m = ir.radon_centred_ir() if name == "radon_centred" else nested_ir()
+    fixed_step_against_oracle(m, oracle(m), eps, C=2, T=10)
 
 
 @pytest.mark.gpu
 def test_lockstep_dense_mass_run_matches_the_oracle_on_the_example():
     m = ir.radon_centred_ir()
-    rng = np.random.default_rng(6)
-    U = rng.standard_normal((m.n, 3)) * 0.03
-    cov = np.diag(np.full(m.n, 0.01)) + U @ U.T
-    _fixed_step_against_oracle(m, 0.3, dense_cov=0.5 * (cov + cov.T), C=2, T=10)
+    fixed_step_against_oracle(m, oracle(m), 0.3, dense_cov=random_dense_cov(m.n, 3, 0.01, 0.03, 6), C=2, T=10)
 
 
 def radon_noncentred_ir(**kw):
@@ -726,16 +692,8 @@ def test_log_likelihood_group_holds_only_the_observed_likelihood():
 
 
 def test_model_create_refuses_malformed_latent_tables():
-    from b200_helpers import create_raw
-
-    def edited(edit):
-        low = ir.lower(nested_ir())
-        assert create_raw(low) is None
-        edit(low.liks[2], low)
-        return create_raw(low)
-
     def setter(**kw):
-        return lambda L, low: L.update(kw)
+        return lambda low: low.liks[2].update(kw)
 
     n_vars = len(nested_ir().vars)
     for edit, msg in [(setter(y_var=-1), "outside [0, n_vars"), (setter(y_var=n_vars + 1), "outside [0, n_vars"),
@@ -743,5 +701,5 @@ def test_model_create_refuses_malformed_latent_tables():
                       (setter(y_var=1), "must equal the size of its variable"),
                       (setter(y_var=0), "missing observations"),
                       (setter(sigma_kind=ir.SIGMA_CONST, sigma_value=-1.0), "sigma must be a finite constant > 0")]:
-        err = edited(edit)
+        err = refusal_after_edit(nested_ir, edit)
         assert err is not None and msg in err, (msg, err)

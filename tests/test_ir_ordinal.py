@@ -18,13 +18,15 @@ import numpy as np
 import pytest
 from mpmath import mp, mpf
 from scipy import special, stats
+from b200_helpers import (adaptive_against_oracle, fd_grad, fixed_step_against_oracle, logp_at_both_team_shapes, random_dense_cov,
+                          refusal_after_edit)
 from test_ir_closed_set import LP_TOL, MP_DPS
 
 from pymc_b200 import ir, models
 from pymc_b200.ir import Likelihood, ModelIR, Prior, Ref, Term, Var
 
 
-def _oracle(m):
+def oracle(m):
     from ir_latent_oracle import make_logp as latent
     from oracle import ir_numpy_ordinal
 
@@ -109,7 +111,7 @@ def _mp_logp(m, q):
 def _conditioning(m, q, power=1):
     """sum over probit observations of (|a| + |b| + 1) / (b - a)^power: the rounding of forming the window from two bounds,
     in log Z (power 1) and in phi / Z, which the gradient carries (power 2)."""
-    f = _oracle(m)
+    f = oracle(m)
     x, _ = f.constrained(np.asarray(q, dtype=np.float64))
     tot = 0.0
     for L in m.likelihoods:
@@ -210,15 +212,6 @@ def _lp_tol(S, C):
     return LP_TOL * S + 1e-15 * C
 
 
-def _fd_grad(f, q, h=1e-6):
-    g = np.empty(len(q))
-    for j in range(len(q)):
-        e = np.zeros(len(q))
-        e[j] = h
-        g[j] = (f(q + e)[0] - f(q - e)[0]) / (2 * h)
-    return g
-
-
 # ------------------------------------------------------------------------------------------------------------------------
 # CPU: the reference and the oracle
 # ------------------------------------------------------------------------------------------------------------------------
@@ -262,12 +255,12 @@ def test_the_catalogue_covers_the_ordinal_forms():
 @pytest.mark.parametrize("cid", CASE_IDS)
 def test_oracle_matches_the_mp_reference_and_central_differences(cid):
     m = build(cid)
-    f = _oracle(m)
+    f = oracle(m)
     Q, lp_mp, S, C = mp_reference(cid)
     for q, want, s, c in zip(Q, lp_mp, S, C):
         lp, g = f(q)
         assert abs(lp - want) <= _lp_tol(s, c), (cid, lp, want)
-        fd = _fd_grad(f, q)
+        fd = fd_grad(f, q)
         np.testing.assert_allclose(g, fd, rtol=2e-5, atol=2e-5 * max(1.0, np.max(np.abs(g))), err_msg=cid)
 
 
@@ -306,11 +299,11 @@ def test_ordered_transform_equals_the_reference_formulas(size, positive):
     np.testing.assert_array_equal(np.reshape(spec.constrain(z)["c"], want.shape), want)
     assert np.all(np.diff(want, axis=-1) > 0)
     # the oracle's log|J| and chain rule, against central differences of logp = log|J| + sum_k N(x_k; 0, 3)
-    f = _oracle(m)
+    f = oracle(m)
     lp, g = f(z[0])
     jac = np.sum(z[0]) if positive else np.sum(z[0, 1:])
     assert abs(lp - (jac + np.sum(stats.norm.logpdf(want[0], 0.0, 3.0)))) <= 1e-12 * max(1.0, abs(lp))
-    np.testing.assert_allclose(g, _fd_grad(f, z[0]), rtol=1e-6, atol=1e-6 * max(1.0, np.max(np.abs(g))))
+    np.testing.assert_allclose(g, fd_grad(f, z[0]), rtol=1e-6, atol=1e-6 * max(1.0, np.max(np.abs(g))))
 
 
 def _ord(link="ordered_logistic", y=(0, 1, 2), cut=Ref("c_ordered__"), tr="ordered", size=2, prior="normal", sigma=None):
@@ -405,26 +398,20 @@ def _device(m):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("cid", CASE_IDS)
-def test_device_logp_matches_the_mp_reference_and_the_oracle(cid, monkeypatch):
+def test_device_logp_matches_the_mp_reference_and_the_oracle(cid):
     m = build(cid)
     cm = _device(m)
-    f = _oracle(m)
+    f = oracle(m)
     Q, lp_mp, S, C = mp_reference(cid)
     lo = np.array([f(q)[0] for q in Q])
     go = np.array([f(q)[1] for q in Q])
     C2 = np.array([_conditioning(m, q, 2) for q in Q])
-    for team in ("warp", "cta"):
-        if team == "cta":
-            monkeypatch.setenv("B200_FORCE_TEAM", "1")
-        lp, g = cm.logp_dlogp(Q)
-        lp2, g2 = cm.logp_dlogp(Q)
-        assert np.array_equal(lp, lp2) and np.array_equal(g, g2), (cid, team)
+    for team, (lp, g) in logp_at_both_team_shapes(cm, Q).items():
         assert np.all(np.abs(lp - lp_mp) <= _lp_tol(S, C)), (cid, team, lp - lp_mp)
         assert np.all(np.abs(lp - lo) <= _lp_tol(S, C)), (cid, team, lp - lo)
         scale = np.maximum(1.0, np.max(np.abs(go), axis=1, keepdims=True))
         err = np.max(np.abs(g - go) / scale, axis=1)
         assert np.all(err <= 1e-11 + 1e-15 * C2), (cid, team, err, C2)
-    monkeypatch.delenv("B200_FORCE_TEAM")
 
 
 @pytest.mark.gpu
@@ -434,7 +421,7 @@ def test_device_function_matches_the_oracle_on_the_builders(name):
     cm = _device(m)
     assert (m.n > 256) == name.endswith("cta")
     assert not cm.supports_constrain
-    f = _oracle(m)
+    f = oracle(m)
     Q = m.initial_point() + np.random.default_rng(0).uniform(-0.5, 0.5, (6, m.n))
     lp, g = cm.logp_dlogp(Q)
     lo, go = np.array([f(q)[0] for q in Q]), np.array([f(q)[1] for q in Q])
@@ -442,44 +429,18 @@ def test_device_function_matches_the_oracle_on_the_builders(name):
     assert np.max(np.abs(g - go) / np.maximum(1.0, np.max(np.abs(go), axis=1, keepdims=True))) <= 1e-11
 
 
-def _fixed_step_against_oracle(m, eps, *, dense_cov=None, C=3, T=12, seed=9):
-    from oracle import nuts_numpy
-    from pymc_b200 import rng as brng
-
-    cm = _device(m)
-    f = _oracle(m)
-    q0 = m.initial_point() + np.random.default_rng(seed).uniform(-0.3, 0.3, (C, m.n))
-    step_rngs, pot_rngs, _ = brng.chain_generators(seed, C)
-    z = brng.momentum_noise(pot_rngs, T, m.n)
-    if dense_cov is not None:
-        cm.set_dense_mass(dense_cov)
-    res = cm.nuts_run(q0, brng.pack_pcg64(step_rngs), tune=0, draws=T, z=z, mass="diag" if dense_cov is None else "dense",
-                      adapt_step_size=False, eps0=np.full(C, eps))
-    for c in range(C):
-        mass = nuts_numpy.DiagMass(np.ones(m.n)) if dense_cov is None else nuts_numpy.DenseMass(dense_cov)
-        o = nuts_numpy.Oracle(f, mass, adapt_step_size=False)
-        o.da = nuts_numpy.DualAveraging(eps)
-        o.rng, o.tune = step_rngs[c], False
-        qs, st = o.run(q0[c], 0, T, z=z[c])
-        for k in ("tree_size", "diverging"):
-            assert np.array_equal(np.asarray(st[k]).astype(float), np.asarray(res.stats[k][c]).astype(float)), (m.name, c, k)
-        assert np.max(np.abs(qs - res.draws[c])) <= 1e-9, (m.name, c)
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("name,eps", [("logistic", 0.1), ("probit", 0.1), ("probit_var", 0.1)])
 def test_fixed_step_nuts_matches_the_oracle_sampler(name, eps):
-    _fixed_step_against_oracle(BUILDERS[name](), eps)
+    m = BUILDERS[name]()
+    fixed_step_against_oracle(m, oracle(m), eps)
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("link", ["logistic", "probit"])
 def test_lockstep_dense_mass_run_matches_the_oracle(link):
     m = ir.ordinal_regression_ir(link, n_obs=120)
-    rng = np.random.default_rng(12)
-    U = rng.standard_normal((m.n, 2)) * 0.05
-    cov = np.diag(np.full(m.n, 0.02)) + U @ U.T
-    _fixed_step_against_oracle(m, 0.3, dense_cov=0.5 * (cov + cov.T), C=2, T=10)
+    fixed_step_against_oracle(m, oracle(m), 0.3, dense_cov=random_dense_cov(m.n, 2, 0.02, 0.05, 12), C=2, T=10)
 
 
 @pytest.mark.gpu
@@ -488,26 +449,9 @@ def test_adaptive_run_matches_the_oracle_posterior_and_returns_ordered_cutpoints
     effective-size-free bound, SE of the mean of the pooled draws), standard deviations within 25 %; the cutpoint draws of
     sample_b200_nuts come back ordered."""
     import pymc_b200
-    from oracle import nuts_numpy
-    from pymc_b200 import rng as brng
 
     m = ir.ordinal_regression_ir("logistic", n_obs=200)
-    cm = _device(m)
-    f = _oracle(m)
-    C = 64
-    sr, _, js = brng.chain_generators(23, C)
-    q0 = np.stack([m.initial_point() + np.random.default_rng(s).uniform(-0.5, 0.5, m.n) for s in js])
-    run = cm.nuts_run(q0, brng.pack_pcg64(sr), tune=400, draws=300, mean0=np.broadcast_to(q0.mean(0), q0.shape).copy(),
-                      store_warmup=False, philox_seed=5)
-    xs = []
-    for c in range(8):
-        o = nuts_numpy.Oracle(f, nuts_numpy.DiagMass(np.ones(m.n), adapt=True, initial_mean=q0[c].copy(), initial_weight=10))
-        o.setup_chain(np.random.default_rng(200 + c))
-        xs.append(o.run(q0[c], 400, 300)[0][400:])
-    xo, xg = np.concatenate(xs), run.draws.reshape(-1, m.n)
-    se = np.sqrt(xo.var(0) / 300 + xg.var(0) / 2000)
-    assert np.max(np.abs(xo.mean(0) - xg.mean(0)) / se) < 4.0
-    assert np.all(np.abs(np.log(xo.std(0) / xg.std(0))) < 0.25)
+    adaptive_against_oracle(m, oracle(m), chain_seed=23, spread=0.5, philox_seed=5, oracle_seed=200, se_bound=4.0)
     res = pymc_b200.sample_b200_nuts(30, tune=100, chains=4, random_seed=3, model=m, compute_convergence_checks=False)
     c = np.asarray(res.posterior["cutpoints"])
     assert c.shape == (4, 30, 4) and np.all(np.diff(c, axis=-1) > 0)
@@ -518,7 +462,7 @@ def test_pointwise_log_likelihood_and_the_log_likelihood_group_match_scipy():
     import pymc_b200
 
     def scipy_ll(m, q):
-        f = _oracle(m)
+        f = oracle(m)
         L = m.likelihoods[0]
         out = np.empty(q.shape[:-1] + (len(L.y),))
         y = np.asarray(L.y).astype(int)
@@ -549,14 +493,6 @@ def test_pointwise_log_likelihood_and_the_log_likelihood_group_match_scipy():
 
 
 def test_model_create_refuses_malformed_ordinal_tables_through_the_c_abi():
-    from b200_helpers import create_raw
-
-    def edited(builder, edit):
-        low = ir.lower(builder())
-        assert create_raw(low) is None
-        edit(low)
-        return create_raw(low)
-
     def set_y(low, v):
         low.liks[0]["y"] = low.liks[0]["y"].copy()
         low.liks[0]["y"][0] = v
@@ -579,5 +515,5 @@ def test_model_create_refuses_malformed_ordinal_tables_through_the_c_abi():
         (pr, lambda low: low.liks[0].update(sigma_kind=ir.SIGMA_NONE), "needs sigma"),
     ]
     for builder, edit, msg in cases:
-        err = edited(builder, edit)
+        err = refusal_after_edit(builder, edit)
         assert err is not None and msg in err, (msg, err)

@@ -19,13 +19,15 @@ import numpy as np
 import pytest
 from mpmath import mp, mpf
 from scipy import special, stats
+from b200_helpers import (adaptive_against_oracle, fd_grad, fixed_step_against_oracle, logp_at_both_team_shapes, random_dense_cov,
+                          refusal_after_edit)
 from test_ir_closed_set import LP_TOL, MP_DPS
 
 from pymc_b200 import ir
 from pymc_b200.ir import Likelihood, Linear, ModelIR, Prior, Ref, Term, Var
 
 
-def _oracle(m):
+def oracle(m):
     from oracle import ir_numpy_zero_inflated
 
     return ir_numpy_zero_inflated.make_logp(m)
@@ -254,15 +256,6 @@ def mp_reference(cid):
     return Q, lp, S
 
 
-def _fd_grad(f, q, h=1e-6):
-    g = np.empty(len(q))
-    for j in range(len(q)):
-        e = np.zeros(len(q))
-        e[j] = h
-        g[j] = (f(q + e)[0] - f(q - e)[0]) / (2 * h)
-    return g
-
-
 # ------------------------------------------------------------------------------------------------------------------------
 # CPU: the reference and the oracle
 # ------------------------------------------------------------------------------------------------------------------------
@@ -315,14 +308,14 @@ def test_the_catalogue_covers_every_form():
 @pytest.mark.parametrize("cid", CASE_IDS)
 def test_oracle_matches_the_mp_reference_and_central_differences(cid):
     m = build(cid)
-    f = _oracle(m)
+    f = oracle(m)
     Q, lp_mp, S = mp_reference(cid)
     for q, want, s in zip(Q, lp_mp, S):
         lp, g = f(q)
         assert np.isfinite(lp) and np.all(np.isfinite(g)), cid
         assert abs(lp - want) <= LP_TOL * s, (cid, lp, want)
         # psi = 1 - 2e-9 at z = 20: differences of the double psi are rounding; take them of the 40-digit one
-        fd = _fd_grad(lambda t: _mp_logp(m, t, exact=True), q) if "psi-z20" in cid else _fd_grad(f, q)
+        fd = fd_grad(lambda t: _mp_logp(m, t, exact=True), q) if "psi-z20" in cid else fd_grad(f, q)
         np.testing.assert_allclose(g, fd, rtol=2e-5, atol=2e-5 * max(1.0, np.max(np.abs(g))), err_msg=cid)
 
 
@@ -438,7 +431,7 @@ def test_lowered_tables_hold_the_psi_block_and_the_constants():
     fz = ir.fuse_design_columns(mz)
     assert len(fz.likelihoods[0].psi.terms) == 1 and np.array_equal(fz.likelihoods[0].psi.terms[0].coef, Z)
     q = np.array([0.1, 0.3, -0.2])
-    assert abs(_oracle(fz)(q)[0] - _oracle(mz)(q)[0]) <= 1e-12 * abs(_oracle(mz)(q)[0])
+    assert abs(oracle(fz)(q)[0] - oracle(mz)(q)[0]) <= 1e-12 * abs(oracle(mz)(q)[0])
 
 
 def test_constants_of_c0_match_the_oracle_split():
@@ -450,7 +443,7 @@ def test_constants_of_c0_match_the_oracle_split():
     y = np.asarray(L.y)
     pos = y > 0
     assert 0 < pos.sum() < len(y)
-    f = _oracle(m)
+    f = oracle(m)
     q = m.initial_point() + 0.1
     x, _ = f.constrained(q)
     ll = f.loglik(L, x)
@@ -471,49 +464,19 @@ def _device(m):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("cid", CASE_IDS)
-def test_device_logp_matches_the_mp_reference_and_the_oracle(cid, monkeypatch):
+def test_device_logp_matches_the_mp_reference_and_the_oracle(cid):
     m = build(cid)
     cm = _device(m)
-    f = _oracle(m)
+    f = oracle(m)
     Q, lp_mp, S = mp_reference(cid)
     lo = np.array([f(q)[0] for q in Q])
     go = np.array([f(q)[1] for q in Q])
-    for team in ("warp", "cta"):
-        if team == "cta":
-            monkeypatch.setenv("B200_FORCE_TEAM", "1")
-        lp, g = cm.logp_dlogp(Q)
-        lp2, g2 = cm.logp_dlogp(Q)
-        assert np.array_equal(lp, lp2) and np.array_equal(g, g2), (cid, team)
+    for team, (lp, g) in logp_at_both_team_shapes(cm, Q).items():
         assert np.all(np.abs(lp - lp_mp) <= LP_TOL * S), (cid, team, lp - lp_mp)
         assert np.all(np.abs(lp - lo) <= LP_TOL * S), (cid, team, lp - lo)
         scale = np.maximum(1.0, np.max(np.abs(go), axis=1, keepdims=True))
         err = np.max(np.abs(g - go) / scale, axis=1)
         assert np.all(err <= 1e-11), (cid, team, err)
-    monkeypatch.delenv("B200_FORCE_TEAM")
-
-
-def _fixed_step_against_oracle(m, eps, *, dense_cov=None, C=3, T=12, seed=9):
-    from oracle import nuts_numpy
-    from pymc_b200 import rng as brng
-
-    cm = _device(m)
-    f = _oracle(m)
-    q0 = m.initial_point() + np.random.default_rng(seed).uniform(-0.3, 0.3, (C, m.n))
-    step_rngs, pot_rngs, _ = brng.chain_generators(seed, C)
-    z = brng.momentum_noise(pot_rngs, T, m.n)
-    if dense_cov is not None:
-        cm.set_dense_mass(dense_cov)
-    res = cm.nuts_run(q0, brng.pack_pcg64(step_rngs), tune=0, draws=T, z=z, mass="diag" if dense_cov is None else "dense",
-                      adapt_step_size=False, eps0=np.full(C, eps))
-    for c in range(C):
-        mass = nuts_numpy.DiagMass(np.ones(m.n)) if dense_cov is None else nuts_numpy.DenseMass(dense_cov)
-        o = nuts_numpy.Oracle(f, mass, adapt_step_size=False)
-        o.da = nuts_numpy.DualAveraging(eps)
-        o.rng, o.tune = step_rngs[c], False
-        qs, st = o.run(q0[c], 0, T, z=z[c])
-        for k in ("tree_size", "diverging"):
-            assert np.array_equal(np.asarray(st[k]).astype(float), np.asarray(res.stats[k][c]).astype(float)), (m.name, c, k)
-        assert np.max(np.abs(qs - res.draws[c])) <= 1e-9, (m.name, c)
 
 
 @pytest.mark.gpu
@@ -521,16 +484,14 @@ def _fixed_step_against_oracle(m, eps, *, dense_cov=None, C=3, T=12, seed=9):
                                       ("hurdle_gamma", "logit"), ("hurdle_negative_binomial", "const"),
                                       ("zero_inflated_binomial", "logit")])
 def test_fixed_step_nuts_matches_the_oracle_sampler(dist, psi):
-    _fixed_step_against_oracle(ir.zero_inflated_ir(dist, psi), 0.05)
+    m = ir.zero_inflated_ir(dist, psi)
+    fixed_step_against_oracle(m, oracle(m), 0.05)
 
 
 @pytest.mark.gpu
 def test_lockstep_dense_mass_run_matches_the_oracle():
     m = ir.zero_inflated_ir("zero_inflated_negative_binomial", "logit", n_obs=120)
-    rng = np.random.default_rng(12)
-    U = rng.standard_normal((m.n, 2)) * 0.05
-    cov = np.diag(np.full(m.n, 0.01)) + U @ U.T
-    _fixed_step_against_oracle(m, 0.3, dense_cov=0.5 * (cov + cov.T), C=2, T=10)
+    fixed_step_against_oracle(m, oracle(m), 0.3, dense_cov=random_dense_cov(m.n, 2, 0.01, 0.05, 12), C=2, T=10)
 
 
 @pytest.mark.gpu
@@ -540,26 +501,9 @@ def test_adaptive_run_matches_the_oracle_posterior_and_recovers_psi():
     psi from sample_b200_nuts holds the simulated 0.6 within three posterior standard deviations (the spread the data
     leave) plus four MCSEs (bounded with an effective size of a tenth of the draws)."""
     import pymc_b200
-    from oracle import nuts_numpy
-    from pymc_b200 import rng as brng
 
     m = ir.zero_inflated_ir("zero_inflated_poisson", "var", n_obs=400)
-    cm = _device(m)
-    f = _oracle(m)
-    C = 64
-    sr, _, js = brng.chain_generators(23, C)
-    q0 = np.stack([m.initial_point() + np.random.default_rng(s).uniform(-0.5, 0.5, m.n) for s in js])
-    run = cm.nuts_run(q0, brng.pack_pcg64(sr), tune=400, draws=300, mean0=np.broadcast_to(q0.mean(0), q0.shape).copy(),
-                      store_warmup=False, philox_seed=5)
-    xs = []
-    for c in range(8):
-        o = nuts_numpy.Oracle(f, nuts_numpy.DiagMass(np.ones(m.n), adapt=True, initial_mean=q0[c].copy(), initial_weight=10))
-        o.setup_chain(np.random.default_rng(200 + c))
-        xs.append(o.run(q0[c], 400, 300)[0][400:])
-    xo, xg = np.concatenate(xs), run.draws.reshape(-1, m.n)
-    se = np.sqrt(xo.var(0) / 300 + xg.var(0) / 2000)
-    assert np.max(np.abs(xo.mean(0) - xg.mean(0)) / se) < 4.0
-    assert np.all(np.abs(np.log(xo.std(0) / xg.std(0))) < 0.25)
+    adaptive_against_oracle(m, oracle(m), chain_seed=23, spread=0.5, philox_seed=5, oracle_seed=200, se_bound=4.0)
     res = pymc_b200.sample_b200_nuts(300, tune=300, chains=8, random_seed=3, model=m, compute_convergence_checks=False)
     psi = np.asarray(res.posterior["psi"]).ravel()
     assert np.all((psi > 0) & (psi < 1))
@@ -571,7 +515,7 @@ def test_pointwise_log_likelihood_and_the_log_likelihood_group_match_scipy():
     import pymc_b200
 
     def scipy_ll(m, q):
-        f = _oracle(m)
+        f = oracle(m)
         L = m.likelihoods[0]
         fam = ir.ZI_FAMILY[L.dist]
         y = np.asarray(L.y)
@@ -607,14 +551,6 @@ def test_pointwise_log_likelihood_and_the_log_likelihood_group_match_scipy():
 
 
 def test_model_create_refuses_malformed_psi_and_y_tables_through_the_c_abi():
-    from b200_helpers import create_raw
-
-    def edited(builder, edit):
-        low = ir.lower(builder())
-        assert create_raw(low) is None
-        edit(low)
-        return create_raw(low)
-
     def set_y(low, v, i=0):
         low.liks[0]["y"] = low.liks[0]["y"].copy()
         low.liks[0]["y"][i] = v
@@ -651,5 +587,5 @@ def test_model_create_refuses_malformed_psi_and_y_tables_through_the_c_abi():
         (hnb, lambda low: low.liks[0].update(y_var=1), "latent factor"),
     ]
     for builder, edit, msg in cases:
-        err = edited(builder, edit)
+        err = refusal_after_edit(builder, edit)
         assert err is not None and msg in err, (msg, err)

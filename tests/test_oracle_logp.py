@@ -3,19 +3,11 @@ compositions (pymc/testing.py:311-418 check_logp), closed-form values from the r
 and central finite differences for the hand-derived gradients."""
 import numpy as np
 import pytest
+from b200_helpers import fd_grad
 from scipy import stats as st
 
 from oracle import logp_numpy as L
 from pymc_b200 import models
-
-
-def fd_grad(f, q, h=1e-6):
-    g = np.empty_like(q)
-    for i in range(len(q)):
-        e = np.zeros_like(q)
-        e[i] = h
-        g[i] = (f(q + e)[0] - f(q - e)[0]) / (2 * h)
-    return g
 
 
 def test_normal_matches_scipy():

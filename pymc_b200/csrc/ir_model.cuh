@@ -100,23 +100,144 @@ struct IrLikD { int dist, n_terms, term0, sigma_kind; long long N; const double*
                 const signed char* cens; const double* bnd; };
 struct IrAr1D { int offset, size; IrParamD phi, sigma; double init_sigma; };
 
-// eta_i = sum_t coef_t[i] prod_f x_f[idx_f[i]] over the likelihood's terms, t ascending (as eval's observation loop)
-__device__ __forceinline__ double ir_eta(const IrTermD* terms, int n_terms, const double* x, int i, int N) {
+// ---- per-observation pieces, shared by eval's observation loops and the pointwise kernel
+
+// x_f[idx_f[i]]: factor F at observation i (indexed, scalar or elementwise)
+__device__ __forceinline__ double ir_factor(const IrFactorD& F, const double* x, int i) {
+    return x[F.offset + (F.idx ? F.idx[i] : (F.size == 1 ? 0 : i))];
+}
+
+// eta_i = sum_t coef_t[i] prod_f x_f[idx_f[i]] over the block terms[term0 .. term0 + n_terms), t ascending.
+// terms is taken by reference so that eval, which passes the member P.terms, loads it inside the loop, after the
+// n_terms check, and indexes it with term0 + t; the out-of-line passes pass the block's start with term0 = 0.  Each
+// caller thereby keeps the code it had with its own inline loop, and the kernels that reach eval keep their register
+// allocation (stack and spills are sensitive to any change in eval's code).
+__device__ __forceinline__ double ir_eta(const IrTermD* const& terms, int term0, int n_terms, const double* x, int i,
+                                         int N) {
     double eta = 0.0;
     for (int t = 0; t < n_terms; ++t) {
-        const IrTermD& Tm = terms[t];
+        const IrTermD& Tm = terms[term0 + t];
         if (Tm.n_cols) {
             eta += ir_design_row(Tm, x + Tm.f[0].offset, i, N);
             continue;
         }
         double pr = Tm.coef ? Tm.coef[i] : 1.0;
-        for (int f = 0; f < Tm.n_factors; ++f) {
-            const IrFactorD& Fc = Tm.f[f];
-            pr *= x[Fc.offset + (Fc.idx ? Fc.idx[i] : (Fc.size == 1 ? 0 : i))];
-        }
+        for (int f = 0; f < Tm.n_factors; ++f) pr *= ir_factor(Tm.f[f], x, i);
         eta += pr;
     }
     return eta;
+}
+
+// x = backward(z) of one element of a log / interval variable, log|dx/dz| added to lj (transforms.py:880-891, :1026-1073)
+__device__ __forceinline__ double ir_backward(const IrVarD& V, double z, double& lj) {
+    double xv = z;
+    if (V.transform == IRT_LOG) {
+        xv = exp(z);
+        lj += z;
+    } else if (V.transform == IRT_INTERVAL) {
+        xv = V.lo + (V.hi - V.lo) * sigmoid(z);
+        lj += log(V.hi - V.lo) - softplus(-z) - softplus(z);
+    }
+    return xv;
+}
+
+// the value of the slot (sigma, the Binomial's trials or alpha) where it is a constant or a scalar variable
+__device__ __forceinline__ double ir_slot(const IrLikD& L, const double* x) {
+    return (L.sigma_kind == IRS_REF) ? x[L.sigma.ref] : L.sigma.value;
+}
+
+// the scale (or the Binomial's trials) of observation i: its own value, or the slot's sg_s
+__device__ __forceinline__ double ir_scale(const IrLikD& L, int i, double sg_s) {
+    return (L.sigma_kind == IRS_OBS) ? L.sigma_obs[i] : sg_s;
+}
+
+// The NegativeBinomial (discrete.py:700-745, n = a, p = a / (mu + a)) at d = eta - log a: lse = logaddexp(eta, log a) =
+// log a + softplus(d) = eta + softplus(-d), with s = mu / (mu + a) and sc = a / (mu + a) from one exp, so nothing
+// overflows for any finite eta.  e = exp(-|d|), l1 = log1p(e), sp = softplus(d) = lse - log a.
+struct IrNegBin { double d, e, l1, s, sc, sp; };
+__device__ __forceinline__ IrNegBin ir_negbin(double eta, double la) {
+    const double d = eta - la, e = exp(-fabs(d)), l1 = log1p(e), h = 1.0 / (1.0 + e);
+    return {d, e, l1, d >= 0 ? h : e * h, d >= 0 ? e * h : h, fmax(d, 0.0) + l1};
+}
+
+// log p(y_i | eta) of one observation of the eight base families, less the constants of ir_obs_const, added to lp, and
+// d / d sigma (NegativeBinomial, Gamma: d / d alpha; the NegativeBinomial's without psi(y + a) - psi(a)) added to s_sig.
+// Returns r_i = d / d eta.  It adds in place rather than returning its parts, so eval's running sums take exactly the
+// additions written here, in this order, and a family without a sigma adds nothing to s_sig.
+__device__ __forceinline__ double ir_base_term(const IrLikD& L, int i, double yi, double eta, double sg_s, double la,
+                                               double& lp, double& s_sig) {
+    double ri = 0.0;
+    switch (L.dist) {
+        case IRL_NORMAL: {  // continuous.py:526-527
+            const double sg = ir_scale(L, i, sg_s);
+            const double z = (yi - eta) / sg;
+            lp += -0.5 * z * z - log(sg);
+            ri = z / sg; s_sig += (z * z - 1.0) / sg;
+        } break;
+        case IRL_BERNOULLI_LOGIT:  // discrete.py:362-367 in PyTensor's stabilised forms
+            lp += yi * eta - softplus(eta);
+            ri = yi - sigmoid(eta);
+            break;
+        case IRL_POISSON_LOG: {  // discrete.py:581-586
+            const double mu = exp(eta);
+            lp += yi * eta - mu;
+            ri = yi - mu;
+        } break;
+        case IRL_STUDENTT: {  // continuous.py:1936-1944
+            const double sg = ir_scale(L, i, sg_s);
+            const double z = (yi - eta) / sg;
+            lp += -log(sg) - 0.5 * (L.nu + 1.0) * log1p(z * z / L.nu);
+            ri = (L.nu + 1.0) * z / (sg * (L.nu + z * z)); s_sig += -1.0 / sg + ri * z;
+        } break;
+        case IRL_NORMAL_LOGVAR: {  // Normal(0, exp(eta / 2))
+            const double w = yi * yi * exp(-eta);
+            lp += -0.5 * w - 0.5 * eta;
+            ri = 0.5 * w - 0.5;
+        } break;
+        case IRL_BINOMIAL_LOGIT: {  // discrete.py:141-152 in PyTensor's stabilised forms
+            const double nt = ir_scale(L, i, sg_s);
+            lp += yi * eta - nt * softplus(eta);
+            ri = yi - nt * sigmoid(eta);
+        } break;
+        case IRL_NEGBINOMIAL_LOG:  // the lgamma part is in c0 / eval's alpha terms
+            if (sg_s > kNegBinPoissonAlpha) {  // uniform branch: the Poisson(mu) limit
+                const double mu = exp(eta);
+                lp += yi * eta - mu;
+                ri = yi - mu;
+            } else {
+                const IrNegBin nb = ir_negbin(eta, la);
+                lp -= yi * (fmax(-nb.d, 0.0) + nb.l1) + sg_s * nb.sp;
+                ri = yi * nb.sc - sg_s * nb.s;                     // a (y - mu) / (mu + a)
+                s_sig += 1.0 - nb.sp - nb.sc * (1.0 + yi / sg_s);  // d/da except psi(y + a) - psi(a)
+            }
+            break;
+        case IRL_GAMMA_LOG: {  // continuous.py:2512-2521, beta = a exp(-eta); the eta-free part: c0 / alpha terms
+            const double w = yi * exp(-eta);
+            lp -= sg_s * (eta + w);
+            ri = sg_s * (w - 1.0);
+            s_sig -= eta + w;
+        } break;
+        default: break;
+    }
+    return ri;
+}
+
+// The per-observation constant of log f(y_i) that eval folds into c0 or the alpha terms (csrc/b200nuts.cu: prepare_ir):
+// of a base family, and of the count / positive component f of a zero-inflated or hurdle likelihood at y > 0.
+__device__ __forceinline__ double ir_obs_const(const IrLikD& L, int i, double y, double sg_s, double la) {
+    switch (L.dist) {
+        case IRL_NORMAL: case IRL_NORMAL_LOGVAR: return -B200_HALF_LOG_2PI;
+        case IRL_STUDENTT: return lgamma(0.5 * (L.nu + 1.0)) - lgamma(0.5 * L.nu) - 0.5 * log(L.nu * 3.14159265358979323846);
+        case IRL_POISSON_LOG: case IRL_ZI_POISSON: case IRL_HURDLE_POISSON: return -lgamma(y + 1.0);
+        case IRL_BINOMIAL_LOGIT: case IRL_ZI_BINOMIAL: {  // binomln(n, y)
+            const double nt = ir_scale(L, i, sg_s);
+            return lgamma(nt + 1.0) - lgamma(y + 1.0) - lgamma(nt - y + 1.0);
+        }
+        case IRL_NEGBINOMIAL_LOG: case IRL_ZI_NEGBINOMIAL: case IRL_HURDLE_NEGBINOMIAL:
+            return sg_s > kNegBinPoissonAlpha ? -lgamma(y + 1.0) : lgamma(y + sg_s) - lgamma(sg_s) - lgamma(y + 1.0);
+        case IRL_GAMMA_LOG: case IRL_HURDLE_GAMMA: return sg_s * la - lgamma(sg_s) + (sg_s - 1.0) * log(y);
+        default: return 0.0;
+    }
 }
 
 // log p(y_i | eta) of one censored / truncated Normal observation without its constant -log(2 pi) / 2 (in c0), with
@@ -152,19 +273,13 @@ __device__ __noinline__ IrPartials ir_bounded_pass(const IrLikD* Lp, const IrTer
     const int N = (int)L.N;
     double lp = 0.0, s_sig = 0.0;
     for (int i = tid; i < N; i += TS) {
-        const double eta = ir_eta(terms + L.term0, L.n_terms, x, i, N);
-        const IrBoundedTerm b = ir_bounded_term(L, i, eta, (L.sigma_kind == IRS_OBS) ? L.sigma_obs[i] : sg_s);
+        const double eta = ir_eta(terms + L.term0, 0, L.n_terms, x, i, N);
+        const IrBoundedTerm b = ir_bounded_term(L, i, eta, ir_scale(L, i, sg_s));
         lp += b.lp;
         s_sig += b.s;
         r[i] = b.r;
     }
     return {lp, s_sig};
-}
-
-// the pointwise pass's share of the same: log p(y_i | eta) with every constant (a censored value at its bound has none)
-__device__ __noinline__ double ir_bounded_loglik(const IrLikD& L, int i, double eta, double sg) {
-    const bool at_bound = L.dist == IRL_CENSORED_NORMAL && L.cens[i] != 0;
-    return ir_bounded_term(L, i, eta, sg).lp - (at_bound ? 0.0 : B200_HALF_LOG_2PI);
 }
 
 // ---- ordinal observations: OrderedLogistic / OrderedProbit (discrete.py:1231-1432) as the Categorical they build
@@ -211,8 +326,8 @@ __device__ __noinline__ IrPartials ir_ordinal_pass(const IrLikD* Lp, const IrTer
     const IrTermD& C = terms[L.term0 + L.n_terms];
     double lp = 0.0, s_sig = 0.0;
     for (int i = tid; i < N; i += TS) {
-        const double eta = ir_eta(terms + L.term0, L.n_terms, x, i, N);
-        const double s = L.sigma_kind == IRS_OBS ? L.sigma_obs[i] : (L.sigma_kind == IRS_NONE ? 1.0 : sg_s);
+        const double eta = ir_eta(terms + L.term0, 0, L.n_terms, x, i, N);
+        const double s = ir_scale(L, i, L.sigma_kind == IRS_NONE ? 1.0 : sg_s);  // the logistic link: s = 1
         const IrOrdinalTerm o = ir_ordinal_term(L, C, x, i, eta, s);
         lp += o.lp;
         s_sig += o.ds;
@@ -241,12 +356,6 @@ __device__ __noinline__ void ir_cutpoint_grad(const IrLikD* Lp, const IrTermD* t
     }
 }
 
-// the pointwise pass's share: log p(y_i | eta), which has no constant
-__device__ __noinline__ double ir_ordinal_loglik(const IrLikD& L, const IrTermD* terms, const double* x, int i, double eta) {
-    const double s = L.sigma_kind == IRS_NONE ? 1.0 : (L.sigma_kind == IRS_OBS ? L.sigma_obs[i] : (L.sigma_kind == IRS_REF ? x[L.sigma.ref] : L.sigma.value));
-    return ir_ordinal_term(L, terms[L.term0 + L.n_terms], x, i, eta, s).lp;
-}
-
 // ---- zero-inflated and hurdle observations (mixture.py:560-1035).  psi is the probability of the count / positive
 // component f, the family at mu = exp(eta) (Binomial: p = sigmoid(eta)), P0 = f(0):
 //   zero-inflated (mixture_logprob, :469-494)  y = 0: logaddexp(log(1 - psi), log psi + log P0);  y > 0: log psi + log f(y)
@@ -254,14 +363,25 @@ __device__ __noinline__ double ir_ordinal_loglik(const IrLikD& L, const IrTermD*
 //                                              component being Truncated(f, lower=1) (:826-829); Gamma has P0 = 0
 // log P0 is -e^eta (Poisson), -n softplus(eta) (Binomial), -a softplus(eta - log a) (NegativeBinomial, whose a > 1e10
 // Poisson limit is kept).  log(1 - P0) = log1mexp(log P0), and log m (m = -log P0) where m is below 1e-304, so the density
-// stays finite for every finite eta.  The psi block is terms[term0 + n_terms ..]: nu = 0, psi itself, one constant
-// (coef[0]) or one scalar variable; nu = m >= 1, psi = sigmoid(zeta), zeta the sum of the m terms, with log psi =
-// -softplus(-zeta) and log(1 - psi) = -softplus(zeta).  The constants of f (-lgamma(y + 1), binomln(n, y), and the
-// NegativeBinomial's lgamma(y + a) - lgamma(a), the Gamma normaliser over the y > 0) are in c0 / the alpha terms of eval.
-// Returns lp, r = d lp / d eta, dz = d lp / d zeta, dpsi = d lp / d psi, da = d lp / d alpha.
+// stays finite for every finite eta.  The constants of f (-lgamma(y + 1), binomln(n, y), and the NegativeBinomial's
+// lgamma(y + a) - lgamma(a), the Gamma normaliser over the y > 0) are in c0 / the alpha terms of eval, and in
+// ir_obs_const.  Returns lp, r = d lp / d eta, dz = d lp / d zeta, dpsi = d lp / d psi, da = d lp / d alpha.
+//
+// psi, log psi and log(1 - psi) at observation i from the psi block pt = terms + term0 + n_terms: m = nu = 0, psi itself,
+// one constant (coef[0]) or one scalar variable; m >= 1, psi = sigmoid(zeta), zeta the sum of the m terms, with log psi =
+// -softplus(-zeta) and log(1 - psi) = -softplus(zeta).
+struct IrPsi { double psi, lpsi, l1psi; };
+__device__ __forceinline__ IrPsi ir_psi(const IrTermD* pt, int m, const double* x, int i, int N) {
+    if (m == 0) {
+        const double psi = pt->n_factors ? x[pt->f[0].offset] : pt->coef[0];
+        return {psi, log(psi), log1p(-psi)};
+    }
+    const double z = ir_eta(pt, 0, m, x, i, N);
+    return {sigmoid(z), -softplus(-z), -softplus(z)};
+}
 struct IrZiTerm { double lp, r, dz, dpsi, da; };
-__device__ __forceinline__ IrZiTerm ir_zi_term(int dist, double y, double eta, double nt, double a, double la, double lpsi,
-                                               double l1psi, double psi) {
+__device__ __forceinline__ IrZiTerm ir_zi_term(int dist, double y, double eta, double nt, double a, double la, const IrPsi& ps) {
+    const double psi = ps.psi, lpsi = ps.lpsi, l1psi = ps.l1psi;
     // the family: lf = log f(y) less its constants, rf / af = its eta / alpha derivatives; lP0 = log P0 with r0 / a0;
     // lm = log(-lP0)
     double lf, rf, af = 0.0, lP0 = -INFINITY, r0 = 0.0, a0 = 0.0, lm = INFINITY;
@@ -276,16 +396,14 @@ __device__ __forceinline__ IrZiTerm ir_zi_term(int dist, double y, double eta, d
         lf = y * eta + lP0;
         rf = y + r0;
     } else if (dist != IRL_ZI_POISSON && dist != IRL_HURDLE_POISSON && a <= kNegBinPoissonAlpha) {  // discrete.py:700-745
-        const double d = eta - la, e = exp(-fabs(d)), l1 = log1p(e), h = 1.0 / (1.0 + e);
-        const double s = d >= 0 ? h : e * h, sc = d >= 0 ? e * h : h;
-        const double sp = fmax(d, 0.0) + l1;  // softplus(d)
-        lP0 = -a * sp;
-        r0 = -a * s;
-        a0 = s - sp;
-        lf = lP0 - y * (fmax(-d, 0.0) + l1);
-        rf = y * sc + r0;
-        af = 1.0 - sp - sc * (1.0 + y / a);
-        lm = la + (d < -30.0 ? d - 0.5 * e : log(sp));  // log softplus(d) = d - e^d / 2 to rounding below -30
+        const IrNegBin nb = ir_negbin(eta, la);
+        lP0 = -a * nb.sp;
+        r0 = -a * nb.s;
+        a0 = nb.s - nb.sp;
+        lf = lP0 - y * (fmax(-nb.d, 0.0) + nb.l1);
+        rf = y * nb.sc + r0;
+        af = 1.0 - nb.sp - nb.sc * (1.0 + y / a);
+        lm = la + (nb.d < -30.0 ? nb.d - 0.5 * nb.e : log(nb.sp));  // log softplus(d) = d - e^d / 2 to rounding below -30
     } else {  // discrete.py:581-586, and the NegativeBinomial's Poisson limit (:727-735)
         const double mu = exp(eta);
         lP0 = -mu;
@@ -322,11 +440,6 @@ __device__ __forceinline__ IrZiTerm ir_zi_term(int dist, double y, double eta, d
 // d eta_i and, for a logit psi, z_i = d logp / d zeta_i; returns this thread's partial sums of logp, d logp / d alpha and
 // d logp / d psi.
 struct IrZiPartials { double lp, s_a, s_psi; };
-__device__ __forceinline__ void ir_zi_psi(const IrTermD& T, const double* x, double* psi, double* lpsi, double* l1psi) {
-    *psi = T.n_factors ? x[T.f[0].offset] : T.coef[0];  // nu = 0: one constant or one scalar variable
-    *lpsi = log(*psi);
-    *l1psi = log1p(-*psi);
-}
 template <int W>
 __device__ __noinline__ IrZiPartials ir_zi_pass(const IrLikD* Lp, const IrTermD* terms, const double* x, double* r,
                                                 double* zr, double sg_s, double la, int tid) {
@@ -334,19 +447,14 @@ __device__ __noinline__ IrZiPartials ir_zi_pass(const IrLikD* Lp, const IrTermD*
     const IrLikD& L = *Lp;
     const int N = (int)L.N, m = (int)L.nu;
     const IrTermD* pt = terms + L.term0 + L.n_terms;  // the psi block
-    double psi = 0.0, lpsi = 0.0, l1psi = 0.0;
-    if (m == 0) ir_zi_psi(*pt, x, &psi, &lpsi, &l1psi);
+    IrPsi ps{0.0, 0.0, 0.0};
+    if (m == 0) ps = ir_psi(pt, 0, x, 0, N);
     double lp = 0.0, s_a = 0.0, s_psi = 0.0;
     for (int i = tid; i < N; i += TS) {
-        const double eta = ir_eta(terms + L.term0, L.n_terms, x, i, N);
-        if (m > 0) {
-            const double z = ir_eta(pt, m, x, i, N);
-            psi = sigmoid(z);
-            lpsi = -softplus(-z);
-            l1psi = -softplus(z);
-        }
-        const double nt = L.sigma_kind == IRS_OBS ? L.sigma_obs[i] : sg_s;
-        const IrZiTerm o = ir_zi_term(L.dist, L.y[i], eta, nt, sg_s, la, lpsi, l1psi, psi);
+        const double eta = ir_eta(terms + L.term0, 0, L.n_terms, x, i, N);
+        if (m > 0) ps = ir_psi(pt, m, x, i, N);
+        const double nt = ir_scale(L, i, sg_s);
+        const IrZiTerm o = ir_zi_term(L.dist, L.y[i], eta, nt, sg_s, la, ps);
         lp += o.lp;
         s_a += o.da;
         s_psi += o.dpsi;
@@ -354,35 +462,6 @@ __device__ __noinline__ IrZiPartials ir_zi_pass(const IrLikD* Lp, const IrTermD*
         if (m > 0) zr[i] = o.dz;
     }
     return {lp, s_a, s_psi};
-}
-
-// the pointwise pass's share: log p(y_i | eta, psi) with every constant of f
-__device__ __noinline__ double ir_zi_loglik(const IrLikD& L, const IrTermD* terms, const double* x, int i, double eta,
-                                            double sg_s) {
-    const int N = (int)L.N, m = (int)L.nu;
-    const IrTermD* pt = terms + L.term0 + L.n_terms;
-    double psi, lpsi, l1psi;
-    if (m == 0) {
-        ir_zi_psi(*pt, x, &psi, &lpsi, &l1psi);
-    } else {
-        const double z = ir_eta(pt, m, x, i, N);
-        psi = sigmoid(z);
-        lpsi = -softplus(-z);
-        l1psi = -softplus(z);
-    }
-    const double y = L.y[i], nt = L.sigma_kind == IRS_OBS ? L.sigma_obs[i] : sg_s, la = log(sg_s);
-    double lp = ir_zi_term(L.dist, y, eta, nt, sg_s, la, lpsi, l1psi, psi).lp;
-    if (y > 0.0) {
-        if (L.dist == IRL_HURDLE_GAMMA)
-            lp += sg_s * la - lgamma(sg_s) + (sg_s - 1.0) * log(y);
-        else if (L.dist == IRL_ZI_BINOMIAL)
-            lp += lgamma(nt + 1.0) - lgamma(y + 1.0) - lgamma(nt - y + 1.0);
-        else if (L.dist == IRL_ZI_POISSON || L.dist == IRL_HURDLE_POISSON || sg_s > kNegBinPoissonAlpha)
-            lp -= lgamma(y + 1.0);
-        else
-            lp += lgamma(y + sg_s) - lgamma(sg_s) - lgamma(y + 1.0);
-    }
-    return lp;
 }
 
 // ---- the ordered transform (transforms.py:79-120): x_0 = z_0 (positive: e^{z_0}), x_k = x_{k-1} + e^{z_k}; log|J| =
@@ -454,11 +533,8 @@ struct IrModel {
                 const IrFactorD& Fc = Tm.f[f];
                 auto others = [&](int i) -> double {
                     double pr = Tm.coef ? Tm.coef[i] : 1.0;
-                    for (int f2 = 0; f2 < Tm.n_factors; ++f2) {
-                        if (f2 == f) continue;
-                        const IrFactorD& F2 = Tm.f[f2];
-                        pr *= x[F2.offset + (F2.idx ? F2.idx[i] : (F2.size == 1 ? 0 : i))];
-                    }
+                    for (int f2 = 0; f2 < Tm.n_factors; ++f2)
+                        if (f2 != f) pr *= ir_factor(Tm.f[f2], x, i);
                     return pr;
                 };
                 if (!Fc.idx && Fc.size == 1) {  // scalar target: team reduction over the observations
@@ -510,17 +586,7 @@ struct IrModel {
             }
             for (int j = tid; j < V.size; j += TS) {
                 const int i = V.offset + j;
-                const double z = q_s[i];
-                double xv = z;
-                if (V.transform == IRT_LOG) {
-                    xv = exp(z);
-                    lp += z;
-                } else if (V.transform == IRT_INTERVAL) {
-                    const double sg = sigmoid(z);
-                    xv = V.lo + (V.hi - V.lo) * sg;
-                    lp += log(V.hi - V.lo) - softplus(-z) - softplus(z);
-                }
-                x[i] = xv;
+                x[i] = ir_backward(V, q_s[i], lp);
                 g_s[i] = 0.0;
             }
         }
@@ -602,7 +668,7 @@ struct IrModel {
         for (int l = 0; l < P.n_liks; ++l) {
             const IrLikD L = P.liks[l];
             const int N = (int)L.N;
-            const double sg_s = (L.sigma_kind == IRS_REF) ? x[L.sigma.ref] : L.sigma.value;
+            const double sg_s = ir_slot(L, x);
             const bool zi = EXTENDED && L.dist >= IRL_ZI_POISSON;  // zero-inflated / hurdle
             const bool gamma = L.dist == IRL_GAMMA_LOG || (EXTENDED && L.dist == IRL_HURDLE_GAMMA);
             const bool disp = L.dist == IRL_NEGBINOMIAL_LOG || gamma ||  // sg_s is the dispersion alpha
@@ -625,78 +691,9 @@ struct IrModel {
                 }
             }
             if (!bounded) for (int i = tid; i < N; i += TS) {
-                double eta = 0.0;
-                for (int t = 0; t < L.n_terms; ++t) {
-                    const IrTermD& Tm = P.terms[L.term0 + t];
-                    if (Tm.n_cols) {
-                        eta += ir_design_row(Tm, x + Tm.f[0].offset, i, N);
-                        continue;
-                    }
-                    double pr = Tm.coef ? Tm.coef[i] : 1.0;
-                    for (int f = 0; f < Tm.n_factors; ++f) {
-                        const IrFactorD& Fc = Tm.f[f];
-                        pr *= x[Fc.offset + (Fc.idx ? Fc.idx[i] : (Fc.size == 1 ? 0 : i))];
-                    }
-                    eta += pr;
-                }
+                const double eta = ir_eta(P.terms, L.term0, L.n_terms, x, i, N);
                 const double yi = L.yoff >= 0 ? x[L.yoff + i] : L.y[i];
-                double ri = 0.0;
-                switch (L.dist) {
-                    case IRL_NORMAL: {  // continuous.py:526-527
-                        const double sg = (L.sigma_kind == IRS_OBS) ? L.sigma_obs[i] : sg_s;
-                        const double z = (yi - eta) / sg;
-                        lp += -0.5 * z * z - log(sg);
-                        ri = z / sg; s_sig += (z * z - 1.0) / sg;
-                    } break;
-                    case IRL_BERNOULLI_LOGIT:  // discrete.py:362-367 in PyTensor's stabilised forms
-                        lp += yi * eta - softplus(eta);
-                        ri = yi - sigmoid(eta);
-                        break;
-                    case IRL_POISSON_LOG: {  // discrete.py:581-586
-                        const double mu = exp(eta);
-                        lp += yi * eta - mu;
-                        ri = yi - mu;
-                    } break;
-                    case IRL_STUDENTT: {  // continuous.py:1936-1944
-                        const double sg = (L.sigma_kind == IRS_OBS) ? L.sigma_obs[i] : sg_s;
-                        const double z = (yi - eta) / sg;
-                        lp += -log(sg) - 0.5 * (L.nu + 1.0) * log1p(z * z / L.nu);
-                        ri = (L.nu + 1.0) * z / (sg * (L.nu + z * z)); s_sig += -1.0 / sg + ri * z;
-                    } break;
-                    case IRL_NORMAL_LOGVAR: {  // Normal(0, exp(eta / 2))
-                        const double w = yi * yi * exp(-eta);
-                        lp += -0.5 * w - 0.5 * eta;
-                        ri = 0.5 * w - 0.5;
-                    } break;
-                    case IRL_BINOMIAL_LOGIT: {  // discrete.py:141-152 in PyTensor's stabilised forms; binomln(n, y) is in c0
-                        const double nt = (L.sigma_kind == IRS_OBS) ? L.sigma_obs[i] : sg_s;
-                        lp += yi * eta - nt * softplus(eta);
-                        ri = yi - nt * sigmoid(eta);
-                    } break;
-                    case IRL_NEGBINOMIAL_LOG:  // discrete.py:700-745, n = a, p = a / (mu + a); the lgamma part is in c0 / below
-                        if (sg_s > kNegBinPoissonAlpha) {  // uniform branch: the Poisson(mu) limit
-                            const double mu = exp(eta);
-                            lp += yi * eta - mu;
-                            ri = yi - mu;
-                        } else {
-                            // d = eta - log a: lse = logaddexp(eta, log a) = log a + softplus(d) = eta + softplus(-d), with
-                            // s = mu / (mu + a) and sc = a / (mu + a) from one exp, so nothing overflows for any finite eta
-                            const double d = eta - la, e = exp(-fabs(d)), l1 = log1p(e), h = 1.0 / (1.0 + e);
-                            const double s = d >= 0 ? h : e * h, sc = d >= 0 ? e * h : h;
-                            const double sp = fmax(d, 0.0) + l1;  // lse - log a
-                            lp -= yi * (fmax(-d, 0.0) + l1) + sg_s * sp;
-                            ri = yi * sc - sg_s * s;                         // a (y - mu) / (mu + a)
-                            s_sig += 1.0 - sp - sc * (1.0 + yi / sg_s);      // d/da except psi(y + a) - psi(a)
-                        }
-                        break;
-                    case IRL_GAMMA_LOG: {  // continuous.py:2512-2521, beta = a exp(-eta); the eta-free part once below
-                        const double w = yi * exp(-eta);
-                        lp -= sg_s * (eta + w);
-                        ri = sg_s * (w - 1.0);
-                        s_sig -= eta + w;
-                    } break;
-                    default: break;
-                }
+                const double ri = ir_base_term(L, i, yi, eta, sg_s, la, lp, s_sig);
                 r[i] = ri;
                 if (L.yoff >= 0) g_s[L.yoff + i] -= ri;  // this thread owns element i of the latent variable
             }
@@ -827,14 +824,40 @@ struct IrExtendedModel : IrModel {
 // team scratch slice like in eval().  Elementwise constants (log 2pi, lgamma) are included, unlike in eval() where they are
 // folded into one constant per factor.
 // ---------------------------------------------------------------------------------------------------------------------
+
+// log p(y_i | eta) of observation i with every constant, through the term function eval's pass uses: a base family's
+// term plus ir_obs_const; a zero-inflated / hurdle count's plus that of f at y > 0; a censored / truncated Normal's plus
+// -log(2 pi) / 2 except at a censoring bound; an ordinal one's has none.
 template <bool EXTENDED>  // as IrModel / IrExtendedModel
+__device__ __forceinline__ double ir_obs_loglik(const IrLikD& L, const IrTermD* terms, const double* x, int i, double eta,
+                                                double sg_s, double la) {
+    const double y = L.y[i];
+    if (EXTENDED && L.dist >= IRL_ZI_POISSON) {
+        const IrPsi ps = ir_psi(terms + L.term0 + L.n_terms, (int)L.nu, x, i, (int)L.N);
+        const double lp = ir_zi_term(L.dist, y, eta, ir_scale(L, i, sg_s), sg_s, la, ps).lp;
+        return y > 0.0 ? lp + ir_obs_const(L, i, y, sg_s, la) : lp;
+    }
+    if (EXTENDED && L.dist >= IRL_ORDERED_LOGISTIC) {
+        const double s = ir_scale(L, i, L.sigma_kind == IRS_NONE ? 1.0 : sg_s);  // the logistic link: s = 1
+        return ir_ordinal_term(L, terms[L.term0 + L.n_terms], x, i, eta, s).lp;
+    }
+    if (EXTENDED && L.dist >= IRL_CENSORED_NORMAL) {
+        const bool at_bound = L.dist == IRL_CENSORED_NORMAL && L.cens[i] != 0;
+        return ir_bounded_term(L, i, eta, ir_scale(L, i, sg_s)).lp - (at_bound ? 0.0 : B200_HALF_LOG_2PI);
+    }
+    double lp = 0.0, s_sig = 0.0;
+    ir_base_term(L, i, y, eta, sg_s, la, lp, s_sig);
+    return lp + ir_obs_const(L, i, y, sg_s, la);
+}
+
+template <bool EXTENDED>
 __global__ void __launch_bounds__(256) ir_pointwise_kernel(const IrModel::Params P, int lik, long long D,
                                                            const double* __restrict__ draws /*[D][n]*/,
                                                            double* __restrict__ out /*[D][N]*/) {
     const int lane = threadIdx.x & 31;
     const int slot = (int)(blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5));
     double* x = P.scratch + (long long)slot * P.stride;
-    const IrLikD L = P.liks[lik];
+    const IrLikD& L = P.liks[lik];
     const int N = (int)L.N, n = P.n;
     const long long stride = (long long)gridDim.x * (blockDim.x >> 5);
     for (long long d = slot; d < D; d += stride) {
@@ -847,67 +870,14 @@ __global__ void __launch_bounds__(256) ir_pointwise_kernel(const IrModel::Params
                     continue;
                 }
             }
-            for (int j = lane; j < V.size; j += 32) {
-                const double z = q[V.offset + j];
-                x[V.offset + j] = V.transform == IRT_LOG ? exp(z) : (V.transform == IRT_INTERVAL ? V.lo + (V.hi - V.lo) * sigmoid(z) : z);
-            }
+            double lj = 0.0;  // the log-Jacobian is not part of the likelihood
+            for (int j = lane; j < V.size; j += 32) x[V.offset + j] = ir_backward(V, q[V.offset + j], lj);
         }
         __syncwarp();
-        const double sg_s = (L.sigma_kind == IRS_REF) ? x[L.sigma.ref] : L.sigma.value;
-        const double la = (L.dist == IRL_NEGBINOMIAL_LOG || L.dist == IRL_GAMMA_LOG) ? log(sg_s) : 0.0;
+        const double sg_s = ir_slot(L, x), la = log(sg_s);  // la: log alpha, read only by the families with a dispersion
         for (int i = lane; i < N; i += 32) {
-            double eta = 0.0;
-            for (int t = 0; t < L.n_terms; ++t) {
-                const IrTermD& Tm = P.terms[L.term0 + t];
-                if (Tm.n_cols) {
-                    eta += ir_design_row(Tm, x + Tm.f[0].offset, i, N);
-                    continue;
-                }
-                double pr = Tm.coef ? Tm.coef[i] : 1.0;
-                for (int f = 0; f < Tm.n_factors; ++f) {
-                    const IrFactorD& Fc = Tm.f[f];
-                    pr *= x[Fc.offset + (Fc.idx ? Fc.idx[i] : (Fc.size == 1 ? 0 : i))];
-                }
-                eta += pr;
-            }
-            const double yi = L.y[i];
-            double lp = 0.0;
-            switch (L.dist) {
-                case IRL_NORMAL: {
-                    const double sg = (L.sigma_kind == IRS_OBS) ? L.sigma_obs[i] : sg_s, z = (yi - eta) / sg;
-                    lp = -0.5 * z * z - log(sg) - B200_HALF_LOG_2PI;
-                } break;
-                case IRL_BERNOULLI_LOGIT: lp = yi * eta - softplus(eta); break;
-                case IRL_POISSON_LOG: lp = yi * eta - exp(eta) - lgamma(yi + 1.0); break;
-                case IRL_STUDENTT: {
-                    const double sg = (L.sigma_kind == IRS_OBS) ? L.sigma_obs[i] : sg_s, z = (yi - eta) / sg;
-                    lp = lgamma(0.5 * (L.nu + 1.0)) - lgamma(0.5 * L.nu) - 0.5 * log(L.nu * 3.14159265358979323846) - log(sg) -
-                         0.5 * (L.nu + 1.0) * log1p(z * z / L.nu);
-                } break;
-                case IRL_NORMAL_LOGVAR: lp = -0.5 * yi * yi * exp(-eta) - 0.5 * eta - B200_HALF_LOG_2PI; break;
-                case IRL_BINOMIAL_LOGIT: {
-                    const double nt = (L.sigma_kind == IRS_OBS) ? L.sigma_obs[i] : sg_s;
-                    lp = lgamma(nt + 1.0) - lgamma(yi + 1.0) - lgamma(nt - yi + 1.0) + yi * eta - nt * softplus(eta);
-                } break;
-                case IRL_NEGBINOMIAL_LOG:
-                    if (sg_s > kNegBinPoissonAlpha) {
-                        lp = yi * eta - exp(eta) - lgamma(yi + 1.0);
-                    } else {
-                        const double d = eta - la, l1 = log1p(exp(-fabs(d)));
-                        lp = lgamma(yi + sg_s) - lgamma(sg_s) - lgamma(yi + 1.0) - yi * (fmax(-d, 0.0) + l1) - sg_s * (fmax(d, 0.0) + l1);
-                    }
-                    break;
-                case IRL_GAMMA_LOG: lp = sg_s * (la - eta) - lgamma(sg_s) + (sg_s - 1.0) * log(yi) - sg_s * yi * exp(-eta); break;
-                case IRL_CENSORED_NORMAL: case IRL_TRUNCATED_NORMAL:
-                    if constexpr (EXTENDED) lp = ir_bounded_loglik(L, i, eta, (L.sigma_kind == IRS_OBS) ? L.sigma_obs[i] : sg_s);
-                    break;
-                default:  // the ordinal, zero-inflated and hurdle likelihoods
-                    if constexpr (EXTENDED)
-                        lp = L.dist >= IRL_ZI_POISSON ? ir_zi_loglik(L, P.terms, x, i, eta, sg_s)
-                                                      : ir_ordinal_loglik(L, P.terms, x, i, eta);
-                    break;
-            }
-            out[d * N + i] = lp;
+            const double eta = ir_eta(P.terms, L.term0, L.n_terms, x, i, N);
+            out[d * N + i] = ir_obs_loglik<EXTENDED>(L, P.terms, x, i, eta, sg_s, la);
         }
         __syncwarp();
     }

@@ -131,6 +131,23 @@ extern "C" {
 #define B200_IR_L_HURDLE_POISSON 15                  /* pm.HurdlePoisson mixture.py:873-922                 */
 #define B200_IR_L_HURDLE_NEGATIVE_BINOMIAL 16        /* pm.HurdleNegativeBinomial mixture.py:925-978        */
 #define B200_IR_L_HURDLE_GAMMA 17                    /* pm.HurdleGamma mixture.py:981-1034                  */
+/* Survival (time-to-event) observations y > 0 with a log link.  With u = log y - eta and t(y) = exp(alpha u) = (y / beta)^alpha:
+ *   WEIBULL_LOG        y ~ Weibull(alpha, beta = exp(eta)): log f = log alpha - eta + (alpha - 1) u - t.  The Exponential
+ *                      with scale exp(eta) is alpha = 1.  sigma: alpha, CONST (> 0) or REF (a scalar of positive support).
+ *   LOGNORMAL          y ~ LogNormal(mu = eta, sigma): the Normal of log y at (eta, sigma), minus log y.  sigma as for NORMAL.
+ *   CENSORED_*         `y` is the [3][N] block (y, lower, upper) of CENSORED_NORMAL: log F(y) where y_i == lower_i (Weibull:
+ *                      log(1 - e^-t); LogNormal: log Phi of log y), log S(y) where y_i == upper_i (-t; log(1 - Phi)), the
+ *                      density elsewhere
+ *   TRUNCATED_*        the same block: the density minus log(S(lower) - S(upper)), a one-sided form where a side is open
+ * y finite and > 0; lower >= 0 or -inf and upper > 0 or +inf, where lower 0 / -inf and upper +inf are open sides;
+ * lower_i < upper_i and lower_i <= y_i <= upper_i; a truncated factor has a finite lower bound > 0 or a finite upper bound.
+ * nu is unused.  y_var must be 0. */
+#define B200_IR_L_WEIBULL_LOG 18            /* pm.Weibull continuous.py:2740-2831; pm.Exponential :1461-1480 */
+#define B200_IR_L_LOGNORMAL 19              /* pm.LogNormal continuous.py:1723-1846                          */
+#define B200_IR_L_CENSORED_WEIBULL_LOG 20   /* pm.Censored(pm.Weibull.dist(...)) logprob/censoring.py:213-248 */
+#define B200_IR_L_CENSORED_LOGNORMAL 21     /* pm.Censored(pm.LogNormal.dist(...))                            */
+#define B200_IR_L_TRUNCATED_WEIBULL_LOG 22  /* pm.Truncated(pm.Weibull.dist(...)) truncated.py                */
+#define B200_IR_L_TRUNCATED_LOGNORMAL 23    /* pm.Truncated(pm.LogNormal.dist(...))                           */
 /* The support rule b200_model_create enforces (as ModelIR.validate does): HalfNormal, HalfCauchy, Exponential, Gamma and
  * LogNormal priors sit on a LOG variable or an INTERVAL with lo >= 0, Beta on an INTERVAL inside [0, 1], Uniform(a, b) on an
  * INTERVAL inside [a, b]; every scale (a prior's sigma / beta / lam, Normal and StudentT sigma including each sigma_obs, an
@@ -176,7 +193,7 @@ typedef struct b200_ir_term {
 typedef struct b200_ir_lik {
     int32_t dist, n_terms;
     int64_t N;
-    const double* y; /* [N]; [3][N] (y, lower, upper) for CENSORED_NORMAL / TRUNCATED_NORMAL; NULL allowed when y_var > 0 */
+    const double* y; /* [N]; [3][N] (y, lower, upper) for the CENSORED_* / TRUNCATED_* dists; NULL allowed when y_var > 0 */
     const b200_ir_term* terms;
     int32_t sigma_kind, y_var;
     b200_ir_param sigma;

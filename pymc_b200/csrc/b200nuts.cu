@@ -130,7 +130,7 @@ struct b200_model {
     IrModel::Params ir{};
     std::vector<IrLikD> ir_liks;  // the host copy of ir.liks
     DevBuf ir_tables;             // the data arrays ir's tables point into (prepare_ir)
-    bool ir_extended = false;  // a censored / truncated Normal, ordinal, zero-inflated or hurdle likelihood, or an ordered
+    bool ir_extended = false;  // a censored / truncated Normal, ordinal, zero-inflated, hurdle or survival likelihood, or an ordered
                                // variable: the kernels run IrExtendedModel
     DevBuf ir_scratch;  // per-team scratch of the generic IR device function: [teams][n_pad + max N] doubles
     // lock-step (GEMM-shaped) models; every matrix is row-major with rows `ld` doubles apart (n rounded up to 4, zero pad)
@@ -472,6 +472,10 @@ static bool ir_scale_ok(const b200_ir_param& p, const std::vector<IrVarD>& vars)
 #define B200_IR_BOUND_ORDER "lower < upper must hold for every observation"
 #define B200_IR_BOUND_Y "y must be finite and lie in [lower, upper] for every observation"
 #define B200_IR_TRUNC_OPEN "truncated_normal needs a finite lower or upper bound; with neither side bounded, write the likelihood as normal"
+// Survival observations (ModelIR._validate_survival, same wording)
+#define B200_IR_SURV_Y "y must be finite and > 0 for every observation"
+#define B200_IR_SURV_SIDES "lower must be finite and >= 0 or -inf (0 and -inf: open) and upper > 0 or +inf (open), neither NaN"
+#define B200_IR_SURV_TRUNC_OPEN "a truncated survival likelihood needs a finite lower bound > 0 or a finite upper bound; with neither, write the plain likelihood"
 // Ordered variables and ordinal observations (ModelIR.validate, same wording)
 #define B200_IR_ORDERED_PRIOR "an ordered variable takes only real-line priors (flat, normal, studentt, cauchy, or a latent normal / studentt); ordered_positive also admits the positive priors"
 #define B200_IR_ORD_K "an ordinal likelihood needs K >= 2 categories"
@@ -678,6 +682,53 @@ static int ir_bounds(IrPass& c, const b200_ir_lik& L, int l, IrLikD& D) {
     return 0;
 }
 
+// Weibull / LogNormal, plain, censored or truncated (y: [N], or the [3][N] block (y, lower, upper)).  The device reads log y;
+// the censoring codes as for the censored Normal; the truncated forms' bounds, 0 / +inf where open (Weibull) or their logs,
+// -inf / +inf where open (LogNormal).  A LogNormal's -log(2 pi) / 2 - log y_i of every observation with a density is in c0.
+static int ir_survival(IrPass& c, const b200_ir_lik& L, int l, const b200_ir_param& slot, IrLikD& D) {
+    static const char* const names[] = {"weibull_log", "lognormal", "censored_weibull_log", "censored_lognormal",
+                                        "truncated_weibull_log", "truncated_lognormal"};
+    const long long N = L.N;
+    const int k = L.dist - B200_IR_L_WEIBULL_LOG;
+    const bool weibull = k % 2 == 0, cens = k / 2 == 1, trunc = k / 2 == 2;
+    const char* what = names[k];
+    if (weibull && L.sigma_kind != B200_IR_S_CONST && L.sigma_kind != B200_IR_S_REF)
+        return fail("ir: likelihood %d: %s: alpha must be a constant or a scalar variable", l, what);
+    if (weibull && !ir_scale_ok(slot, c.vars)) return fail("ir: likelihood %d: %s: alpha " B200_IR_SCALE_RULE, l, what);
+    const double *y = L.y, *lo = L.y + N, *hi = L.y + 2 * N;  // lo, hi: the censored / truncated forms only
+    std::vector<double>& ly = c.reals.emplace_back((size_t)N);
+    std::vector<double>& bnd = c.reals.emplace_back(trunc ? 2 * (size_t)N : 0);
+    std::vector<signed char>& code = c.codes.emplace_back(cens ? (size_t)N : 0);
+    long long n_dens = 0;
+    double sly = 0.0;  // sum of log y over the observations with a density
+    bool bounded = false;
+    for (long long i = 0; i < N; ++i) {
+        if (!(std::isfinite(y[i]) && y[i] > 0)) return fail("ir: likelihood %d: %s: " B200_IR_SURV_Y " (at %lld)", l, what, i);
+        ly[i] = std::log(y[i]);
+        int ci = 0;
+        if (cens || trunc) {
+            if (std::isnan(lo[i]) || std::isnan(hi[i]) || !(lo[i] >= 0 || lo[i] == -INFINITY) || lo[i] == INFINITY || !(hi[i] > 0))
+                return fail("ir: likelihood %d: %s: " B200_IR_SURV_SIDES " (at %lld)", l, what, i);
+            if (!(lo[i] < hi[i])) return fail("ir: likelihood %d: %s: " B200_IR_BOUND_ORDER " (at %lld)", l, what, i);
+            if (!(lo[i] <= y[i] && y[i] <= hi[i])) return fail("ir: likelihood %d: %s: " B200_IR_BOUND_Y " (at %lld)", l, what, i);
+            bounded = bounded || (lo[i] > 0 && std::isfinite(lo[i])) || std::isfinite(hi[i]);
+        }
+        if (cens) code[i] = (signed char)(ci = y[i] == lo[i] ? 1 : (y[i] == hi[i] ? 2 : 0));  // lo[i] = y[i] > 0: finite
+        if (trunc) {
+            const double a = lo[i] > 0 ? lo[i] : 0.0;
+            bnd[i] = weibull ? a : (a > 0 ? std::log(a) : -INFINITY);
+            bnd[N + i] = weibull ? hi[i] : std::log(hi[i]);
+        }
+        if (ci == 0) { ++n_dens; sly += ly[i]; }
+    }
+    if (trunc && !bounded) return fail("ir: likelihood %d: %s: " B200_IR_SURV_TRUNC_OPEN, l, what);
+    if (!weibull) D.c0 = -(double)n_dens * B200_HALF_LOG_2PI - sly;
+    c.add(&D.y, ly.data(), ly.size());
+    if (cens) c.add(&D.cens, code.data(), code.size());
+    if (trunc) c.add(&D.bnd, bnd.data(), bnd.size());
+    return 0;
+}
+
 // ordered logistic / probit: nu = K
 static int ir_ordinal(IrPass& c, const b200_ir_lik& L, int l) {
     const double K = L.nu;
@@ -807,7 +858,8 @@ static int ir_lik(IrPass& c, const b200_ir_lik& L, int l, IrLikD& D) {
     c.max_obs = std::max(c.max_obs, N);
     D.dist = L.dist; D.n_terms = L.n_terms; D.term0 = (int)c.terms.size(); D.sigma_kind = L.sigma_kind; D.N = N; D.nu = L.nu;
     D.yoff = latent ? c.vars[L.y_var - 1].offset : -1;
-    if (!latent) c.add(&D.y, L.y, (size_t)N);
+    const bool survival = L.dist >= B200_IR_L_WEIBULL_LOG && L.dist <= B200_IR_L_TRUNCATED_LOGNORMAL;
+    if (!latent && !survival) c.add(&D.y, L.y, (size_t)N);  // a survival likelihood's device y is log y (ir_survival)
     if (ir_param(L.sigma, c.n, &D.sigma, "likelihood sigma")) return -1;
     if (L.sigma_kind == B200_IR_S_REF && L.sigma.kind != 1) return fail("ir: likelihood %d: sigma_kind REF needs a reference", l);
     b200_ir_param slot = L.sigma;  // the parameter slot as the device reads it: x[ref] for REF, else the value
@@ -833,6 +885,10 @@ static int ir_lik(IrPass& c, const b200_ir_lik& L, int l, IrLikD& D) {
         case B200_IR_L_GAMMA_LOG: rc = ir_family(c, L, l, slot, L.dist, "Gamma y must be > 0", false, D); break;
         case B200_IR_L_CENSORED_NORMAL: case B200_IR_L_TRUNCATED_NORMAL: rc = ir_bounds(c, L, l, D); break;
         case B200_IR_L_ORDERED_LOGISTIC: case B200_IR_L_ORDERED_PROBIT: rc = ir_ordinal(c, L, l); break;
+        case B200_IR_L_WEIBULL_LOG: case B200_IR_L_LOGNORMAL: case B200_IR_L_CENSORED_WEIBULL_LOG:
+        case B200_IR_L_CENSORED_LOGNORMAL: case B200_IR_L_TRUNCATED_WEIBULL_LOG: case B200_IR_L_TRUNCATED_LOGNORMAL:
+            rc = ir_survival(c, L, l, slot, D);
+            break;
         case B200_IR_L_ZERO_INFLATED_POISSON: case B200_IR_L_ZERO_INFLATED_BINOMIAL:
         case B200_IR_L_ZERO_INFLATED_NEGATIVE_BINOMIAL: case B200_IR_L_HURDLE_POISSON:
         case B200_IR_L_HURDLE_NEGATIVE_BINOMIAL: case B200_IR_L_HURDLE_GAMMA: {  // nu: the form of the psi block
@@ -847,7 +903,9 @@ static int ir_lik(IrPass& c, const b200_ir_lik& L, int l, IrLikD& D) {
     }
     if (rc) return rc;
     const bool has_sigma = L.dist == B200_IR_L_NORMAL || L.dist == B200_IR_L_STUDENTT || L.dist == B200_IR_L_CENSORED_NORMAL ||
-                           L.dist == B200_IR_L_TRUNCATED_NORMAL || L.dist == B200_IR_L_ORDERED_PROBIT;
+                           L.dist == B200_IR_L_TRUNCATED_NORMAL || L.dist == B200_IR_L_ORDERED_PROBIT ||
+                           L.dist == B200_IR_L_LOGNORMAL || L.dist == B200_IR_L_CENSORED_LOGNORMAL ||
+                           L.dist == B200_IR_L_TRUNCATED_LOGNORMAL;
     if (has_sigma && L.sigma_kind == B200_IR_S_NONE) return fail("ir: likelihood %d needs sigma", l);
     if (has_sigma && L.sigma_kind == B200_IR_S_OBS) {
         for (long long i = 0; i < N; ++i)
@@ -858,7 +916,7 @@ static int ir_lik(IrPass& c, const b200_ir_lik& L, int l, IrLikD& D) {
     }
     if (ir_terms(c, L, l, 0, L.n_terms)) return -1;
     if (L.dist == B200_IR_L_ORDERED_LOGISTIC || L.dist == B200_IR_L_ORDERED_PROBIT) return ir_cutpoints(c, L, l);
-    return L.dist >= B200_IR_L_ZERO_INFLATED_POISSON ? ir_psi(c, L, l) : 0;
+    return L.dist >= B200_IR_L_ZERO_INFLATED_POISSON && L.dist <= B200_IR_L_HURDLE_GAMMA ? ir_psi(c, L, l) : 0;
 }
 
 static int ir_ar1(const IrPass& c, const b200_ir_ar1& A, int k, IrAr1D& D) {

@@ -28,7 +28,8 @@ enum { IRP_FLAT = 0, IRP_NORMAL, IRP_HALFNORMAL, IRP_CAUCHY, IRP_HALFCAUCHY, IRP
 enum { IRL_NORMAL = 0, IRL_BERNOULLI_LOGIT, IRL_POISSON_LOG, IRL_STUDENTT, IRL_NORMAL_LOGVAR, IRL_BINOMIAL_LOGIT,
        IRL_NEGBINOMIAL_LOG, IRL_GAMMA_LOG, IRL_CENSORED_NORMAL, IRL_TRUNCATED_NORMAL, IRL_ORDERED_LOGISTIC,
        IRL_ORDERED_PROBIT, IRL_ZI_POISSON, IRL_ZI_BINOMIAL, IRL_ZI_NEGBINOMIAL, IRL_HURDLE_POISSON, IRL_HURDLE_NEGBINOMIAL,
-       IRL_HURDLE_GAMMA };
+       IRL_HURDLE_GAMMA, IRL_WEIBULL_LOG, IRL_LOGNORMAL, IRL_CENSORED_WEIBULL_LOG, IRL_CENSORED_LOGNORMAL,
+       IRL_TRUNCATED_WEIBULL_LOG, IRL_TRUNCATED_LOGNORMAL };
 enum { IRS_NONE = 0, IRS_CONST, IRS_REF, IRS_OBS };
 constexpr double kNegBinPoissonAlpha = 1e10;  // above: NegativeBinomial -> Poisson(mu) limit (discrete.py:727-735)
 
@@ -93,6 +94,8 @@ __device__ __forceinline__ void ir_design_grad(const IrTermD& Tm, const double* 
 // and n_tab = N+, the number of such y_i.
 // Censored Normal: cens[i] = 0 (observed), 1 (y_i at its lower bound), 2 (at its upper bound); the censoring point is y_i
 // itself.  Truncated Normal: bnd = [2][N], the lower and upper bound of each observation, -inf / +inf where open.
+// Survival likelihoods: y = log y_i; cens as above for the censored forms and null otherwise; bnd of the truncated forms
+// holds the bounds themselves (Weibull, 0 / +inf where open) or their logs (LogNormal, -inf / +inf where open).
 // yoff >= 0: a latent factor (a Normal / StudentT prior whose location is a linear predictor): y_i = x[yoff + i], the
 // constrained values of a variable of size N, which also receives d logp / d y_i = -r_i; y is null.  -1: y is data.
 struct IrLikD { int dist, n_terms, term0, sigma_kind; long long N; const double* y; const double* sigma_obs; IrParamD sigma;
@@ -243,12 +246,14 @@ __device__ __forceinline__ double ir_obs_const(const IrLikD& L, int i, double y,
 // log p(y_i | eta) of one censored / truncated Normal observation without its constant -log(2 pi) / 2 (in c0), with
 // r = d / d eta and s = d / d sigma.  Censored (logprob/censoring.py:213-248 over Normal): the Normal density where y_i is
 // observed, log Phi(zc) at a bound, zc = z at the lower one and -z at the upper one (normal_lccdf(z) = normal_lcdf(-z)).
-// Truncated (continuous.py:720-747): the Normal density minus log(Phi(b) - Phi(a)) of the standardised bounds.
+// Truncated (continuous.py:720-747): the Normal density minus log(Phi(b) - Phi(a)) of the standardised bounds.  The
+// LogNormal likelihoods run the same arithmetic on log y and log bounds (a plain one as censored with no code); their
+// -log y_i is in c0.
 struct IrBoundedTerm { double lp, r, s; };
 __device__ __forceinline__ IrBoundedTerm ir_bounded_term(const IrLikD& L, int i, double eta, double sg) {
     const double z = (L.y[i] - eta) / sg;
-    if (L.dist == IRL_CENSORED_NORMAL) {
-        const int c = L.cens[i];
+    if (L.dist != IRL_TRUNCATED_NORMAL && L.dist != IRL_TRUNCATED_LOGNORMAL) {
+        const int c = L.cens ? L.cens[i] : 0;
         if (c == 0) return {-0.5 * z * z - log(sg), z / sg, (z * z - 1.0) / sg};
         const double zc = c == 1 ? z : -z;
         const NormalTail t = normal_tail(zc);
@@ -261,8 +266,62 @@ __device__ __forceinline__ IrBoundedTerm ir_bounded_term(const IrLikD& L, int i,
     return {-0.5 * z * z - log(sg) - M.log_z, (z + M.rb - M.ra) / sg, (z * z - 1.0 + tb - ta) / sg};
 }
 
-// The observation loop of a censored / truncated Normal likelihood, out of line: IrExtendedModel::eval calls it once per
-// such likelihood, so the erfcx() tail math stays out of eval's own observation loop.  Writes r_i = d logp / d eta_i;
+// ---- survival observations (continuous.py:2740-2831 / :1461-1480 / :1723-1846).  The Weibull with beta = e^eta, at
+// u = log y - eta and t = e^{alpha u} = (y / beta)^alpha:  log f = log alpha - eta + (alpha - 1) u - t,  log S = -t,
+// log F = log(1 - e^-t).  log S is written directly (the reference has no Weibull logccdf and takes log(1 - F), which
+// loses every digit for small t); log F takes log t - t / 2 where t < 2e-9, so it stays finite after t underflows.  t
+// overflowing for y far above beta gives log S = -inf, which is the value.
+__device__ __forceinline__ bool ir_weibull(int dist) {
+    return dist == IRL_WEIBULL_LOG || dist == IRL_CENSORED_WEIBULL_LOG || dist == IRL_TRUNCATED_WEIBULL_LOG;
+}
+__device__ __forceinline__ bool ir_survival(int dist) { return dist >= IRL_WEIBULL_LOG && dist <= IRL_TRUNCATED_LOGNORMAL; }
+// log(1 - e^-t) given v = log t and t
+__device__ __forceinline__ double ir_log1mexp_neg(double v, double t) {
+    return v < -20.0 ? v - 0.5 * t : (t < 0.6931471805599453 ? log(-expm1(-t)) : log1p(-exp(-t)));
+}
+// t / (e^t - 1) given v = log t and t: 1 as t -> 0, 0 once e^t overflows
+__device__ __forceinline__ double ir_t_over_expm1(double v, double t) {
+    return v < -20.0 ? 1.0 - 0.5 * t : (v > 700.0 ? 0.0 : t / expm1(t));
+}
+// One Weibull observation: lp, r = d / d eta and s = d / d alpha.  Uncensored: r = alpha (t - 1), s = 1 / alpha + u - u t;
+// right-censored (cens 2): r = alpha t, s = -u t; left-censored (cens 1): r = -alpha t / expm1(t), s = u t / expm1(t).
+// Truncated to [A, B]: the density minus log Z, Z = S(A) - S(B) = e^{-tA} (1 - e^{-D}), D = tB - tA taken as
+// log D = alpha uB + log(1 - e^{-alpha log(B / A)}) with log(B / A) = log1p((B - A) / A), so a window with D ~ 1e-6 keeps
+// its digits; an open side drops its factor (A = 0: log Z = log(1 - e^{-tB}); B = +inf: log Z = -tA).
+__device__ __forceinline__ IrBoundedTerm ir_weibull_term(const IrLikD& L, int i, double eta, double a, double la) {
+    const double u = L.y[i] - eta, v = a * u, t = exp(v);
+    const int c = L.cens ? L.cens[i] : 0;
+    if (c == 2) return {-t, a * t, -u * t};
+    if (c == 1) {
+        const double q = ir_t_over_expm1(v, t);
+        return {ir_log1mexp_neg(v, t), -a * q, u * q};
+    }
+    IrBoundedTerm o{la - eta + (a - 1.0) * u - t, a * (t - 1.0), 1.0 / a + u - u * t};
+    if (L.bnd) {  // truncated
+        const int N = (int)L.N;
+        const double A = L.bnd[i], B = L.bnd[N + i];
+        double ta = 0.0, ua = 0.0;
+        if (A > 0.0) {  // -log Z gains +tA
+            ua = log(A) - eta;
+            ta = exp(a * ua);
+            o.lp += ta;
+            o.r -= a * ta;
+            o.s += ua * ta;
+        }
+        if (B != INFINITY) {  // -log Z gains -log(1 - e^-D)
+            const double ub = log(B) - eta, lr = A > 0.0 ? log1p((B - A) / A) : 0.0;
+            const double ld = A > 0.0 ? a * ub + log(-expm1(-a * lr)) : a * ub, d = exp(ld);
+            const double q = ir_t_over_expm1(ld, d);  // D / expm1(D)
+            o.lp -= ir_log1mexp_neg(ld, d);
+            o.r += a * q;  // dD / d eta = -alpha D
+            o.s -= q * (ub + (A > 0.0 ? lr / expm1(a * lr) : 0.0));  // dD / d alpha = uB tB - uA tA = log(B / A) tA + uB D
+        }
+    }
+    return o;
+}
+
+// The observation loop of a censored / truncated Normal or a survival likelihood, out of line: IrExtendedModel::eval calls
+// it once per such likelihood, so the erfcx() tail math stays out of eval's own observation loop.  Writes r_i = d logp / d eta_i;
 // returns this thread's partial sums of logp and d logp / d sigma.
 struct IrPartials { double lp, s_sig; };
 template <int W>
@@ -271,10 +330,12 @@ __device__ __noinline__ IrPartials ir_bounded_pass(const IrLikD* Lp, const IrTer
     constexpr int TS = 32 * W;
     const IrLikD& L = *Lp;
     const int N = (int)L.N;
+    const bool weibull = ir_weibull(L.dist);  // sg_s is alpha
+    const double la = weibull ? log(sg_s) : 0.0;
     double lp = 0.0, s_sig = 0.0;
     for (int i = tid; i < N; i += TS) {
         const double eta = ir_eta(terms + L.term0, 0, L.n_terms, x, i, N);
-        const IrBoundedTerm b = ir_bounded_term(L, i, eta, ir_scale(L, i, sg_s));
+        const IrBoundedTerm b = weibull ? ir_weibull_term(L, i, eta, sg_s, la) : ir_bounded_term(L, i, eta, ir_scale(L, i, sg_s));
         lp += b.lp;
         s_sig += b.s;
         r[i] = b.r;
@@ -493,8 +554,8 @@ __device__ __noinline__ void ir_ordered_chain(const IrVarD* Vp, const double* q,
     }
 }
 
-// IrModel evaluates every factor of the closed set except the censored / truncated Normal, the ordinal, the zero-inflated
-// and the hurdle likelihoods and the ordered transform; IrExtendedModel (below) is the same function with those added,
+// IrModel evaluates every factor of the closed set except the censored / truncated Normal, the ordinal, the zero-inflated,
+// the hurdle and the survival likelihoods and the ordered transform; IrExtendedModel (below) is the same function with those added,
 // each out of line.  A kernel's
 // register allocation covers every function it can reach, and the tail math takes about 128 registers, so the engine
 // instantiates its kernels twice and runs a model on IrExtendedModel only when it has one of them (b200_model.ir_extended):
@@ -669,14 +730,15 @@ struct IrModel {
             const IrLikD L = P.liks[l];
             const int N = (int)L.N;
             const double sg_s = ir_slot(L, x);
-            const bool zi = EXTENDED && L.dist >= IRL_ZI_POISSON;  // zero-inflated / hurdle
+            const bool zi = EXTENDED && L.dist >= IRL_ZI_POISSON && L.dist <= IRL_HURDLE_GAMMA;  // zero-inflated / hurdle
             const bool gamma = L.dist == IRL_GAMMA_LOG || (EXTENDED && L.dist == IRL_HURDLE_GAMMA);
             const bool disp = L.dist == IRL_NEGBINOMIAL_LOG || gamma ||  // sg_s is the dispersion alpha
                               (EXTENDED && (L.dist == IRL_ZI_NEGBINOMIAL || L.dist == IRL_HURDLE_NEGBINOMIAL));
             const double la = disp ? log(sg_s) : 0.0;
             double s_sig = 0.0, s_psi = 0.0;
             const bool ordinal = EXTENDED && (L.dist == IRL_ORDERED_LOGISTIC || L.dist == IRL_ORDERED_PROBIT);
-            const bool bounded = EXTENDED && (ordinal || zi || L.dist == IRL_CENSORED_NORMAL || L.dist == IRL_TRUNCATED_NORMAL);
+            const bool bounded = EXTENDED && (ordinal || zi || L.dist == IRL_CENSORED_NORMAL || L.dist == IRL_TRUNCATED_NORMAL ||
+                                              ir_survival(L.dist));
             if constexpr (EXTENDED) {
                 if (zi) {  // uniform branch: out of line
                     const IrZiPartials b = ir_zi_pass<W>(P.liks + l, P.terms, x, r, x + P.ord_row, sg_s, la, tid);
@@ -827,23 +889,26 @@ struct IrExtendedModel : IrModel {
 
 // log p(y_i | eta) of observation i with every constant, through the term function eval's pass uses: a base family's
 // term plus ir_obs_const; a zero-inflated / hurdle count's plus that of f at y > 0; a censored / truncated Normal's plus
-// -log(2 pi) / 2 except at a censoring bound; an ordinal one's has none.
+// -log(2 pi) / 2 except at a censoring bound, a LogNormal's plus -log(2 pi) / 2 - log y_i there; an ordinal or Weibull
+// one's has none.
 template <bool EXTENDED>  // as IrModel / IrExtendedModel
 __device__ __forceinline__ double ir_obs_loglik(const IrLikD& L, const IrTermD* terms, const double* x, int i, double eta,
                                                 double sg_s, double la) {
     const double y = L.y[i];
-    if (EXTENDED && L.dist >= IRL_ZI_POISSON) {
+    if (EXTENDED && L.dist >= IRL_ZI_POISSON && L.dist <= IRL_HURDLE_GAMMA) {
         const IrPsi ps = ir_psi(terms + L.term0 + L.n_terms, (int)L.nu, x, i, (int)L.N);
         const double lp = ir_zi_term(L.dist, y, eta, ir_scale(L, i, sg_s), sg_s, la, ps).lp;
         return y > 0.0 ? lp + ir_obs_const(L, i, y, sg_s, la) : lp;
     }
-    if (EXTENDED && L.dist >= IRL_ORDERED_LOGISTIC) {
+    if (EXTENDED && (L.dist == IRL_ORDERED_LOGISTIC || L.dist == IRL_ORDERED_PROBIT)) {
         const double s = ir_scale(L, i, L.sigma_kind == IRS_NONE ? 1.0 : sg_s);  // the logistic link: s = 1
         return ir_ordinal_term(L, terms[L.term0 + L.n_terms], x, i, eta, s).lp;
     }
-    if (EXTENDED && L.dist >= IRL_CENSORED_NORMAL) {
-        const bool at_bound = L.dist == IRL_CENSORED_NORMAL && L.cens[i] != 0;
-        return ir_bounded_term(L, i, eta, ir_scale(L, i, sg_s)).lp - (at_bound ? 0.0 : B200_HALF_LOG_2PI);
+    if (EXTENDED && ir_weibull(L.dist)) return ir_weibull_term(L, i, eta, sg_s, la).lp;
+    if (EXTENDED && (L.dist == IRL_CENSORED_NORMAL || L.dist == IRL_TRUNCATED_NORMAL || ir_survival(L.dist))) {
+        const bool at_bound = L.cens && L.cens[i] != 0;
+        const double ly = L.dist >= IRL_WEIBULL_LOG ? y : 0.0;  // a LogNormal's y is log y_i
+        return ir_bounded_term(L, i, eta, ir_scale(L, i, sg_s)).lp - (at_bound ? 0.0 : B200_HALF_LOG_2PI + ly);
     }
     double lp = 0.0, s_sig = 0.0;
     ir_base_term(L, i, y, eta, sg_s, la, lp, s_sig);

@@ -16,6 +16,9 @@ pymc/model/fgraph.py:76-81, :139) -- and pattern-matches them onto the closed fa
                      Gamma(alpha, beta = alpha / exp(eta) | alpha * exp(-eta)), alpha a constant or a scalar free RV;
                      pm.Censored(pm.Normal.dist(eta, sigma), lower, upper), pm.TruncatedNormal(eta, sigma, lower, upper)
                      and pm.Truncated(pm.Normal.dist(eta, sigma), lower, upper) with constant bounds;
+                     survival: pm.Weibull(alpha, beta=exp(eta)), pm.Exponential(scale=exp(eta)) or (lam=exp(-eta)) (the
+                     Weibull with alpha = 1) and pm.LogNormal(eta, sigma), plain, or under pm.Censored / pm.Truncated with
+                     constant bounds;
                      pm.OrderedLogistic / pm.OrderedProbit: the Categorical whose p is their compute_p graph, with or
                      without the {name}_probs Deterministic (recorded, evaluated from the draws);
                      pm.ZeroInflatedPoisson / Binomial / NegativeBinomial and pm.HurdlePoisson / NegativeBinomial / Gamma:
@@ -490,8 +493,8 @@ def from_pymc(model) -> _ir.ModelIR:
         comp = comps[1]
         cop = _op_name(comp)
         if hurdle and cop == "lognormal":
-            raise NotImplementedError(f"{rv.name}: pm.HurdleLogNormal is outside the closed set (there is no LogNormal "
-                                      "likelihood)")
+            raise NotImplementedError(f"{rv.name}: pm.HurdleLogNormal is outside the closed set (the hurdle likelihoods "
+                                      "are HurdlePoisson, HurdleNegativeBinomial and HurdleGamma)")
         cps = _dist_params(comp)
         truncated = cop == "truncated"
         if hurdle and truncated:  # Truncated(f, lower=1): f's own parameters, then lower and upper
@@ -512,6 +515,44 @@ def from_pymc(model) -> _ir.ModelIR:
         dist = next(d for d, f in _ir.ZI_FAMILY.items() if f == fam and d.startswith("hurdle" if hurdle else "zero"))
         return dist, eta, slot, psi_of(w, rv.name, N)
 
+    def survival_of(op, ps, name, sigma_of):
+        """(family, eta, parameter slot) of a survival RV (op, its dist params ps): pm.Weibull(alpha, beta=exp(eta)),
+        pm.Exponential(scale=exp(eta)) or (lam=exp(-eta)) -- the Weibull with alpha = 1 -- or pm.LogNormal(eta, sigma)"""
+        if op in ("weibullbeta", "weibull"):  # WeibullBetaRV: (alpha, beta), continuous.py:2717-2737
+            form = "pm.Weibull(alpha, beta=pm.math.exp(linear predictor)) with alpha a constant or a scalar free RV"
+            a = ps[0]
+            while a.owner is not None and isinstance(a.owner.op, DimShuffle):
+                a = a.owner.inputs[0]
+            c = _const_value(a)
+            if (a in name_of and size_of[name_of[a]] != 1) or (a not in name_of and c is not None and c.size != 1):
+                raise NotImplementedError(f"{name}: a per-observation or vector Weibull alpha is outside the closed set "
+                                          f"({form})")
+            try:
+                alpha = param(a, name + ".alpha")
+            except NotImplementedError:
+                raise NotImplementedError(f"{name}: a Weibull alpha that is an expression of random variables is outside "
+                                          f"the closed set ({form})") from None
+            e = inputs_of(ps[1], "exp")
+            if e is None:
+                raise NotImplementedError(f"{name}: write the likelihood as {form}")
+            return "weibull_log", e[0], {"alpha": alpha}
+        if op == "exponential":  # ExponentialRV: (scale,), scale = reciprocal(lam), continuous.py:1461-1471
+            form = ("pm.Exponential(scale=pm.math.exp(linear predictor)) or "
+                    "pm.Exponential(lam=pm.math.exp(-linear predictor))")
+            e, eta = inputs_of(ps[0], "exp"), None
+            if e is not None:
+                eta = e[0]
+            else:
+                r = inputs_of(ps[0], "reciprocal")
+                e = inputs_of(r[0], "exp") if r is not None else None
+                ng = inputs_of(e[0], "neg") if e is not None else None
+                eta = ng[0] if ng is not None else None
+            if eta is None:
+                raise NotImplementedError(f"{name}: write the likelihood as {form}")
+            return "weibull_log", eta, {"alpha": 1.0}
+        return "lognormal", ps[0], {"sigma": sigma_of(ps[1])}  # LogNormalRV: (mu, sigma)
+
+    survival_ops = ("weibullbeta", "weibull", "exponential", "lognormal")
     probs_of = {}  # id of a {name}_probs Deterministic's expression -> the ordinal likelihood's name
     liks = []
     for rv in model.observed_RVs:
@@ -559,16 +600,13 @@ def from_pymc(model) -> _ir.ModelIR:
         elif op in ("mixture", "_hurdle", "hurdle"):  # pm.ZeroInflated* / pm.Hurdle*
             dist, eta, slot, psi = zero_inflated_of(rv, ps, N)
             liks.append(_ir.Likelihood(dist, y, make_terms(eta, N), name=rv.name, psi=psi, **slot))
-        elif op == "truncated":
-            # TruncatedRV (truncated.py:53-130): the base RV's own inputs followed by lower and upper, its op in base_rv_op.
-            # A Normal base never arrives here: pm.Truncated dispatches it to TruncatedNormal (truncated.py:499-505).
-            base_op = getattr(rv.owner.op, "base_rv_op", None)
-            what = type(base_op).__name__ if base_op is not None else type(rv.owner.op).__name__
-            raise NotImplementedError(f"{rv.name}: pm.Truncated of {what} is outside the closed set (only a Normal base "
-                                      "distribution can be truncated)")
-        elif op in ("censored", "truncatednormal"):
+        elif op in survival_ops:
+            dist, eta, slot = survival_of(op, ps, rv.name, sigma_of)
+            liks.append(_ir.Likelihood(dist, y, make_terms(eta, N), name=rv.name, **slot))
+        elif op in ("censored", "truncatednormal", "truncated"):
             # CensoredRV: dist params (base, lower, upper) (censored.py:45-76); TruncatedNormalRV: (mu, sigma, lower, upper)
-            # (continuous.py:558-583), which pm.Truncated of a Normal also becomes (truncated.py:499-505)
+            # (continuous.py:558-583), which pm.Truncated of a Normal also becomes (truncated.py:499-505); TruncatedRV
+            # (truncated.py:53-130): the base RV's own inputs followed by lower and upper, its op in base_rv_op
             def bound(x, open_value):
                 v = _const_value(x)
                 if v is None:
@@ -579,14 +617,35 @@ def from_pymc(model) -> _ir.ModelIR:
                     return None if float(v.reshape(())) == open_value else float(v.reshape(()))
                 return np.ravel(np.broadcast_to(v, (N,))).astype(np.float64)
 
+            if op == "truncated":
+                base_op = getattr(rv.owner.op, "base_rv_op", None)
+                what = type(base_op).__name__ if base_op is not None else type(rv.owner.op).__name__
+                bop = _op_class_name(base_op) if base_op is not None else ""
+                if bop not in survival_ops:
+                    raise NotImplementedError(f"{rv.name}: pm.Truncated of {what} is outside the closed set (only a "
+                                              "Normal, Weibull, Exponential or LogNormal base distribution can be truncated)")
+                lo, hi = ps[-2], ps[-1]
+                fam, eta, slot = survival_of(bop, ps[:-2][-(1 if bop == "exponential" else 2):], rv.name, sigma_of)
+                liks.append(_ir.Likelihood(f"truncated_{fam}", y, make_terms(eta, N), lower=bound(lo, -np.inf),
+                                           upper=bound(hi, np.inf), name=rv.name, **slot))
+                continue
             if op == "truncatednormal":
                 mu, s, lo, hi = ps[:4]
             else:
                 base, lo, hi = ps[:3]
-                if base.owner is None or _op_name(base) != "normal":
+                bop = _op_name(base) if base.owner is not None else ""
+                if bop == "truncated":
+                    raise NotImplementedError(f"{rv.name}: pm.Censored of a pm.Truncated distribution is outside the closed "
+                                              "set (censor or truncate, not both)")
+                if bop in survival_ops:
+                    fam, eta, slot = survival_of(bop, _dist_params(base), rv.name, sigma_of)
+                    liks.append(_ir.Likelihood(f"censored_{fam}", y, make_terms(eta, N), lower=bound(lo, -np.inf),
+                                               upper=bound(hi, np.inf), name=rv.name, **slot))
+                    continue
+                if bop != "normal":
                     what = type(base.owner.op).__name__ if base.owner is not None else str(base)
-                    raise NotImplementedError(f"{rv.name}: pm.Censored of {what} is outside the closed set (only a Normal "
-                                              "base distribution can be censored)")
+                    raise NotImplementedError(f"{rv.name}: pm.Censored of {what} is outside the closed set (only a Normal, "
+                                              "Weibull, Exponential or LogNormal base distribution can be censored)")
                 mu, s = _dist_params(base)[:2]
             dist = "censored_normal" if op == "censored" else "truncated_normal"
             liks.append(_ir.Likelihood(dist, y, make_terms(mu, N), sigma=sigma_of(s), lower=bound(lo, -np.inf),

@@ -70,6 +70,12 @@ LIK_DISTS = {
     "hurdle_poisson": 15,                   # HurdlePoisson(psi, mu = exp(eta_i))                  mixture.py:873-922
     "hurdle_negative_binomial": 16,         # HurdleNegativeBinomial(psi, exp(eta_i), alpha)       mixture.py:925-978
     "hurdle_gamma": 17,                     # HurdleGamma(psi, alpha, beta = alpha / exp(eta_i))   mixture.py:981-1034
+    "weibull_log": 18,             # y_i ~ Weibull(alpha, beta = exp(eta_i)); Exponential(scale = exp(eta_i)): alpha = 1
+    "lognormal": 19,               # y_i ~ LogNormal(mu = eta_i, sigma)                          continuous.py:1723-1846
+    "censored_weibull_log": 20,    # y_i ~ Censored(Weibull(alpha, exp(eta_i)), lower, upper)     continuous.py:2740-2831
+    "censored_lognormal": 21,      # y_i ~ Censored(LogNormal(eta_i, sigma), lower, upper)
+    "truncated_weibull_log": 22,   # y_i ~ Truncated(Weibull(alpha, exp(eta_i)), lower, upper)
+    "truncated_lognormal": 23,     # y_i ~ Truncated(LogNormal(eta_i, sigma), lower, upper)
 }
 # Zero-inflated and hurdle observations: ``Likelihood.psi`` is the probability of the count / positive component, a
 # constant in (0, 1), a Ref to a scalar variable with an interval transform inside [0, 1], or a Linear: the logit of psi.
@@ -104,12 +110,27 @@ LOGISTIC_SIGMA = "ordered_logistic has no sigma"
 # Normal observations with bounds: ``Likelihood.lower`` / ``.upper`` (None, a constant or one value per observation, -inf /
 # +inf where that side is open); lowered as the [3][N] block (y, lower, upper) of include/b200nuts.h
 BOUNDED_LIKS = ("censored_normal", "truncated_normal")
-SIGMA_LIKS = ("normal", "studentt") + BOUNDED_LIKS + ("ordered_probit",)  # likelihoods whose parameter slot is sigma
+# Survival (time-to-event) observations y_i > 0 with a log link: the Weibull (the Exponential is its alpha = 1) and the
+# LogNormal, plain, censored or truncated.  Bounds as for the Normal ones (``Likelihood.lower`` / ``.upper``, lowered as the
+# [3][N] block), where a lower bound of 0 or -inf is an open side; the Weibull's shape is ``Likelihood.alpha``, the
+# LogNormal's scale ``Likelihood.sigma`` (include/b200nuts.h)
+WEIBULL_LIKS = ("weibull_log", "censored_weibull_log", "truncated_weibull_log")
+LOGNORMAL_LIKS = ("lognormal", "censored_lognormal", "truncated_lognormal")
+SURVIVAL_LIKS = WEIBULL_LIKS + LOGNORMAL_LIKS
+SURVIVAL_BOUNDED = ("censored_weibull_log", "censored_lognormal", "truncated_weibull_log", "truncated_lognormal")
+SIGMA_LIKS = ("normal", "studentt") + BOUNDED_LIKS + ("ordered_probit",) + LOGNORMAL_LIKS  # parameter slot: sigma
 # the support rule of bounded observations (csrc/b200nuts.cu: prepare_ir, same words)
 BOUND_SIDES = "lower must not be +inf or NaN and upper must not be -inf or NaN"
 BOUND_ORDER = "lower < upper must hold for every observation"
 BOUND_Y = "y must be finite and lie in [lower, upper] for every observation"
 TRUNC_OPEN = "truncated_normal needs a finite lower or upper bound; with neither side bounded, write the likelihood as normal"
+# the support rule of survival observations (csrc/b200nuts.cu: prepare_ir, same words)
+SURV_Y = "y must be finite and > 0 for every observation"
+SURV_SIDES = "lower must be finite and >= 0 or -inf (0 and -inf: open) and upper > 0 or +inf (open), neither NaN"
+SURV_TRUNC_OPEN = ("a truncated survival likelihood needs a finite lower bound > 0 or a finite upper bound; with neither, "
+                   "write the plain likelihood")
+SURV_PLAIN = "lower / upper belong to the censored_ and truncated_ forms"
+WEIBULL_SIGMA = "a Weibull likelihood has no sigma (its parameter is alpha)"
 DISPERSION_LIKS = ("negative_binomial_log", "gamma_log")  # their `alpha` is a constant or a Ref
 # The support rule.  The device evaluates a density's formula wherever it is asked to, so every variable must be kept
 # inside its prior's support by its transform, and every scale parameter must be positive:
@@ -205,10 +226,10 @@ class Likelihood:
     sigma: float | Ref | np.ndarray | None = None
     nu: float = 0.0
     name: str = "y"
-    alpha: float | Ref | None = None           # negative_binomial_log / gamma_log: dispersion (shape)
+    alpha: float | Ref | None = None           # negative_binomial_log / gamma_log: dispersion (shape); Weibull: shape
     trials: float | np.ndarray | None = None   # binomial_logit: number of trials, one for all or one per observation
-    lower: float | np.ndarray | None = None    # censored_normal / truncated_normal: None (open), a constant or one per
-    upper: float | np.ndarray | None = None    # observation, -inf / +inf where that observation's side is open
+    lower: float | np.ndarray | None = None    # censored / truncated: None (open), a constant or one per observation,
+    upper: float | np.ndarray | None = None    # -inf / +inf where that observation's side is open (survival: lower 0 too)
     cutpoints: Ref | np.ndarray | None = None  # ordered_logistic / ordered_probit: K - 1 cutpoints (see ORDINAL_LIKS)
     psi: float | Ref | Linear | None = None    # the zero-inflated / hurdle likelihoods (ZI_LIKS): a Linear is logit(psi)
 
@@ -368,6 +389,7 @@ class ModelIR:
             self._validate_bounds(L)
             self._validate_ordinal(L)
             self._validate_psi(L)
+            self._validate_survival(L)
         for a in self.ar1:
             if self.var(a.var).size < 2:
                 raise ValueError("AR1 needs at least two steps")
@@ -479,7 +501,7 @@ class ModelIR:
                 raise ValueError("gamma_log: y must be > 0")
             if L.dist == "hurdle_gamma" and not (np.all(np.isfinite(y)) and np.all(y >= 0)):
                 raise ValueError(f"hurdle_gamma: {HG_Y}")
-        elif L.alpha is not None:
+        elif L.alpha is not None and L.dist not in WEIBULL_LIKS:
             raise ValueError(f"{L.dist}: alpha belongs to the negative_binomial_log / gamma_log likelihoods")
         if fam in ("binomial_logit",) + DISPERSION_LIKS and L.sigma is not None:
             raise ValueError(f"{L.dist} has no sigma (its parameter is {'trials' if L.dist == 'binomial_logit' else 'alpha'})")
@@ -487,6 +509,8 @@ class ModelIR:
     def _validate_bounds(self, L) -> None:
         """Bounds of censored / truncated Normal observations (the checks prepare_ir makes, in the same words)."""
         what = f"{L.dist} likelihood {L.name}"
+        if L.dist in SURVIVAL_LIKS:  # _validate_survival
+            return
         if L.dist not in BOUNDED_LIKS:
             if L.lower is not None or L.upper is not None:
                 raise ValueError(f"{what}: lower / upper belong to the censored_normal / truncated_normal likelihoods")
@@ -507,6 +531,45 @@ class ModelIR:
             raise ValueError(f"{what}: {BOUND_Y}")
         if L.dist == "truncated_normal" and not np.any(np.isfinite(lo) | np.isfinite(hi)):
             raise ValueError(f"{what}: {TRUNC_OPEN}")
+
+    def _validate_survival(self, L) -> None:
+        """y, bounds and the shape alpha of Weibull / LogNormal observations (the checks prepare_ir makes, in the same
+        words).  A lower bound of 0 is an open side, as -inf is: every y is > 0."""
+        if L.dist not in SURVIVAL_LIKS:
+            return
+        what = f"{L.dist} likelihood {L.name}"
+        if L.dist in WEIBULL_LIKS:
+            if L.alpha is None:
+                raise ValueError(f"{L.dist} needs alpha")
+            if isinstance(L.alpha, Ref) and self.var(L.alpha.var).size != 1:
+                raise ValueError(f"{L.dist}: alpha must be a scalar variable")
+            if not isinstance(L.alpha, Ref) and np.ndim(L.alpha) != 0:
+                raise ValueError(f"{what}: alpha must be one constant or a scalar variable")
+            self._check_scale(L.alpha, f"{L.dist}: alpha")
+            if L.sigma is not None:
+                raise ValueError(f"{what}: {WEIBULL_SIGMA}")
+        y = np.asarray(L.y, dtype=np.float64)
+        if not (np.all(np.isfinite(y)) and np.all(y > 0)):
+            raise ValueError(f"{what}: {SURV_Y}")
+        if L.dist not in SURVIVAL_BOUNDED:
+            if L.lower is not None or L.upper is not None:
+                raise ValueError(f"{what}: {SURV_PLAIN}")
+            return
+        N = len(y)
+        for side in (L.lower, L.upper):
+            if isinstance(side, Ref):
+                raise ValueError(f"{what}: lower and upper are data (None, a constant or one per observation), not variables")
+            if side is not None and not (np.ndim(side) == 0 or (np.ndim(side) == 1 and len(side) == N)):
+                raise ValueError(f"{what}: lower and upper must be None, a constant or one value per observation (N = {N})")
+        lo, hi = L.bounds()
+        if np.any(np.isnan(lo) | np.isnan(hi) | ~((lo >= 0) | (lo == -np.inf)) | (lo == np.inf) | ~(hi > 0)):
+            raise ValueError(f"{what}: {SURV_SIDES}")
+        if not np.all(lo < hi):
+            raise ValueError(f"{what}: {BOUND_ORDER}")
+        if not np.all((lo <= y) & (y <= hi)):
+            raise ValueError(f"{what}: {BOUND_Y}")
+        if L.dist.startswith("truncated") and not np.any((np.isfinite(lo) & (lo > 0)) | np.isfinite(hi)):
+            raise ValueError(f"{what}: {SURV_TRUNC_OPEN}")
 
     def _validate_ordinal(self, L) -> None:
         """Cutpoints and categories of ordinal observations (the checks prepare_ir makes, in the same words)."""
@@ -962,6 +1025,66 @@ def zero_inflated_ir(dist: str = "zero_inflated_poisson", psi: str = "const", n_
                    likelihoods=[Likelihood(dist, y, terms, alpha=alpha, trials=trials, psi=p)])
 
 
+def survival_regression_ir(dist: str = "weibull", observe: str = "right_censored", alpha: float | None = None,
+                           n_obs: int = 400, n_groups: int = 8, n_features: int = 3, seed: int = 61) -> ModelIR:
+    """Survival regression on simulated event times, accelerated-failure-time style: eta_i = b0 + sigma_a z[g_i] + x_i . beta
+    with b0 ~ Normal(0, 2), z_g ~ Normal(0, 1) and sigma_a ~ HalfNormal(1) (a non-centred group frailty), beta ~ Normal(0,
+    1)^F as a design term, and T_i ~ Weibull(alpha, beta = exp(eta_i)) (``dist="weibull"``), Exponential(scale =
+    exp(eta_i)), the Weibull with alpha = 1 (``"exponential"``), or LogNormal(eta_i, sigma) (``"lognormal"``).  The shape
+    alpha ~ HalfNormal(2), the LogNormal's sigma ~ HalfNormal(1), or the constant ``alpha`` for either.
+    observe: "plain" records every T_i; "right_censored" records y_i = min(T_i, c_i) at per-observation follow-up times
+    c_i, which end about 30 % of the observations before their event; "entry_truncated" records subjects only if they are
+    still event-free at their own entry time e_i (delayed entry; e_i = 0 for a third of them), i.e. T_i truncated to
+    (e_i, inf)."""
+    if dist not in ("weibull", "exponential", "lognormal"):
+        raise ValueError("dist must be 'weibull', 'exponential' or 'lognormal'")
+    if observe not in ("plain", "right_censored", "entry_truncated"):
+        raise ValueError("observe must be 'plain', 'right_censored' or 'entry_truncated'")
+    if dist == "exponential" and alpha is not None:
+        raise ValueError("the exponential's shape is 1: leave alpha None")
+    rng = np.random.default_rng(seed)
+    g = rng.integers(0, n_groups, n_obs).astype(np.int32)
+    X = rng.standard_normal((n_obs, n_features))
+    eta = 1.0 + rng.normal(0.0, 0.4, n_groups)[g] + X @ rng.normal(0.0, 0.4, n_features)
+    shape = 1.0 if dist == "exponential" else (1.5 if alpha is None else float(alpha))  # the Weibull's alpha
+    scale = 0.8 if alpha is None else float(alpha)  # the LogNormal's sigma
+
+    def draw(i):
+        if dist == "lognormal":
+            return float(np.exp(eta[i] + scale * rng.standard_normal()))
+        return float(np.exp(eta[i]) * rng.exponential() ** (1.0 / shape))
+
+    lower = upper = None
+    entry = np.where(rng.random(n_obs) < 1 / 3, 0.0, np.exp(eta) * rng.uniform(0.05, 1.0, n_obs))
+    y = np.empty(n_obs)
+    for i in range(n_obs):
+        y[i] = draw(i)
+        while observe == "entry_truncated" and not y[i] > entry[i]:  # rejection: T_i given T_i > e_i
+            y[i] = draw(i)
+    if observe == "right_censored":
+        u = np.exp(eta) * rng.uniform(0.5, 3.0, n_obs)
+        upper = u * np.quantile(y / u, 0.7)  # 30 % of the T_i lie past their follow-up time
+        y = np.minimum(y, upper)
+    elif observe == "entry_truncated":
+        lower = entry
+    vars_ = [Var("b0", "b0", 1), Var("z", "z", n_groups), Var("sigma_a_log__", "sigma_a", 1, "log"),
+             Var("beta", "beta", n_features)]
+    priors = [Prior("normal", "b0", (0.0, 2.0)), Prior("normal", "z", (0.0, 1.0)), Prior("halfnormal", "sigma_a_log__", (1.0,)),
+              Prior("normal", "beta", (0.0, 1.0))]
+    par = 1.0 if dist == "exponential" else alpha
+    if par is None:
+        name = "sigma" if dist == "lognormal" else "alpha"
+        vars_.append(Var(f"{name}_log__", name, 1, "log"))
+        priors.append(Prior("halfnormal", f"{name}_log__", (1.0 if dist == "lognormal" else 2.0,)))
+        par = Ref(f"{name}_log__")
+    base = "lognormal" if dist == "lognormal" else "weibull_log"
+    lik = {"plain": base, "right_censored": f"censored_{base}", "entry_truncated": f"truncated_{base}"}[observe]
+    terms = [Term([("b0", None)]), Term([("sigma_a_log__", None), ("z", g)]), Term([("beta", None)], coef=X)]
+    slot = dict(sigma=par) if dist == "lognormal" else dict(alpha=par)
+    return ModelIR(name=f"survival_{dist}_{observe}", vars=vars_, priors=priors,
+                   likelihoods=[Likelihood(lik, y, terms, lower=lower, upper=upper, **slot)])
+
+
 # ------------------------------------------------------------------------------------------------------------------------
 # lowering: ModelIR -> flat arrays of the C ABI (include/b200nuts.h: b200_ir)
 # ------------------------------------------------------------------------------------------------------------------------
@@ -975,7 +1098,8 @@ class LoweredIR:
     priors: list            # [(dist, var, [(kind, value, ref_offset)] * 3)]
     liks: list              # [dict(dist, N, y, terms=[dict(coef, factors=[(offset, size, idx)])], sigma_kind, sigma_value, sigma_ref, sigma_obs, nu, y_var)]
                             # a design term's dict also has n_cols = K, with coef = X [N][K]
-                            # censored_normal / truncated_normal: y is the [3][N] block (y, lower, upper)
+                            # censored_normal / truncated_normal and the censored_ / truncated_ survival likelihoods:
+                            # y is the [3][N] block (y, lower, upper); the Weibull's alpha is the sigma slot
                             # ordered_logistic / ordered_probit: nu = K, and cut = the cutpoint term (a term dict)
                             # zero-inflated / hurdle: nu = 0 or m, and psi = the psi block (a list of term dicts)
                             # y_var 0: y is observed data; v + 1: a latent factor, y is None and its values are variable v's
@@ -1049,9 +1173,9 @@ def lower(ir: ModelIR) -> LoweredIR:
     for L in ir.likelihoods:
         # the likelihood's one parameter slot: sigma, or the trials / alpha of the count and positive families
         fam = ZI_FAMILY.get(L.dist, L.dist)
-        par = L.trials if fam == "binomial_logit" else (L.alpha if fam in DISPERSION_LIKS else L.sigma)
+        par = L.trials if fam == "binomial_logit" else (L.alpha if fam in DISPERSION_LIKS + WEIBULL_LIKS else L.sigma)
         y = np.ascontiguousarray(L.y, dtype=np.float64)
-        if L.dist in BOUNDED_LIKS:  # the [3][N] block: y, lower, upper
+        if L.dist in BOUNDED_LIKS + SURVIVAL_BOUNDED:  # the [3][N] block: y, lower, upper
             y = np.ascontiguousarray(np.stack([y, *L.bounds()]))
         extra = {}
         if L.dist in ORDINAL_LIKS:  # nu = K; the cutpoint term goes one past the predictor's terms

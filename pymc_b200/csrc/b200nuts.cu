@@ -1956,3 +1956,20 @@ extern "C" int b200_measure_dmma_tflops(double* tflops) {
     *tflops = best;
     return 0;
 }
+
+#ifdef B200_PHASE_CLOCKS
+// Phase profile of nuts_warp_kernel (built by scripts/profile_radon_phases.py only): copy out, or clear, the per-chain
+// cycle counters [chain][phase] of chains 0 .. chains-1.
+extern "C" int b200_phase_clocks(unsigned long long* out, int chains, int clear) {
+    const size_t bytes = (size_t)std::min(chains, b200::kPhaseMaxChains) * b200::PH_COUNT * sizeof(unsigned long long);
+    if (clear) {
+        void* p = nullptr;
+        CU(cudaGetSymbolAddress(&p, b200::b200_phase_cycles));
+        CU(cudaMemset(p, 0, bytes));
+    } else {
+        CU(cudaMemcpyFromSymbol(out, b200::b200_phase_cycles, bytes));
+    }
+    CU(cudaDeviceSynchronize());
+    return b200::PH_COUNT;
+}
+#endif

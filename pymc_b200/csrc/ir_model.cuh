@@ -561,6 +561,7 @@ __device__ __noinline__ void ir_ordered_chain(const IrVarD* Vp, const double* q,
 // instantiates its kernels twice and runs a model on IrExtendedModel only when it has one of them (b200_model.ir_extended):
 // every other IR model keeps the kernels it had before.
 struct IrModel {
+    static constexpr bool kEvalOutOfLine = true;  // eval is __noinline__ (see nuts_model_eval)
     struct Params {
         const IrVarD* vars; const IrPriorD* priors; const IrLikD* liks; const IrTermD* terms; const IrAr1D* ar1;
         int n_vars, n_priors, n_liks, n_ar1, n;

@@ -16,6 +16,7 @@ namespace b200 {
 // x ~ Normal(0,1)^n  (test model; Normal.logp distributions/continuous.py:526-527)
 // ------------------------------------------------------------------------------------------------
 struct StdNormalModel {
+    static constexpr bool kEvalOutOfLine = false;  // see nuts_model_eval
     struct Params {
         int n;
     };
@@ -43,6 +44,7 @@ struct StdNormalModel {
 // + Jacobian logprob/transforms.py:880-891.  Gradient: SURVEY Appendix C-1.
 // ------------------------------------------------------------------------------------------------
 struct EightSchoolsModel {
+    static constexpr bool kEvalOutOfLine = false;  // see nuts_model_eval
     struct Params {
         const double* y;       // [J]
         const double* inv_s2;  // [J] 1/sigma^2
@@ -96,6 +98,7 @@ struct EightSchoolsModel {
 // double2 staged once per CTA into shared memory by bulk TMA and shared by all the CTA's chains.
 // ------------------------------------------------------------------------------------------------
 struct RadonModel {
+    static constexpr bool kEvalOutOfLine = false;  // see nuts_model_eval
     struct Params {
         const double2* xy;   // [K][32]  (floor_i, y_i); row j occupies 4 * nblk_j consecutive k, rows back to back,
                              //          followed by 4 all-zero k (the block prefetched past the last row)
@@ -231,6 +234,7 @@ struct RadonModel {
 // from the chain's shared-memory copy of q; y_t^2 is read through L1 (24 KB, shared by all CTAs of the SM).
 // ------------------------------------------------------------------------------------------------
 struct StochVolModel {
+    static constexpr bool kEvalOutOfLine = false;  // see nuts_model_eval
     struct Params {
         const double* y2;  // [T] y_t^2
         int T;

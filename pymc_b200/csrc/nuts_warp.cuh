@@ -91,6 +91,26 @@ __host__ __device__ inline size_t nuts_warp_smem_bytes(int NP, int hot, int W) {
 
 constexpr int kNutsWarpChains = 8;  // chain = warp (W = 1): chains per CTA (256 threads, one CTA per SM)
 
+// Phase profile of the persistent kernel (scripts/profile_radon_phases.py), compiled in only with -DB200_PHASE_CLOCKS: the
+// team's first thread adds the clock64() cycles since the previous mark to the chain's counter of the phase that just ended.
+// The cycles are the team's own elapsed time, stalls included, so the phases of a chain add up to its time on the SM.
+#ifdef B200_PHASE_CLOCKS
+enum { PH_LEAPFROG, PH_EVAL, PH_ENERGY, PH_MERGE0, PH_MERGE, PH_PARK, PH_DOUBLING, PH_ITER, PH_SEGMENT, PH_COUNT };
+constexpr int kPhaseMaxChains = 8192;
+__device__ unsigned long long b200_phase_cycles[kPhaseMaxChains * PH_COUNT];
+#define B200_PHASE(ph)                                                                                          \
+    do {                                                                                                        \
+        const long long t_ = clock64();                                                                         \
+        if (lane == 0 && chain < kPhaseMaxChains)                                                               \
+            atomicAdd(&b200_phase_cycles[chain * PH_COUNT + (ph)], (unsigned long long)(t_ - ph_t));            \
+        ph_t = t_;                                                                                              \
+    } while (0)
+#else
+#define B200_PHASE(ph) \
+    do {               \
+    } while (0)
+#endif
+
 // CTA prologue of the model kernels: stage the model's observed data into the start of the dynamic shared memory (bulk
 // TMA).  Returns the bytes it occupies, padded to 16.
 template <class Model>
@@ -104,6 +124,43 @@ __device__ __forceinline__ size_t stage_model_data(const typename Model::Params&
         mbar_wait(&tma_bar, 0);
     }
     return data_bytes;
+}
+
+// The persistent kernel's model evaluation, team-synchronised on both sides.  The start state, the HMC steps, every tree
+// leaf and the final DIAG_ADAPT_GRAD update all call ONE out-of-line copy (nuts_model_eval_call), so the kernel holds the
+// model's code once and the leaf loop around it stays compact.  A model whose eval is out of line already
+// (kEvalOutOfLine) is called directly: a second call level would only cost registers.
+template <class Model, int NPL, int W>
+__device__ __forceinline__ double team_model_eval(const typename Model::Params& M, const char* data_s, const double* q_s,
+                                                  double* g_s, int lane, double* red) {
+    team_sync<W>();
+    const double lp = Model::template eval<NPL, W, true>(M, data_s, q_s, g_s, lane, red);
+    team_sync<W>();
+    return lp;
+}
+template <class Model, int NPL, int W>
+__device__ __noinline__ double nuts_model_eval_call(const typename Model::Params M, const char* data_s, const double* q_s,
+                                                    double* g_s, int lane, double* red) {
+    return team_model_eval<Model, NPL, W>(M, data_s, q_s, g_s, lane, red);
+}
+template <class Model, int NPL, int W>
+__device__ __forceinline__ double nuts_model_eval(const typename Model::Params& M, const char* data_s, const double* q_s,
+                                                  double* g_s, int lane, double* red) {
+    if constexpr (Model::kEvalOutOfLine) return team_model_eval<Model, NPL, W>(M, data_s, q_s, g_s, lane, red);
+    else return nuts_model_eval_call<Model, NPL, W>(M, data_s, q_s, g_s, lane, red);
+}
+
+// _WeightedVariance.add_sample of one draw x on both diagonal estimators, for the NPL elements of a team thread: out of line
+// (it runs once per tuning draw, and its divisions would otherwise be inlined NPL times into the kernel)
+template <int TS, int NPL>
+__device__ __noinline__ void welford_add_team(const double* x, double fg_n, double bg_n, double* fm, double* fv, double* bm,
+                                              double* bv, int lane) {
+#pragma unroll 1
+    for (int k = 0; k < NPL; ++k) {
+        const int i = lane + TS * k;
+        welford_add(x[i], fg_n, fm[i], fv[i]);
+        welford_add(x[i], bg_n, bm[i], bv[i]);
+    }
 }
 
 // W = warps per chain (team).
@@ -150,6 +207,9 @@ __global__ void __launch_bounds__(W > 1 ? 32 * W : 32 * kNutsWarpChains, 1)
     const int seg_iters = P.seg_iters > 0 ? P.seg_iters : P.n_iter;
     const unsigned int n_seg = (unsigned int)((P.n_iter + seg_iters - 1) / seg_iters);
     const unsigned int n_units = n_seg * (unsigned int)P.C;
+#ifdef B200_PHASE_CLOCKS
+    long long ph_t = clock64();
+#endif
 
     // ---- work loop: one (chain, segment) unit per turn ---------------------------------------------------
     for (;;) {
@@ -242,6 +302,7 @@ __global__ void __launch_bounds__(W > 1 ? 32 * W : 32 * kNutsWarpChains, 1)
         rng.load(r.state_hi, r.state_lo, r.inc_hi, r.inc_lo);
     }
     team_sync<W>();
+    B200_PHASE(PH_SEGMENT);
 
     // QuadPotentialDiagAdaptExp.update with use_grads (quadpotential.py:531-579); sample = q_s, grad = g_s.  The four
     // Welford slots of the scratch hold (mean, var) of the draws and of the gradients.
@@ -282,9 +343,8 @@ __global__ void __launch_bounds__(W > 1 ? 32 * W : 32 * kNutsWarpChains, 1)
 
         // ---- start = integrator.compute_state(q0, p0)  (integration.py:68-75): the evaluation at q0 does not depend on
         //      p0, so it runs first ...
-        team_sync<W>();
-        const double logp0 = Model::template eval<NPL, W, true>(M, data_s, q_s, g_s, lane, red);
-        team_sync<W>();
+        const double logp0 = nuts_model_eval<Model, NPL, W>(M, data_s, q_s, g_s, lane, red);
+        B200_PHASE(PH_EVAL);
         ++n_grad;
         // ---- ... which lets QuadPotentialDiagAdaptExp.update(sample, grad) (quadpotential.py:531-567) of the PREVIOUS
         //      iteration run here, where the accepted position's gradient is at hand (the reference calls it at the end of
@@ -296,7 +356,7 @@ __global__ void __launch_bounds__(W > 1 ? 32 * W : 32 * kNutsWarpChains, 1)
 #pragma unroll
         for (int k = 0; k < NPL; ++k) {
             const int i = lane + TS * k;
-            const double zz = (i < n) ? momentum_z(P, chain, it, i) : 0.0;
+            const double zz = (i < n) ? momentum_z<true>(P, chain, it, i) : 0.0;
             p[k] = (1.0 / sqrt(VAR(k))) * zz;
         }
         double kin = 0.0;
@@ -309,6 +369,7 @@ __global__ void __launch_bounds__(W > 1 ? 32 * W : 32 * kNutsWarpChains, 1)
         }
         const double eps = ss.current(adapting);  // step_adapt.current (step_sizes.py:60-64)
         const int maxd = (tuning && it < 200) ? P.early_td : P.max_td;  // nuts.py:205-208
+        B200_PHASE(PH_ITER);
 
         double m_logw = 0.0, m_pe = E0, m_plogp = logp0;
         double m_s = 1.0;
@@ -337,9 +398,7 @@ __global__ void __launch_bounds__(W > 1 ? 32 * W : 32 * kNutsWarpChains, 1)
                     p[k] = fma(dt, g_s[i], p[k]);
                     q_s[i] = fma(es, VAR(k) * p[k], q_s[i]);
                 }
-                team_sync<W>();
-                logp = Model::template eval<NPL, W, true>(M, data_s, q_s, g_s, lane, red);
-                team_sync<W>();
+                logp = nuts_model_eval<Model, NPL, W>(M, data_s, q_s, g_s, lane, red);
                 double kk = 0.0;
 #pragma unroll
                 for (int k = 0; k < NPL; ++k) {
@@ -377,6 +436,7 @@ __global__ void __launch_bounds__(W > 1 ? 32 * W : 32 * kNutsWarpChains, 1)
             }
             int L_idx = 0, R_idx = 0;
             for (; d_iter < maxd; ++d_iter) {
+                B200_PHASE(PH_DOUBLING);  // the tree's start state, or the previous doubling's exit
                 const int dir = (rng.next_double() < 0.5) ? 1 : -1;  // nuts.py:215
                 // ---- load the edge we grow from into the integrator state; remember its p ----------------
                 const double* Eq = dir > 0 ? Rq : Lq;
@@ -399,6 +459,7 @@ __global__ void __launch_bounds__(W > 1 ? 32 * W : 32 * kNutsWarpChains, 1)
                 double c_s = 1.0;
                 int c_pidx = 0;
                 const int n_leaf = 1 << depth;
+                B200_PHASE(PH_DOUBLING);
                 for (int leaf = 0; leaf < n_leaf; ++leaf) {
                     // -- one leapfrog (integration.py:109-145)
     #pragma unroll
@@ -407,9 +468,9 @@ __global__ void __launch_bounds__(W > 1 ? 32 * W : 32 * kNutsWarpChains, 1)
                         p[k] = fma(dt, g_s[i], p[k]);
                         q_s[i] = fma(es, VAR(k) * p[k], q_s[i]);
                     }
-                    team_sync<W>();
-                    const double logp = Model::template eval<NPL, W, true>(M, data_s, q_s, g_s, lane, red);
-                    team_sync<W>();
+                    B200_PHASE(PH_LEAPFROG);
+                    const double logp = nuts_model_eval<Model, NPL, W>(M, data_s, q_s, g_s, lane, red);
+                    B200_PHASE(PH_EVAL);
                     double kk = 0.0;
     #pragma unroll
                     for (int k = 0; k < NPL; ++k) {
@@ -417,6 +478,7 @@ __global__ void __launch_bounds__(W > 1 ? 32 * W : 32 * kNutsWarpChains, 1)
                         p[k] = fma(dt, g_s[i], p[k]);
                         kk = fma(p[k], VAR(k) * p[k], kk);
                     }
+                    B200_PHASE(PH_LEAPFROG);
                     const double E = 0.5 * team_sum<W>(kk, lane, red) - logp;
                     w_idx += dir;
                     // -- _single_step bookkeeping (nuts.py:406-440)
@@ -438,6 +500,7 @@ __global__ void __launch_bounds__(W > 1 ? 32 * W : 32 * kNutsWarpChains, 1)
                     }
                     c_logw = -dE; c_pe = E; c_plogp = logp; c_pidx = w_idx;
                     c_s = 1.0;
+                    B200_PHASE(PH_ENERGY);
 
                     // -- merge with pending left siblings while the counter carries (nuts.py:452-476)
                     int h = 0;
@@ -498,6 +561,7 @@ __global__ void __launch_bounds__(W > 1 ? 32 * W : 32 * kNutsWarpChains, 1)
                         }
                         c_logw = fmax(c_logw, t_m);
                         c_s = ws;
+                        B200_PHASE(h == 0 ? PH_MERGE0 : PH_MERGE);
                         if (turn) {
                             sub_turn = true;
                             break;
@@ -532,6 +596,7 @@ __global__ void __launch_bounds__(W > 1 ? 32 * W : 32 * kNutsWarpChains, 1)
                             sc_s[h] = c_s;
                         }
                         team_sync<W>();
+                        B200_PHASE(PH_PARK);
                     }
                 }
                 ++depth;  // nuts.py:365 (counts the aborted doubling too)
@@ -598,6 +663,7 @@ __global__ void __launch_bounds__(W > 1 ? 32 * W : 32 * kNutsWarpChains, 1)
                 }
             }
         }
+        B200_PHASE(PH_DOUBLING);  // the last doubling's exit (HMC: its trajectory)
         if (d_iter == maxd) hit_max = !tuning;  // for/else of nuts.py:220-221
         n_grad += n_prop;  // one gradient per leapfrog
 
@@ -619,12 +685,7 @@ __global__ void __launch_bounds__(W > 1 ? 32 * W : 32 * kNutsWarpChains, 1)
             if (dw.add_sample(P.discard)) {
                 double* fm = gvec(dw.fg_m); double* fv = gvec(dw.fg_v);
                 double* bm = gvec(dw.bg_m); double* bv = gvec(dw.bg_v);
-#pragma unroll
-                for (int k = 0; k < NPL; ++k) {
-                    const int i = lane + TS * k;
-                    welford_add(PQ(k), dw.fg_n, fm[i], fv[i]);
-                    welford_add(PQ(k), dw.bg_n, bm[i], bv[i]);
-                }
+                welford_add_team<TS, NPL>(q_s, dw.fg_n, dw.bg_n, fm, fv, bm, bv, lane);  // q_s holds the draw
             }
             if (dw.var_ready()) {
                 const double* fv = gvec(dw.fg_v);
@@ -650,6 +711,7 @@ __global__ void __launch_bounds__(W > 1 ? 32 * W : 32 * kNutsWarpChains, 1)
                               (P.sampler == B200_SAMPLER_HMC) ? max_de : m_pe - E0, max_de, m_plogp);
         (void)turned;
         team_sync<W>();
+        B200_PHASE(PH_ITER);
     }
 
     if (bad_at >= 0) freeze_outputs<TS>(P, chain, max(bad_at, it_begin), it_end, rec_lo, T_out, lane);
@@ -686,9 +748,7 @@ __global__ void __launch_bounds__(W > 1 ? 32 * W : 32 * kNutsWarpChains, 1)
         if (P.mass_kind == B200_MASS_DIAG_ADAPT_GRAD && it_hi >= P.tune + P.draws && P.draws == 0 && bad_at < 0 && P.sm.final_var &&
             !P.save.log_step) {
             // the update that follows the last tuning iteration needs that position's gradient: one more evaluation
-            team_sync<W>();
-            (void)Model::template eval<NPL, W, true>(M, data_s, q_s, g_s, lane, red);
-            team_sync<W>();
+            (void)nuts_model_eval<Model, NPL, W>(M, data_s, q_s, g_s, lane, red);
             grad_mass_update(gvec(G_FGM), gvec(G_FGV), gvec(G_BGM), gvec(G_BGV));
         }
         if (P.sm.final_var) {
@@ -710,10 +770,12 @@ __global__ void __launch_bounds__(W > 1 ? 32 * W : 32 * kNutsWarpChains, 1)
         team_sync<W>();
         if (lane == 0) st_release_i32(P.done + chain, seg + 1);
     }
+    B200_PHASE(PH_SEGMENT);
     }  // work loop
 }
 
 #undef VAR
+#undef B200_PHASE
 
 // ---------------------------------------------------------------------------------------------------
 // Batched logp + gradient: one warp per point.  Replaces ValueGradFunction._pytensor_function

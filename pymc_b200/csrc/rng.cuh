@@ -64,4 +64,10 @@ __device__ __forceinline__ double philox_normal(uint64_t key, uint32_t chain, ui
     return sqrt(-2.0 * log(u1)) * c;
 }
 
+// The same draw from one out-of-line copy: a caller that unrolls its element loop holds the Philox rounds, log, sincospi
+// and sqrt once instead of once per element.
+__device__ __noinline__ double philox_normal_call(uint64_t key, uint32_t chain, uint32_t draw, uint32_t elem) {
+    return philox_normal(key, chain, draw, elem);
+}
+
 }  // namespace b200

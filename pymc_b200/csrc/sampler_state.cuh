@@ -152,10 +152,13 @@ __device__ __forceinline__ void record_chain_summary(const b200_chain_summary& s
 // Standard-normal momentum noise of (chain, iteration `it`, element i): the caller's buffer z, which holds the n_iter
 // iterations this call runs, or the counter-based Philox stream.  The lock-step engine always runs whole schedules
 // (it0 = 0, n_iter = tune + draws: b200_nuts_run refuses anything else), so both engines index z by `it - it0`.
+// OUT_OF_LINE: the Philox draw from its one out-of-line copy, for a caller that unrolls its element loop.
+template <bool OUT_OF_LINE = false>
 __device__ __forceinline__ double momentum_z(const RunCfg& P, int chain, int it, int i) {
     return (P.momentum_source == B200_MOMENTUM_HOST_BUFFER)
                ? P.z[((long long)chain * P.n_iter + (it - P.it0)) * P.n + i]
-               : philox_normal(P.philox_seed, (uint32_t)(chain + P.chain_offset), (uint32_t)it, (uint32_t)i);
+           : OUT_OF_LINE ? philox_normal_call(P.philox_seed, (uint32_t)(chain + P.chain_offset), (uint32_t)it, (uint32_t)i)
+                         : philox_normal(P.philox_seed, (uint32_t)(chain + P.chain_offset), (uint32_t)it, (uint32_t)i);
 }
 
 // Merge of two multinomial log-weights a (the subtree just built) and b as the lock-step engine carries them:

@@ -72,6 +72,11 @@ extern "C" {
  * studentt); ORDERED_POSITIVE also counts as positive support. */
 #define B200_IR_T_ORDERED 3
 #define B200_IR_T_ORDERED_POSITIVE 4
+/* Simplex (transforms.py:1091-1116): a variable of size K - 1 whose constrained value is the K weights
+ * w = softmax([z, -sum z]); log|J| = log K + sum_k log w_k.  It carries exactly one prior, a DIRICHLET of length K, and is
+ * used only as the weights of a NORMAL_MIXTURE / POISSON_MIXTURE (never as a parameter, a term factor, cutpoints, psi, an
+ * AR(1) variable or a latent factor).  The draws of a model with such a variable are constrained on the host. */
+#define B200_IR_T_SIMPLEX 5
 /* prior densities (pymc/distributions/continuous.py): parameters in p[0..2] */
 #define B200_IR_P_FLAT 0        /*                       :364-419   */
 #define B200_IR_P_NORMAL 1      /* mu, sigma             :526-527   */
@@ -84,6 +89,8 @@ extern "C" {
 #define B200_IR_P_GAMMA 8       /* alpha, beta (const)   :2512-2515 */
 #define B200_IR_P_BETA 9        /* alpha, beta (const)   :1250-1256 */
 #define B200_IR_P_LOGNORMAL 10  /* mu, sigma             :1807-1814 */
+#define B200_IR_P_DIRICHLET 11  /* a (const), the concentration of every one of the K components; only on a SIMPLEX
+                                 * variable of size K - 1    multivariate.py:557-585 */
 /* likelihoods of a linear predictor eta_i = sum_t coef_t[i] * prod_f x_f[idx_f[i]] */
 #define B200_IR_L_NORMAL 0          /* y ~ Normal(eta, sigma)                    continuous.py:526-527  */
 #define B200_IR_L_BERNOULLI_LOGIT 1 /* y ~ Bernoulli(logit_p = eta)              discrete.py:362-367    */
@@ -148,6 +155,21 @@ extern "C" {
 #define B200_IR_L_CENSORED_LOGNORMAL 21     /* pm.Censored(pm.LogNormal.dist(...))                            */
 #define B200_IR_L_TRUNCATED_WEIBULL_LOG 22  /* pm.Truncated(pm.Weibull.dist(...)) truncated.py                */
 #define B200_IR_L_TRUNCATED_LOGNORMAL 23    /* pm.Truncated(pm.LogNormal.dist(...))                           */
+/* Finite mixtures of K >= 2 components: log p(y_i) = logsumexp_k(log w_k + log f_k(y_i))  (mixture.py:469-494)
+ *   NORMAL_MIXTURE     f_k = Normal(eta_i + mu_k, sigma_k); y finite
+ *   POISSON_MIXTURE    f_k = Poisson(lam_k exp(eta_i)); y integers >= 0
+ *   nu             K
+ *   n_terms        the predictor's terms, which may be none (eta = 0)
+ *   terms[n_terms]     the weights: one unindexed factor on a SIMPLEX variable of size K - 1, or n_factors = 0 and coef = K
+ *                      constants, finite, >= 0, summing to 1 (a zero weight drops its component)
+ *   terms[n_terms + 1] the components mu_k (Normal) / lam_k (Poisson): one unindexed factor on a variable of size K (Normal:
+ *                      no transform or ORDERED; Poisson: positive support), or n_factors = 0 and coef = K constants (finite;
+ *                      Poisson: > 0)
+ *   terms[n_terms + 2] NORMAL_MIXTURE only, sigma_k: one unindexed factor on a variable of size 1 or K with positive support,
+ *                      or n_factors = 0 and coef = K constants > 0
+ *   sigma_kind NONE, y_var 0. */
+#define B200_IR_L_NORMAL_MIXTURE 24         /* pm.NormalMixture mixture.py:529-546                            */
+#define B200_IR_L_POISSON_MIXTURE 25        /* pm.Mixture(w, pm.Poisson.dist(lam, shape=K))                   */
 /* The support rule b200_model_create enforces (as ModelIR.validate does): HalfNormal, HalfCauchy, Exponential, Gamma and
  * LogNormal priors sit on a LOG variable or an INTERVAL with lo >= 0, Beta on an INTERVAL inside [0, 1], Uniform(a, b) on an
  * INTERVAL inside [a, b]; every scale (a prior's sigma / beta / lam, Normal and StudentT sigma including each sigma_obs, an

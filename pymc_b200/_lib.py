@@ -116,8 +116,8 @@ def build_ir(low):
             pri[k].p[a] = param(pars[a])
     liks = (IrLik * max(1, len(low.liks)))()
     for k, L in enumerate(low.liks):
-        # an ordinal likelihood's cutpoint term, or a zero-inflated / hurdle likelihood's psi block, goes last
-        all_terms = L["terms"] + ([L["cut"]] if "cut" in L else []) + L.get("psi", [])
+        # an ordinal likelihood's cutpoint term, a zero-inflated / hurdle likelihood's psi block or a mixture's blocks go last
+        all_terms = L["terms"] + ([L["cut"]] if "cut" in L else []) + L.get("psi", []) + L.get("mix", [])
         terms = (IrTerm * len(all_terms))()
         for t, T in enumerate(all_terms):
             terms[t].coef = addr(T["coef"])

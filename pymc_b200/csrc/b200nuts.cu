@@ -494,6 +494,18 @@ static bool ir_scale_ok(const b200_ir_param& p, const std::vector<IrVarD>& vars)
 #define B200_IR_ZIB_Y "y must be integers with 0 <= y <= trials"
 #define B200_IR_HG_Y "y must be finite and >= 0"
 #define B200_IR_ZIP_SLOT "zero_inflated_poisson and hurdle_poisson take no sigma, trials or alpha"
+// Simplex variables, Dirichlet priors and mixture observations (ModelIR.validate, same wording)
+#define B200_IR_SIMPLEX_USE "a simplex variable may be used only as a mixture's weights"
+#define B200_IR_SIMPLEX_PRIOR "a simplex variable carries exactly one prior, a dirichlet of length K = size + 1"
+#define B200_IR_DIRICHLET_VAR "a dirichlet prior is only allowed on a simplex variable"
+#define B200_IR_DIRICHLET_A "a dirichlet's a must be one finite constant > 0 (K equal constants lower to it)"
+#define B200_IR_MIX_K "a mixture needs K >= 2 components; with K = 1, write the plain likelihood (normal or poisson_log)"
+#define B200_IR_MIX_Y_NORMAL "y must be finite"
+#define B200_IR_MIX_WEIGHTS "the weights must be a simplex variable of size K - 1 or K finite constants >= 0 that sum to 1"
+#define B200_IR_MIX_MU "mu must be a variable of size K with no transform or an ordered one, or K finite constants"
+#define B200_IR_MIX_LAM "lam must be a variable of size K with positive support (log, ordered_positive, or an interval with lo >= 0), or K finite constants > 0"
+#define B200_IR_MIX_SIGMA "sigma must be a finite constant > 0, K of them, or a variable of size 1 or K with positive support"
+#define B200_IR_MIX_SLOTS "a mixture takes no alpha, trials, lower / upper, cutpoints or psi, and poisson_mixture no sigma"
 static constexpr double LOG_PI = 1.1447298858494001741, LOG_2 = 0.69314718055994530942;
 
 // The pass over a b200_ir.  Its steps return 0 or fail(...); the arrays they record in `sg` stay put until the upload.
@@ -506,8 +518,11 @@ struct IrPass {
     std::deque<std::vector<double>> reals;  // Xt, the distinct-count tables
     std::deque<std::vector<signed char>> codes;  // the censoring codes
     // the largest N of any likelihood / of an ordinal one (its w row) / of a logit psi (its zeta row)
-    long long max_obs = 0, ord_obs = 0, zeta_obs = 0;
+    // and twice that of a mixture (its lse and eta rows)
+    long long max_obs = 0, ord_obs = 0, zeta_obs = 0, mix_obs = 0;
     bool has_design = false;
+    int simplex_rows = 0;  // doubles of the simplex variables' (log w, G) rows, after x in the team slice
+    std::vector<int> n_priors_of;  // priors on each variable
     template <class T> void add(const T** dst, const T* host, size_t count) { sg.add(dst, host, count, Staging::IN); }
 };
 
@@ -515,6 +530,16 @@ static const IrVarD* ir_var_at(const std::vector<IrVarD>& vars, int offset) {
     for (const IrVarD& V : vars)
         if (V.offset == offset) return &V;
     return nullptr;
+}
+
+// does q[offset .. offset + size) touch a simplex variable (whose only use is a mixture's weights)?
+static bool ir_touches_simplex(const std::vector<IrVarD>& vars, int offset, int size) {
+    for (const IrVarD& V : vars)
+        if (V.transform == IRT_SIMPLEX && offset < V.offset + V.size && V.offset < offset + size) return true;
+    return false;
+}
+static bool ir_ref_simplex(const std::vector<IrVarD>& vars, const b200_ir_param& p) {
+    return p.kind == 1 && ir_touches_simplex(vars, p.ref, 1);
 }
 
 // CSR transpose of key[0 .. N) in [0, K): rowobs[rowptr[k] .. rowptr[k + 1]) are the i with key[i] = k, ascending
@@ -536,21 +561,39 @@ static int ir_vars(IrPass& c, const b200_ir& R) {
     for (int v = 0; v < R.n_vars; ++v) {
         const b200_ir_var& V = R.vars[v];
         if (V.offset != off || V.size <= 0) return fail("ir: variable %d: offsets must be contiguous in registration order", v);
-        if (V.transform < B200_IR_T_NONE || V.transform > B200_IR_T_ORDERED_POSITIVE) return fail("ir: variable %d: transform %d", v, V.transform);
+        if (V.transform < B200_IR_T_NONE || V.transform > B200_IR_T_SIMPLEX) return fail("ir: variable %d: transform %d", v, V.transform);
         if (V.transform == B200_IR_T_INTERVAL && !(V.lo < V.hi)) return fail("ir: variable %d: interval needs lo < hi", v);
-        c.vars.push_back(IrVarD{V.offset, V.size, V.transform, 0, V.lo, V.hi});
+        int rows = 0;  // a simplex variable's rows: log w and G, K = size + 1 each, after x (padded) in the team slice
+        if (V.transform == B200_IR_T_SIMPLEX) {
+            rows = ((c.n + 3) & ~3) + c.simplex_rows;
+            c.simplex_rows += (2 * (V.size + 1) + 3) & ~3;
+        }
+        c.vars.push_back(IrVarD{V.offset, V.size, V.transform, rows, V.lo, V.hi});
         off += V.size;
     }
     if (off != c.n) return fail("ir: variables cover %d elements but n = %d", off, c.n);
+    c.n_priors_of.assign(c.vars.size(), 0);
     return 0;
 }
 
-static int ir_prior(const IrPass& c, const b200_ir_prior& F, int k, IrPriorD& P) {
+static int ir_prior(IrPass& c, const b200_ir_prior& F, int k, IrPriorD& P) {
     if (F.var < 0 || F.var >= (int)c.vars.size()) return fail("ir: prior %d: variable index %d", k, F.var);
     const IrVarD& PV = c.vars[F.var];
     P.dist = F.dist; P.offset = PV.offset; P.size = PV.size;
     for (int a = 0; a < 3; ++a)
         if (ir_param(F.p[a], c.n, &P.p[a], "prior")) return -1;
+    for (int a = 0; a < 3; ++a)
+        if (ir_ref_simplex(c.vars, F.p[a])) return fail("ir: prior %d: " B200_IR_SIMPLEX_USE, k);
+    if (PV.transform == IRT_SIMPLEX && (F.dist != B200_IR_P_DIRICHLET || ++c.n_priors_of[F.var] > 1))
+        return fail("ir: prior %d: " B200_IR_SIMPLEX_PRIOR, k);
+    if (F.dist == B200_IR_P_DIRICHLET) {  // c0 = lgamma(K a) - K lgamma(a) (multivariate.py:557-585); pad: the rows
+        if (PV.transform != IRT_SIMPLEX) return fail("ir: prior %d: " B200_IR_DIRICHLET_VAR, k);
+        const double a = F.p[0].value, K = PV.size + 1.0;
+        if (F.p[0].kind != 0 || !(std::isfinite(a) && a > 0)) return fail("ir: prior %d: " B200_IR_DIRICHLET_A, k);
+        P.c0 = std::lgamma(K * a) - K * std::lgamma(a);
+        P.pad = PV.pad;
+        return 0;
+    }
     auto cst = [&](int a) { return F.p[a].kind == 0; };
     int scale = -1;  // which parameter is the prior's scale
     switch (F.dist) {
@@ -757,6 +800,7 @@ static int ir_terms(IrPass& c, const b200_ir_lik& L, int l, int t0, int t1) {
             if (K < 0 || T.f[0].size != K || !T.coef)
                 return fail("ir: likelihood %d term %d: X must have shape (N, size of the variable)", l, t);
             if (T.f[0].offset < 0 || T.f[0].offset + K > c.n) return fail("ir: likelihood %d term %d: factor slice outside q", l, t);
+            if (ir_touches_simplex(c.vars, T.f[0].offset, K)) return fail("ir: likelihood %d term %d: " B200_IR_SIMPLEX_USE, l, t);
             std::vector<double>& xt = c.reals.emplace_back((size_t)N * K);
             for (long long i = 0; i < N; ++i)
                 for (int k = 0; k < K; ++k) {
@@ -775,6 +819,7 @@ static int ir_terms(IrPass& c, const b200_ir_lik& L, int l, int t0, int t1) {
         for (int f = 0; f < T.n_factors; ++f) {
             const b200_ir_factor& F = T.f[f];
             if (F.offset < 0 || F.size <= 0 || F.offset + F.size > c.n) return fail("ir: likelihood %d term %d: factor slice outside q", l, t);
+            if (ir_touches_simplex(c.vars, F.offset, F.size)) return fail("ir: likelihood %d term %d: " B200_IR_SIMPLEX_USE, l, t);
             IrFactorD& FD = TD.f[f];
             FD.offset = F.offset; FD.size = F.size;
             if (F.idx) {
@@ -808,6 +853,7 @@ static int ir_psi(IrPass& c, const b200_ir_lik& L, int l) {
     } else {
         const b200_ir_factor& F = T.f[0];
         const IrVarD* V = ir_var_at(c.vars, F.offset);
+        if (ir_touches_simplex(c.vars, F.offset, std::max(F.size, 1))) return fail("ir: likelihood %d: " B200_IR_SIMPLEX_USE, l);
         if (F.idx || !V || V->size != 1 || F.size != 1 || V->transform != IRT_INTERVAL || !(V->lo >= 0.0 && V->hi <= 1.0))
             return fail("ir: likelihood %d: " B200_IR_PSI_VAR, l);
         TD.n_factors = 1;
@@ -826,6 +872,7 @@ static int ir_cutpoints(IrPass& c, const b200_ir_lik& L, int l) {
     if (T.n_factors == 1) {
         const b200_ir_factor& F = T.f[0];
         const IrVarD* V = ir_var_at(c.vars, F.offset);
+        if (ir_touches_simplex(c.vars, F.offset, std::max(F.size, 1))) return fail("ir: likelihood %d: " B200_IR_SIMPLEX_USE, l);
         if (F.idx || !V || V->size != F.size) return fail("ir: likelihood %d: the cutpoint factor must be a whole variable, unindexed", l);
         if (F.size != K - 1) return fail("ir: likelihood %d: " B200_IR_CUT_SIZE " (%d, K = %d)", l, F.size, K);
         if (F.size > 1 && V->transform != IRT_ORDERED && V->transform != IRT_ORDERED_POSITIVE)
@@ -843,6 +890,63 @@ static int ir_cutpoints(IrPass& c, const b200_ir_lik& L, int l) {
     return 0;
 }
 
+// normal_mixture / poisson_mixture: nu = K, the slots, y and the constants -log(2 pi) / 2 or -lgamma(y + 1) (c0)
+static int ir_mixture_obs(IrPass& c, const b200_ir_lik& L, int l, IrLikD& D) {
+    const bool normal = L.dist == B200_IR_L_NORMAL_MIXTURE;
+    if (!(L.nu >= 2 && L.nu == std::floor(L.nu) && L.nu <= 0x7fffffff)) return fail("ir: likelihood %d: " B200_IR_MIX_K, l);
+    if (L.sigma_kind != B200_IR_S_NONE || L.y_var != 0) return fail("ir: likelihood %d: " B200_IR_MIX_SLOTS, l);
+    double c0 = 0.0;
+    for (long long i = 0; i < L.N; ++i) {
+        const double y = L.y[i];
+        if (normal && !std::isfinite(y)) return fail("ir: likelihood %d: " B200_IR_MIX_Y_NORMAL " (at %lld)", l, i);
+        if (!normal && !(y >= 0 && y == std::floor(y) && !std::isinf(y))) return fail("ir: likelihood %d: " B200_IR_ZI_Y " (at %lld)", l, i);
+        c0 -= normal ? B200_HALF_LOG_2PI : std::lgamma(y + 1.0);
+    }
+    D.c0 = c0;
+    c.mix_obs = std::max(c.mix_obs, 2 * (long long)L.N);  // its rows: lse_i and eta_i
+    return 0;
+}
+
+// The weights, component and (Normal) sigma blocks at terms[n_terms ..].  A simplex weights factor's device offset is its
+// rows (log w, G); constant weights go up as their logs (-inf for a zero weight), a constant sigma as K values.
+static int ir_mixture_blocks(IrPass& c, const b200_ir_lik& L, int l) {
+    const bool normal = L.dist == B200_IR_L_NORMAL_MIXTURE;
+    const int K = (int)L.nu;
+    for (int b = 0; b < (normal ? 3 : 2); ++b) {
+        const b200_ir_term& T = L.terms[L.n_terms + b];
+        const char* what = b == 0 ? B200_IR_MIX_WEIGHTS : (b == 2 ? B200_IR_MIX_SIGMA : (normal ? B200_IR_MIX_MU : B200_IR_MIX_LAM));
+        if (T.n_cols != 0 || T.n_factors < 0 || T.n_factors > 1 || (T.n_factors == 0) != (T.coef != nullptr))
+            return fail("ir: likelihood %d: %s", l, what);
+        IrTermD& TD = c.terms.emplace_back();
+        if (T.n_factors == 1) {
+            const b200_ir_factor& F = T.f[0];
+            const IrVarD* V = ir_var_at(c.vars, F.offset);
+            const bool whole = V && !F.idx && F.size == V->size;
+            if (b != 0 && whole && V->transform == IRT_SIMPLEX) return fail("ir: likelihood %d: " B200_IR_SIMPLEX_USE, l);
+            const bool ok = whole && (b == 0   ? V->transform == IRT_SIMPLEX && V->size == K - 1
+                                      : b == 2 ? (V->size == 1 || V->size == K) && ir_positive_support(*V)
+                                      : normal ? V->size == K && (V->transform == IRT_NONE || V->transform == IRT_ORDERED)
+                                               : V->size == K && ir_positive_support(*V));
+            if (!ok) return fail("ir: likelihood %d: %s", l, what);
+            TD.n_factors = 1;
+            TD.f[0] = IrFactorD{b == 0 ? V->pad : F.offset, F.size, nullptr, nullptr, nullptr};
+            continue;
+        }
+        std::vector<double>& v = c.reals.emplace_back(T.coef, T.coef + K);
+        double sum = 0.0;
+        for (int k = 0; k < K; ++k) {
+            const double a = v[k];
+            const bool ok = b == 0 ? std::isfinite(a) && a >= 0 : std::isfinite(a) && (b == 1 && normal ? true : a > 0);
+            if (!ok) return fail("ir: likelihood %d: %s (at %d)", l, what, k);
+            sum += a;
+            if (b == 0) v[k] = std::log(a);
+        }
+        if (b == 0 && !(std::fabs(sum - 1.0) <= 1e-8 + 1e-5)) return fail("ir: likelihood %d: %s", l, what);  // np.isclose
+        c.add(&TD.coef, v.data(), v.size());
+    }
+    return 0;
+}
+
 static int ir_lik(IrPass& c, const b200_ir_lik& L, int l, IrLikD& D) {
     const int n_vars = (int)c.vars.size();
     // y_var = v + 1: a latent factor, a Normal / StudentT prior on variable v with a linear-predictor location
@@ -852,8 +956,10 @@ static int ir_lik(IrPass& c, const b200_ir_lik& L, int l, IrLikD& D) {
         return fail("ir: likelihood %d: a latent factor (y_var > 0) is a normal or studentt prior with a Linear location; dist %d is neither", l, L.dist);
     if (latent && L.N != c.vars[L.y_var - 1].size)
         return fail("ir: likelihood %d: a latent factor's N (%lld) must equal the size of its variable (%d)", l, (long long)L.N, c.vars[L.y_var - 1].size);
+    if (latent && c.vars[L.y_var - 1].transform == IRT_SIMPLEX) return fail("ir: likelihood %d: " B200_IR_SIMPLEX_USE, l);
     if (L.N <= 0 || L.N > 0x7fffffff || (!latent && !L.y)) return fail("ir: likelihood %d: missing observations", l);
-    if (L.n_terms <= 0 || !L.terms) return fail("ir: likelihood %d: no linear-predictor terms", l);
+    const bool mixture = L.dist == B200_IR_L_NORMAL_MIXTURE || L.dist == B200_IR_L_POISSON_MIXTURE;  // eta may be 0
+    if (L.n_terms < (mixture ? 0 : 1) || !L.terms) return fail("ir: likelihood %d: no linear-predictor terms", l);
     const long long N = L.N;
     c.max_obs = std::max(c.max_obs, N);
     D.dist = L.dist; D.n_terms = L.n_terms; D.term0 = (int)c.terms.size(); D.sigma_kind = L.sigma_kind; D.N = N; D.nu = L.nu;
@@ -862,6 +968,7 @@ static int ir_lik(IrPass& c, const b200_ir_lik& L, int l, IrLikD& D) {
     if (!latent && !survival) c.add(&D.y, L.y, (size_t)N);  // a survival likelihood's device y is log y (ir_survival)
     if (ir_param(L.sigma, c.n, &D.sigma, "likelihood sigma")) return -1;
     if (L.sigma_kind == B200_IR_S_REF && L.sigma.kind != 1) return fail("ir: likelihood %d: sigma_kind REF needs a reference", l);
+    if (L.sigma_kind == B200_IR_S_REF && ir_ref_simplex(c.vars, L.sigma)) return fail("ir: likelihood %d: " B200_IR_SIMPLEX_USE, l);
     b200_ir_param slot = L.sigma;  // the parameter slot as the device reads it: x[ref] for REF, else the value
     slot.kind = L.sigma_kind == B200_IR_S_REF ? 1 : 0;
     if (L.sigma_kind == B200_IR_S_OBS) {
@@ -899,6 +1006,7 @@ static int ir_lik(IrPass& c, const b200_ir_lik& L, int l, IrLikD& D) {
             if (fam == B200_IR_L_POISSON_LOG && L.sigma_kind != B200_IR_S_NONE) return fail("ir: likelihood %d: " B200_IR_ZIP_SLOT, l);
             rc = ir_family(c, L, l, slot, fam, fam == B200_IR_L_GAMMA_LOG ? B200_IR_HG_Y : B200_IR_ZI_Y, true, D);
         } break;
+        case B200_IR_L_NORMAL_MIXTURE: case B200_IR_L_POISSON_MIXTURE: rc = ir_mixture_obs(c, L, l, D); break;
         default: return fail("ir: likelihood %d: density %d is not in the closed set", l, L.dist);
     }
     if (rc) return rc;
@@ -915,12 +1023,15 @@ static int ir_lik(IrPass& c, const b200_ir_lik& L, int l, IrLikD& D) {
         return fail("ir: likelihood %d: sigma " B200_IR_SCALE_RULE, l);
     }
     if (ir_terms(c, L, l, 0, L.n_terms)) return -1;
+    if (mixture) return ir_mixture_blocks(c, L, l);
     if (L.dist == B200_IR_L_ORDERED_LOGISTIC || L.dist == B200_IR_L_ORDERED_PROBIT) return ir_cutpoints(c, L, l);
     return L.dist >= B200_IR_L_ZERO_INFLATED_POISSON && L.dist <= B200_IR_L_HURDLE_GAMMA ? ir_psi(c, L, l) : 0;
 }
 
 static int ir_ar1(const IrPass& c, const b200_ir_ar1& A, int k, IrAr1D& D) {
     if (A.var < 0 || A.var >= (int)c.vars.size() || c.vars[A.var].size < 2) return fail("ir: ar1 %d: bad variable", k);
+    if (c.vars[A.var].transform == IRT_SIMPLEX || ir_ref_simplex(c.vars, A.phi) || ir_ref_simplex(c.vars, A.sigma))
+        return fail("ir: ar1 %d: " B200_IR_SIMPLEX_USE, k);
     if (!(A.init_sigma > 0)) return fail("ir: ar1 %d: init_sigma must be > 0", k);
     D.offset = c.vars[A.var].offset; D.size = c.vars[A.var].size; D.init_sigma = A.init_sigma;
     if (ir_param(A.phi, c.n, &D.phi, "ar1 phi") || ir_param(A.sigma, c.n, &D.sigma, "ar1 sigma")) return -1;
@@ -937,6 +1048,8 @@ static int prepare_ir(b200_model* m, const b200_model_desc* d) {
     std::vector<IrPriorD> priors(std::max(R->n_priors, 0));
     for (int k = 0; k < R->n_priors; ++k)
         if (ir_prior(c, R->priors[k], k, priors[k])) return -1;
+    for (size_t v = 0; v < c.vars.size(); ++v)
+        if (c.vars[v].transform == IRT_SIMPLEX && c.n_priors_of[v] != 1) return fail("ir: variable %d: " B200_IR_SIMPLEX_PRIOR, (int)v);
     m->ir_liks.assign(std::max(R->n_liks, 0), IrLikD{});  // filled in place: sg holds the addresses of their pointers
     for (int l = 0; l < R->n_liks; ++l)
         if (ir_lik(c, R->liks[l], l, m->ir_liks[l])) return -1;
@@ -951,8 +1064,9 @@ static int prepare_ir(b200_model* m, const b200_model_desc* d) {
     if (upload(m, c.vars, &P.vars) || upload(m, priors, &P.priors) || upload(m, m->ir_liks, &P.liks) || upload(m, terms, &P.terms) ||
         upload(m, ars, &P.ar1))
         return -1;
-    P.n_pad = (c.n + 3) & ~3;
-    const long long row2 = std::max(c.ord_obs, c.zeta_obs);  // likelihoods are evaluated one after another: they share the row
+    P.n_pad = ((c.n + 3) & ~3) + c.simplex_rows;  // x, then the simplex variables' rows
+    // likelihoods are evaluated one after another: they share the row
+    const long long row2 = std::max(std::max(c.ord_obs, c.zeta_obs), c.mix_obs);
     P.ord_row = row2 ? (int)(P.n_pad + ((c.max_obs + 3) & ~3LL)) : 0;  // after r, before the design partials
     P.stride = P.n_pad + ((c.max_obs + 3) & ~3LL) + ((row2 + 3) & ~3LL) + (c.has_design ? kIrPartDoubles : 0);
     m->ir_extended = std::any_of(c.vars.begin(), c.vars.end(), [](const IrVarD& V) { return V.transform >= IRT_ORDERED; }) ||

@@ -22,20 +22,21 @@
 
 namespace b200 {
 
-enum { IRT_NONE = 0, IRT_LOG = 1, IRT_INTERVAL = 2, IRT_ORDERED = 3, IRT_ORDERED_POSITIVE = 4 };
+enum { IRT_NONE = 0, IRT_LOG = 1, IRT_INTERVAL = 2, IRT_ORDERED = 3, IRT_ORDERED_POSITIVE = 4, IRT_SIMPLEX = 5 };
 enum { IRP_FLAT = 0, IRP_NORMAL, IRP_HALFNORMAL, IRP_CAUCHY, IRP_HALFCAUCHY, IRP_EXPONENTIAL, IRP_STUDENTT, IRP_UNIFORM,
-       IRP_GAMMA, IRP_BETA, IRP_LOGNORMAL };
+       IRP_GAMMA, IRP_BETA, IRP_LOGNORMAL, IRP_DIRICHLET };
 enum { IRL_NORMAL = 0, IRL_BERNOULLI_LOGIT, IRL_POISSON_LOG, IRL_STUDENTT, IRL_NORMAL_LOGVAR, IRL_BINOMIAL_LOGIT,
        IRL_NEGBINOMIAL_LOG, IRL_GAMMA_LOG, IRL_CENSORED_NORMAL, IRL_TRUNCATED_NORMAL, IRL_ORDERED_LOGISTIC,
        IRL_ORDERED_PROBIT, IRL_ZI_POISSON, IRL_ZI_BINOMIAL, IRL_ZI_NEGBINOMIAL, IRL_HURDLE_POISSON, IRL_HURDLE_NEGBINOMIAL,
        IRL_HURDLE_GAMMA, IRL_WEIBULL_LOG, IRL_LOGNORMAL, IRL_CENSORED_WEIBULL_LOG, IRL_CENSORED_LOGNORMAL,
-       IRL_TRUNCATED_WEIBULL_LOG, IRL_TRUNCATED_LOGNORMAL };
+       IRL_TRUNCATED_WEIBULL_LOG, IRL_TRUNCATED_LOGNORMAL, IRL_NORMAL_MIXTURE, IRL_POISSON_MIXTURE };
 enum { IRS_NONE = 0, IRS_CONST, IRS_REF, IRS_OBS };
 constexpr double kNegBinPoissonAlpha = 1e10;  // above: NegativeBinomial -> Poisson(mu) limit (discrete.py:727-735)
 
 struct IrParamD { int kind, ref; double value; };                     // kind 0: constant; 1: x[ref] (a scalar variable)
-struct IrVarD { int offset, size, transform, pad; double lo, hi; };
+struct IrVarD { int offset, size, transform, pad; double lo, hi; };  // pad: a simplex variable's rows (below)
 struct IrPriorD { int dist, offset, size, pad; IrParamD p[3]; double c0; };      // c0: per-element constant of the density
+                                                                                 // (dirichlet: of the whole vector; pad: the rows)
 struct IrFactorD { int offset, size; const int* idx; const int* rowptr; const int* rowobs; };  // CSR: element -> observations
 // n_cols > 0: a design term, eta_i += sum_k X[i][k] x[f[0].offset + k], with coef = X row-major [N][n_cols] (the gradient
 // reads it) and xt = X column-major [n_cols][N] (the forward pass reads it: consecutive threads take consecutive rows).
@@ -554,6 +555,158 @@ __device__ __noinline__ void ir_ordered_chain(const IrVarD* Vp, const double* q,
     }
 }
 
+// ---- the simplex transform (transforms.py:1091-1116): a variable of size K - 1, w = softmax([z, -sum z]).  Its K weights
+// never live at the variable's offset of x: V.pad is the offset in the team slice of two rows of K, lw = log w_k and
+// G = d logp / d log w_k, which the Dirichlet prior and the mixture passes read and add to.  The forward pass forms
+// log w_k = z_k - lse(z), finite where w_k underflows; log|J| = log K + sum_k log w_k (the reference's log_jac_det), whose
+// d / d log w_k = 1 starts G.  One thread, k ascending, like the ordered transform.
+__device__ __noinline__ double ir_simplex_forward(const IrVarD* Vp, const double* q, double* x) {
+    const int o = Vp->offset, K = Vp->size + 1;
+    double* lw = x + Vp->pad;
+    double* G = lw + K;
+    double zs = 0.0, m = -INFINITY;
+    for (int k = 0; k < K - 1; ++k) {
+        zs += q[o + k];
+        m = fmax(m, q[o + k]);
+    }
+    m = fmax(m, -zs);
+    double s = 0.0;
+    for (int k = 0; k < K; ++k) s += exp((k < K - 1 ? q[o + k] : -zs) - m);
+    const double lse = m + log(s);
+    double lj = log((double)K);
+    for (int k = 0; k < K; ++k) {
+        lw[k] = (k < K - 1 ? q[o + k] : -zs) - lse;
+        lj += lw[k];
+        G[k] = 1.0;
+    }
+    return lj;
+}
+
+// The Dirichlet prior of a simplex variable (multivariate.py:557-585): c0 + (a - 1) sum_k log w_k, with d / d log w_k = a - 1
+// added to G.  One thread, k ascending.
+__device__ __noinline__ double ir_dirichlet(const IrPriorD* Fp, double* x) {
+    const int K = Fp->size + 1;
+    const double am1 = Fp->p[0].value - 1.0;
+    double* lw = x + Fp->pad;
+    double s = 0.0;
+    for (int j = 0; j < K; ++j) {
+        s += lw[j];
+        lw[K + j] += am1;
+    }
+    return fma(am1, s, Fp->c0);
+}
+
+// The chain rule through it: d/dz_j = (G_j - w_j S) - (G_K - w_K S), S = sum_k G_k, with no division by any w.
+__device__ __noinline__ void ir_simplex_chain(const IrVarD* Vp, const double* x, double* g) {
+    const int o = Vp->offset, K = Vp->size + 1;
+    const double* lw = x + Vp->pad;
+    const double* G = lw + K;
+    double S = 0.0;
+    for (int k = 0; k < K; ++k) S += G[k];
+    const double last = G[K - 1] - exp(lw[K - 1]) * S;
+    for (int j = 0; j < K - 1; ++j) g[o + j] = (G[j] - exp(lw[j]) * S) - last;
+}
+
+// ---- finite mixtures (mixture.py:469-494): log p(y_i) = lse_k(l_ik), l_ik = log w_k + log f_k(y_i), over K = L.nu
+// components, with the weights, component and (Normal) sigma blocks at terms[term0 + n_terms ..] (include/b200nuts.h).
+// f_k is Normal(eta + mu_k, sigma_k) or Poisson(lam_k e^eta), less the constants -log(2 pi) / 2 and -lgamma(y + 1) (in c0:
+// they leave the lse unchanged).  The block pointers: lw (x + the simplex row, or the host-logged constants), G (null for
+// constant weights), the components c and sigma s with their gradient targets (null for constants).
+struct IrMix { const double* lw; double* G; const double* c; double* gc; const double* s; double* gs; bool s_vec; };
+__device__ __forceinline__ IrMix ir_mix_block(const IrLikD& L, const IrTermD* terms, const double* x, double* g) {
+    const IrTermD* b = terms + L.term0 + L.n_terms;
+    const int K = (int)L.nu;
+    IrMix M{b[0].n_factors ? x + b[0].f[0].offset : b[0].coef, b[0].n_factors ? (double*)x + b[0].f[0].offset + K : nullptr,
+            b[1].n_factors ? x + b[1].f[0].offset : b[1].coef, b[1].n_factors && g ? g + b[1].f[0].offset : nullptr,
+            nullptr, nullptr, true};
+    if (L.dist == IRL_NORMAL_MIXTURE) {
+        M.s = b[2].n_factors ? x + b[2].f[0].offset : b[2].coef;
+        M.gs = b[2].n_factors && g ? g + b[2].f[0].offset : nullptr;
+        M.s_vec = !b[2].n_factors || b[2].f[0].size > 1;
+    }
+    return M;
+}
+// log f_k(y) less its constant, with d / d eta (= d / d mu_k for the Normal), d / d lam_k or d / d sigma_k in dt.
+struct IrMixTerm { double lf, de, dc, ds; };
+__device__ __forceinline__ IrMixTerm ir_mix_term(int dist, const IrMix& M, int k, double y, double eta) {
+    if (dist == IRL_NORMAL_MIXTURE) {
+        const double sg = M.s[M.s_vec ? k : 0], z = (y - eta - M.c[k]) / sg;
+        return {-0.5 * z * z - log(sg), z / sg, z / sg, (z * z - 1.0) / sg};
+    }
+    const double lam = M.c[k], mu = lam * exp(eta);
+    return {y * (log(lam) + eta) - mu, y - mu, (y - mu) / lam, 0.0};
+}
+// lse_i and r_i = sum_k rho_ik d log f_k / d eta with the max-shifted sum formed in one pass over k (the running maximum
+// rescales the partial sums); a term l = -inf (a component of weight 0, or a density that underflows to 0) is skipped, so
+// it adds nothing and no NaN, as logsumexp does.
+struct IrMixObs { double lse, r; };
+__device__ __forceinline__ IrMixObs ir_mix_obs(int dist, int K, const IrMix& M, double y, double eta) {
+    double m = -INFINITY, s = 0.0, rr = 0.0;
+    for (int k = 0; k < K; ++k) {
+        if (M.lw[k] == -INFINITY) continue;
+        const IrMixTerm t = ir_mix_term(dist, M, k, y, eta);
+        const double l = M.lw[k] + t.lf;
+        if (l == -INFINITY) continue;
+        if (l > m) {
+            const double c = exp(m - l);
+            s = fma(s, c, 1.0);
+            rr = fma(rr, c, t.de);
+            m = l;
+        } else {
+            const double e = exp(l - m);
+            s += e;
+            rr = fma(e, t.de, rr);
+        }
+    }
+    return {m + log(s), rr / s};
+}
+
+// The observation loop of a mixture, out of line like ir_zi_pass: r_i = d logp / d eta_i, lse_i and eta_i (in the rows
+// lr = [lse | eta], 2N doubles), then one team reduction per component k, ascending, that recomputes l_ik from the stored
+// eta_i and lse_i and pulls sum_i rho_ik into G_k, sum_i rho_ik
+// d log f_k / d theta_k into the component and sum_i rho_ik d log f_k / d sigma_k into sigma: a fixed order, no atomics,
+// no bound on K.  Returns this thread's partial sum of logp.
+template <int W>
+__device__ __noinline__ double ir_mixture_pass(const IrLikD* Lp, const IrTermD* terms, const double* x, double* r, double* lr,
+                                               double* g, int tid, double* red) {
+    constexpr int TS = 32 * W;
+    const IrLikD& L = *Lp;
+    const int N = (int)L.N, K = (int)L.nu;
+    const IrMix M = ir_mix_block(L, terms, x, g);
+    double* er = lr + N;
+    double lp = 0.0;
+    for (int i = tid; i < N; i += TS) {
+        const double eta = ir_eta(terms + L.term0, 0, L.n_terms, x, i, N);
+        const IrMixObs o = ir_mix_obs(L.dist, K, M, L.y[i], eta);
+        lp += o.lse;
+        r[i] = o.r;
+        lr[i] = o.lse;
+        er[i] = eta;
+    }
+    team_sync<W>();
+    for (int k = 0; k < K; ++k) {
+        if (M.lw[k] == -INFINITY) continue;  // uniform: a dropped component
+        double a[3] = {0.0, 0.0, 0.0};
+        for (int i = tid; i < N; i += TS) {  // each thread reads back the rows it wrote
+            const IrMixTerm t = ir_mix_term(L.dist, M, k, L.y[i], er[i]);
+            const double l = M.lw[k] + t.lf;
+            if (l == -INFINITY) continue;  // rho = 0, and its derivatives may be infinite
+            const double rho = exp(l - lr[i]);
+            a[0] += rho;
+            a[1] = fma(rho, t.dc, a[1]);
+            a[2] = fma(rho, t.ds, a[2]);
+        }
+        team_sum_n<W>(a, tid, red);
+        if (tid == 0) {
+            if (M.G) M.G[k] += a[0];
+            if (M.gc) M.gc[k] += a[1];
+            if (M.gs) M.gs[M.s_vec ? k : 0] += a[2];
+        }
+        team_sync<W>();
+    }
+    return lp;
+}
+
 // IrModel evaluates every factor of the closed set except the censored / truncated Normal, the ordinal, the zero-inflated,
 // the hurdle and the survival likelihoods and the ordered transform; IrExtendedModel (below) is the same function with those added,
 // each out of line.  A kernel's
@@ -640,8 +793,9 @@ struct IrModel {
         for (int v = 0; v < P.n_vars; ++v) {
             const IrVarD V = P.vars[v];
             if constexpr (EXTENDED) {
-                if (V.transform >= IRT_ORDERED) {  // uniform branch: a prefix sum, on one thread
-                    if (tid == 0) lp += ir_ordered_forward(P.vars + v, q_s, x);
+                if (V.transform >= IRT_ORDERED) {  // uniform branch: a prefix sum or a softmax, on one thread
+                    if (tid == 0)
+                        lp += V.transform == IRT_SIMPLEX ? ir_simplex_forward(P.vars + v, q_s, x) : ir_ordered_forward(P.vars + v, q_s, x);
                     for (int j = tid; j < V.size; j += TS) g_s[V.offset + j] = 0.0;
                     continue;
                 }
@@ -658,6 +812,13 @@ struct IrModel {
         for (int k = 0; k < P.n_priors; ++k) {
             const IrPriorD F = P.priors[k];
             if (F.dist == IRP_FLAT) continue;
+            if constexpr (EXTENDED) {
+                if (F.dist == IRP_DIRICHLET) {  // uniform branch: out of line, on one thread
+                    if (tid == 0) lp += ir_dirichlet(P.priors + k, x);
+                    team_sync<W>();
+                    continue;
+                }
+            }
             const double a0 = par(F.p[0], x), a1 = par(F.p[1], x), a2 = par(F.p[2], x);
             double s[3] = {0.0, 0.0, 0.0};  // sums for the parameter gradients
             for (int j = tid; j < F.size; j += TS) {
@@ -738,10 +899,13 @@ struct IrModel {
             const double la = disp ? log(sg_s) : 0.0;
             double s_sig = 0.0, s_psi = 0.0;
             const bool ordinal = EXTENDED && (L.dist == IRL_ORDERED_LOGISTIC || L.dist == IRL_ORDERED_PROBIT);
-            const bool bounded = EXTENDED && (ordinal || zi || L.dist == IRL_CENSORED_NORMAL || L.dist == IRL_TRUNCATED_NORMAL ||
-                                              ir_survival(L.dist));
+            const bool mixture = EXTENDED && (L.dist == IRL_NORMAL_MIXTURE || L.dist == IRL_POISSON_MIXTURE);
+            const bool bounded = EXTENDED && (ordinal || zi || mixture || L.dist == IRL_CENSORED_NORMAL ||
+                                              L.dist == IRL_TRUNCATED_NORMAL || ir_survival(L.dist));
             if constexpr (EXTENDED) {
-                if (zi) {  // uniform branch: out of line
+                if (mixture) {  // uniform branch: out of line, with the per-component gradients
+                    lp += ir_mixture_pass<W>(P.liks + l, P.terms, x, r, x + P.ord_row, g_s, tid, red);
+                } else if (zi) {  // uniform branch: out of line
                     const IrZiPartials b = ir_zi_pass<W>(P.liks + l, P.terms, x, r, x + P.ord_row, sg_s, la, tid);
                     lp += b.lp;
                     s_sig = b.s_a;
@@ -848,8 +1012,11 @@ struct IrModel {
             const IrVarD V = P.vars[v];
             if (V.transform == IRT_NONE) continue;
             if constexpr (EXTENDED) {
-                if (V.transform >= IRT_ORDERED) {  // uniform branch: a reverse prefix sum, on one thread
-                    if (tid == 0) ir_ordered_chain(P.vars + v, q_s, g_s);
+                if (V.transform >= IRT_ORDERED) {  // uniform branch: a reverse prefix sum or the softmax's, on one thread
+                    if (tid == 0) {
+                        if (V.transform == IRT_SIMPLEX) ir_simplex_chain(P.vars + v, x, g_s);
+                        else ir_ordered_chain(P.vars + v, q_s, g_s);
+                    }
                     continue;
                 }
             }
@@ -896,6 +1063,10 @@ template <bool EXTENDED>  // as IrModel / IrExtendedModel
 __device__ __forceinline__ double ir_obs_loglik(const IrLikD& L, const IrTermD* terms, const double* x, int i, double eta,
                                                 double sg_s, double la) {
     const double y = L.y[i];
+    if (EXTENDED && (L.dist == IRL_NORMAL_MIXTURE || L.dist == IRL_POISSON_MIXTURE)) {
+        const double lse = ir_mix_obs(L.dist, (int)L.nu, ir_mix_block(L, terms, x, nullptr), y, eta).lse;
+        return lse - (L.dist == IRL_NORMAL_MIXTURE ? B200_HALF_LOG_2PI : lgamma(y + 1.0));
+    }
     if (EXTENDED && L.dist >= IRL_ZI_POISSON && L.dist <= IRL_HURDLE_GAMMA) {
         const IrPsi ps = ir_psi(terms + L.term0 + L.n_terms, (int)L.nu, x, i, (int)L.N);
         const double lp = ir_zi_term(L.dist, y, eta, ir_scale(L, i, sg_s), sg_s, la, ps).lp;
@@ -932,7 +1103,10 @@ __global__ void __launch_bounds__(256) ir_pointwise_kernel(const IrModel::Params
             const IrVarD V = P.vars[v];
             if constexpr (EXTENDED) {
                 if (V.transform >= IRT_ORDERED) {
-                    if (lane == 0) ir_ordered_forward(P.vars + v, q, x);
+                    if (lane == 0) {
+                        if (V.transform == IRT_SIMPLEX) ir_simplex_forward(P.vars + v, q, x);
+                        else ir_ordered_forward(P.vars + v, q, x);
+                    }
                     continue;
                 }
             }

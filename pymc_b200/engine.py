@@ -140,9 +140,10 @@ class CompiledModel:
             elif v.transform == "interval":
                 kind[sl], lo[sl], hi[sl] = 2, v.bounds[0], v.bounds[1]
         _lib.check(self._lib.b200_model_set_transforms(self._h, kind.ctypes.data, lo.ctypes.data, hi.ctypes.data))
-        # the record step's transform is per element, which an ordered variable (a cumulative sum) is not: such a model's
-        # draws are constrained on the host (ModelSpec.constrain)
-        self.supports_constrain = not any(v.transform in ("ordered", "ordered_positive") for v in spec.vars)
+        # the record step's transform is per element, which an ordered variable (a cumulative sum) and a simplex one (a
+        # softmax with one more value than coordinates) are not: such a model's draws are constrained on the host
+        # (ModelSpec.constrain)
+        self.supports_constrain = not any(v.transform in ("ordered", "ordered_positive", "simplex") for v in spec.vars)
 
     def pointwise_loglik(self, draws, lik: int = 0):
         """log p(y_i | draw) for every draw: ``draws[..., n]`` (unconstrained) -> ``[..., N]`` (IR models on the generic

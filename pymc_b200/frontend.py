@@ -23,8 +23,13 @@ pymc/model/fgraph.py:76-81, :139) -- and pattern-matches them onto the closed fa
                      without the {name}_probs Deterministic (recorded, evaluated from the draws);
                      pm.ZeroInflatedPoisson / Binomial / NegativeBinomial and pm.HurdlePoisson / NegativeBinomial / Gamma:
                      the mixture of DiracDelta(0) and the family above with weights stack([1 - psi, psi]), psi a
-                     constant, a scalar free RV or pm.math.invlogit(linear predictor)
-    transform    ->  None, log, interval, and Ordered() / Ordered(positive=True) -> "ordered" / "ordered_positive"
+                     constant, a scalar free RV or pm.math.invlogit(linear predictor);
+                     finite mixtures: pm.NormalMixture(w, mu, sigma) and pm.Mixture(w, pm.Poisson.dist(lam, shape=K)), the
+                     Mixture of ONE batched component, with w a free pm.Dirichlet or a constant K-vector, mu optionally
+                     linear_predictor[:, None] + mu and lam optionally pm.math.exp(linear_predictor)[:, None] * lam
+    free RV      ->  pm.Dirichlet with a constant a -> the dirichlet prior on a simplex variable
+    transform    ->  None, log, interval, Ordered() / Ordered(positive=True) -> "ordered" / "ordered_positive", and
+                     SimplexTransform -> "simplex"
 
 Anything outside the closed set raises ``NotImplementedError`` naming the offending op, so a model either lowers exactly
 or not at all.  PyMC and PyTensor are NOT importable in the build image (SURVEY 8c); this module imports them lazily and
@@ -129,6 +134,8 @@ def from_pymc(model) -> _ir.ModelIR:
                 raise NotImplementedError(f"{rv.name}: Ordered(ascending=False) is outside the closed set (only ascending "
                                           "ordered transforms)")
             transform = "ordered_positive" if getattr(tr, "positive", False) else "ordered"
+        elif tname == "simplextransform":  # transforms.py:1091-1116: the value variable has K - 1 elements
+            transform = "simplex"
         elif "log" in tname and "odds" not in tname and "interval" not in tname:
             transform = "log"
         elif "interval" in tname or "logodds" in tname:
@@ -147,9 +154,17 @@ def from_pymc(model) -> _ir.ModelIR:
         vars_.append(_ir.Var(val.name, rv.name, size, transform, bounds, initial=np.ravel(ip[val.name]).astype(np.float64)))
         name_of[rv] = val.name
     size_of = {v.name: v.size for v in vars_}
+    simplex = {v.name for v in vars_ if v.transform == "simplex"}
+
+    def use(x):
+        """the value variable of free RV x, which may enter any factor except a simplex (Dirichlet) one"""
+        if name_of[x] in simplex:
+            raise NotImplementedError(f"{x.name}: {_ir.SIMPLEX_USE} (pm.NormalMixture / pm.Mixture w)")
+        return name_of[x]
 
     def param(x, what):
         if x in name_of:
+            use(x)
             if size_of[name_of[x]] != 1:
                 raise NotImplementedError(f"{what}: a vector random variable as a distribution parameter")
             return _ir.Ref(name_of[x])
@@ -167,7 +182,7 @@ def from_pymc(model) -> _ir.ModelIR:
     def terms_of(x, N):
         """-> list of (coef: ndarray[N] | float, factors: [(var name, idx or None)])"""
         if x in name_of:
-            return [(1.0, [(name_of[x], None)])]
+            return [(1.0, [(use(x), None)])]
         c = _const_value(x)
         if c is not None:
             c = np.broadcast_to(np.asarray(c, dtype=np.float64), (N,)).copy() if c.size > 1 else float(c.reshape(()))
@@ -185,13 +200,13 @@ def from_pymc(model) -> _ir.ModelIR:
                 iv = _const_value(ix[0])
                 if iv is None:
                     raise NotImplementedError("linear predictor: indexing by a non-constant index")
-                return [(1.0, [(name_of[base], np.broadcast_to(np.asarray(iv, dtype=np.int32), (N,)).copy())])]
+                return [(1.0, [(use(base), np.broadcast_to(np.asarray(iv, dtype=np.int32), (N,)).copy())])]
             raise NotImplementedError("linear predictor: indexing of a non-variable expression")
         if isinstance(node.op, Dot):
             a, b = node.inputs
             A, B = _const_value(a), _const_value(b)
             if A is not None and b in name_of and A.ndim == 2:
-                return [(np.ascontiguousarray(A[:, k], dtype=np.float64), [(name_of[b], np.full(N, k, dtype=np.int32))])
+                return [(np.ascontiguousarray(A[:, k], dtype=np.float64), [(use(b), np.full(N, k, dtype=np.int32))])
                         for k in range(A.shape[1])]
             raise NotImplementedError("linear predictor: dot() is supported as constant_matrix @ vector_variable")
         son = scalar_op_name(node)
@@ -248,6 +263,13 @@ def from_pymc(model) -> _ir.ModelIR:
             rho = rhos.owner.inputs[0] if (rhos.owner is not None and not isinstance(rhos.owner.op, type(None)) and rhos not in name_of
                                            and _const_value(rhos) is None and len(rhos.owner.inputs) == 1) else rhos
             ar1.append(_ir.AR1(vn, param(rho, rv.name + ".rho"), param(sigma, rv.name + ".sigma"), float(_const_value(ipar[1]))))
+            continue
+        if op == "dirichlet":  # multivariate.py:557-585; its value variable is the simplex of K - 1 coordinates
+            a = _const_value(ps[0])
+            if a is None:
+                raise NotImplementedError(f"{rv.name}: a pm.Dirichlet with a random a is outside the closed set (a is a "
+                                          "constant)")
+            priors.append(_ir.Prior("dirichlet", vn, (np.asarray(a, dtype=np.float64),)))
             continue
         if op in ("gaussianrandomwalk", "randomwalk"):
             raise NotImplementedError(f"{rv.name}: write the random walk as pm.AR(rho=[1.0], ...) for this front-end")
@@ -323,7 +345,7 @@ def from_pymc(model) -> _ir.ModelIR:
         while x.owner is not None and isinstance(x.owner.op, DimShuffle):
             x = x.owner.inputs[0]
         if x in name_of:
-            return _ir.Ref(name_of[x])
+            return _ir.Ref(use(x))
         c = _const_value(x)
         return np.asarray(c, dtype=np.float64) if c is not None and c.ndim == 1 else None
 
@@ -488,8 +510,10 @@ def from_pymc(model) -> _ir.ModelIR:
         zero = comps[0] if comps else None
         if len(comps) != 2 or zero.owner is None or _op_name(zero) != "diracdelta" or \
                 _const_value(_dist_params(zero)[0]) is None or np.any(_const_value(_dist_params(zero)[0]) != 0):
-            raise NotImplementedError(f"{rv.name}: pm.Mixture / pm.NormalMixture is outside the closed set (only the "
-                                      "zero-inflated Poisson, Binomial and NegativeBinomial mixtures)")
+            raise NotImplementedError(f"{rv.name}: a list-of-components pm.Mixture / pm.NormalMixture is outside the closed "
+                                      "set (write the K components as one batched distribution: pm.NormalMixture(w, mu, "
+                                      "sigma) or pm.Mixture(w, pm.Poisson.dist(lam, shape=K)); the other two-component "
+                                      "mixtures are the zero-inflated Poisson, Binomial and NegativeBinomial)")
         comp = comps[1]
         cop = _op_name(comp)
         if hurdle and cop == "lognormal":
@@ -514,6 +538,94 @@ def from_pymc(model) -> _ir.ModelIR:
         fam, eta, slot = family_of(cop, cps, rv.name, N)
         dist = next(d for d, f in _ir.ZI_FAMILY.items() if f == fam and d.startswith("hurdle" if hurdle else "zero"))
         return dist, eta, slot, psi_of(w, rv.name, N)
+
+    def peel(x):
+        while x.owner is not None and isinstance(x.owner.op, DimShuffle):
+            x = x.owner.inputs[0]
+        return x
+
+    def mixture_of(rv, ps, N):
+        """Likelihood arguments of a Mixture of ONE batched component (mixture.py:469-494, :529-546): pm.NormalMixture(w,
+        mu, sigma) -> normal_mixture, pm.Mixture(w, pm.Poisson.dist(lam, shape=K)) -> poisson_mixture, seen through the
+        DimShuffle / broadcast layers of PyMC's resizing to (N, K)"""
+        name, comp = rv.name, ps[1]
+        cop = _op_name(comp) if comp.owner is not None else ""
+        if cop not in ("normal", "poisson"):
+            what = type(comp.owner.op).__name__ if comp.owner is not None else str(comp)
+            raise NotImplementedError(f"{name}: a mixture of {what} components is outside the closed set (only Normal "
+                                      "and Poisson components)")
+        # the weights: a free pm.Dirichlet (simplex) or a constant K-vector
+        wv = peel(ps[0])
+        wform = "the weights of a mixture are a free pm.Dirichlet or a constant K-vector"
+        if wv in name_of:
+            if name_of[wv] not in simplex:
+                raise NotImplementedError(f"{name}: {wform}")
+            weights, K = _ir.Ref(name_of[wv]), size_of[name_of[wv]] + 1
+        else:
+            c = _const_value(wv)
+            if c is None:
+                raise NotImplementedError(f"{name}: {wform}")
+            c = np.asarray(c, dtype=np.float64)
+            if c.ndim > 1 and not np.all(c.reshape(-1, c.shape[-1]) == c.reshape(-1, c.shape[-1])[0]):
+                raise NotImplementedError(f"{name}: per-observation weights are outside the closed set ({wform})")
+            weights = c.reshape(-1, c.shape[-1])[0] if c.ndim else c
+            K = int(np.size(weights))
+
+        def per_component(x, what):
+            """a free RV of size K (or 1 where allowed: -> Ref) or a constant of 1 or K values, else None"""
+            x = peel(x)
+            if x in name_of:
+                vn = name_of[x]
+                if vn in simplex:
+                    raise NotImplementedError(f"{x.name}: {_ir.SIMPLEX_USE} (pm.NormalMixture / pm.Mixture w)")
+                if size_of[vn] not in (1, K):
+                    raise NotImplementedError(f"{name}: a per-observation {what} is outside the closed set (one per "
+                                              "component)")
+                return _ir.Ref(vn), size_of[vn]
+            c = _const_value(x)
+            if c is None:
+                return None
+            c = np.asarray(c, dtype=np.float64)
+            if c.ndim > 1 and not np.all(c.reshape(-1, c.shape[-1]) == c.reshape(-1, c.shape[-1])[0]):
+                raise NotImplementedError(f"{name}: a per-observation {what} is outside the closed set (one per component)")
+            v = c.reshape(-1, c.shape[-1])[0] if c.ndim else c.reshape(1)
+            return (float(v[0]) if v.size == 1 and what == "sigma" else v), v.size
+
+        def split(x, join, what, mark):
+            """(component, eta or None) of x = component, or x = join(eta-part, component) where mark(eta-part) gives eta"""
+            ins = inputs_of(x, join)
+            if ins is not None and len(ins) == 2:
+                for a, b in ((ins[0], ins[1]), (ins[1], ins[0])):  # the component is the part with K values
+                    eta = mark(a)
+                    try:
+                        got = per_component(b, what) if eta is not None else None
+                    except NotImplementedError:
+                        got = None
+                    if got is not None and got[1] == K:
+                        return got[0], eta
+            got = per_component(x, what)
+            return (got[0], None) if got is not None else (None, None)
+
+        cps = _dist_params(comp)
+        if cop == "normal":
+            form = ("pm.NormalMixture(w, mu, sigma) with mu a K-vector free RV or constant, optionally "
+                    "linear_predictor[:, None] + mu, and sigma a constant, a scalar free RV or a K-vector free RV")
+            mu, eta = split(cps[0], "add", "mu", peel)
+            if mu is None:
+                raise NotImplementedError(f"{name}: {form}")
+            s = peel(cps[1])
+            if s.owner is not None and scalar_op_name(s.owner) in ("pow", "reciprocal", "sqrt", "invsqrt", "truediv"):
+                raise NotImplementedError(f"{name}: pm.NormalMixture(tau=...) is outside the closed set (give sigma)")
+            got = per_component(s, "sigma")
+            if got is None:
+                raise NotImplementedError(f"{name}: {form}")
+            return "normal_mixture", eta, dict(weights=weights, components=mu, sigma=got[0])
+        form = ("pm.Mixture(w, pm.Poisson.dist(lam, shape=K)) with lam a K-vector free RV or constant, optionally "
+                "pm.math.exp(linear_predictor)[:, None] * lam")
+        lam, eta = split(cps[0], "mul", "lam", lambda a: (inputs_of(a, "exp") or [None])[0])
+        if lam is None:
+            raise NotImplementedError(f"{name}: {form}")
+        return "poisson_mixture", eta, dict(weights=weights, components=lam)
 
     def survival_of(op, ps, name, sigma_of):
         """(family, eta, parameter slot) of a survival RV (op, its dist params ps): pm.Weibull(alpha, beta=exp(eta)),
@@ -597,6 +709,9 @@ def from_pymc(model) -> _ir.ModelIR:
         elif op in ("poisson", "binomial", "negbinomial", "nbinom", "gamma"):
             dist, eta, slot = family_of(op, ps, rv.name, N)
             liks.append(_ir.Likelihood(dist, y, make_terms(eta, N), name=rv.name, **slot))
+        elif op == "mixture" and len(ps) == 2:  # pm.NormalMixture / pm.Mixture of one batched component
+            dist, eta, kw = mixture_of(rv, ps, N)
+            liks.append(_ir.Likelihood(dist, y, [] if eta is None else make_terms(eta, N), name=rv.name, **kw))
         elif op in ("mixture", "_hurdle", "hurdle"):  # pm.ZeroInflated* / pm.Hurdle*
             dist, eta, slot, psi = zero_inflated_of(rv, ps, N)
             liks.append(_ir.Likelihood(dist, y, make_terms(eta, N), name=rv.name, psi=psi, **slot))

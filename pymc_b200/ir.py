@@ -29,7 +29,8 @@ import numpy as np
 
 # ids shared with include/b200nuts.h ------------------------------------------------------------------------------------
 TRANSFORMS = {None: 0, "log": 1, "interval": 2,
-              "ordered": 3, "ordered_positive": 4}  # Ordered() / Ordered(positive=True), transforms.py:79-120
+              "ordered": 3, "ordered_positive": 4,  # Ordered() / Ordered(positive=True), transforms.py:79-120
+              "simplex": 5}  # SimplexTransform, transforms.py:1091-1116: Var.size is K - 1, the constrained value K weights
 ORDERED_TRANSFORMS = ("ordered", "ordered_positive")
 # An ordered variable is not constrained elementwise (a cumulative sum): it takes only real-line priors, and
 # ordered_positive also counts as positive support (csrc/b200nuts.cu: prepare_ir, same words)
@@ -49,6 +50,7 @@ PRIOR_DISTS = {
     "gamma": (8, 2),         # (alpha, beta) constants                                  continuous.py:2512-2515
     "beta": (9, 2),          # (alpha, beta) constants                                  continuous.py:1250-1256
     "lognormal": (10, 2),    # (mu, sigma)                                              continuous.py:1807-1814
+    "dirichlet": (11, 1),    # (a): K constants > 0 or one broadcast; on a simplex only  multivariate.py:557-585
 }
 # likelihoods: name -> id
 LIK_DISTS = {
@@ -76,6 +78,8 @@ LIK_DISTS = {
     "censored_lognormal": 21,      # y_i ~ Censored(LogNormal(eta_i, sigma), lower, upper)
     "truncated_weibull_log": 22,   # y_i ~ Truncated(Weibull(alpha, exp(eta_i)), lower, upper)
     "truncated_lognormal": 23,     # y_i ~ Truncated(LogNormal(eta_i, sigma), lower, upper)
+    "normal_mixture": 24,    # y_i ~ NormalMixture(w, eta_i + mu_k, sigma_k)                mixture.py:469-494, :529-546
+    "poisson_mixture": 25,   # y_i ~ Mixture(w, Poisson(lam_k exp(eta_i)))
 }
 # Zero-inflated and hurdle observations: ``Likelihood.psi`` is the probability of the count / positive component, a
 # constant in (0, 1), a Ref to a scalar variable with an interval transform inside [0, 1], or a Linear: the logit of psi.
@@ -132,6 +136,24 @@ SURV_TRUNC_OPEN = ("a truncated survival likelihood needs a finite lower bound >
 SURV_PLAIN = "lower / upper belong to the censored_ and truncated_ forms"
 WEIBULL_SIGMA = "a Weibull likelihood has no sigma (its parameter is alpha)"
 DISPERSION_LIKS = ("negative_binomial_log", "gamma_log")  # their `alpha` is a constant or a Ref
+# Finite mixtures of K >= 2 components, log p(y_i) = logsumexp_k(log w_k + log f_k(y_i)): ``Likelihood.weights`` (a Ref to a
+# simplex variable or K constants) and ``.components`` (mu_k / lam_k: a Ref to a variable of size K or K constants); the
+# Normal's ``sigma`` is one or K constants or a Ref to a variable of size 1 or K.  The predictor's terms may be empty.
+# Lowered with nu = K and the weights, component and sigma blocks one past the predictor's terms (include/b200nuts.h).
+MIXTURE_LIKS = ("normal_mixture", "poisson_mixture")
+# the rules of simplex variables, Dirichlet priors and mixtures (csrc/b200nuts.cu: prepare_ir, same words)
+SIMPLEX_USE = "a simplex variable may be used only as a mixture's weights"
+SIMPLEX_PRIOR = "a simplex variable carries exactly one prior, a dirichlet of length K = size + 1"
+DIRICHLET_VAR = "a dirichlet prior is only allowed on a simplex variable"
+DIRICHLET_A = "a dirichlet's a must be one finite constant > 0 (K equal constants lower to it)"
+MIX_K = "a mixture needs K >= 2 components; with K = 1, write the plain likelihood (normal or poisson_log)"
+MIX_Y_NORMAL = "y must be finite"
+MIX_WEIGHTS = "the weights must be a simplex variable of size K - 1 or K finite constants >= 0 that sum to 1"
+MIX_MU = "mu must be a variable of size K with no transform or an ordered one, or K finite constants"
+MIX_LAM = ("lam must be a variable of size K with positive support (log, ordered_positive, or an interval with lo >= 0), "
+           "or K finite constants > 0")
+MIX_SIGMA = "sigma must be a finite constant > 0, K of them, or a variable of size 1 or K with positive support"
+MIX_SLOTS = "a mixture takes no alpha, trials, lower / upper, cutpoints or psi, and poisson_mixture no sigma"
 # The support rule.  The device evaluates a density's formula wherever it is asked to, so every variable must be kept
 # inside its prior's support by its transform, and every scale parameter must be positive:
 POSITIVE_PRIORS = ("halfnormal", "halfcauchy", "exponential", "gamma", "lognormal")  # a log transform, or interval lo >= 0
@@ -157,6 +179,14 @@ def ordered_backward(z: np.ndarray, positive: bool) -> np.ndarray:
     if not positive:
         d[..., 0] = z[..., 0]
     return np.cumsum(d, axis=-1)
+
+
+def simplex_backward(z: np.ndarray) -> np.ndarray:
+    """SimplexTransform.backward (transforms.py:1101-1105) along the last axis: w = softmax([z, -sum z])."""
+    z = np.asarray(z, dtype=np.float64)
+    ze = np.concatenate([z, -np.sum(z, axis=-1, keepdims=True)], axis=-1)
+    e = np.exp(ze - np.max(ze, axis=-1, keepdims=True))
+    return e / np.sum(e, axis=-1, keepdims=True)
 
 
 def is_design(t) -> bool:
@@ -232,6 +262,14 @@ class Likelihood:
     upper: float | np.ndarray | None = None    # -inf / +inf where that observation's side is open (survival: lower 0 too)
     cutpoints: Ref | np.ndarray | None = None  # ordered_logistic / ordered_probit: K - 1 cutpoints (see ORDINAL_LIKS)
     psi: float | Ref | Linear | None = None    # the zero-inflated / hurdle likelihoods (ZI_LIKS): a Linear is logit(psi)
+    weights: Ref | np.ndarray | None = None     # mixtures (MIXTURE_LIKS): a simplex variable or K constants
+    components: Ref | np.ndarray | None = None  # mixtures: mu_k (normal_mixture) or lam_k (poisson_mixture)
+
+    def n_components(self, model: "ModelIR") -> int:
+        """K of a mixture: the size of its components."""
+        if isinstance(self.components, Ref):
+            return model.var(self.components.var).size
+        return int(np.size(self.components))
 
     def n_categories(self, model: "ModelIR") -> int:
         """K of an ordinal likelihood: one more than its number of cutpoints."""
@@ -331,12 +369,17 @@ class ModelIR:
                 raise ValueError(f"{v.name}: interval transform needs bounds lo < hi")
             if v.size < 1:
                 raise ValueError(f"{v.name}: size must be positive")
+        self._validate_simplex_use()
+        n_simplex_priors = {}
         for p in self.priors:
             if p.dist not in PRIOR_DISTS:
                 raise ValueError(f"prior {p.dist!r} is not in the closed set {sorted(PRIOR_DISTS)}")
             if len(p.params) != PRIOR_DISTS[p.dist][1]:
                 raise ValueError(f"prior {p.dist} on {p.var}: expected {PRIOR_DISTS[p.dist][1]} parameters")
             v = self.var(p.var)
+            if v.transform == "simplex" or p.dist == "dirichlet":
+                self._check_dirichlet(p, v, n_simplex_priors)
+                continue
             loc, scale = LINEAR_PRIORS.get(p.dist, (None, None))
             for k, a in enumerate(p.params):
                 what = f"prior {p.dist} on {v.name}"
@@ -360,11 +403,19 @@ class ModelIR:
                 if k in SCALE_PARAMS.get(p.dist, {}):
                     self._check_scale(a, f"{what}: {SCALE_PARAMS[p.dist][k]}")
             self._check_prior_support(p, v)
+        for v in self.vars:
+            if v.transform == "simplex" and n_simplex_priors.get(v.name, 0) != 1:
+                raise ValueError(f"{v.name}: {SIMPLEX_PRIOR}")
         for L in self.likelihoods:
             if L.dist not in LIK_DISTS:
                 raise ValueError(f"likelihood {L.dist!r} is not in the closed set {sorted(LIK_DISTS)}")
             N = len(L.y)
             self._check_terms(L.terms, N, f"likelihood {L.name}", "the number of observations")
+            if L.dist in MIXTURE_LIKS:
+                self._validate_mixture(L)
+                continue
+            if L.weights is not None or L.components is not None:
+                raise ValueError(f"{L.dist} likelihood {L.name}: weights and components belong to the mixture likelihoods")
             if L.dist in SIGMA_LIKS and L.sigma is None:
                 raise ValueError(f"{L.dist} likelihood needs sigma")
             if isinstance(L.sigma, Ref) and self.var(L.sigma.var).size != 1:
@@ -399,6 +450,104 @@ class ModelIR:
             self._check_scale(a.sigma, f"AR1 on {a.var}: sigma")
             if not (np.isfinite(a.init_sigma) and a.init_sigma > 0):
                 raise ValueError(f"AR1 on {a.var}: init_sigma must be > 0")
+
+    def _validate_simplex_use(self) -> None:
+        """A simplex variable is used only as a mixture's weights: never as a parameter, a term factor (of a likelihood, a
+        Linear location, logit(psi) or a Deterministic), cutpoints, psi, a mixture's components or sigma, or in an AR(1)."""
+        simplex = {v.name for v in self.vars if v.transform == "simplex"}
+        if not simplex:
+            return
+        used = []
+
+        def terms(ts):
+            used.extend(vn for t in ts for vn, _ in t.factors)
+
+        def par(a):
+            if isinstance(a, Ref):
+                used.append(a.var)
+            elif isinstance(a, Linear):
+                terms(a.terms)
+
+        for p in self.priors:
+            for a in p.params:
+                par(a)
+        for L in self.likelihoods:
+            terms(L.terms)
+            for a in (L.sigma, L.alpha, L.psi, L.cutpoints, L.components):
+                par(a)
+        for a in self.ar1:
+            used.append(a.var)
+            par(a.phi)
+            par(a.sigma)
+        for d in self.deterministics:
+            terms(d.terms)
+        if any(self.var(vn).name in simplex for vn in used):
+            raise ValueError(SIMPLEX_USE)
+
+    def _check_dirichlet(self, p, v, count: dict) -> None:
+        """A prior on a simplex variable is its one Dirichlet; a Dirichlet sits on a simplex variable and its a is one
+        constant > 0, or K equal ones (the checks prepare_ir makes, in the same words)."""
+        what = f"prior {p.dist} on {v.name}"
+        if v.transform == "simplex":
+            if p.dist != "dirichlet" or count.get(v.name, 0) > 0:
+                raise ValueError(f"{what}: {SIMPLEX_PRIOR}")
+            count[v.name] = 1
+        if v.transform != "simplex":
+            raise ValueError(f"{what}: {DIRICHLET_VAR}")
+        a = p.params[0]
+        if isinstance(a, (Ref, Linear)):
+            raise ValueError(f"{what}: {DIRICHLET_A}")
+        a = np.asarray(a, dtype=np.float64)
+        if not (a.ndim == 0 or (a.ndim == 1 and len(a) == v.size + 1)) or not (np.all(np.isfinite(a)) and np.all(a > 0)) \
+                or np.any(a != a.ravel()[0]):
+            raise ValueError(f"{what}: {DIRICHLET_A}")
+
+    def _validate_mixture(self, L) -> None:
+        """K, y, weights, components and sigma of a mixture (the checks prepare_ir makes, in the same words)."""
+        what = f"{L.dist} likelihood {L.name}"
+        normal = L.dist == "normal_mixture"
+        if any(a is not None for a in (L.alpha, L.trials, L.lower, L.upper, L.cutpoints, L.psi)) or \
+                (not normal and L.sigma is not None):
+            raise ValueError(f"{what}: {MIX_SLOTS}")
+        comp_words = MIX_MU if normal else MIX_LAM
+        if L.components is None or not (isinstance(L.components, Ref) or np.ndim(L.components) == 1):
+            raise ValueError(f"{what}: {comp_words}")
+        K = L.n_components(self)
+        if K < 2:
+            raise ValueError(f"{what}: {MIX_K}")
+        y = np.asarray(L.y, dtype=np.float64)
+        if normal and not np.all(np.isfinite(y)):
+            raise ValueError(f"{what}: {MIX_Y_NORMAL}")
+        if not normal and not (np.all(np.isfinite(y)) and np.all(y == np.floor(y)) and np.all(y >= 0)):
+            raise ValueError(f"{what}: {ZI_Y}")
+        w = L.weights
+        if isinstance(w, Ref):
+            v = self.var(w.var)
+            if not (v.transform == "simplex" and v.size == K - 1):
+                raise ValueError(f"{what}: {MIX_WEIGHTS}")
+        else:
+            wa = None if w is None else np.asarray(w, dtype=np.float64)
+            if wa is None or wa.shape != (K,) or not (np.all(np.isfinite(wa)) and np.all(wa >= 0)) or not np.isclose(wa.sum(), 1.0):
+                raise ValueError(f"{what}: {MIX_WEIGHTS}")
+        c = L.components
+        if isinstance(c, Ref):
+            v = self.var(c.var)
+            ok = v.size == K and (v.transform in (None, "ordered") if normal else _positive_support(v))
+        else:
+            ca = np.asarray(c, dtype=np.float64)
+            ok = bool(np.all(np.isfinite(ca)) and (normal or np.all(ca > 0)))
+        if not ok:
+            raise ValueError(f"{what}: {comp_words}")
+        if normal:
+            s = L.sigma
+            if isinstance(s, Ref):
+                v = self.var(s.var)
+                ok = v.size in (1, K) and _positive_support(v)
+            else:
+                sa = None if s is None else np.asarray(s, dtype=np.float64)
+                ok = sa is not None and sa.shape in ((), (K,)) and bool(np.all(np.isfinite(sa)) and np.all(sa > 0))
+            if not ok:
+                raise ValueError(f"{what}: {MIX_SIGMA}")
 
     def _check_terms(self, terms, N: int, where: str, length: str) -> None:
         """Terms of a predictor of length N (a likelihood's observations, or the elements of a prior's variable)."""
@@ -636,6 +785,10 @@ class ModelIR:
                 x = s * hi + (1.0 - s) * lo
             elif v.transform in ORDERED_TRANSFORMS:
                 x = ordered_backward(np.array(x, dtype=np.float64), v.transform == "ordered_positive")
+            elif v.transform == "simplex":  # the K weights, as PyMC's posterior holds a Dirichlet
+                x = simplex_backward(x)
+                out[v.rv_name] = x
+                continue
             out[v.rv_name] = x[..., 0] if v.size == 1 else x
         return out
 
@@ -709,6 +862,10 @@ class ModelIR:
                             out[f"{L.name}_psi_{vn}_idx"] = np.asarray(idx)
             elif L.psi is not None and not isinstance(L.psi, Ref):  # a constant psi
                 out[f"{L.name}_psi"] = np.asarray(float(L.psi))
+            for part in ("weights", "components"):  # the constant blocks of a mixture
+                a = getattr(L, part)
+                if a is not None and not isinstance(a, Ref):
+                    out[f"{L.name}_{part}"] = np.asarray(a)
         return out
 
 
@@ -1085,6 +1242,55 @@ def survival_regression_ir(dist: str = "weibull", observe: str = "right_censored
                    likelihoods=[Likelihood(lik, y, terms, lower=lower, upper=upper, **slot)])
 
 
+def mixture_ir(dist: str = "normal", K: int = 3, weights: str = "dirichlet", covariates: int = 0, n_obs: int = 300,
+               seed: int = 67) -> ModelIR:
+    """A finite mixture on simulated data, the NormalMixture example of mixture.py:529-546: w ~ Dirichlet(ones(K)) on the
+    simplex (``weights="dirichlet"``) or the constant weights of the simulation (``"const"``), and
+    ``dist="normal"``: mu ~ Normal(0, 10)^K with the ordered transform, sigma ~ HalfNormal(2)^K,
+    y_i ~ NormalMixture(w, eta_i + mu, sigma);  ``dist="poisson"``: lam ~ Normal(0, 20)^K with the ordered_positive
+    transform (a HalfNormal(20) up to its constant), y_i ~ Mixture(w, Poisson(lam exp(eta_i))).  Ordered locations / rates keep the posterior free of label
+    switching.  ``covariates`` > 0 adds beta ~ Normal(0, 1)^F as a design term, eta_i = x_i . beta (a shared shift, or a
+    shared rate multiplier); with none, eta = 0.  A large K or a design term makes n > 256 (a chain per CTA)."""
+    if dist not in ("normal", "poisson"):
+        raise ValueError("dist must be 'normal' or 'poisson'")
+    if weights not in ("dirichlet", "const"):
+        raise ValueError("weights must be 'dirichlet' or 'const'")
+    rng = np.random.default_rng(seed)
+    w_true = np.linspace(1.0, 2.0, K)
+    w_true /= w_true.sum()
+    X = rng.standard_normal((n_obs, covariates))
+    eta = X @ rng.normal(0.0, 0.3, covariates) if covariates else np.zeros(n_obs)
+    z = rng.choice(K, n_obs, p=w_true)
+    vars_, priors = [], []
+    if weights == "dirichlet":
+        vars_.append(Var("w_simplex__", "w", K - 1, "simplex"))
+        priors.append(Prior("dirichlet", "w_simplex__", (np.ones(K),)))
+        wt = Ref("w_simplex__")
+    else:
+        wt = w_true
+    if dist == "normal":
+        mu_true = np.linspace(-3.0 * (K - 1), 3.0 * (K - 1), K) / max(K - 1, 1)
+        y = eta + mu_true[z] + 0.8 * rng.standard_normal(n_obs)
+        z0 = np.concatenate([[mu_true[0]], np.log(np.diff(mu_true))])
+        vars_ += [Var("mu_ordered__", "mu", K, "ordered", initial=z0), Var("sigma_log__", "sigma", K, "log")]
+        priors += [Prior("normal", "mu_ordered__", (0.0, 10.0)), Prior("halfnormal", "sigma_log__", (2.0,))]
+        comp, sg, lik = Ref("mu_ordered__"), Ref("sigma_log__"), "normal_mixture"
+    else:
+        lam_true = 2.0 * 3.0 ** np.arange(K) / 3.0 ** ((K - 1) / 2)
+        y = rng.poisson(lam_true[z] * np.exp(eta)).astype(np.float64)
+        z0 = np.concatenate([[np.log(lam_true[0])], np.log(np.diff(lam_true))])
+        vars_.append(Var("lam_ordered__", "lam", K, "ordered_positive", initial=z0))
+        priors.append(Prior("normal", "lam_ordered__", (0.0, 20.0)))
+        comp, sg, lik = Ref("lam_ordered__"), None, "poisson_mixture"
+    terms = []
+    if covariates:
+        vars_.append(Var("beta", "beta", covariates))
+        priors.append(Prior("normal", "beta", (0.0, 1.0)))
+        terms = [Term([("beta", None)], coef=X)]
+    return ModelIR(name=f"{dist}_mixture_{K}_{weights}", vars=vars_, priors=priors,
+                   likelihoods=[Likelihood(lik, y, terms, sigma=sg, weights=wt, components=comp)])
+
+
 # ------------------------------------------------------------------------------------------------------------------------
 # lowering: ModelIR -> flat arrays of the C ABI (include/b200nuts.h: b200_ir)
 # ------------------------------------------------------------------------------------------------------------------------
@@ -1102,6 +1308,8 @@ class LoweredIR:
                             # y is the [3][N] block (y, lower, upper); the Weibull's alpha is the sigma slot
                             # ordered_logistic / ordered_probit: nu = K, and cut = the cutpoint term (a term dict)
                             # zero-inflated / hurdle: nu = 0 or m, and psi = the psi block (a list of term dicts)
+                            # normal_mixture / poisson_mixture: nu = K, and mix = the weights, component (and sigma)
+                            # blocks (term dicts)
                             # y_var 0: y is observed data; v + 1: a latent factor, y is None and its values are variable v's
     ar1: list               # [(var, phi(kind, value, ref), sigma(kind, value, ref), init_sigma)]
 
@@ -1167,6 +1375,10 @@ def lower(ir: ModelIR) -> LoweredIR:
         if is_latent(p):
             latent.append(p)
             continue
+        if p.dist == "dirichlet":  # its one concentration (validate: one constant or K equal ones)
+            pars = [(0, float(np.ravel(p.params[0])[0]), -1)] + [(0, 0.0, -1)] * 2
+            priors.append((PRIOR_DISTS[p.dist][0], index[ir.var(p.var).name], pars))
+            continue
         pars = [_param(ir, a, off) for a in p.params] + [(0, 0.0, -1)] * (3 - len(p.params))
         priors.append((PRIOR_DISTS[p.dist][0], index[ir.var(p.var).name], pars))
     liks = []
@@ -1174,6 +1386,8 @@ def lower(ir: ModelIR) -> LoweredIR:
         # the likelihood's one parameter slot: sigma, or the trials / alpha of the count and positive families
         fam = ZI_FAMILY.get(L.dist, L.dist)
         par = L.trials if fam == "binomial_logit" else (L.alpha if fam in DISPERSION_LIKS + WEIBULL_LIKS else L.sigma)
+        if L.dist in MIXTURE_LIKS:
+            par = None  # sigma is a block
         y = np.ascontiguousarray(L.y, dtype=np.float64)
         if L.dist in BOUNDED_LIKS + SURVIVAL_BOUNDED:  # the [3][N] block: y, lower, upper
             y = np.ascontiguousarray(np.stack([y, *L.bounds()]))
@@ -1183,6 +1397,17 @@ def lower(ir: ModelIR) -> LoweredIR:
             extra = dict(nu=float(L.n_categories(ir)),
                          cut=dict(coef=None, factors=[(off[ir.var(c.var).name], ir.var(c.var).size, None)])
                          if isinstance(c, Ref) else dict(coef=np.ascontiguousarray(c, dtype=np.float64), factors=[]))
+        if L.dist in MIXTURE_LIKS:  # nu = K; the weights, component and (normal) sigma blocks one past the predictor's terms
+            K = L.n_components(ir)
+
+            def block(a, n):
+                if isinstance(a, Ref):
+                    v = ir.var(a.var)
+                    return dict(coef=None, factors=[(off[v.name], v.size, None)])
+                return dict(coef=np.ascontiguousarray(np.broadcast_to(np.asarray(a, dtype=np.float64), (n,))), factors=[])
+
+            mix = [block(L.weights, K), block(L.components, K)] + ([block(L.sigma, K)] if L.dist == "normal_mixture" else [])
+            extra = dict(nu=float(K), mix=mix)
         if L.dist in ZI_LIKS:  # the psi block goes one past the predictor's terms; nu = 0 (psi) or its number of terms
             psi = L.psi
             if isinstance(psi, Linear):
@@ -1283,7 +1508,7 @@ def specialise(ir: ModelIR, extended: bool = False):
         return not isinstance(p.params[k], Ref) and (want is None or float(p.params[k]) == want)
 
     pri = {ir.var(p.var).name: p for p in ir.priors}
-    if len(pri) != len(ir.priors) or len(ir.likelihoods) != 1 or ir.likelihoods[0].dist in ZI_LIKS:
+    if len(pri) != len(ir.priors) or len(ir.likelihoods) != 1 or ir.likelihoods[0].dist in ZI_LIKS + MIXTURE_LIKS:
         return None
     if any(isinstance(a, Linear) or (not isinstance(a, Ref) and np.ndim(a) > 0) for p in ir.priors for a in p.params):
         return None

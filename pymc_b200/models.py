@@ -45,7 +45,7 @@ class VarInfo:
     rv_name: str  # random-variable name, e.g. "tau"
     offset: int
     size: int
-    transform: str | None = None  # None | "log" | "interval" | "ordered" | "ordered_positive"
+    transform: str | None = None  # None | "log" | "interval" | "ordered" | "ordered_positive" | "simplex"
     bounds: tuple[float, float] | None = None  # for "interval"
 
 
@@ -86,6 +86,11 @@ class ModelSpec:
                 if v.transform == "ordered":
                     d[..., 0] = x[..., 0]
                 x = np.cumsum(d, axis=-1)
+            elif v.transform == "simplex":  # SimplexTransform.backward, transforms.py:1101-1105: size + 1 weights
+                from .ir import simplex_backward
+
+                out[v.rv_name] = simplex_backward(x)
+                continue
             if v.size == 1:
                 x = x[..., 0]
             out[v.rv_name] = x

@@ -130,8 +130,7 @@ struct b200_model {
     IrModel::Params ir{};
     std::vector<IrLikD> ir_liks;  // the host copy of ir.liks
     DevBuf ir_tables;             // the data arrays ir's tables point into (prepare_ir)
-    bool ir_extended = false;  // a censored / truncated Normal, ordinal, zero-inflated, hurdle or survival likelihood, or an ordered
-                               // variable: the kernels run IrExtendedModel
+    bool ir_extended = false;  // a factor of ir_extended_liks / ir_extended_transforms: the kernels run IrExtendedModel
     DevBuf ir_scratch;  // per-team scratch of the generic IR device function: [teams][n_pad + max N] doubles
     // lock-step (GEMM-shaped) models; every matrix is row-major with rows `ld` doubles apart (n rounded up to 4, zero pad)
     long long ld = 0;
@@ -455,7 +454,7 @@ static int ir_param(const b200_ir_param& p, int n, IrParamD* out, const char* wh
 // it is asked to, so a variable must be kept inside its prior's support by its transform, and every scale parameter must
 // be positive.  A variable has positive support under a log transform or an interval with lo >= 0.
 static bool ir_positive_support(const IrVarD& V) {
-    return V.transform == IRT_LOG || V.transform == IRT_ORDERED_POSITIVE || (V.transform == IRT_INTERVAL && V.lo >= 0);
+    return V.transform == B200_IR_T_LOG || V.transform == B200_IR_T_ORDERED_POSITIVE || (V.transform == B200_IR_T_INTERVAL && V.lo >= 0);
 }
 
 // A scale slot (a prior's sigma / beta / lam, a likelihood's sigma, an AR(1) sigma, a dispersion alpha): a finite constant
@@ -535,7 +534,7 @@ static const IrVarD* ir_var_at(const std::vector<IrVarD>& vars, int offset) {
 // does q[offset .. offset + size) touch a simplex variable (whose only use is a mixture's weights)?
 static bool ir_touches_simplex(const std::vector<IrVarD>& vars, int offset, int size) {
     for (const IrVarD& V : vars)
-        if (V.transform == IRT_SIMPLEX && offset < V.offset + V.size && V.offset < offset + size) return true;
+        if (V.transform == B200_IR_T_SIMPLEX && offset < V.offset + V.size && V.offset < offset + size) return true;
     return false;
 }
 static bool ir_ref_simplex(const std::vector<IrVarD>& vars, const b200_ir_param& p) {
@@ -584,10 +583,10 @@ static int ir_prior(IrPass& c, const b200_ir_prior& F, int k, IrPriorD& P) {
         if (ir_param(F.p[a], c.n, &P.p[a], "prior")) return -1;
     for (int a = 0; a < 3; ++a)
         if (ir_ref_simplex(c.vars, F.p[a])) return fail("ir: prior %d: " B200_IR_SIMPLEX_USE, k);
-    if (PV.transform == IRT_SIMPLEX && (F.dist != B200_IR_P_DIRICHLET || ++c.n_priors_of[F.var] > 1))
+    if (PV.transform == B200_IR_T_SIMPLEX && (F.dist != B200_IR_P_DIRICHLET || ++c.n_priors_of[F.var] > 1))
         return fail("ir: prior %d: " B200_IR_SIMPLEX_PRIOR, k);
     if (F.dist == B200_IR_P_DIRICHLET) {  // c0 = lgamma(K a) - K lgamma(a) (multivariate.py:557-585); pad: the rows
-        if (PV.transform != IRT_SIMPLEX) return fail("ir: prior %d: " B200_IR_DIRICHLET_VAR, k);
+        if (PV.transform != B200_IR_T_SIMPLEX) return fail("ir: prior %d: " B200_IR_DIRICHLET_VAR, k);
         const double a = F.p[0].value, K = PV.size + 1.0;
         if (F.p[0].kind != 0 || !(std::isfinite(a) && a > 0)) return fail("ir: prior %d: " B200_IR_DIRICHLET_A, k);
         P.c0 = std::lgamma(K * a) - K * std::lgamma(a);
@@ -607,7 +606,7 @@ static int ir_prior(IrPass& c, const b200_ir_prior& F, int k, IrPriorD& P) {
                           F.dist == B200_IR_P_GAMMA || F.dist == B200_IR_P_LOGNORMAL;
     const bool real_line = F.dist == B200_IR_P_FLAT || F.dist == B200_IR_P_NORMAL || F.dist == B200_IR_P_STUDENTT ||
                            F.dist == B200_IR_P_CAUCHY;
-    if (PV.transform >= IRT_ORDERED && !(real_line || (positive && PV.transform == IRT_ORDERED_POSITIVE)))
+    if (ir_extended_transforms(PV.transform) && !(real_line || (positive && PV.transform == B200_IR_T_ORDERED_POSITIVE)))
         return fail("ir: prior %d: " B200_IR_ORDERED_PRIOR, k);
     if (positive && !ir_positive_support(PV))
         return fail("ir: prior %d: the variable needs a log transform or an interval with lo >= 0 (positive support)", k);
@@ -624,7 +623,7 @@ static int ir_prior(IrPass& c, const b200_ir_prior& F, int k, IrPriorD& P) {
         } break;
         case B200_IR_P_UNIFORM:
             if (!cst(0) || !cst(1) || !(F.p[0].value < F.p[1].value)) return fail("ir: prior %d: Uniform bounds must be constants lo < hi", k);
-            if (!(PV.transform == IRT_INTERVAL && PV.lo >= F.p[0].value && PV.hi <= F.p[1].value))
+            if (!(PV.transform == B200_IR_T_INTERVAL && PV.lo >= F.p[0].value && PV.hi <= F.p[1].value))
                 return fail("ir: prior %d: the variable needs an interval inside the Uniform bounds", k);
             P.c0 = -std::log(F.p[1].value - F.p[0].value);
             break;
@@ -634,7 +633,7 @@ static int ir_prior(IrPass& c, const b200_ir_prior& F, int k, IrPriorD& P) {
             break;
         case B200_IR_P_BETA:
             if (!cst(0) || !cst(1) || !(F.p[0].value > 0) || !(F.p[1].value > 0)) return fail("ir: prior %d: Beta needs constant alpha, beta > 0", k);
-            if (!(PV.transform == IRT_INTERVAL && PV.lo >= 0 && PV.hi <= 1)) return fail("ir: prior %d: the variable needs an interval inside [0, 1]", k);
+            if (!(PV.transform == B200_IR_T_INTERVAL && PV.lo >= 0 && PV.hi <= 1)) return fail("ir: prior %d: the variable needs an interval inside [0, 1]", k);
             P.c0 = -(std::lgamma(F.p[0].value) + std::lgamma(F.p[1].value) - std::lgamma(F.p[0].value + F.p[1].value));
             break;
         default: return fail("ir: prior %d: density %d is not in the closed set", k, F.dist);
@@ -725,16 +724,17 @@ static int ir_bounds(IrPass& c, const b200_ir_lik& L, int l, IrLikD& D) {
     return 0;
 }
 
+static const char* ir_survival_name(int d) {  // SURVIVAL_LIKS' names in LIK_DISTS
+    return d == B200_IR_L_WEIBULL_LOG ? "weibull_log" : d == B200_IR_L_LOGNORMAL ? "lognormal" : d == B200_IR_L_CENSORED_WEIBULL_LOG ? "censored_weibull_log"
+         : d == B200_IR_L_CENSORED_LOGNORMAL ? "censored_lognormal" : d == B200_IR_L_TRUNCATED_WEIBULL_LOG ? "truncated_weibull_log" : "truncated_lognormal";
+}
 // Weibull / LogNormal, plain, censored or truncated (y: [N], or the [3][N] block (y, lower, upper)).  The device reads log y;
 // the censoring codes as for the censored Normal; the truncated forms' bounds, 0 / +inf where open (Weibull) or their logs,
 // -inf / +inf where open (LogNormal).  A LogNormal's -log(2 pi) / 2 - log y_i of every observation with a density is in c0.
 static int ir_survival(IrPass& c, const b200_ir_lik& L, int l, const b200_ir_param& slot, IrLikD& D) {
-    static const char* const names[] = {"weibull_log", "lognormal", "censored_weibull_log", "censored_lognormal",
-                                        "truncated_weibull_log", "truncated_lognormal"};
     const long long N = L.N;
-    const int k = L.dist - B200_IR_L_WEIBULL_LOG;
-    const bool weibull = k % 2 == 0, cens = k / 2 == 1, trunc = k / 2 == 2;
-    const char* what = names[k];
+    const bool weibull = ir_weibull_liks(L.dist), cens = ir_censored_survival_liks(L.dist), trunc = ir_truncated_survival_liks(L.dist);
+    const char* what = ir_survival_name(L.dist);
     if (weibull && L.sigma_kind != B200_IR_S_CONST && L.sigma_kind != B200_IR_S_REF)
         return fail("ir: likelihood %d: %s: alpha must be a constant or a scalar variable", l, what);
     if (weibull && !ir_scale_ok(slot, c.vars)) return fail("ir: likelihood %d: %s: alpha " B200_IR_SCALE_RULE, l, what);
@@ -854,7 +854,7 @@ static int ir_psi(IrPass& c, const b200_ir_lik& L, int l) {
         const b200_ir_factor& F = T.f[0];
         const IrVarD* V = ir_var_at(c.vars, F.offset);
         if (ir_touches_simplex(c.vars, F.offset, std::max(F.size, 1))) return fail("ir: likelihood %d: " B200_IR_SIMPLEX_USE, l);
-        if (F.idx || !V || V->size != 1 || F.size != 1 || V->transform != IRT_INTERVAL || !(V->lo >= 0.0 && V->hi <= 1.0))
+        if (F.idx || !V || V->size != 1 || F.size != 1 || V->transform != B200_IR_T_INTERVAL || !(V->lo >= 0.0 && V->hi <= 1.0))
             return fail("ir: likelihood %d: " B200_IR_PSI_VAR, l);
         TD.n_factors = 1;
         TD.f[0] = IrFactorD{F.offset, 1, nullptr, nullptr, nullptr};
@@ -875,7 +875,7 @@ static int ir_cutpoints(IrPass& c, const b200_ir_lik& L, int l) {
         if (ir_touches_simplex(c.vars, F.offset, std::max(F.size, 1))) return fail("ir: likelihood %d: " B200_IR_SIMPLEX_USE, l);
         if (F.idx || !V || V->size != F.size) return fail("ir: likelihood %d: the cutpoint factor must be a whole variable, unindexed", l);
         if (F.size != K - 1) return fail("ir: likelihood %d: " B200_IR_CUT_SIZE " (%d, K = %d)", l, F.size, K);
-        if (F.size > 1 && V->transform != IRT_ORDERED && V->transform != IRT_ORDERED_POSITIVE)
+        if (F.size > 1 && V->transform != B200_IR_T_ORDERED && V->transform != B200_IR_T_ORDERED_POSITIVE)
             return fail("ir: likelihood %d: " B200_IR_CUT_ORDERED, l);
         TD.n_factors = 1;
         TD.f[0] = IrFactorD{F.offset, F.size, nullptr, nullptr, nullptr};
@@ -922,10 +922,10 @@ static int ir_mixture_blocks(IrPass& c, const b200_ir_lik& L, int l) {
             const b200_ir_factor& F = T.f[0];
             const IrVarD* V = ir_var_at(c.vars, F.offset);
             const bool whole = V && !F.idx && F.size == V->size;
-            if (b != 0 && whole && V->transform == IRT_SIMPLEX) return fail("ir: likelihood %d: " B200_IR_SIMPLEX_USE, l);
-            const bool ok = whole && (b == 0   ? V->transform == IRT_SIMPLEX && V->size == K - 1
+            if (b != 0 && whole && V->transform == B200_IR_T_SIMPLEX) return fail("ir: likelihood %d: " B200_IR_SIMPLEX_USE, l);
+            const bool ok = whole && (b == 0   ? V->transform == B200_IR_T_SIMPLEX && V->size == K - 1
                                       : b == 2 ? (V->size == 1 || V->size == K) && ir_positive_support(*V)
-                                      : normal ? V->size == K && (V->transform == IRT_NONE || V->transform == IRT_ORDERED)
+                                      : normal ? V->size == K && (V->transform == B200_IR_T_NONE || V->transform == B200_IR_T_ORDERED)
                                                : V->size == K && ir_positive_support(*V));
             if (!ok) return fail("ir: likelihood %d: %s", l, what);
             TD.n_factors = 1;
@@ -956,16 +956,15 @@ static int ir_lik(IrPass& c, const b200_ir_lik& L, int l, IrLikD& D) {
         return fail("ir: likelihood %d: a latent factor (y_var > 0) is a normal or studentt prior with a Linear location; dist %d is neither", l, L.dist);
     if (latent && L.N != c.vars[L.y_var - 1].size)
         return fail("ir: likelihood %d: a latent factor's N (%lld) must equal the size of its variable (%d)", l, (long long)L.N, c.vars[L.y_var - 1].size);
-    if (latent && c.vars[L.y_var - 1].transform == IRT_SIMPLEX) return fail("ir: likelihood %d: " B200_IR_SIMPLEX_USE, l);
+    if (latent && c.vars[L.y_var - 1].transform == B200_IR_T_SIMPLEX) return fail("ir: likelihood %d: " B200_IR_SIMPLEX_USE, l);
     if (L.N <= 0 || L.N > 0x7fffffff || (!latent && !L.y)) return fail("ir: likelihood %d: missing observations", l);
-    const bool mixture = L.dist == B200_IR_L_NORMAL_MIXTURE || L.dist == B200_IR_L_POISSON_MIXTURE;  // eta may be 0
+    const bool mixture = ir_mixture_liks(L.dist);  // eta may be 0
     if (L.n_terms < (mixture ? 0 : 1) || !L.terms) return fail("ir: likelihood %d: no linear-predictor terms", l);
     const long long N = L.N;
     c.max_obs = std::max(c.max_obs, N);
     D.dist = L.dist; D.n_terms = L.n_terms; D.term0 = (int)c.terms.size(); D.sigma_kind = L.sigma_kind; D.N = N; D.nu = L.nu;
     D.yoff = latent ? c.vars[L.y_var - 1].offset : -1;
-    const bool survival = L.dist >= B200_IR_L_WEIBULL_LOG && L.dist <= B200_IR_L_TRUNCATED_LOGNORMAL;
-    if (!latent && !survival) c.add(&D.y, L.y, (size_t)N);  // a survival likelihood's device y is log y (ir_survival)
+    if (!latent && !ir_survival_liks(L.dist)) c.add(&D.y, L.y, (size_t)N);  // a survival likelihood's device y is log y (ir_survival)
     if (ir_param(L.sigma, c.n, &D.sigma, "likelihood sigma")) return -1;
     if (L.sigma_kind == B200_IR_S_REF && L.sigma.kind != 1) return fail("ir: likelihood %d: sigma_kind REF needs a reference", l);
     if (L.sigma_kind == B200_IR_S_REF && ir_ref_simplex(c.vars, L.sigma)) return fail("ir: likelihood %d: " B200_IR_SIMPLEX_USE, l);
@@ -976,7 +975,16 @@ static int ir_lik(IrPass& c, const b200_ir_lik& L, int l, IrLikD& D) {
         c.add(&D.sigma_obs, L.sigma_obs, (size_t)N);
     }
     int rc = 0;
-    switch (L.dist) {
+    if (ir_bounded_liks(L.dist)) rc = ir_bounds(c, L, l, D);
+    else if (ir_ordinal_liks(L.dist)) rc = ir_ordinal(c, L, l);
+    else if (ir_survival_liks(L.dist)) rc = ir_survival(c, L, l, slot, D);
+    else if (ir_mixture_liks(L.dist)) rc = ir_mixture_obs(c, L, l, D);
+    else if (ir_zi_liks(L.dist)) {  // nu: the form of the psi block
+        if (!(L.nu >= 0 && L.nu == std::floor(L.nu) && L.nu <= 0x7fff)) return fail("ir: likelihood %d: " B200_IR_PSI_NU, l);
+        const int fam = ir_zi_family(L.dist);
+        if (fam == B200_IR_L_POISSON_LOG && L.sigma_kind != B200_IR_S_NONE) return fail("ir: likelihood %d: " B200_IR_ZIP_SLOT, l);
+        rc = ir_family(c, L, l, slot, fam, fam == B200_IR_L_GAMMA_LOG ? B200_IR_HG_Y : B200_IR_ZI_Y, true, D);
+    } else switch (L.dist) {
         case B200_IR_L_NORMAL: case B200_IR_L_NORMAL_LOGVAR: D.c0 = -(double)N * B200_HALF_LOG_2PI; break;
         case B200_IR_L_BERNOULLI_LOGIT:
             for (long long i = 0; i < N; ++i)
@@ -990,30 +998,10 @@ static int ir_lik(IrPass& c, const b200_ir_lik& L, int l, IrLikD& D) {
         case B200_IR_L_BINOMIAL_LOGIT: rc = ir_family(c, L, l, slot, L.dist, "Binomial y must be an integer in [0, n]", false, D); break;
         case B200_IR_L_NEGBINOMIAL_LOG: rc = ir_family(c, L, l, slot, L.dist, "NegativeBinomial y must be an integer >= 0", false, D); break;
         case B200_IR_L_GAMMA_LOG: rc = ir_family(c, L, l, slot, L.dist, "Gamma y must be > 0", false, D); break;
-        case B200_IR_L_CENSORED_NORMAL: case B200_IR_L_TRUNCATED_NORMAL: rc = ir_bounds(c, L, l, D); break;
-        case B200_IR_L_ORDERED_LOGISTIC: case B200_IR_L_ORDERED_PROBIT: rc = ir_ordinal(c, L, l); break;
-        case B200_IR_L_WEIBULL_LOG: case B200_IR_L_LOGNORMAL: case B200_IR_L_CENSORED_WEIBULL_LOG:
-        case B200_IR_L_CENSORED_LOGNORMAL: case B200_IR_L_TRUNCATED_WEIBULL_LOG: case B200_IR_L_TRUNCATED_LOGNORMAL:
-            rc = ir_survival(c, L, l, slot, D);
-            break;
-        case B200_IR_L_ZERO_INFLATED_POISSON: case B200_IR_L_ZERO_INFLATED_BINOMIAL:
-        case B200_IR_L_ZERO_INFLATED_NEGATIVE_BINOMIAL: case B200_IR_L_HURDLE_POISSON:
-        case B200_IR_L_HURDLE_NEGATIVE_BINOMIAL: case B200_IR_L_HURDLE_GAMMA: {  // nu: the form of the psi block
-            if (!(L.nu >= 0 && L.nu == std::floor(L.nu) && L.nu <= 0x7fff)) return fail("ir: likelihood %d: " B200_IR_PSI_NU, l);
-            static const int family[] = {B200_IR_L_POISSON_LOG, B200_IR_L_BINOMIAL_LOGIT, B200_IR_L_NEGBINOMIAL_LOG,
-                                         B200_IR_L_POISSON_LOG, B200_IR_L_NEGBINOMIAL_LOG, B200_IR_L_GAMMA_LOG};
-            const int fam = family[L.dist - B200_IR_L_ZERO_INFLATED_POISSON];
-            if (fam == B200_IR_L_POISSON_LOG && L.sigma_kind != B200_IR_S_NONE) return fail("ir: likelihood %d: " B200_IR_ZIP_SLOT, l);
-            rc = ir_family(c, L, l, slot, fam, fam == B200_IR_L_GAMMA_LOG ? B200_IR_HG_Y : B200_IR_ZI_Y, true, D);
-        } break;
-        case B200_IR_L_NORMAL_MIXTURE: case B200_IR_L_POISSON_MIXTURE: rc = ir_mixture_obs(c, L, l, D); break;
         default: return fail("ir: likelihood %d: density %d is not in the closed set", l, L.dist);
     }
     if (rc) return rc;
-    const bool has_sigma = L.dist == B200_IR_L_NORMAL || L.dist == B200_IR_L_STUDENTT || L.dist == B200_IR_L_CENSORED_NORMAL ||
-                           L.dist == B200_IR_L_TRUNCATED_NORMAL || L.dist == B200_IR_L_ORDERED_PROBIT ||
-                           L.dist == B200_IR_L_LOGNORMAL || L.dist == B200_IR_L_CENSORED_LOGNORMAL ||
-                           L.dist == B200_IR_L_TRUNCATED_LOGNORMAL;
+    const bool has_sigma = ir_sigma_liks(L.dist);
     if (has_sigma && L.sigma_kind == B200_IR_S_NONE) return fail("ir: likelihood %d needs sigma", l);
     if (has_sigma && L.sigma_kind == B200_IR_S_OBS) {
         for (long long i = 0; i < N; ++i)
@@ -1024,13 +1012,13 @@ static int ir_lik(IrPass& c, const b200_ir_lik& L, int l, IrLikD& D) {
     }
     if (ir_terms(c, L, l, 0, L.n_terms)) return -1;
     if (mixture) return ir_mixture_blocks(c, L, l);
-    if (L.dist == B200_IR_L_ORDERED_LOGISTIC || L.dist == B200_IR_L_ORDERED_PROBIT) return ir_cutpoints(c, L, l);
-    return L.dist >= B200_IR_L_ZERO_INFLATED_POISSON && L.dist <= B200_IR_L_HURDLE_GAMMA ? ir_psi(c, L, l) : 0;
+    if (ir_ordinal_liks(L.dist)) return ir_cutpoints(c, L, l);
+    return ir_zi_liks(L.dist) ? ir_psi(c, L, l) : 0;
 }
 
 static int ir_ar1(const IrPass& c, const b200_ir_ar1& A, int k, IrAr1D& D) {
     if (A.var < 0 || A.var >= (int)c.vars.size() || c.vars[A.var].size < 2) return fail("ir: ar1 %d: bad variable", k);
-    if (c.vars[A.var].transform == IRT_SIMPLEX || ir_ref_simplex(c.vars, A.phi) || ir_ref_simplex(c.vars, A.sigma))
+    if (c.vars[A.var].transform == B200_IR_T_SIMPLEX || ir_ref_simplex(c.vars, A.phi) || ir_ref_simplex(c.vars, A.sigma))
         return fail("ir: ar1 %d: " B200_IR_SIMPLEX_USE, k);
     if (!(A.init_sigma > 0)) return fail("ir: ar1 %d: init_sigma must be > 0", k);
     D.offset = c.vars[A.var].offset; D.size = c.vars[A.var].size; D.init_sigma = A.init_sigma;
@@ -1049,7 +1037,7 @@ static int prepare_ir(b200_model* m, const b200_model_desc* d) {
     for (int k = 0; k < R->n_priors; ++k)
         if (ir_prior(c, R->priors[k], k, priors[k])) return -1;
     for (size_t v = 0; v < c.vars.size(); ++v)
-        if (c.vars[v].transform == IRT_SIMPLEX && c.n_priors_of[v] != 1) return fail("ir: variable %d: " B200_IR_SIMPLEX_PRIOR, (int)v);
+        if (c.vars[v].transform == B200_IR_T_SIMPLEX && c.n_priors_of[v] != 1) return fail("ir: variable %d: " B200_IR_SIMPLEX_PRIOR, (int)v);
     m->ir_liks.assign(std::max(R->n_liks, 0), IrLikD{});  // filled in place: sg holds the addresses of their pointers
     for (int l = 0; l < R->n_liks; ++l)
         if (ir_lik(c, R->liks[l], l, m->ir_liks[l])) return -1;
@@ -1069,8 +1057,8 @@ static int prepare_ir(b200_model* m, const b200_model_desc* d) {
     const long long row2 = std::max(std::max(c.ord_obs, c.zeta_obs), c.mix_obs);
     P.ord_row = row2 ? (int)(P.n_pad + ((c.max_obs + 3) & ~3LL)) : 0;  // after r, before the design partials
     P.stride = P.n_pad + ((c.max_obs + 3) & ~3LL) + ((row2 + 3) & ~3LL) + (c.has_design ? kIrPartDoubles : 0);
-    m->ir_extended = std::any_of(c.vars.begin(), c.vars.end(), [](const IrVarD& V) { return V.transform >= IRT_ORDERED; }) ||
-                     std::any_of(m->ir_liks.begin(), m->ir_liks.end(), [](const IrLikD& L) { return L.dist >= B200_IR_L_CENSORED_NORMAL; });
+    m->ir_extended = std::any_of(c.vars.begin(), c.vars.end(), [](const IrVarD& V) { return ir_extended_transforms(V.transform); }) ||
+                     std::any_of(m->ir_liks.begin(), m->ir_liks.end(), [](const IrLikD& L) { return ir_extended_liks(L.dist); });
     return 0;
 }
 
@@ -1192,7 +1180,7 @@ static int dispatch(const b200_model* m, F&& f) {
             B200_TEAM(StochVolModel, m->stochvol)
             return fail("stochvol: n=%d exceeds 4096", m->n);
         case B200_MODEL_IR:
-            if (m->ir_extended) {  // a censored / truncated Normal likelihood: the kernels that can evaluate it
+            if (m->ir_extended) {  // a factor IrModel leaves out: the kernels that can evaluate it
                 if (m->n <= 256 && !env_flag("B200_FORCE_TEAM")) { B200_WARP(IrExtendedModel, m->ir) }
                 B200_TEAM(IrExtendedModel, m->ir)
             } else {

@@ -18,20 +18,37 @@
 // sigma.  Its normalising terms are not per observation: Gamma's once per evaluation, NegativeBinomial's over a table of
 // the distinct nonzero counts (csrc/b200nuts.cu: prepare_ir), with digamma() of common.cuh for the gradient.
 #pragma once
+#include "../../include/b200nuts.h"
 #include "common.cuh"
 
 namespace b200 {
 
-enum { IRT_NONE = 0, IRT_LOG = 1, IRT_INTERVAL = 2, IRT_ORDERED = 3, IRT_ORDERED_POSITIVE = 4, IRT_SIMPLEX = 5 };
-enum { IRP_FLAT = 0, IRP_NORMAL, IRP_HALFNORMAL, IRP_CAUCHY, IRP_HALFCAUCHY, IRP_EXPONENTIAL, IRP_STUDENTT, IRP_UNIFORM,
-       IRP_GAMMA, IRP_BETA, IRP_LOGNORMAL, IRP_DIRICHLET };
-enum { IRL_NORMAL = 0, IRL_BERNOULLI_LOGIT, IRL_POISSON_LOG, IRL_STUDENTT, IRL_NORMAL_LOGVAR, IRL_BINOMIAL_LOGIT,
-       IRL_NEGBINOMIAL_LOG, IRL_GAMMA_LOG, IRL_CENSORED_NORMAL, IRL_TRUNCATED_NORMAL, IRL_ORDERED_LOGISTIC,
-       IRL_ORDERED_PROBIT, IRL_ZI_POISSON, IRL_ZI_BINOMIAL, IRL_ZI_NEGBINOMIAL, IRL_HURDLE_POISSON, IRL_HURDLE_NEGBINOMIAL,
-       IRL_HURDLE_GAMMA, IRL_WEIBULL_LOG, IRL_LOGNORMAL, IRL_CENSORED_WEIBULL_LOG, IRL_CENSORED_LOGNORMAL,
-       IRL_TRUNCATED_WEIBULL_LOG, IRL_TRUNCATED_LOGNORMAL, IRL_NORMAL_MIXTURE, IRL_POISSON_MIXTURE };
-enum { IRS_NONE = 0, IRS_CONST, IRS_REF, IRS_OBS };
 constexpr double kNegBinPoissonAlpha = 1e10;  // above: NegativeBinomial -> Poisson(mu) limit (discrete.py:727-735)
+
+// ---- the likelihood groups prepare_ir and the device branch on, each named after its pymc_b200/ir.py tuple; ranges: static_assert
+__host__ __device__ __forceinline__ constexpr bool ir_bounded_liks(int d) { return d == B200_IR_L_CENSORED_NORMAL || d == B200_IR_L_TRUNCATED_NORMAL; }
+__host__ __device__ __forceinline__ constexpr bool ir_ordinal_liks(int d) { return d == B200_IR_L_ORDERED_LOGISTIC || d == B200_IR_L_ORDERED_PROBIT; }
+static_assert(B200_IR_L_ZERO_INFLATED_POISSON == 12 && B200_IR_L_ZERO_INFLATED_BINOMIAL == 13 && B200_IR_L_ZERO_INFLATED_NEGATIVE_BINOMIAL == 14 &&
+              B200_IR_L_HURDLE_POISSON == 15 && B200_IR_L_HURDLE_NEGATIVE_BINOMIAL == 16 && B200_IR_L_HURDLE_GAMMA == 17, "ZI_LIKS, the hurdles last");
+__host__ __device__ __forceinline__ constexpr bool ir_zi_liks(int d) { return d >= B200_IR_L_ZERO_INFLATED_POISSON && d <= B200_IR_L_HURDLE_GAMMA; }
+__host__ __device__ __forceinline__ constexpr bool ir_hurdle_liks(int d) { return d >= B200_IR_L_HURDLE_POISSON; }  // of a ZI_LIKS id
+__host__ __device__ __forceinline__ constexpr int ir_zi_family(int d) {  // ZI_FAMILY: a ZI_LIKS id's family, whose slot (trials, alpha) it takes
+    return d == B200_IR_L_ZERO_INFLATED_BINOMIAL ? B200_IR_L_BINOMIAL_LOGIT : d == B200_IR_L_HURDLE_GAMMA ? B200_IR_L_GAMMA_LOG
+         : d == B200_IR_L_ZERO_INFLATED_NEGATIVE_BINOMIAL || d == B200_IR_L_HURDLE_NEGATIVE_BINOMIAL ? B200_IR_L_NEGBINOMIAL_LOG : B200_IR_L_POISSON_LOG;
+}
+__host__ __device__ __forceinline__ constexpr bool ir_weibull_liks(int d) { return d == B200_IR_L_WEIBULL_LOG || d == B200_IR_L_CENSORED_WEIBULL_LOG || d == B200_IR_L_TRUNCATED_WEIBULL_LOG; }
+__host__ __device__ __forceinline__ constexpr bool ir_lognormal_liks(int d) { return d == B200_IR_L_LOGNORMAL || d == B200_IR_L_CENSORED_LOGNORMAL || d == B200_IR_L_TRUNCATED_LOGNORMAL; }
+static_assert(B200_IR_L_WEIBULL_LOG == 18 && B200_IR_L_LOGNORMAL == 19 && B200_IR_L_CENSORED_WEIBULL_LOG == 20 && B200_IR_L_CENSORED_LOGNORMAL == 21 &&
+              B200_IR_L_TRUNCATED_WEIBULL_LOG == 22 && B200_IR_L_TRUNCATED_LOGNORMAL == 23, "SURVIVAL_LIKS");
+__host__ __device__ __forceinline__ constexpr bool ir_survival_liks(int d) { return d >= B200_IR_L_WEIBULL_LOG && d <= B200_IR_L_TRUNCATED_LOGNORMAL; }
+__host__ __device__ __forceinline__ constexpr bool ir_censored_survival_liks(int d) { return d == B200_IR_L_CENSORED_WEIBULL_LOG || d == B200_IR_L_CENSORED_LOGNORMAL; }
+__host__ __device__ __forceinline__ constexpr bool ir_truncated_survival_liks(int d) { return d == B200_IR_L_TRUNCATED_WEIBULL_LOG || d == B200_IR_L_TRUNCATED_LOGNORMAL; }
+__host__ __device__ __forceinline__ constexpr bool ir_mixture_liks(int d) { return d == B200_IR_L_NORMAL_MIXTURE || d == B200_IR_L_POISSON_MIXTURE; }
+__host__ __device__ __forceinline__ constexpr bool ir_sigma_liks(int d) { return d == B200_IR_L_NORMAL || d == B200_IR_L_STUDENTT || ir_bounded_liks(d) || d == B200_IR_L_ORDERED_PROBIT || ir_lognormal_liks(d); }
+// the likelihoods and transforms that IrModel leaves out and IrExtendedModel evaluates out of line (below)
+__host__ __device__ __forceinline__ constexpr bool ir_extended_liks(int d) { return ir_ordinal_liks(d) || ir_zi_liks(d) || ir_mixture_liks(d) || ir_bounded_liks(d) || ir_survival_liks(d); }
+static_assert(B200_IR_T_ORDERED == 3 && B200_IR_T_ORDERED_POSITIVE == 4 && B200_IR_T_SIMPLEX == 5, "the last three transforms");
+__host__ __device__ __forceinline__ constexpr bool ir_extended_transforms(int t) { return t >= B200_IR_T_ORDERED; }  // ORDERED_TRANSFORMS and simplex
 
 struct IrParamD { int kind, ref; double value; };                     // kind 0: constant; 1: x[ref] (a scalar variable)
 struct IrVarD { int offset, size, transform, pad; double lo, hi; };  // pad: a simplex variable's rows (below)
@@ -135,10 +152,10 @@ __device__ __forceinline__ double ir_eta(const IrTermD* const& terms, int term0,
 // x = backward(z) of one element of a log / interval variable, log|dx/dz| added to lj (transforms.py:880-891, :1026-1073)
 __device__ __forceinline__ double ir_backward(const IrVarD& V, double z, double& lj) {
     double xv = z;
-    if (V.transform == IRT_LOG) {
+    if (V.transform == B200_IR_T_LOG) {
         xv = exp(z);
         lj += z;
-    } else if (V.transform == IRT_INTERVAL) {
+    } else if (V.transform == B200_IR_T_INTERVAL) {
         xv = V.lo + (V.hi - V.lo) * sigmoid(z);
         lj += log(V.hi - V.lo) - softplus(-z) - softplus(z);
     }
@@ -147,12 +164,12 @@ __device__ __forceinline__ double ir_backward(const IrVarD& V, double z, double&
 
 // the value of the slot (sigma, the Binomial's trials or alpha) where it is a constant or a scalar variable
 __device__ __forceinline__ double ir_slot(const IrLikD& L, const double* x) {
-    return (L.sigma_kind == IRS_REF) ? x[L.sigma.ref] : L.sigma.value;
+    return (L.sigma_kind == B200_IR_S_REF) ? x[L.sigma.ref] : L.sigma.value;
 }
 
 // the scale (or the Binomial's trials) of observation i: its own value, or the slot's sg_s
 __device__ __forceinline__ double ir_scale(const IrLikD& L, int i, double sg_s) {
-    return (L.sigma_kind == IRS_OBS) ? L.sigma_obs[i] : sg_s;
+    return (L.sigma_kind == B200_IR_S_OBS) ? L.sigma_obs[i] : sg_s;
 }
 
 // The NegativeBinomial (discrete.py:700-745, n = a, p = a / (mu + a)) at d = eta - log a: lse = logaddexp(eta, log a) =
@@ -172,38 +189,38 @@ __device__ __forceinline__ double ir_base_term(const IrLikD& L, int i, double yi
                                                double& lp, double& s_sig) {
     double ri = 0.0;
     switch (L.dist) {
-        case IRL_NORMAL: {  // continuous.py:526-527
+        case B200_IR_L_NORMAL: {  // continuous.py:526-527
             const double sg = ir_scale(L, i, sg_s);
             const double z = (yi - eta) / sg;
             lp += -0.5 * z * z - log(sg);
             ri = z / sg; s_sig += (z * z - 1.0) / sg;
         } break;
-        case IRL_BERNOULLI_LOGIT:  // discrete.py:362-367 in PyTensor's stabilised forms
+        case B200_IR_L_BERNOULLI_LOGIT:  // discrete.py:362-367 in PyTensor's stabilised forms
             lp += yi * eta - softplus(eta);
             ri = yi - sigmoid(eta);
             break;
-        case IRL_POISSON_LOG: {  // discrete.py:581-586
+        case B200_IR_L_POISSON_LOG: {  // discrete.py:581-586
             const double mu = exp(eta);
             lp += yi * eta - mu;
             ri = yi - mu;
         } break;
-        case IRL_STUDENTT: {  // continuous.py:1936-1944
+        case B200_IR_L_STUDENTT: {  // continuous.py:1936-1944
             const double sg = ir_scale(L, i, sg_s);
             const double z = (yi - eta) / sg;
             lp += -log(sg) - 0.5 * (L.nu + 1.0) * log1p(z * z / L.nu);
             ri = (L.nu + 1.0) * z / (sg * (L.nu + z * z)); s_sig += -1.0 / sg + ri * z;
         } break;
-        case IRL_NORMAL_LOGVAR: {  // Normal(0, exp(eta / 2))
+        case B200_IR_L_NORMAL_LOGVAR: {  // Normal(0, exp(eta / 2))
             const double w = yi * yi * exp(-eta);
             lp += -0.5 * w - 0.5 * eta;
             ri = 0.5 * w - 0.5;
         } break;
-        case IRL_BINOMIAL_LOGIT: {  // discrete.py:141-152 in PyTensor's stabilised forms
+        case B200_IR_L_BINOMIAL_LOGIT: {  // discrete.py:141-152 in PyTensor's stabilised forms
             const double nt = ir_scale(L, i, sg_s);
             lp += yi * eta - nt * softplus(eta);
             ri = yi - nt * sigmoid(eta);
         } break;
-        case IRL_NEGBINOMIAL_LOG:  // the lgamma part is in c0 / eval's alpha terms
+        case B200_IR_L_NEGBINOMIAL_LOG:  // the lgamma part is in c0 / eval's alpha terms
             if (sg_s > kNegBinPoissonAlpha) {  // uniform branch: the Poisson(mu) limit
                 const double mu = exp(eta);
                 lp += yi * eta - mu;
@@ -215,7 +232,7 @@ __device__ __forceinline__ double ir_base_term(const IrLikD& L, int i, double yi
                 s_sig += 1.0 - nb.sp - nb.sc * (1.0 + yi / sg_s);  // d/da except psi(y + a) - psi(a)
             }
             break;
-        case IRL_GAMMA_LOG: {  // continuous.py:2512-2521, beta = a exp(-eta); the eta-free part: c0 / alpha terms
+        case B200_IR_L_GAMMA_LOG: {  // continuous.py:2512-2521, beta = a exp(-eta); the eta-free part: c0 / alpha terms
             const double w = yi * exp(-eta);
             lp -= sg_s * (eta + w);
             ri = sg_s * (w - 1.0);
@@ -230,16 +247,16 @@ __device__ __forceinline__ double ir_base_term(const IrLikD& L, int i, double yi
 // of a base family, and of the count / positive component f of a zero-inflated or hurdle likelihood at y > 0.
 __device__ __forceinline__ double ir_obs_const(const IrLikD& L, int i, double y, double sg_s, double la) {
     switch (L.dist) {
-        case IRL_NORMAL: case IRL_NORMAL_LOGVAR: return -B200_HALF_LOG_2PI;
-        case IRL_STUDENTT: return lgamma(0.5 * (L.nu + 1.0)) - lgamma(0.5 * L.nu) - 0.5 * log(L.nu * 3.14159265358979323846);
-        case IRL_POISSON_LOG: case IRL_ZI_POISSON: case IRL_HURDLE_POISSON: return -lgamma(y + 1.0);
-        case IRL_BINOMIAL_LOGIT: case IRL_ZI_BINOMIAL: {  // binomln(n, y)
+        case B200_IR_L_NORMAL: case B200_IR_L_NORMAL_LOGVAR: return -B200_HALF_LOG_2PI;
+        case B200_IR_L_STUDENTT: return lgamma(0.5 * (L.nu + 1.0)) - lgamma(0.5 * L.nu) - 0.5 * log(L.nu * 3.14159265358979323846);
+        case B200_IR_L_POISSON_LOG: case B200_IR_L_ZERO_INFLATED_POISSON: case B200_IR_L_HURDLE_POISSON: return -lgamma(y + 1.0);
+        case B200_IR_L_BINOMIAL_LOGIT: case B200_IR_L_ZERO_INFLATED_BINOMIAL: {  // binomln(n, y)
             const double nt = ir_scale(L, i, sg_s);
             return lgamma(nt + 1.0) - lgamma(y + 1.0) - lgamma(nt - y + 1.0);
         }
-        case IRL_NEGBINOMIAL_LOG: case IRL_ZI_NEGBINOMIAL: case IRL_HURDLE_NEGBINOMIAL:
+        case B200_IR_L_NEGBINOMIAL_LOG: case B200_IR_L_ZERO_INFLATED_NEGATIVE_BINOMIAL: case B200_IR_L_HURDLE_NEGATIVE_BINOMIAL:
             return sg_s > kNegBinPoissonAlpha ? -lgamma(y + 1.0) : lgamma(y + sg_s) - lgamma(sg_s) - lgamma(y + 1.0);
-        case IRL_GAMMA_LOG: case IRL_HURDLE_GAMMA: return sg_s * la - lgamma(sg_s) + (sg_s - 1.0) * log(y);
+        case B200_IR_L_GAMMA_LOG: case B200_IR_L_HURDLE_GAMMA: return sg_s * la - lgamma(sg_s) + (sg_s - 1.0) * log(y);
         default: return 0.0;
     }
 }
@@ -253,7 +270,7 @@ __device__ __forceinline__ double ir_obs_const(const IrLikD& L, int i, double y,
 struct IrBoundedTerm { double lp, r, s; };
 __device__ __forceinline__ IrBoundedTerm ir_bounded_term(const IrLikD& L, int i, double eta, double sg) {
     const double z = (L.y[i] - eta) / sg;
-    if (L.dist != IRL_TRUNCATED_NORMAL && L.dist != IRL_TRUNCATED_LOGNORMAL) {
+    if (L.dist != B200_IR_L_TRUNCATED_NORMAL && L.dist != B200_IR_L_TRUNCATED_LOGNORMAL) {
         const int c = L.cens ? L.cens[i] : 0;
         if (c == 0) return {-0.5 * z * z - log(sg), z / sg, (z * z - 1.0) / sg};
         const double zc = c == 1 ? z : -z;
@@ -272,10 +289,6 @@ __device__ __forceinline__ IrBoundedTerm ir_bounded_term(const IrLikD& L, int i,
 // log F = log(1 - e^-t).  log S is written directly (the reference has no Weibull logccdf and takes log(1 - F), which
 // loses every digit for small t); log F takes log t - t / 2 where t < 2e-9, so it stays finite after t underflows.  t
 // overflowing for y far above beta gives log S = -inf, which is the value.
-__device__ __forceinline__ bool ir_weibull(int dist) {
-    return dist == IRL_WEIBULL_LOG || dist == IRL_CENSORED_WEIBULL_LOG || dist == IRL_TRUNCATED_WEIBULL_LOG;
-}
-__device__ __forceinline__ bool ir_survival(int dist) { return dist >= IRL_WEIBULL_LOG && dist <= IRL_TRUNCATED_LOGNORMAL; }
 // log(1 - e^-t) given v = log t and t
 __device__ __forceinline__ double ir_log1mexp_neg(double v, double t) {
     return v < -20.0 ? v - 0.5 * t : (t < 0.6931471805599453 ? log(-expm1(-t)) : log1p(-exp(-t)));
@@ -331,7 +344,7 @@ __device__ __noinline__ IrPartials ir_bounded_pass(const IrLikD* Lp, const IrTer
     constexpr int TS = 32 * W;
     const IrLikD& L = *Lp;
     const int N = (int)L.N;
-    const bool weibull = ir_weibull(L.dist);  // sg_s is alpha
+    const bool weibull = ir_weibull_liks(L.dist);  // sg_s is alpha
     const double la = weibull ? log(sg_s) : 0.0;
     double lp = 0.0, s_sig = 0.0;
     for (int i = tid; i < N; i += TS) {
@@ -362,7 +375,7 @@ __device__ __forceinline__ IrOrdinalTerm ir_ordinal_term(const IrLikD& L, const 
     const double* c = C.n_factors ? x + C.f[0].offset : C.coef;
     const bool lo_open = y == 0, hi_open = y == K - 1;
     const double a = lo_open ? -INFINITY : (c[y - 1] - eta) / s, b = hi_open ? INFINITY : (c[y] - eta) / s;
-    if (L.dist == IRL_ORDERED_PROBIT) {
+    if (L.dist == B200_IR_L_ORDERED_PROBIT) {
         const NormalMass M = normal_log_mass(a, b);
         const double ta = M.ra == 0.0 ? 0.0 : a * M.ra, tb = M.rb == 0.0 ? 0.0 : b * M.rb;  // inf * 0 = 0
         return {M.log_z, M.ra - M.rb, M.rb / s, (ta - tb) / s};
@@ -389,7 +402,7 @@ __device__ __noinline__ IrPartials ir_ordinal_pass(const IrLikD* Lp, const IrTer
     double lp = 0.0, s_sig = 0.0;
     for (int i = tid; i < N; i += TS) {
         const double eta = ir_eta(terms + L.term0, 0, L.n_terms, x, i, N);
-        const double s = ir_scale(L, i, L.sigma_kind == IRS_NONE ? 1.0 : sg_s);  // the logistic link: s = 1
+        const double s = ir_scale(L, i, L.sigma_kind == B200_IR_S_NONE ? 1.0 : sg_s);  // the logistic link: s = 1
         const IrOrdinalTerm o = ir_ordinal_term(L, C, x, i, eta, s);
         lp += o.lp;
         s_sig += o.ds;
@@ -447,17 +460,17 @@ __device__ __forceinline__ IrZiTerm ir_zi_term(int dist, double y, double eta, d
     // the family: lf = log f(y) less its constants, rf / af = its eta / alpha derivatives; lP0 = log P0 with r0 / a0;
     // lm = log(-lP0)
     double lf, rf, af = 0.0, lP0 = -INFINITY, r0 = 0.0, a0 = 0.0, lm = INFINITY;
-    if (dist == IRL_HURDLE_GAMMA) {  // continuous.py:2512-2521, beta = a exp(-eta)
+    if (dist == B200_IR_L_HURDLE_GAMMA) {  // continuous.py:2512-2521, beta = a exp(-eta)
         const double w = y * exp(-eta);
         lf = -a * (eta + w);
         rf = a * (w - 1.0);
         af = -(eta + w);
-    } else if (dist == IRL_ZI_BINOMIAL) {  // discrete.py:141-152 in PyTensor's stabilised forms
+    } else if (dist == B200_IR_L_ZERO_INFLATED_BINOMIAL) {  // discrete.py:141-152 in PyTensor's stabilised forms
         lP0 = -nt * softplus(eta);
         r0 = -nt * sigmoid(eta);
         lf = y * eta + lP0;
         rf = y + r0;
-    } else if (dist != IRL_ZI_POISSON && dist != IRL_HURDLE_POISSON && a <= kNegBinPoissonAlpha) {  // discrete.py:700-745
+    } else if (dist != B200_IR_L_ZERO_INFLATED_POISSON && dist != B200_IR_L_HURDLE_POISSON && a <= kNegBinPoissonAlpha) {  // discrete.py:700-745
         const IrNegBin nb = ir_negbin(eta, la);
         lP0 = -a * nb.sp;
         r0 = -a * nb.s;
@@ -474,7 +487,7 @@ __device__ __forceinline__ IrZiTerm ir_zi_term(int dist, double y, double eta, d
         rf = y - mu;
         lm = eta;
     }
-    const bool hurdle = dist >= IRL_HURDLE_POISSON;
+    const bool hurdle = ir_hurdle_liks(dist);
     if (y == 0.0) {
         if (hurdle) return {l1psi, 0.0, -psi, -exp(-l1psi), 0.0};
         const double t = lpsi + lP0, u = t - l1psi;  // u: the log-odds of the count component at a zero
@@ -484,7 +497,7 @@ __device__ __forceinline__ IrZiTerm ir_zi_term(int dist, double y, double eta, d
         return {lp, w * r0, w - psi, expm1(lP0) * exp(-lp), w * a0};
     }
     IrZiTerm o{lpsi + lf, rf, 1.0 - psi, exp(-lpsi), af};
-    if (hurdle && dist != IRL_HURDLE_GAMMA) {  // - log(1 - P0)
+    if (hurdle && dist != B200_IR_L_HURDLE_GAMMA) {  // - log(1 - P0)
         if (lm < -700.0) {  // m = -log P0 < 1e-304: log(1 - e^-m) = log m, d log m / d eta = 1, d log m / d a = 0
             o.lp -= lm;
             o.r -= 1.0;
@@ -531,7 +544,7 @@ __device__ __noinline__ IrZiPartials ir_zi_pass(const IrLikD* Lp, const IrTermD*
 // order): O(size) serial work per evaluation, for vectors as short as cutpoints are.
 __device__ __noinline__ double ir_ordered_forward(const IrVarD* Vp, const double* q, double* x) {
     const int o = Vp->offset, n = Vp->size;
-    const bool pos = Vp->transform == IRT_ORDERED_POSITIVE;
+    const bool pos = Vp->transform == B200_IR_T_ORDERED_POSITIVE;
     double acc = pos ? exp(q[o]) : q[o], lj = pos ? q[o] : 0.0;
     x[o] = acc;
     for (int k = 1; k < n; ++k) {
@@ -547,7 +560,7 @@ __device__ __noinline__ double ir_ordered_forward(const IrVarD* Vp, const double
 // d/dz_0 = sum_k g_k otherwise.  The reverse cumulative sum runs k descending, on one thread.
 __device__ __noinline__ void ir_ordered_chain(const IrVarD* Vp, const double* q, double* g) {
     const int o = Vp->offset, n = Vp->size;
-    const bool pos = Vp->transform == IRT_ORDERED_POSITIVE;
+    const bool pos = Vp->transform == B200_IR_T_ORDERED_POSITIVE;
     double s = 0.0;
     for (int k = n - 1; k >= 0; --k) {
         s += g[o + k];
@@ -619,7 +632,7 @@ __device__ __forceinline__ IrMix ir_mix_block(const IrLikD& L, const IrTermD* te
     IrMix M{b[0].n_factors ? x + b[0].f[0].offset : b[0].coef, b[0].n_factors ? (double*)x + b[0].f[0].offset + K : nullptr,
             b[1].n_factors ? x + b[1].f[0].offset : b[1].coef, b[1].n_factors && g ? g + b[1].f[0].offset : nullptr,
             nullptr, nullptr, true};
-    if (L.dist == IRL_NORMAL_MIXTURE) {
+    if (L.dist == B200_IR_L_NORMAL_MIXTURE) {
         M.s = b[2].n_factors ? x + b[2].f[0].offset : b[2].coef;
         M.gs = b[2].n_factors && g ? g + b[2].f[0].offset : nullptr;
         M.s_vec = !b[2].n_factors || b[2].f[0].size > 1;
@@ -629,7 +642,7 @@ __device__ __forceinline__ IrMix ir_mix_block(const IrLikD& L, const IrTermD* te
 // log f_k(y) less its constant, with d / d eta (= d / d mu_k for the Normal), d / d lam_k or d / d sigma_k in dt.
 struct IrMixTerm { double lf, de, dc, ds; };
 __device__ __forceinline__ IrMixTerm ir_mix_term(int dist, const IrMix& M, int k, double y, double eta) {
-    if (dist == IRL_NORMAL_MIXTURE) {
+    if (dist == B200_IR_L_NORMAL_MIXTURE) {
         const double sg = M.s[M.s_vec ? k : 0], z = (y - eta - M.c[k]) / sg;
         return {-0.5 * z * z - log(sg), z / sg, z / sg, (z * z - 1.0) / sg};
     }
@@ -707,9 +720,8 @@ __device__ __noinline__ double ir_mixture_pass(const IrLikD* Lp, const IrTermD* 
     return lp;
 }
 
-// IrModel evaluates every factor of the closed set except the censored / truncated Normal, the ordinal, the zero-inflated,
-// the hurdle and the survival likelihoods and the ordered transform; IrExtendedModel (below) is the same function with those added,
-// each out of line.  A kernel's
+// IrModel evaluates every factor of the closed set except the likelihoods of ir_extended_liks and the transforms of
+// ir_extended_transforms; IrExtendedModel (below) is the same function with those added, each out of line.  A kernel's
 // register allocation covers every function it can reach, and the tail math takes about 128 registers, so the engine
 // instantiates its kernels twice and runs a model on IrExtendedModel only when it has one of them (b200_model.ir_extended):
 // every other IR model keeps the kernels it had before.
@@ -793,9 +805,9 @@ struct IrModel {
         for (int v = 0; v < P.n_vars; ++v) {
             const IrVarD V = P.vars[v];
             if constexpr (EXTENDED) {
-                if (V.transform >= IRT_ORDERED) {  // uniform branch: a prefix sum or a softmax, on one thread
+                if (ir_extended_transforms(V.transform)) {  // uniform branch: a prefix sum or a softmax, on one thread
                     if (tid == 0)
-                        lp += V.transform == IRT_SIMPLEX ? ir_simplex_forward(P.vars + v, q_s, x) : ir_ordered_forward(P.vars + v, q_s, x);
+                        lp += V.transform == B200_IR_T_SIMPLEX ? ir_simplex_forward(P.vars + v, q_s, x) : ir_ordered_forward(P.vars + v, q_s, x);
                     for (int j = tid; j < V.size; j += TS) g_s[V.offset + j] = 0.0;
                     continue;
                 }
@@ -811,9 +823,9 @@ struct IrModel {
         // ---- 2a. priors ---------------------------------------------------------------------------------------------
         for (int k = 0; k < P.n_priors; ++k) {
             const IrPriorD F = P.priors[k];
-            if (F.dist == IRP_FLAT) continue;
+            if (F.dist == B200_IR_P_FLAT) continue;
             if constexpr (EXTENDED) {
-                if (F.dist == IRP_DIRICHLET) {  // uniform branch: out of line, on one thread
+                if (F.dist == B200_IR_P_DIRICHLET) {  // uniform branch: out of line, on one thread
                     if (tid == 0) lp += ir_dirichlet(P.priors + k, x);
                     team_sync<W>();
                     continue;
@@ -826,46 +838,46 @@ struct IrModel {
                 const double xv = x[i];
                 double gxi = 0.0;
                 switch (F.dist) {
-                    case IRP_NORMAL: {  // continuous.py:526-527
+                    case B200_IR_P_NORMAL: {  // continuous.py:526-527
                         const double z = (xv - a0) / a1;
                         lp += -0.5 * z * z + F.c0 - log(a1);
                         gxi = -z / a1; s[0] += z / a1; s[1] += (z * z - 1.0) / a1;
                     } break;
-                    case IRP_HALFNORMAL: {  // continuous.py:909-911
+                    case B200_IR_P_HALFNORMAL: {  // continuous.py:909-911
                         const double z = xv / a0;
                         lp += -0.5 * z * z + F.c0 - log(a0);
                         gxi = -z / a0; s[0] += (z * z - 1.0) / a0;
                     } break;
-                    case IRP_CAUCHY: {  // continuous.py:2287-2288
+                    case B200_IR_P_CAUCHY: {  // continuous.py:2287-2288
                         const double u = xv - a0, den = a1 * a1 + u * u, t = u / a1;
                         lp += F.c0 - log(a1) - log1p(t * t);
                         gxi = -2.0 * u / den; s[0] += 2.0 * u / den; s[1] += (u * u - a1 * a1) / (a1 * den);
                     } break;
-                    case IRP_HALFCAUCHY: {  // continuous.py:2383-2385
+                    case B200_IR_P_HALFCAUCHY: {  // continuous.py:2383-2385
                         const double den = a0 * a0 + xv * xv, t = xv / a0;
                         lp += F.c0 - log(a0) - log1p(t * t);
                         gxi = -2.0 * xv / den; s[0] += (xv * xv - a0 * a0) / (a0 * den);
                     } break;
-                    case IRP_EXPONENTIAL:  // continuous.py:1478-1480 (mu = 1 / lam)
+                    case B200_IR_P_EXPONENTIAL:  // continuous.py:1478-1480 (mu = 1 / lam)
                         lp += log(a0) - a0 * xv;
                         gxi = -a0; s[0] += 1.0 / a0 - xv;
                         break;
-                    case IRP_STUDENTT: {  // continuous.py:1936-1944; a0 = nu (constant), a1 = mu, a2 = sigma
+                    case B200_IR_P_STUDENTT: {  // continuous.py:1936-1944; a0 = nu (constant), a1 = mu, a2 = sigma
                         const double z = (xv - a1) / a2;
                         lp += F.c0 - log(a2) - 0.5 * (a0 + 1.0) * log1p(z * z / a0);
                         const double w = (a0 + 1.0) * z / (a2 * (a0 + z * z));
                         gxi = -w; s[1] += w; s[2] += -1.0 / a2 + w * z;
                     } break;
-                    case IRP_UNIFORM: lp += F.c0; break;  // continuous.py:309-314
-                    case IRP_GAMMA:  // continuous.py:2512-2515
+                    case B200_IR_P_UNIFORM: lp += F.c0; break;  // continuous.py:309-314
+                    case B200_IR_P_GAMMA:  // continuous.py:2512-2515
                         lp += F.c0 + (a0 - 1.0) * log(xv) - a1 * xv;
                         gxi = (a0 - 1.0) / xv - a1;
                         break;
-                    case IRP_BETA:  // continuous.py:1250-1256
+                    case B200_IR_P_BETA:  // continuous.py:1250-1256
                         lp += F.c0 + (a0 - 1.0) * log(xv) + (a1 - 1.0) * log1p(-xv);
                         gxi = (a0 - 1.0) / xv - (a1 - 1.0) / (1.0 - xv);
                         break;
-                    case IRP_LOGNORMAL: {  // continuous.py:1807-1814
+                    case B200_IR_P_LOGNORMAL: {  // continuous.py:1807-1814
                         const double lx = log(xv), z = (lx - a0) / a1;
                         lp += -0.5 * z * z - lx + F.c0 - log(a1);
                         gxi = (-z / a1 - 1.0) / xv; s[0] += z / a1; s[1] += (z * z - 1.0) / a1;
@@ -892,16 +904,15 @@ struct IrModel {
             const IrLikD L = P.liks[l];
             const int N = (int)L.N;
             const double sg_s = ir_slot(L, x);
-            const bool zi = EXTENDED && L.dist >= IRL_ZI_POISSON && L.dist <= IRL_HURDLE_GAMMA;  // zero-inflated / hurdle
-            const bool gamma = L.dist == IRL_GAMMA_LOG || (EXTENDED && L.dist == IRL_HURDLE_GAMMA);
-            const bool disp = L.dist == IRL_NEGBINOMIAL_LOG || gamma ||  // sg_s is the dispersion alpha
-                              (EXTENDED && (L.dist == IRL_ZI_NEGBINOMIAL || L.dist == IRL_HURDLE_NEGBINOMIAL));
+            const bool zi = EXTENDED && ir_zi_liks(L.dist);  // zero-inflated / hurdle
+            const bool gamma = L.dist == B200_IR_L_GAMMA_LOG || (EXTENDED && L.dist == B200_IR_L_HURDLE_GAMMA);
+            const bool disp = L.dist == B200_IR_L_NEGBINOMIAL_LOG || gamma ||  // sg_s is the dispersion alpha
+                              (EXTENDED && (L.dist == B200_IR_L_ZERO_INFLATED_NEGATIVE_BINOMIAL || L.dist == B200_IR_L_HURDLE_NEGATIVE_BINOMIAL));
             const double la = disp ? log(sg_s) : 0.0;
             double s_sig = 0.0, s_psi = 0.0;
-            const bool ordinal = EXTENDED && (L.dist == IRL_ORDERED_LOGISTIC || L.dist == IRL_ORDERED_PROBIT);
-            const bool mixture = EXTENDED && (L.dist == IRL_NORMAL_MIXTURE || L.dist == IRL_POISSON_MIXTURE);
-            const bool bounded = EXTENDED && (ordinal || zi || mixture || L.dist == IRL_CENSORED_NORMAL ||
-                                              L.dist == IRL_TRUNCATED_NORMAL || ir_survival(L.dist));
+            const bool ordinal = EXTENDED && ir_ordinal_liks(L.dist);
+            const bool mixture = EXTENDED && ir_mixture_liks(L.dist);
+            const bool bounded = EXTENDED && (ordinal || zi || mixture || ir_bounded_liks(L.dist) || ir_survival_liks(L.dist));
             if constexpr (EXTENDED) {
                 if (mixture) {  // uniform branch: out of line, with the per-component gradients
                     lp += ir_mixture_pass<W>(P.liks + l, P.terms, x, r, x + P.ord_row, g_s, tid, red);
@@ -924,13 +935,13 @@ struct IrModel {
                 r[i] = ri;
                 if (L.yoff >= 0) g_s[L.yoff + i] -= ri;  // this thread owns element i of the latent variable
             }
-            if (disp && L.sigma_kind == IRS_REF) {  // uniform branch: the alpha-dependent normalising terms
+            if (disp && L.sigma_kind == B200_IR_S_REF) {  // uniform branch: the alpha-dependent normalising terms
                 const double a = sg_s;
                 const IrLikD& Lt = P.liks[l];  // read here, not kept live through the observation loop
                 if (gamma) {
                     if (tid == 0) {
                         const double sly = Lt.sum_log_y;
-                        const double Ny = (EXTENDED && L.dist == IRL_HURDLE_GAMMA) ? (double)Lt.n_tab : (double)N;  // N+
+                        const double Ny = (EXTENDED && L.dist == B200_IR_L_HURDLE_GAMMA) ? (double)Lt.n_tab : (double)N;  // hurdle_gamma: N+
                         lp += Ny * (a * la - lgamma(a)) + (a - 1.0) * sly;
                         s_sig += Ny * (la + 1.0 - digamma(a)) + sly;
                     }
@@ -965,7 +976,7 @@ struct IrModel {
                     }
                 }
             }
-            if (L.sigma_kind == IRS_REF) {
+            if (L.sigma_kind == B200_IR_S_REF) {
                 const double tot = team_sum<W>(s_sig, tid, red);
                 if (tid == 0) g_s[L.sigma.ref] += tot;
                 team_sync<W>();
@@ -1010,11 +1021,11 @@ struct IrModel {
         // ---- 3. chain rule through the transforms -------------------------------------------------------------------------
         for (int v = 0; v < P.n_vars; ++v) {
             const IrVarD V = P.vars[v];
-            if (V.transform == IRT_NONE) continue;
+            if (V.transform == B200_IR_T_NONE) continue;
             if constexpr (EXTENDED) {
-                if (V.transform >= IRT_ORDERED) {  // uniform branch: a reverse prefix sum or the softmax's, on one thread
+                if (ir_extended_transforms(V.transform)) {  // uniform branch: a reverse prefix sum or the softmax's, on one thread
                     if (tid == 0) {
-                        if (V.transform == IRT_SIMPLEX) ir_simplex_chain(P.vars + v, x, g_s);
+                        if (V.transform == B200_IR_T_SIMPLEX) ir_simplex_chain(P.vars + v, x, g_s);
                         else ir_ordered_chain(P.vars + v, q_s, g_s);
                     }
                     continue;
@@ -1023,7 +1034,7 @@ struct IrModel {
             for (int j = tid; j < V.size; j += TS) {
                 const int i = V.offset + j;
                 const double xv = x[i];
-                if (V.transform == IRT_LOG) {
+                if (V.transform == B200_IR_T_LOG) {
                     g_s[i] = fma(g_s[i], xv, 1.0);
                 } else {
                     // dx/dz = (hi - lo) s (1 - s), s = sigmoid(z), in the form e / (1 + e)^2 with e = exp(-|z|): s recovered
@@ -1063,23 +1074,23 @@ template <bool EXTENDED>  // as IrModel / IrExtendedModel
 __device__ __forceinline__ double ir_obs_loglik(const IrLikD& L, const IrTermD* terms, const double* x, int i, double eta,
                                                 double sg_s, double la) {
     const double y = L.y[i];
-    if (EXTENDED && (L.dist == IRL_NORMAL_MIXTURE || L.dist == IRL_POISSON_MIXTURE)) {
+    if (EXTENDED && ir_mixture_liks(L.dist)) {
         const double lse = ir_mix_obs(L.dist, (int)L.nu, ir_mix_block(L, terms, x, nullptr), y, eta).lse;
-        return lse - (L.dist == IRL_NORMAL_MIXTURE ? B200_HALF_LOG_2PI : lgamma(y + 1.0));
+        return lse - (L.dist == B200_IR_L_NORMAL_MIXTURE ? B200_HALF_LOG_2PI : lgamma(y + 1.0));
     }
-    if (EXTENDED && L.dist >= IRL_ZI_POISSON && L.dist <= IRL_HURDLE_GAMMA) {
+    if (EXTENDED && ir_zi_liks(L.dist)) {
         const IrPsi ps = ir_psi(terms + L.term0 + L.n_terms, (int)L.nu, x, i, (int)L.N);
         const double lp = ir_zi_term(L.dist, y, eta, ir_scale(L, i, sg_s), sg_s, la, ps).lp;
         return y > 0.0 ? lp + ir_obs_const(L, i, y, sg_s, la) : lp;
     }
-    if (EXTENDED && (L.dist == IRL_ORDERED_LOGISTIC || L.dist == IRL_ORDERED_PROBIT)) {
-        const double s = ir_scale(L, i, L.sigma_kind == IRS_NONE ? 1.0 : sg_s);  // the logistic link: s = 1
+    if (EXTENDED && ir_ordinal_liks(L.dist)) {
+        const double s = ir_scale(L, i, L.sigma_kind == B200_IR_S_NONE ? 1.0 : sg_s);  // the logistic link: s = 1
         return ir_ordinal_term(L, terms[L.term0 + L.n_terms], x, i, eta, s).lp;
     }
-    if (EXTENDED && ir_weibull(L.dist)) return ir_weibull_term(L, i, eta, sg_s, la).lp;
-    if (EXTENDED && (L.dist == IRL_CENSORED_NORMAL || L.dist == IRL_TRUNCATED_NORMAL || ir_survival(L.dist))) {
+    if (EXTENDED && ir_weibull_liks(L.dist)) return ir_weibull_term(L, i, eta, sg_s, la).lp;
+    if (EXTENDED && (ir_bounded_liks(L.dist) || ir_survival_liks(L.dist))) {
         const bool at_bound = L.cens && L.cens[i] != 0;
-        const double ly = L.dist >= IRL_WEIBULL_LOG ? y : 0.0;  // a LogNormal's y is log y_i
+        const double ly = ir_bounded_liks(L.dist) ? 0.0 : y;  // a LogNormal's y is log y_i
         return ir_bounded_term(L, i, eta, ir_scale(L, i, sg_s)).lp - (at_bound ? 0.0 : B200_HALF_LOG_2PI + ly);
     }
     double lp = 0.0, s_sig = 0.0;
@@ -1102,9 +1113,9 @@ __global__ void __launch_bounds__(256) ir_pointwise_kernel(const IrModel::Params
         for (int v = 0; v < P.n_vars; ++v) {
             const IrVarD V = P.vars[v];
             if constexpr (EXTENDED) {
-                if (V.transform >= IRT_ORDERED) {
+                if (ir_extended_transforms(V.transform)) {
                     if (lane == 0) {
-                        if (V.transform == IRT_SIMPLEX) ir_simplex_forward(P.vars + v, q, x);
+                        if (V.transform == B200_IR_T_SIMPLEX) ir_simplex_forward(P.vars + v, q, x);
                         else ir_ordered_forward(P.vars + v, q, x);
                     }
                     continue;

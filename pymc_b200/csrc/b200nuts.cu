@@ -90,10 +90,10 @@ static size_t point_smem_bytes(size_t model_shared, int NP, int W) {
     const int wpb = (W == 1) ? 8 : 1;
     return staged_bytes(model_shared) + (size_t)wpb * (2 * NP + (W > 1 ? 8 * W : 0)) * sizeof(double);
 }
-// the persistent NUTS kernel with `hot` tree levels in shared memory
-static size_t nuts_smem_bytes(size_t model_shared, int NP, int hot, int W) {
+// the persistent NUTS kernel with `hot` tree levels, and with or without the main tree, in shared memory
+static size_t nuts_smem_bytes(size_t model_shared, int NP, int hot, int W, bool tree_smem = false) {
     const int wpb = (W == 1) ? kNutsWarpChains : 1;
-    return staged_bytes(model_shared) + (size_t)wpb * nuts_warp_smem_bytes(NP, hot, W);
+    return staged_bytes(model_shared) + (size_t)wpb * nuts_team_smem_bytes(NP, hot, W, tree_smem);
 }
 static int npl_warp(int n);
 
@@ -1759,6 +1759,11 @@ struct NutsLaunch {
             smem = nuts_smem_bytes(shared, NP, hot, W);
         }
         if (smem > kMaxDynSmem) return fail("nuts: shared memory request %zu B exceeds 227 KB", smem);
+        // the main tree of each draw goes to shared memory too when it fits after the hot levels (it is touched at every
+        // doubling)
+        const size_t smem_tree = nuts_smem_bytes(shared, NP, hot, W, true);
+        P.tree_smem = smem_tree <= kMaxDynSmem;
+        if (P.tree_smem) smem = smem_tree;
         P.hot_levels = hot;
         P.scratch_stride = nuts_scratch_doubles(NP, P.max_td);
         // tree scratch [C][stride] | ChainCtx [C] | done [C] | ticket

@@ -19,9 +19,10 @@
 //               construction: left.p, p_sum, proposal q   -> 5*NPL doubles per lane
 //   shared    : q and grad of the integrator state (the model function needs all of q), the HOT lowest
 //               levels of the pending-subtree stack (level h is touched every 2^h leapfrogs), per-level
-//               scalars, and the model's observed data (staged once per CTA by bulk TMA)
-//   global/L2 : the colder stack levels, the main tree (both edge states, p_sum, proposal q) and the
-//               Welford accumulators -- touched once per doubling / per draw
+//               scalars, and the model's observed data (staged once per CTA by bulk TMA); then, when the
+//               CTA still fits, the main tree (both edge states, p_sum, proposal q) -- touched every doubling
+//   global/L2 : the colder stack levels, the main tree when it does not fit, the Welford accumulators and
+//               the segment hand-over -- touched once per merge at a cold level / per draw / per segment
 #pragma once
 #include "sampler_state.cuh"
 
@@ -37,6 +38,7 @@ constexpr int kMaxLevels = 12;  // pending-subtree levels (max_treedepth <= 12)
 
 struct NutsDev : RunCfg {
     int hot_levels;
+    int tree_smem;                             // the main tree's kTreeVecs vectors live in shared memory (else: scratch)
     b200_chain_state resume, save;             // optional per-chain state in / out (null pointers: not used)
     int sampler, max_steps, stop_adaptation;   // B200_SAMPLER_*; HMC: max leapfrogs; DIAG_ADAPT_GRAD: stop after this many
     double path_length, mass_alpha;            // HMC trajectory length; DIAG_ADAPT_GRAD decay rate
@@ -75,8 +77,12 @@ __device__ __forceinline__ void st_release_i32(int* p, int v) {
     asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
 }
 
-// global scratch layout per chain, in units of NP doubles
-enum { G_LQ = 0, G_LP, G_LG, G_RQ, G_RP, G_RG, G_PS, G_PQ, G_NEARP, G_FGM, G_FGV, G_BGM, G_BGV, G_Q, G_VAR, G_STACK };
+// per-chain vector slots, in units of NP doubles.  The first kTreeVecs are the main tree of one draw (p_sum, proposal q,
+// both edge states): in shared memory when the launch has room for them after the hot levels (NutsDev::tree_smem),
+// otherwise in the chain's global scratch.  The Welford estimators and the segment hand-over outlive a draw and are
+// always global.
+enum { G_PS = 0, G_PQ, G_LP, G_RP, G_LQ, G_RQ, G_LG, G_RG, G_FGM, G_FGV, G_BGM, G_BGV, G_Q, G_VAR, G_STACK };
+constexpr int kTreeVecs = G_FGM;
 
 __host__ __device__ inline long long nuts_scratch_doubles(int NP, int levels) {
     return (long long)(G_STACK + 4 * levels) * NP;
@@ -87,6 +93,10 @@ __host__ __device__ inline size_t nuts_warp_smem_bytes(int NP, int hot, int W) {
     const int vecs = 2 + (W > 1 ? 3 : 0) + (hot > 0 ? 2 + 4 * (hot - 1) : 0);
     return (size_t)vecs * NP * sizeof(double) + 5 * kMaxLevels * sizeof(double) +
            (W > 1 ? W * 8 * sizeof(double) : 0);
+}
+// ... plus the main tree when it is placed in shared memory, after everything above
+__host__ __device__ inline size_t nuts_team_smem_bytes(int NP, int hot, int W, bool tree_smem) {
+    return nuts_warp_smem_bytes(NP, hot, W) + (tree_smem ? (size_t)kTreeVecs * NP * sizeof(double) : 0);
 }
 
 constexpr int kNutsWarpChains = 8;  // chain = warp (W = 1): chains per CTA (256 threads, one CTA per SM)
@@ -151,15 +161,31 @@ __device__ __forceinline__ double nuts_model_eval(const typename Model::Params& 
 }
 
 // _WeightedVariance.add_sample of one draw x on both diagonal estimators, for the NPL elements of a team thread: out of line
-// (it runs once per tuning draw, and its divisions would otherwise be inlined NPL times into the kernel)
+// (it runs once per tuning draw, and its divisions would otherwise be inlined NPL times into the kernel).  Two elements at
+// a time: both elements' loads are issued before their divisions, which halves the chain of dependent L2 round trips.  All
+// NPL elements at once would cost the bench kernel <6,1> 20 B more spill stores and 52 B more spill loads around the call.
 template <int TS, int NPL>
 __device__ __noinline__ void welford_add_team(const double* x, double fg_n, double bg_n, double* fm, double* fv, double* bm,
                                               double* bv, int lane) {
+    constexpr int G = NPL % 2 == 0 ? 2 : 1;
 #pragma unroll 1
-    for (int k = 0; k < NPL; ++k) {
-        const int i = lane + TS * k;
-        welford_add(x[i], fg_n, fm[i], fv[i]);
-        welford_add(x[i], bg_n, bm[i], bv[i]);
+    for (int k0 = 0; k0 < NPL; k0 += G) {
+        double xs[G], m1[G], v1[G], m2[G], v2[G];
+#pragma unroll
+        for (int k = 0; k < G; ++k) {
+            const int i = lane + TS * (k0 + k);
+            xs[k] = x[i]; m1[k] = fm[i]; v1[k] = fv[i]; m2[k] = bm[i]; v2[k] = bv[i];
+        }
+#pragma unroll
+        for (int k = 0; k < G; ++k) {
+            welford_add(xs[k], fg_n, m1[k], v1[k]);
+            welford_add(xs[k], bg_n, m2[k], v2[k]);
+        }
+#pragma unroll
+        for (int k = 0; k < G; ++k) {
+            const int i = lane + TS * (k0 + k);
+            fm[i] = m1[k]; fv[i] = v1[k]; bm[i] = m2[k]; bv[i] = v2[k];
+        }
     }
 }
 
@@ -181,7 +207,8 @@ __global__ void __launch_bounds__(W > 1 ? 32 * W : 32 * kNutsWarpChains, 1)
     __shared__ unsigned int ticket_s;  // W > 1: the CTA's current ticket
 
     const int hot = P.hot_levels;
-    double* ws = reinterpret_cast<double*>(smem_raw + data_bytes + wib * nuts_warp_smem_bytes(NP, hot, W));
+    double* ws = reinterpret_cast<double*>(smem_raw + data_bytes + wib * nuts_team_smem_bytes(NP, hot, W, P.tree_smem));
+    double* tree_s = ws + nuts_warp_smem_bytes(NP, hot, W) / sizeof(double);  // tree_smem: the main tree's slots
     double* q_s = ws;
     double* g_s = ws + NP;
     double* sub_s = ws + 2 * NP + lane;            // SUBS: left.p, p_sum, proposal q of the subtree under construction
@@ -239,7 +266,10 @@ __global__ void __launch_bounds__(W > 1 ? 32 * W : 32 * kNutsWarpChains, 1)
         if (h < hot) return hot_base + (h == 0 ? (which - 2) : (2 + 4 * (h - 1) + which)) * NP;
         return gs + (long long)(G_STACK + 4 * h + which) * NP;
     };
+    // the state that outlives a draw (always global) and the main tree (shared or global: generic pointers)
     auto gvec = [&](int which) -> double* { return gs + (long long)which * NP; };
+    double* tree = P.tree_smem ? tree_s : gs;
+    auto tvec = [&](int which) -> double* { return tree + which * NP; };
 
     // ---- per-chain state: initialised by the first segment, carried through global memory afterwards ------------
     double var[NPL], p[NPL];
@@ -378,7 +408,7 @@ __global__ void __launch_bounds__(W > 1 ? 32 * W : 32 * kNutsWarpChains, 1)
         int n_prop = 0, depth = 0;
         bool diverged = false, turned = false, hit_max = false;
         double hmc_accept = 0.0;
-        double* PQv = gvec(G_PQ);
+        double* PQv = tvec(G_PQ);
         int d_iter = 0;
         if (P.sampler == B200_SAMPLER_HMC) {
             // ---- HamiltonianMC._hamiltonian_step (hmc/hmc.py:143-200): a fixed-length trajectory, Metropolis accept ----
@@ -423,9 +453,9 @@ __global__ void __launch_bounds__(W > 1 ? 32 * W : 32 * kNutsWarpChains, 1)
             diverged = div; m_pe = E; m_plogp = logp; max_de = dE;  // stats report the trajectory's LAST state (hmc.py:180-188)
         } else {
             // ---- _Tree.__init__ (nuts.py:292-332): both edges, proposal and p_sum are the start state ----
-            double* Lq = gvec(G_LQ); double* Lp = gvec(G_LP); double* Lg = gvec(G_LG);
-            double* Rq = gvec(G_RQ); double* Rp = gvec(G_RP); double* Rg = gvec(G_RG);
-            double* PSv = gvec(G_PS); double* NEARP = gvec(G_NEARP);
+            double* Lq = tvec(G_LQ); double* Lp = tvec(G_LP); double* Lg = tvec(G_LG);
+            double* Rq = tvec(G_RQ); double* Rp = tvec(G_RP); double* Rg = tvec(G_RG);
+            double* PSv = tvec(G_PS);
     #pragma unroll
             for (int k = 0; k < NPL; ++k) {
                 const int i = lane + TS * k;
@@ -438,18 +468,26 @@ __global__ void __launch_bounds__(W > 1 ? 32 * W : 32 * kNutsWarpChains, 1)
             for (; d_iter < maxd; ++d_iter) {
                 B200_PHASE(PH_DOUBLING);  // the tree's start state, or the previous doubling's exit
                 const int dir = (rng.next_double() < 0.5) ? 1 : -1;  // nuts.py:215
-                // ---- load the edge we grow from into the integrator state; remember its p ----------------
+                // ---- load the edge we grow from into the integrator state (the first doubling grows from the start
+                //      state, which the integrator state still holds) -------------------------------------------------
                 const double* Eq = dir > 0 ? Rq : Lq;
                 const double* Ep = dir > 0 ? Rp : Lp;
                 const double* Eg = dir > 0 ? Rg : Lg;
                 int w_idx = dir > 0 ? R_idx : L_idx;
+                if (d_iter > 0) {  // every load is issued before the first store (a generic store may alias q_s, g_s)
+                    double eq[NPL], eg[NPL];
     #pragma unroll
-                for (int k = 0; k < NPL; ++k) {
-                    const int i = lane + TS * k;
-                    q_s[i] = Eq[i];
-                    g_s[i] = Eg[i];
-                    p[k] = Ep[i];
-                    NEARP[i] = p[k];
+                    for (int k = 0; k < NPL; ++k) {
+                        const int i = lane + TS * k;
+                        eq[k] = Eq[i];
+                        eg[k] = Eg[i];
+                        p[k] = Ep[i];
+                    }
+    #pragma unroll
+                    for (int k = 0; k < NPL; ++k) {
+                        q_s[lane + TS * k] = eq[k];
+                        g_s[lane + TS * k] = eg[k];
+                    }
                 }
                 const double es = dir * eps, dt = 0.5 * es;
 
@@ -605,20 +643,7 @@ __global__ void __launch_bounds__(W > 1 ? 32 * W : 32 * kNutsWarpChains, 1)
                     turned = sub_turn;
                     break;
                 }
-                // ---- the new outer edge is the integrator state (self.right/left = tree.right) ------------
-                {
-                    double* Nq = dir > 0 ? Rq : Lq;
-                    double* Np = dir > 0 ? Rp : Lp;
-                    double* Ng = dir > 0 ? Rg : Lg;
-    #pragma unroll
-                    for (int k = 0; k < NPL; ++k) {
-                        const int i = lane + TS * k;
-                        Nq[i] = q_s[i];
-                        Ng[i] = g_s[i];
-                        Np[i] = p[k];
-                    }
-                    if (dir > 0) R_idx = w_idx; else L_idx = w_idx;
-                }
+                if (dir > 0) R_idx = w_idx; else L_idx = w_idx;
                 // ---- biased progressive pick (nuts.py:370-374), drawn before the full-tree U-turn checks --
                 {
                     // accept the new subtree's proposal iff u < w_new / w_old  (log(u) < log_size_new - log_size_old)
@@ -634,14 +659,16 @@ __global__ void __launch_bounds__(W > 1 ? 32 * W : 32 * kNutsWarpChains, 1)
                     m_logw = fmax(c_logw, m_logw);
                     m_s = wo + wn;
                 }
-                // ---- U-turn checks on the whole tree (nuts.py:376-390) ------------------------------------
+                // ---- U-turn checks on the whole tree (nuts.py:376-390); the old edge the subtree grew from is still
+                //      in Ep, and the new outer edge, the integrator state, replaces it afterwards (self.right/left =
+                //      tree.right) ----------------------------------------------------------------------------------
                 {
                     const double* FARP = dir > 0 ? Lp : Rp;
                     double dots[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
     #pragma unroll
                     for (int k = 0; k < NPL; ++k) {
                         const int i = lane + TS * k;
-                        const double so = PSv[i], fp = FARP[i], np_ = NEARP[i];
+                        const double so = PSv[i], fp = FARP[i], np_ = Ep[i];
                         const double s = so + PS(k);
                         PSv[i] = s;
                         const double vf = VAR(k) * fp, vw = VAR(k) * p[k];
@@ -653,6 +680,16 @@ __global__ void __launch_bounds__(W > 1 ? 32 * W : 32 * kNutsWarpChains, 1)
                         const double b = np_ + PS(k);  // (old tree's edge adjacent to the new subtree).p + new p_sum
                         dots[4] = fma(b, VAR(k) * np_, dots[4]);
                         dots[5] = fma(b, vw, dots[5]);
+                    }
+                    double* Nq = dir > 0 ? Rq : Lq;
+                    double* Np = dir > 0 ? Rp : Lp;
+                    double* Ng = dir > 0 ? Rg : Lg;
+    #pragma unroll
+                    for (int k = 0; k < NPL; ++k) {
+                        const int i = lane + TS * k;
+                        Nq[i] = q_s[i];
+                        Ng[i] = g_s[i];
+                        Np[i] = p[k];
                     }
                     team_sum_n<W>(dots, lane, red);
                     if ((dots[0] <= 0) || (dots[1] <= 0) || (dots[2] <= 0) || (dots[3] <= 0) || (dots[4] <= 0) ||
@@ -672,11 +709,12 @@ __global__ void __launch_bounds__(W > 1 ? 32 * W : 32 * kNutsWarpChains, 1)
         const bool rec = P.store_warmup || !tuning;
         const int t_out = it - rec_lo;
 #pragma unroll
+        for (int k = 0; k < NPL; ++k) PQ(k) = PQv[lane + TS * k];
+#pragma unroll
         for (int k = 0; k < NPL; ++k) {
             const int i = lane + TS * k;
-            const double qi = PQv[i];
+            const double qi = PQ(k);
             q_s[i] = qi;
-            PQ(k) = qi;
             if (rec && i < n) P.draws_out[((long long)chain * T_out + t_out) * n + i] = constrained(qi, i, P.tr_kind, P.tr_lo, P.tr_hi);
         }
         if (adapting) ss.update(P, accept);

@@ -170,6 +170,13 @@ extern "C" {
  *   sigma_kind NONE, y_var 0. */
 #define B200_IR_L_NORMAL_MIXTURE 24         /* pm.NormalMixture mixture.py:529-546                            */
 #define B200_IR_L_POISSON_MIXTURE 25        /* pm.Mixture(w, pm.Poisson.dist(lam, shape=K))                   */
+/* Beta regression with a logit mean: mu = sigmoid(eta), precision phi, a = phi mu, b = phi (1 - mu).  sigma: phi, CONST (> 0)
+ * or REF (a scalar variable with positive support).  y_var must be 0.
+ *   BETA_LOGIT           y ~ Beta(mu, nu = phi): y finite with 0 < y < 1 (0 and 1 are outside the support)
+ *   BETA_BINOMIAL_LOGIT  y ~ BetaBinomial(n, a, b): `y` is the [2][N] block (y, trials); trials finite integers >= 0, y an
+ *                        integer with 0 <= y <= trials */
+#define B200_IR_L_BETA_LOGIT 26             /* pm.Beta(mu, nu) continuous.py:1131-1262, alpha = mu nu :1238-1240 */
+#define B200_IR_L_BETA_BINOMIAL_LOGIT 27    /* pm.BetaBinomial discrete.py:178-262                            */
 /* The support rule b200_model_create enforces (as ModelIR.validate does): HalfNormal, HalfCauchy, Exponential, Gamma and
  * LogNormal priors sit on a LOG variable or an INTERVAL with lo >= 0, Beta on an INTERVAL inside [0, 1], Uniform(a, b) on an
  * INTERVAL inside [a, b]; every scale (a prior's sigma / beta / lam, Normal and StudentT sigma including each sigma_obs, an
@@ -215,7 +222,8 @@ typedef struct b200_ir_term {
 typedef struct b200_ir_lik {
     int32_t dist, n_terms;
     int64_t N;
-    const double* y; /* [N]; [3][N] (y, lower, upper) for the CENSORED_* / TRUNCATED_* dists; NULL allowed when y_var > 0 */
+    const double* y; /* [N]; [3][N] (y, lower, upper) for the CENSORED_* / TRUNCATED_* dists; [2][N] (y, trials) for
+                      * BETA_BINOMIAL_LOGIT; NULL allowed when y_var > 0 */
     const b200_ir_term* terms;
     int32_t sigma_kind, y_var;
     b200_ir_param sigma;

@@ -505,6 +505,10 @@ static bool ir_scale_ok(const b200_ir_param& p, const std::vector<IrVarD>& vars)
 #define B200_IR_MIX_LAM "lam must be a variable of size K with positive support (log, ordered_positive, or an interval with lo >= 0), or K finite constants > 0"
 #define B200_IR_MIX_SIGMA "sigma must be a finite constant > 0, K of them, or a variable of size 1 or K with positive support"
 #define B200_IR_MIX_SLOTS "a mixture takes no alpha, trials, lower / upper, cutpoints or psi, and poisson_mixture no sigma"
+// Beta and BetaBinomial observations (ModelIR._validate_beta, same wording)
+#define B200_IR_BETA_Y "y must be finite with 0 < y < 1 for every observation (0 and 1 are outside the Beta's support; a zero/one-inflated Beta is not provided)"
+#define B200_IR_BB_TRIALS "trials must be finite integers >= 0"
+#define B200_IR_BETA_SLOTS "beta_logit and beta_binomial_logit take phi, and no sigma, alpha, cutpoints, psi, weights, components or lower / upper"
 static constexpr double LOG_PI = 1.1447298858494001741, LOG_2 = 0.69314718055994530942;
 
 // The pass over a b200_ir.  Its steps return 0 or fail(...); the arrays they record in `sg` stay put until the upload.
@@ -772,6 +776,62 @@ static int ir_survival(IrPass& c, const b200_ir_lik& L, int l, const b200_ir_par
     return 0;
 }
 
+// sum_{j<m} log(a + j), as ir_rising (csrc/ir_model.cuh) forms it on the device: lgamma(a + m) - lgamma(a) from
+// kIrBetaSumMax on
+static double ir_log_rising(double a, double m) {
+    if (m >= kIrBetaSumMax) return std::lgamma(a + m) - std::lgamma(a);
+    double l = 0.0;
+    for (int j = 0; j < (int)m; ++j) l += std::log(a + j);
+    return l;
+}
+// beta_logit / beta_binomial_logit: phi in the slot, and the device's [2][N] y block, (log y, log1p(-y)) or (y, trials).
+// c0: -sum (log y + log1p(-y)) and, for a constant phi, N lgamma(phi) (Beta); sum binomln(n, y) and, for a constant phi,
+// sum lgamma(phi) - lgamma(n + phi) (BetaBinomial), whose random phi sums over the table of distinct nonzero trials.
+static int ir_beta(IrPass& c, const b200_ir_lik& L, int l, const b200_ir_param& slot, IrLikD& D) {
+    const long long N = L.N;
+    const bool bb = L.dist == B200_IR_L_BETA_BINOMIAL_LOGIT;
+    const char* what = bb ? "beta_binomial_logit" : "beta_logit";
+    if (L.nu != 0.0) return fail("ir: likelihood %d: %s: " B200_IR_BETA_SLOTS, l, what);
+    if (L.sigma_kind != B200_IR_S_CONST && L.sigma_kind != B200_IR_S_REF)
+        return fail("ir: likelihood %d: %s: phi must be a constant or a scalar variable", l, what);
+    if (!ir_scale_ok(slot, c.vars)) return fail("ir: likelihood %d: %s: phi " B200_IR_SCALE_RULE, l, what);
+    const double phi = L.sigma.value;
+    const bool fold = L.sigma_kind == B200_IR_S_CONST;
+    std::vector<double>& blk = c.reals.emplace_back(2 * (size_t)N);
+    std::map<double, double> count;  // distinct nonzero trials -> multiplicity, ascending
+    double c0 = 0.0;
+    for (long long i = 0; i < N; ++i) {
+        const double y = L.y[i];
+        if (!bb) {
+            if (!(std::isfinite(y) && y > 0.0 && y < 1.0)) return fail("ir: likelihood %d: %s: " B200_IR_BETA_Y " (at %lld)", l, what, i);
+            blk[i] = std::log(y);
+            blk[N + i] = std::log1p(-y);
+            c0 -= blk[i] + blk[N + i];
+            continue;
+        }
+        const double n = L.y[N + i];
+        if (!(std::isfinite(n) && n >= 0 && n == std::floor(n))) return fail("ir: likelihood %d: %s: " B200_IR_BB_TRIALS " (at %lld)", l, what, i);
+        if (!(y >= 0 && y == std::floor(y) && y <= n)) return fail("ir: likelihood %d: %s: " B200_IR_ZIB_Y " (at %lld)", l, what, i);
+        blk[i] = y;
+        blk[N + i] = n;
+        c0 += std::lgamma(n + 1.0) - std::lgamma(y + 1.0) - std::lgamma(n - y + 1.0);
+        if (fold) c0 -= ir_log_rising(phi, n);
+        else if (n > 0) count[n] += 1.0;
+    }
+    if (!bb && fold) c0 += (double)N * std::lgamma(phi);
+    D.c0 = c0;
+    c.add(&D.y, blk.data(), blk.size());
+    if (bb && !fold) {
+        std::vector<double>& u = c.reals.emplace_back();
+        std::vector<double>& cnt = c.reals.emplace_back();
+        for (const auto& kv : count) { u.push_back(kv.first); cnt.push_back(kv.second); }
+        D.n_tab = (int)u.size();
+        c.add(&D.tab_u, u.data(), u.size());
+        c.add(&D.tab_cnt, cnt.data(), cnt.size());
+    }
+    return 0;
+}
+
 // ordered logistic / probit: nu = K
 static int ir_ordinal(IrPass& c, const b200_ir_lik& L, int l) {
     const double K = L.nu;
@@ -964,7 +1024,8 @@ static int ir_lik(IrPass& c, const b200_ir_lik& L, int l, IrLikD& D) {
     c.max_obs = std::max(c.max_obs, N);
     D.dist = L.dist; D.n_terms = L.n_terms; D.term0 = (int)c.terms.size(); D.sigma_kind = L.sigma_kind; D.N = N; D.nu = L.nu;
     D.yoff = latent ? c.vars[L.y_var - 1].offset : -1;
-    if (!latent && !ir_survival_liks(L.dist)) c.add(&D.y, L.y, (size_t)N);  // a survival likelihood's device y is log y (ir_survival)
+    if (!latent && !ir_survival_liks(L.dist) && !ir_beta_liks(L.dist))  // a survival / Beta likelihood's device y: ir_survival / ir_beta
+        c.add(&D.y, L.y, (size_t)N);
     if (ir_param(L.sigma, c.n, &D.sigma, "likelihood sigma")) return -1;
     if (L.sigma_kind == B200_IR_S_REF && L.sigma.kind != 1) return fail("ir: likelihood %d: sigma_kind REF needs a reference", l);
     if (L.sigma_kind == B200_IR_S_REF && ir_ref_simplex(c.vars, L.sigma)) return fail("ir: likelihood %d: " B200_IR_SIMPLEX_USE, l);
@@ -979,6 +1040,7 @@ static int ir_lik(IrPass& c, const b200_ir_lik& L, int l, IrLikD& D) {
     else if (ir_ordinal_liks(L.dist)) rc = ir_ordinal(c, L, l);
     else if (ir_survival_liks(L.dist)) rc = ir_survival(c, L, l, slot, D);
     else if (ir_mixture_liks(L.dist)) rc = ir_mixture_obs(c, L, l, D);
+    else if (ir_beta_liks(L.dist)) rc = ir_beta(c, L, l, slot, D);
     else if (ir_zi_liks(L.dist)) {  // nu: the form of the psi block
         if (!(L.nu >= 0 && L.nu == std::floor(L.nu) && L.nu <= 0x7fff)) return fail("ir: likelihood %d: " B200_IR_PSI_NU, l);
         const int fam = ir_zi_family(L.dist);

@@ -44,9 +44,10 @@ __host__ __device__ __forceinline__ constexpr bool ir_survival_liks(int d) { ret
 __host__ __device__ __forceinline__ constexpr bool ir_censored_survival_liks(int d) { return d == B200_IR_L_CENSORED_WEIBULL_LOG || d == B200_IR_L_CENSORED_LOGNORMAL; }
 __host__ __device__ __forceinline__ constexpr bool ir_truncated_survival_liks(int d) { return d == B200_IR_L_TRUNCATED_WEIBULL_LOG || d == B200_IR_L_TRUNCATED_LOGNORMAL; }
 __host__ __device__ __forceinline__ constexpr bool ir_mixture_liks(int d) { return d == B200_IR_L_NORMAL_MIXTURE || d == B200_IR_L_POISSON_MIXTURE; }
+__host__ __device__ __forceinline__ constexpr bool ir_beta_liks(int d) { return d == B200_IR_L_BETA_LOGIT || d == B200_IR_L_BETA_BINOMIAL_LOGIT; }
 __host__ __device__ __forceinline__ constexpr bool ir_sigma_liks(int d) { return d == B200_IR_L_NORMAL || d == B200_IR_L_STUDENTT || ir_bounded_liks(d) || d == B200_IR_L_ORDERED_PROBIT || ir_lognormal_liks(d); }
 // the likelihoods and transforms that IrModel leaves out and IrExtendedModel evaluates out of line (below)
-__host__ __device__ __forceinline__ constexpr bool ir_extended_liks(int d) { return ir_ordinal_liks(d) || ir_zi_liks(d) || ir_mixture_liks(d) || ir_bounded_liks(d) || ir_survival_liks(d); }
+__host__ __device__ __forceinline__ constexpr bool ir_extended_liks(int d) { return ir_ordinal_liks(d) || ir_zi_liks(d) || ir_mixture_liks(d) || ir_bounded_liks(d) || ir_survival_liks(d) || ir_beta_liks(d); }
 static_assert(B200_IR_T_ORDERED == 3 && B200_IR_T_ORDERED_POSITIVE == 4 && B200_IR_T_SIMPLEX == 5, "the last three transforms");
 __host__ __device__ __forceinline__ constexpr bool ir_extended_transforms(int t) { return t >= B200_IR_T_ORDERED; }  // ORDERED_TRANSFORMS and simplex
 
@@ -114,6 +115,8 @@ __device__ __forceinline__ void ir_design_grad(const IrTermD& Tm, const double* 
 // itself.  Truncated Normal: bnd = [2][N], the lower and upper bound of each observation, -inf / +inf where open.
 // Survival likelihoods: y = log y_i; cens as above for the censored forms and null otherwise; bnd of the truncated forms
 // holds the bounds themselves (Weibull, 0 / +inf where open) or their logs (LogNormal, -inf / +inf where open).
+// Beta: y = the [2][N] block (log y_i, log1p(-y_i)).  BetaBinomial: y = the [2][N] block (y_i, n_i); a random phi keeps the
+// distinct nonzero trials in tab_u with their counts in tab_cnt (n_tab of them).
 // yoff >= 0: a latent factor (a Normal / StudentT prior whose location is a linear predictor): y_i = x[yoff + i], the
 // constrained values of a variable of size N, which also receives d logp / d y_i = -r_i; y is null.  -1: y is data.
 struct IrLikD { int dist, n_terms, term0, sigma_kind; long long N; const double* y; const double* sigma_obs; IrParamD sigma;
@@ -243,6 +246,30 @@ __device__ __forceinline__ double ir_base_term(const IrLikD& L, int i, double yi
     return ri;
 }
 
+// ---- Beta regression: the rising-factorial sums of a BetaBinomial bracket and of its phi-only part.
+// sum_{j<m} log(a + j) and sum_{j<m} 1 / (a + j) of a count m: below kIrBetaSumMax from products P of four factors and
+// their a-derivatives D (D / P = the four reciprocals), one log and one division per four terms and no cancellation
+// however large a is against m; from m = kIrBetaSumMax on, lgamma(a + m) - lgamma(a) and digamma(a + m) - digamma(a),
+// which lose about |lgamma(a)| ulp (DESIGN.md section 6).  P overflows above a ~ 1e76.
+constexpr int kIrBetaSumMax = 32;
+struct IrRise { double l, d; };
+__device__ __forceinline__ IrRise ir_rising(double a, double m) {
+    if (m >= kIrBetaSumMax) return {lgamma(a + m) - lgamma(a), digamma(a + m) - digamma(a)};
+    const int n = (int)m;
+    double l = 0.0, d = 0.0;
+    for (int j = 0; j < n; j += 4) {
+        double P = 1.0, D = 0.0;
+        for (int k = j; k < min(j + 4, n); ++k) {
+            const double t = a + k;
+            D = fma(D, t, P);
+            P *= t;
+        }
+        l += log(P);
+        d += D / P;
+    }
+    return {l, d};
+}
+
 // The per-observation constant of log f(y_i) that eval folds into c0 or the alpha terms (csrc/b200nuts.cu: prepare_ir):
 // of a base family, and of the count / positive component f of a zero-inflated or hurdle likelihood at y > 0.
 __device__ __forceinline__ double ir_obs_const(const IrLikD& L, int i, double y, double sg_s, double la) {
@@ -259,6 +286,15 @@ __device__ __forceinline__ double ir_obs_const(const IrLikD& L, int i, double y,
         case B200_IR_L_GAMMA_LOG: case B200_IR_L_HURDLE_GAMMA: return sg_s * la - lgamma(sg_s) + (sg_s - 1.0) * log(y);
         default: return 0.0;
     }
+}
+
+// The per-observation constant of a Beta / BetaBinomial observation that eval folds into c0 or the phi terms, apart from
+// ir_obs_const so that IrModel's pointwise kernel keeps its code: lgamma(phi) - log y_i - log1p(-y_i) (L.y holds the two
+// logs), or binomln(n, y) + lgamma(phi) - lgamma(n + phi).
+__device__ __forceinline__ double ir_beta_const(const IrLikD& L, int i, double phi) {
+    const double y = L.y[i], v = L.y[L.N + i];
+    if (L.dist == B200_IR_L_BETA_LOGIT) return lgamma(phi) - y - v;
+    return lgamma(v + 1.0) - lgamma(y + 1.0) - lgamma(v - y + 1.0) - ir_rising(phi, v).l;
 }
 
 // log p(y_i | eta) of one censored / truncated Normal observation without its constant -log(2 pi) / 2 (in c0), with
@@ -720,6 +756,67 @@ __device__ __noinline__ double ir_mixture_pass(const IrLikD* Lp, const IrTermD* 
     return lp;
 }
 
+// ---- Beta regression (continuous.py:1131-1262 at alpha = mu nu, beta = (1 - mu) nu, :1238-1240; discrete.py:178-262):
+// mu = sigmoid(eta), a = phi mu and b = phi (1 - mu) = phi sigmoid(-eta), both from one e = exp(-|eta|) so that 1 - mu
+// never cancels, and mu (1 - mu) = e / (1 + e)^2.  The brackets of a BetaBinomial are ir_rising (above).
+// One observation: lp, r = d / d eta and s = d / d phi, less the parts that are not per observation.
+//   beta_logit           (a - 1) log y + (b - 1) log1p(-y) - lgamma(a) - lgamma(b) without -log y - log1p(-y) (c0) and
+//                        lgamma(phi) (c0, or once per evaluation), s without psi(phi).  L.y is the [2][N] block
+//                        (log y, log1p(-y)), formed on the host.
+//   beta_binomial_logit  [lgamma(y + a) - lgamma(a)] + [lgamma(n - y + b) - lgamma(b)] without binomln(n, y) (c0) and
+//                        lgamma(phi) - lgamma(n + phi) (c0, or over the distinct-trials table), s without psi(phi) -
+//                        psi(n + phi).  L.y is the [2][N] block (y, trials); a bracket is 0 at y = 0 / y = n (m = 0).
+__device__ __forceinline__ IrBoundedTerm ir_beta_term(const IrLikD& L, int i, double eta, double phi) {
+    const int N = (int)L.N;
+    const double e = exp(-fabs(eta)), h = 1.0 / (1.0 + e);
+    const double mu = eta >= 0 ? h : e * h, mc = eta >= 0 ? e * h : h;  // sigmoid(eta), sigmoid(-eta)
+    const double a = phi * mu, b = phi * mc, w = phi * (e * h * h);      // w = phi mu (1 - mu) = da / d eta = -db / d eta
+    if (L.dist == B200_IR_L_BETA_LOGIT) {
+        const double ly = L.y[i], l1y = L.y[N + i];
+        const double ua = ly - digamma(a), ub = l1y - digamma(b);
+        return {a * ly + b * l1y - lgamma(a) - lgamma(b), w * (ua - ub), mu * ua + mc * ub};
+    }
+    const double y = L.y[i], n = L.y[N + i];
+    const IrRise A = ir_rising(a, y), B = ir_rising(b, n - y);
+    return {A.l + B.l, w * (A.d - B.d), mu * A.d + mc * B.d};
+}
+
+// The observation loop of a Beta / BetaBinomial likelihood, out of line like ir_bounded_pass, with the phi-only terms of a
+// random phi: N lgamma(phi) and N psi(phi) once (Beta), or -sum_{j<u} log(phi + j) and its derivative over the distinct
+// nonzero trials u with their counts (BetaBinomial), team-strided in a fixed order.  Writes r_i = d logp / d eta_i;
+// returns this thread's partial sums of logp and d logp / d phi.
+template <int W>
+__device__ __noinline__ IrPartials ir_beta_pass(const IrLikD* Lp, const IrTermD* terms, const double* x, double* r,
+                                                double phi, int tid) {
+    constexpr int TS = 32 * W;
+    const IrLikD& L = *Lp;
+    const int N = (int)L.N;
+    double lp = 0.0, s = 0.0;
+    for (int i = tid; i < N; i += TS) {
+        const double eta = ir_eta(terms + L.term0, 0, L.n_terms, x, i, N);
+        const IrBoundedTerm b = ir_beta_term(L, i, eta, phi);
+        lp += b.lp;
+        s += b.s;
+        r[i] = b.r;
+    }
+    if (L.sigma_kind == B200_IR_S_REF) {  // uniform branch
+        if (L.dist == B200_IR_L_BETA_LOGIT) {
+            if (tid == 0) {
+                lp = fma((double)N, lgamma(phi), lp);
+                s = fma((double)N, digamma(phi), s);
+            }
+        } else {
+            for (int k = tid; k < L.n_tab; k += TS) {
+                const double c = L.tab_cnt[k];
+                const IrRise R = ir_rising(phi, L.tab_u[k]);
+                lp = fma(-c, R.l, lp);
+                s = fma(-c, R.d, s);
+            }
+        }
+    }
+    return {lp, s};
+}
+
 // IrModel evaluates every factor of the closed set except the likelihoods of ir_extended_liks and the transforms of
 // ir_extended_transforms; IrExtendedModel (below) is the same function with those added, each out of line.  A kernel's
 // register allocation covers every function it can reach, and the tail math takes about 128 registers, so the engine
@@ -912,10 +1009,15 @@ struct IrModel {
             double s_sig = 0.0, s_psi = 0.0;
             const bool ordinal = EXTENDED && ir_ordinal_liks(L.dist);
             const bool mixture = EXTENDED && ir_mixture_liks(L.dist);
-            const bool bounded = EXTENDED && (ordinal || zi || mixture || ir_bounded_liks(L.dist) || ir_survival_liks(L.dist));
+            const bool beta = EXTENDED && ir_beta_liks(L.dist);
+            const bool bounded = EXTENDED && (ordinal || zi || mixture || beta || ir_bounded_liks(L.dist) || ir_survival_liks(L.dist));
             if constexpr (EXTENDED) {
                 if (mixture) {  // uniform branch: out of line, with the per-component gradients
                     lp += ir_mixture_pass<W>(P.liks + l, P.terms, x, r, x + P.ord_row, g_s, tid, red);
+                } else if (beta) {  // uniform branch: out of line, with the phi-only terms of a random phi
+                    const IrPartials b = ir_beta_pass<W>(P.liks + l, P.terms, x, r, sg_s, tid);
+                    lp += b.lp;
+                    s_sig = b.s_sig;
                 } else if (zi) {  // uniform branch: out of line
                     const IrZiPartials b = ir_zi_pass<W>(P.liks + l, P.terms, x, r, x + P.ord_row, sg_s, la, tid);
                     lp += b.lp;
@@ -1088,6 +1190,7 @@ __device__ __forceinline__ double ir_obs_loglik(const IrLikD& L, const IrTermD* 
         return ir_ordinal_term(L, terms[L.term0 + L.n_terms], x, i, eta, s).lp;
     }
     if (EXTENDED && ir_weibull_liks(L.dist)) return ir_weibull_term(L, i, eta, sg_s, la).lp;
+    if (EXTENDED && ir_beta_liks(L.dist)) return ir_beta_term(L, i, eta, sg_s).lp + ir_beta_const(L, i, sg_s);
     if (EXTENDED && (ir_bounded_liks(L.dist) || ir_survival_liks(L.dist))) {
         const bool at_bound = L.cens && L.cens[i] != 0;
         const double ly = ir_bounded_liks(L.dist) ? 0.0 : y;  // a LogNormal's y is log y_i

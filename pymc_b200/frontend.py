@@ -19,6 +19,9 @@ pymc/model/fgraph.py:76-81, :139) -- and pattern-matches them onto the closed fa
                      survival: pm.Weibull(alpha, beta=exp(eta)), pm.Exponential(scale=exp(eta)) or (lam=exp(-eta)) (the
                      Weibull with alpha = 1) and pm.LogNormal(eta, sigma), plain, or under pm.Censored / pm.Truncated with
                      constant bounds;
+                     Beta regression: pm.Beta(mu=invlogit(eta), nu=phi) or pm.Beta(alpha=mu * phi, beta=(1 - mu) * phi)
+                     and pm.BetaBinomial(alpha=mu * phi, beta=(1 - mu) * phi, n=trials) with constant trials, mu =
+                     invlogit(eta), phi a constant or a scalar free RV;
                      pm.OrderedLogistic / pm.OrderedProbit: the Categorical whose p is their compute_p graph, with or
                      without the {name}_probs Deterministic (recorded, evaluated from the draws);
                      pm.ZeroInflatedPoisson / Binomial / NegativeBinomial and pm.HurdlePoisson / NegativeBinomial / Gamma:
@@ -664,6 +667,55 @@ def from_pymc(model) -> _ir.ModelIR:
             return "weibull_log", eta, {"alpha": 1.0}
         return "lognormal", ps[0], {"sigma": sigma_of(ps[1])}  # LogNormalRV: (mu, sigma)
 
+    def beta_of(op, ps, name, N):
+        """(dist, eta, slots) of pm.Beta / pm.BetaBinomial whose alpha = mu * phi and beta = (1 - mu) * phi (the factors of
+        each product in either order), mu = invlogit(eta): BetaRV (alpha, beta), the graph get_alpha_beta builds for
+        Beta(mu, nu) too (continuous.py:1238-1240); BetaBinomialRV (n, alpha, beta), discrete.py:178-262"""
+        bb = op == "betabinomial"
+        form = ("pm.BetaBinomial(alpha=mu * phi, beta=(1 - mu) * phi, n=trials) with constant trials" if bb else
+                "pm.Beta(mu=mu, nu=phi) or pm.Beta(alpha=mu * phi, beta=(1 - mu) * phi)") + \
+            ", mu = pm.math.invlogit(linear predictor) and phi a constant or a scalar free RV"
+        a_, b_ = ps[-2], ps[-1]
+        slots = {}
+        if bb:
+            nt = _const_value(ps[0])
+            if nt is None:
+                raise NotImplementedError(f"{name}: random trials are outside the closed set ({form})")
+            slots["trials"] = float(nt.reshape(())) if nt.size == 1 else np.ravel(np.broadcast_to(nt, (N,))).astype(np.float64)
+        if _const_value(a_) is not None and _const_value(b_) is not None:
+            raise NotImplementedError(f"{name}: constant alpha and beta with no predictor are outside the closed set (write "
+                                      f"{form})")
+        ins = inputs_of(a_, "mul")
+        if ins is None or len(ins) != 2:
+            raise NotImplementedError(f"{name}: write the likelihood as {form}")
+        mu = next(((m_, p_) for m_, p_ in (ins, ins[::-1]) if inputs_of(m_, "sigmoid") is not None), None)
+        if mu is None:
+            raise NotImplementedError(f"{name}: a mean other than invlogit of a linear predictor is outside the closed set "
+                                      f"({form})")
+        mu, p_ = peel(mu[0]), peel(mu[1])
+        if p_.owner is not None and p_ not in name_of and \
+                {scalar_op_name(v.owner) for v in graph_nodes(p_)} & {"pow", "sqr", "sqrt"}:
+            raise NotImplementedError(f"{name}: pm.Beta(mu, sigma), the kappa form, is outside the closed set (write {form})")
+        c = _const_value(p_)
+        if (p_ in name_of and size_of[name_of[p_]] != 1) or (p_ not in name_of and c is not None and c.size != 1):
+            raise NotImplementedError(f"{name}: a per-observation or vector phi is outside the closed set ({form})")
+        try:
+            phi = param(p_, name + ".phi")
+        except NotImplementedError:
+            raise NotImplementedError(f"{name}: a phi that is an expression of random variables is outside the closed set "
+                                      f"({form})") from None
+        ok = False
+        ins = inputs_of(b_, "mul")
+        for one_minus, q_ in (ins, ins[::-1]) if ins is not None and len(ins) == 2 else ():
+            sub = inputs_of(one_minus, "sub")
+            one = _const_value(sub[0]) if sub is not None and len(sub) == 2 else None
+            if one is not None and np.all(one == 1.0) and peel(sub[1]) is mu and same_param(q_, phi):
+                ok = True
+        if not ok:
+            raise NotImplementedError(f"{name}: write the likelihood as {form} (beta must be (1 - mu) * phi with the mu "
+                                      "and phi of alpha)")
+        return ("beta_binomial_logit" if bb else "beta_logit"), inputs_of(mu, "sigmoid")[0], dict(slots, phi=phi)
+
     survival_ops = ("weibullbeta", "weibull", "exponential", "lognormal")
     probs_of = {}  # id of a {name}_probs Deterministic's expression -> the ordinal likelihood's name
     liks = []
@@ -715,6 +767,9 @@ def from_pymc(model) -> _ir.ModelIR:
         elif op in ("mixture", "_hurdle", "hurdle"):  # pm.ZeroInflated* / pm.Hurdle*
             dist, eta, slot, psi = zero_inflated_of(rv, ps, N)
             liks.append(_ir.Likelihood(dist, y, make_terms(eta, N), name=rv.name, psi=psi, **slot))
+        elif op in ("beta", "betabinomial"):
+            dist, eta, slot = beta_of(op, ps, rv.name, N)
+            liks.append(_ir.Likelihood(dist, y, make_terms(eta, N), name=rv.name, **slot))
         elif op in survival_ops:
             dist, eta, slot = survival_of(op, ps, rv.name, sigma_of)
             liks.append(_ir.Likelihood(dist, y, make_terms(eta, N), name=rv.name, **slot))

@@ -80,6 +80,8 @@ LIK_DISTS = {
     "truncated_lognormal": 23,     # y_i ~ Truncated(LogNormal(eta_i, sigma), lower, upper)
     "normal_mixture": 24,    # y_i ~ NormalMixture(w, eta_i + mu_k, sigma_k)                mixture.py:469-494, :529-546
     "poisson_mixture": 25,   # y_i ~ Mixture(w, Poisson(lam_k exp(eta_i)))
+    "beta_logit": 26,            # y_i ~ Beta(mu = sigmoid(eta_i), nu = phi)               continuous.py:1131-1262, :1238-1240
+    "beta_binomial_logit": 27,   # y_i ~ BetaBinomial(n_i, phi mu_i, phi (1 - mu_i))       discrete.py:178-262
 }
 # Zero-inflated and hurdle observations: ``Likelihood.psi`` is the probability of the count / positive component, a
 # constant in (0, 1), a Ref to a scalar variable with an interval transform inside [0, 1], or a Linear: the logit of psi.
@@ -154,6 +156,19 @@ MIX_LAM = ("lam must be a variable of size K with positive support (log, ordered
            "or K finite constants > 0")
 MIX_SIGMA = "sigma must be a finite constant > 0, K of them, or a variable of size 1 or K with positive support"
 MIX_SLOTS = "a mixture takes no alpha, trials, lower / upper, cutpoints or psi, and poisson_mixture no sigma"
+# Beta regression with a logit mean, mu_i = sigmoid(eta_i), and a precision ``Likelihood.phi`` (PyMC's ``nu`` of
+# ``Beta(mu, nu)``): a finite constant > 0 or a Ref to a scalar variable with positive support.  beta_logit observes
+# y_i in (0, 1); beta_binomial_logit observes counts y_i of ``Likelihood.trials`` (one constant or one per observation),
+# with a = phi mu_i and b = phi (1 - mu_i).  Lowered with phi in the parameter slot and, for the BetaBinomial, the
+# [2][N] block (y, trials) (include/b200nuts.h).
+BETA_LIKS = ("beta_logit", "beta_binomial_logit")
+# the support rule of Beta / BetaBinomial observations (csrc/b200nuts.cu: prepare_ir, same words)
+BETA_Y = ("y must be finite with 0 < y < 1 for every observation (0 and 1 are outside the Beta's support; a "
+          "zero/one-inflated Beta is not provided)")
+BB_TRIALS = "trials must be finite integers >= 0"
+BETA_SLOTS = ("beta_logit and beta_binomial_logit take phi, and no sigma, alpha, cutpoints, psi, weights, components or "
+              "lower / upper")
+BETA_TRIALS = "trials belong to beta_binomial_logit (a Beta observes proportions, not counts)"
 # The support rule.  The device evaluates a density's formula wherever it is asked to, so every variable must be kept
 # inside its prior's support by its transform, and every scale parameter must be positive:
 POSITIVE_PRIORS = ("halfnormal", "halfcauchy", "exponential", "gamma", "lognormal")  # a log transform, or interval lo >= 0
@@ -264,6 +279,7 @@ class Likelihood:
     psi: float | Ref | Linear | None = None    # the zero-inflated / hurdle likelihoods (ZI_LIKS): a Linear is logit(psi)
     weights: Ref | np.ndarray | None = None     # mixtures (MIXTURE_LIKS): a simplex variable or K constants
     components: Ref | np.ndarray | None = None  # mixtures: mu_k (normal_mixture) or lam_k (poisson_mixture)
+    phi: float | Ref | None = None              # BETA_LIKS: the precision, PyMC's nu of Beta(mu, nu)
 
     def n_components(self, model: "ModelIR") -> int:
         """K of a mixture: the size of its components."""
@@ -414,6 +430,12 @@ class ModelIR:
             if L.dist in MIXTURE_LIKS:
                 self._validate_mixture(L)
                 continue
+            if L.dist in BETA_LIKS:
+                self._validate_beta(L)
+                continue
+            if L.phi is not None:
+                raise ValueError(f"{L.dist} likelihood {L.name}: phi belongs to the beta_logit / beta_binomial_logit "
+                                 "likelihoods")
             if L.weights is not None or L.components is not None:
                 raise ValueError(f"{L.dist} likelihood {L.name}: weights and components belong to the mixture likelihoods")
             if L.dist in SIGMA_LIKS and L.sigma is None:
@@ -473,7 +495,7 @@ class ModelIR:
                 par(a)
         for L in self.likelihoods:
             terms(L.terms)
-            for a in (L.sigma, L.alpha, L.psi, L.cutpoints, L.components):
+            for a in (L.sigma, L.alpha, L.psi, L.cutpoints, L.components, L.phi):
                 par(a)
         for a in self.ar1:
             used.append(a.var)
@@ -548,6 +570,36 @@ class ModelIR:
                 ok = sa is not None and sa.shape in ((), (K,)) and bool(np.all(np.isfinite(sa)) and np.all(sa > 0))
             if not ok:
                 raise ValueError(f"{what}: {MIX_SIGMA}")
+
+    def _validate_beta(self, L) -> None:
+        """phi, y and trials of Beta / BetaBinomial observations (the checks prepare_ir makes, in the same words)."""
+        what = f"{L.dist} likelihood {L.name}"
+        if any(a is not None for a in (L.sigma, L.alpha, L.cutpoints, L.psi, L.weights, L.components, L.lower, L.upper)):
+            raise ValueError(f"{what}: {BETA_SLOTS}")
+        if L.dist == "beta_logit" and L.trials is not None:
+            raise ValueError(f"{what}: {BETA_TRIALS}")
+        if L.phi is None:
+            raise ValueError(f"{L.dist} needs phi")
+        if isinstance(L.phi, Ref) and self.var(L.phi.var).size != 1:
+            raise ValueError(f"{L.dist}: phi must be a scalar variable")
+        if isinstance(L.phi, Linear) or (not isinstance(L.phi, Ref) and np.ndim(L.phi) != 0):
+            raise ValueError(f"{what}: phi must be one constant or a scalar variable")
+        self._check_scale(L.phi, f"{what}: phi")
+        y = np.asarray(L.y, dtype=np.float64)
+        if L.dist == "beta_logit":
+            if not (np.all(np.isfinite(y)) and np.all((y > 0.0) & (y < 1.0))):
+                raise ValueError(f"{what}: {BETA_Y}")
+            return
+        if L.trials is None or isinstance(L.trials, (Ref, Linear)):
+            raise ValueError(f"{what}: trials must be a constant scalar or a constant array")
+        n = np.asarray(L.trials, dtype=np.float64)
+        if n.ndim > 1 or (n.ndim == 1 and len(n) != len(y)):
+            raise ValueError(f"{what}: trials must be a scalar or one per observation")
+        n = np.broadcast_to(n, y.shape)
+        if not (np.all(np.isfinite(n)) and np.all(n == np.floor(n)) and np.all(n >= 0)):
+            raise ValueError(f"{what}: {BB_TRIALS}")
+        if not (np.all(np.isfinite(y)) and np.all(y == np.floor(y)) and np.all((y >= 0) & (y <= n))):
+            raise ValueError(f"{what}: {ZIB_Y}")
 
     def _check_terms(self, terms, N: int, where: str, length: str) -> None:
         """Terms of a predictor of length N (a likelihood's observations, or the elements of a prior's variable)."""
@@ -1291,6 +1343,46 @@ def mixture_ir(dist: str = "normal", K: int = 3, weights: str = "dirichlet", cov
                    likelihoods=[Likelihood(lik, y, terms, sigma=sg, weights=wt, components=comp)])
 
 
+def beta_regression_ir(dist: str = "beta", phi: str = "var", n_obs: int = 400, n_groups: int = 8, n_features: int = 2,
+                       seed: int = 71) -> ModelIR:
+    """Beta regression on simulated data: eta_i = b0 + sigma_a z[g_i] + x_i . beta with b0 ~ Normal(0, 1.5), z_g ~ Normal(0,
+    1) and sigma_a ~ HalfNormal(1) (non-centred group intercepts), beta ~ Normal(0, 1)^F as a design term, mu_i =
+    sigmoid(eta_i), and ``dist="beta"``: y_i ~ Beta(mu_i, nu = phi), the proportions PyMC writes as
+    ``pm.Beta("y", mu=pm.math.invlogit(eta), nu=phi)``; ``"beta_binomial"``: y_i ~ BetaBinomial(n_i, phi mu_i, phi (1 -
+    mu_i)) with per-observation trials n_i from 5 to 60, whose spread is visibly wider than the Binomial's (phi = 4).
+    ``phi="var"``: phi ~ Gamma(2, 0.1) under a log transform; ``"const"``: phi is the simulation's value."""
+    if dist not in ("beta", "beta_binomial"):
+        raise ValueError("dist must be 'beta' or 'beta_binomial'")
+    if phi not in ("var", "const"):
+        raise ValueError("phi must be 'var' or 'const'")
+    rng = np.random.default_rng(seed)
+    g = rng.integers(0, n_groups, n_obs).astype(np.int32)
+    X = rng.standard_normal((n_obs, n_features))
+    eta = -0.3 + rng.normal(0.0, 0.5, n_groups)[g] + X @ rng.normal(0.0, 0.5, n_features)
+    mu = 1.0 / (1.0 + np.exp(-eta))
+    phi_true = 15.0 if dist == "beta" else 4.0
+    p = rng.beta(mu * phi_true, (1.0 - mu) * phi_true)
+    trials = None
+    if dist == "beta":
+        y = np.clip(p, 1e-12, 1.0 - 1e-12)
+    else:
+        trials = rng.integers(5, 61, n_obs).astype(np.float64)
+        y = rng.binomial(trials.astype(np.int64), p).astype(np.float64)
+    vars_ = [Var("b0", "b0", 1), Var("z", "z", n_groups), Var("sigma_a_log__", "sigma_a", 1, "log"),
+             Var("beta", "beta", n_features)]
+    priors = [Prior("normal", "b0", (0.0, 1.5)), Prior("normal", "z", (0.0, 1.0)), Prior("halfnormal", "sigma_a_log__", (1.0,)),
+              Prior("normal", "beta", (0.0, 1.0))]
+    par = phi_true
+    if phi == "var":
+        vars_.append(Var("phi_log__", "phi", 1, "log", initial=np.log(phi_true)))
+        priors.append(Prior("gamma", "phi_log__", (2.0, 0.1)))
+        par = Ref("phi_log__")
+    terms = [Term([("b0", None)]), Term([("sigma_a_log__", None), ("z", g)]), Term([("beta", None)], coef=X)]
+    lik = "beta_logit" if dist == "beta" else "beta_binomial_logit"
+    return ModelIR(name=f"{dist}_{phi}", vars=vars_, priors=priors,
+                   likelihoods=[Likelihood(lik, y, terms, trials=trials, phi=par)])
+
+
 # ------------------------------------------------------------------------------------------------------------------------
 # lowering: ModelIR -> flat arrays of the C ABI (include/b200nuts.h: b200_ir)
 # ------------------------------------------------------------------------------------------------------------------------
@@ -1310,6 +1402,8 @@ class LoweredIR:
                             # zero-inflated / hurdle: nu = 0 or m, and psi = the psi block (a list of term dicts)
                             # normal_mixture / poisson_mixture: nu = K, and mix = the weights, component (and sigma)
                             # blocks (term dicts)
+                            # beta_logit / beta_binomial_logit: phi is the sigma slot; beta_binomial_logit's y is the
+                            # [2][N] block (y, trials)
                             # y_var 0: y is observed data; v + 1: a latent factor, y is None and its values are variable v's
     ar1: list               # [(var, phi(kind, value, ref), sigma(kind, value, ref), init_sigma)]
 
@@ -1388,7 +1482,11 @@ def lower(ir: ModelIR) -> LoweredIR:
         par = L.trials if fam == "binomial_logit" else (L.alpha if fam in DISPERSION_LIKS + WEIBULL_LIKS else L.sigma)
         if L.dist in MIXTURE_LIKS:
             par = None  # sigma is a block
+        if L.dist in BETA_LIKS:
+            par = L.phi
         y = np.ascontiguousarray(L.y, dtype=np.float64)
+        if L.dist == "beta_binomial_logit":  # the [2][N] block: y, trials
+            y = np.ascontiguousarray(np.stack([y, np.broadcast_to(np.asarray(L.trials, dtype=np.float64), y.shape)]))
         if L.dist in BOUNDED_LIKS + SURVIVAL_BOUNDED:  # the [3][N] block: y, lower, upper
             y = np.ascontiguousarray(np.stack([y, *L.bounds()]))
         extra = {}
@@ -1508,7 +1606,7 @@ def specialise(ir: ModelIR, extended: bool = False):
         return not isinstance(p.params[k], Ref) and (want is None or float(p.params[k]) == want)
 
     pri = {ir.var(p.var).name: p for p in ir.priors}
-    if len(pri) != len(ir.priors) or len(ir.likelihoods) != 1 or ir.likelihoods[0].dist in ZI_LIKS + MIXTURE_LIKS:
+    if len(pri) != len(ir.priors) or len(ir.likelihoods) != 1 or ir.likelihoods[0].dist in ZI_LIKS + MIXTURE_LIKS + BETA_LIKS:
         return None
     if any(isinstance(a, Linear) or (not isinstance(a, Ref) and np.ndim(a) > 0) for p in ir.priors for a in p.params):
         return None

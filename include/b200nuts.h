@@ -91,6 +91,7 @@ extern "C" {
 #define B200_IR_P_LOGNORMAL 10  /* mu, sigma             :1807-1814 */
 #define B200_IR_P_DIRICHLET 11  /* a (const), the concentration of every one of the K components; only on a SIMPLEX
                                  * variable of size K - 1    multivariate.py:557-585 */
+#define B200_IR_P_INVERSEGAMMA 12 /* alpha, beta (const > 0); positive support   :2631-2640 */
 /* likelihoods of a linear predictor eta_i = sum_t coef_t[i] * prod_f x_f[idx_f[i]] */
 #define B200_IR_L_NORMAL 0          /* y ~ Normal(eta, sigma)                    continuous.py:526-527  */
 #define B200_IR_L_BERNOULLI_LOGIT 1 /* y ~ Bernoulli(logit_p = eta)              discrete.py:362-367    */
@@ -177,8 +178,8 @@ extern "C" {
  *                        integer with 0 <= y <= trials */
 #define B200_IR_L_BETA_LOGIT 26             /* pm.Beta(mu, nu) continuous.py:1131-1262, alpha = mu nu :1238-1240 */
 #define B200_IR_L_BETA_BINOMIAL_LOGIT 27    /* pm.BetaBinomial discrete.py:178-262                            */
-/* The support rule b200_model_create enforces (as ModelIR.validate does): HalfNormal, HalfCauchy, Exponential, Gamma and
- * LogNormal priors sit on a LOG variable or an INTERVAL with lo >= 0, Beta on an INTERVAL inside [0, 1], Uniform(a, b) on an
+/* The support rule b200_model_create enforces (as ModelIR.validate does): HalfNormal, HalfCauchy, Exponential, Gamma,
+ * InverseGamma and LogNormal priors sit on a LOG variable or an INTERVAL with lo >= 0, Beta on an INTERVAL inside [0, 1], Uniform(a, b) on an
  * INTERVAL inside [a, b]; every scale (a prior's sigma / beta / lam, Normal and StudentT sigma including each sigma_obs, an
  * AR(1) sigma, alpha) is a finite constant > 0 or a REF to a scalar of positive support; Poisson y are integers >= 0,
  * Bernoulli y are 0 or 1.  Censored and truncated Normal observations: y finite, lower_i < upper_i, lower never +inf and
@@ -207,7 +208,23 @@ typedef struct b200_ir_factor {
 } b200_ir_factor;
 /* A term is coef[i] * prod_f x_f[idx_f[i]] when n_cols == 0.  n_cols > 0 makes it a design term,
  * eta_i += sum_k X[i][k] x[f[0].offset + k]: coef is X, row-major [N][n_cols], finite; n_factors == 1, f[0].size == n_cols
- * and f[0].idx == NULL.  b200_model_create refuses any other design table with the words ModelIR.validate uses. */
+ * and f[0].idx == NULL.  b200_model_create refuses any other design table with the words ModelIR.validate uses.
+ *
+ * A spectral term (a Hilbert-space approximate GP, pm.gp.HSGP non-centred, hsgp_approx.py:453-473) is a design term with
+ * n_factors == 3 whose column weights depend on hyperparameters: eta_i += sum_k Phi[i][k] s_k z_k, with
+ *   s_k = a sqrt(S(omega_k; l)),  Q_k = sum_d l_d^2 omega_kd^2  and the power spectral density S of cov (cov.py):
+ *   EXPQUAD   S = (2 pi)^(D/2) prod_d l_d exp(-Q/2)
+ *   MATERN52  S = 2^D pi^(D/2) Gamma((D+5)/2) 5^(5/2) / (3/4 sqrt(pi)) prod_d l_d (5 + Q)^(-(D+5)/2)
+ *   MATERN32  S = 2^D pi^(D/2) Gamma((D+3)/2) 3^(3/2) / (1/2 sqrt(pi)) prod_d l_d (3 + Q)^(-(D+3)/2)
+ *   n_cols  M;  f[0] z: a variable of size M, no index, no transform
+ *   f[1]    the amplitude a: a scalar variable with positive support (size 1), or size 0 for the constant in the block
+ *   f[2]    the lengthscale(s) l: a variable of size 1 (isotropic) or D with positive support, or size 0 for the constants
+ *   coef    Phi [N][M] row-major, finite, followed by the block (3 + D + M D doubles):
+ *           cov, D, a (> 0; read when f[1].size == 0), l_1 .. l_D (> 0; read when f[2].size == 0), omega [M][D] (finite, >= 0)
+ * Such a term may stand wherever a design term may. */
+#define B200_IR_COV_EXPQUAD 1
+#define B200_IR_COV_MATERN52 2
+#define B200_IR_COV_MATERN32 3
 typedef struct b200_ir_term {
     const double* coef; /* [N] or NULL (= 1); a design term: X [N][n_cols] */
     int32_t n_factors, n_cols;

@@ -509,6 +509,13 @@ static bool ir_scale_ok(const b200_ir_param& p, const std::vector<IrVarD>& vars)
 #define B200_IR_BETA_Y "y must be finite with 0 < y < 1 for every observation (0 and 1 are outside the Beta's support; a zero/one-inflated Beta is not provided)"
 #define B200_IR_BB_TRIALS "trials must be finite integers >= 0"
 #define B200_IR_BETA_SLOTS "beta_logit and beta_binomial_logit take phi, and no sigma, alpha, cutpoints, psi, weights, components or lower / upper"
+// Spectral (HSGP) terms (ModelIR._check_spectral, same wording)
+#define B200_IR_SPEC_PHI "a spectral term's Phi must be finite with shape (N, M), M the size of its variable"
+#define B200_IR_SPEC_Z "a spectral term's variable must be one whole variable with no index and no transform"
+#define B200_IR_SPEC_OMEGA "omega must have shape (M, D), D >= 1, with finite entries >= 0"
+#define B200_IR_SPEC_COV "cov must be expquad, matern52 or matern32"
+#define B200_IR_SPEC_LS "ls must be a finite constant > 0, D of them, or a variable of size 1 or D with positive support"
+#define B200_IR_SPEC_AMP "amplitude must be a finite constant > 0 or a scalar variable with positive support"
 static constexpr double LOG_PI = 1.1447298858494001741, LOG_2 = 0.69314718055994530942;
 
 // The pass over a b200_ir.  Its steps return 0 or fail(...); the arrays they record in `sg` stay put until the upload.
@@ -526,6 +533,9 @@ struct IrPass {
     bool has_design = false;
     int simplex_rows = 0;  // doubles of the simplex variables' (log w, G) rows, after x in the team slice
     std::vector<int> n_priors_of;  // priors on each variable
+    std::deque<IrSpecD> specs;     // the spectral terms
+    int spec_rows = 0;             // doubles of their (s z, g_b, s) rows, after the simplex rows in the team slice
+    bool has_inversegamma = false;
     template <class T> void add(const T** dst, const T* host, size_t count) { sg.add(dst, host, count, Staging::IN); }
 };
 
@@ -607,7 +617,7 @@ static int ir_prior(IrPass& c, const b200_ir_prior& F, int k, IrPriorD& P) {
     }
     if (scale >= 0 && !ir_scale_ok(F.p[scale], c.vars)) return fail("ir: prior %d: parameter %d (the scale) " B200_IR_SCALE_RULE, k, scale);
     const bool positive = F.dist == B200_IR_P_HALFNORMAL || F.dist == B200_IR_P_HALFCAUCHY || F.dist == B200_IR_P_EXPONENTIAL ||
-                          F.dist == B200_IR_P_GAMMA || F.dist == B200_IR_P_LOGNORMAL;
+                          F.dist == B200_IR_P_GAMMA || F.dist == B200_IR_P_LOGNORMAL || F.dist == B200_IR_P_INVERSEGAMMA;
     const bool real_line = F.dist == B200_IR_P_FLAT || F.dist == B200_IR_P_NORMAL || F.dist == B200_IR_P_STUDENTT ||
                            F.dist == B200_IR_P_CAUCHY;
     if (ir_extended_transforms(PV.transform) && !(real_line || (positive && PV.transform == B200_IR_T_ORDERED_POSITIVE)))
@@ -634,6 +644,12 @@ static int ir_prior(IrPass& c, const b200_ir_prior& F, int k, IrPriorD& P) {
         case B200_IR_P_GAMMA:
             if (!cst(0) || !cst(1) || !(F.p[0].value > 0) || !(F.p[1].value > 0)) return fail("ir: prior %d: Gamma needs constant alpha, beta > 0", k);
             P.c0 = F.p[0].value * std::log(F.p[1].value) - std::lgamma(F.p[0].value);
+            break;
+        case B200_IR_P_INVERSEGAMMA:  // evaluated out of line on IrExtendedModel (csrc/ir_model.cuh: ir_inversegamma)
+            if (!cst(0) || !cst(1) || !(F.p[0].value > 0) || !(F.p[1].value > 0) || !std::isfinite(F.p[0].value) || !std::isfinite(F.p[1].value))
+                return fail("ir: prior %d: InverseGamma needs constant alpha, beta > 0", k);
+            P.c0 = F.p[0].value * std::log(F.p[1].value) - std::lgamma(F.p[0].value);
+            c.has_inversegamma = true;
             break;
         case B200_IR_P_BETA:
             if (!cst(0) || !cst(1) || !(F.p[0].value > 0) || !(F.p[1].value > 0)) return fail("ir: prior %d: Beta needs constant alpha, beta > 0", k);
@@ -845,6 +861,83 @@ static int ir_ordinal(IrPass& c, const b200_ir_lik& L, int l) {
     return 0;
 }
 
+// A spectral term (include/b200nuts.h): the checks and words of ModelIR._check_spectral, then its IrSpecD and rows.  Its
+// device term is a design term on the b row whose gradient goes to the g_b row (csrc/ir_model.cuh: IrSpecD).
+static int ir_spectral(IrPass& c, const b200_ir_term& T, long long N, int l, int t, IrTermD& TD) {
+    const int M = T.n_cols;
+    const b200_ir_factor& Z = T.f[0];
+    const IrVarD* V = ir_var_at(c.vars, Z.offset);
+    if (Z.idx || !V || V->transform != B200_IR_T_NONE) return fail("ir: likelihood %d term %d: " B200_IR_SPEC_Z, l, t);
+    if (M < 0 || Z.size != M || V->size != M || !T.coef) return fail("ir: likelihood %d term %d: " B200_IR_SPEC_PHI, l, t);
+    const double* blk = T.coef + (size_t)N * M;
+    const double cov = blk[0], Dd = blk[1];
+    if (cov != B200_IR_COV_EXPQUAD && cov != B200_IR_COV_MATERN52 && cov != B200_IR_COV_MATERN32)
+        return fail("ir: likelihood %d term %d: " B200_IR_SPEC_COV, l, t);
+    if (!(Dd >= 1 && Dd <= 4096 && Dd == std::floor(Dd))) return fail("ir: likelihood %d term %d: " B200_IR_SPEC_OMEGA, l, t);
+    const int D = (int)Dd;
+    const double* ls = blk + 3;
+    const double* omega = ls + D;
+    for (long long i = 0; i < (long long)M * D; ++i)
+        if (!(std::isfinite(omega[i]) && omega[i] >= 0)) return fail("ir: likelihood %d term %d: " B200_IR_SPEC_OMEGA, l, t);
+    IrSpecD S{};
+    S.z = Z.offset; S.M = M; S.D = D; S.a_ref = -1; S.ls_size = 0;
+    const b200_ir_factor& A = T.f[1];
+    if (A.size == 0) {
+        if (!(std::isfinite(blk[2]) && blk[2] > 0)) return fail("ir: likelihood %d term %d: " B200_IR_SPEC_AMP, l, t);
+        S.a = blk[2];
+    } else {
+        const IrVarD* AV = ir_var_at(c.vars, A.offset);
+        if (A.idx || A.size != 1 || !AV || AV->size != 1 || !ir_positive_support(*AV))
+            return fail("ir: likelihood %d term %d: " B200_IR_SPEC_AMP, l, t);
+        S.a_ref = A.offset;
+    }
+    const b200_ir_factor& Lf = T.f[2];
+    if (Lf.size == 0) {
+        for (int d = 0; d < D; ++d)
+            if (!(std::isfinite(ls[d]) && ls[d] > 0)) return fail("ir: likelihood %d term %d: " B200_IR_SPEC_LS, l, t);
+    } else {
+        const IrVarD* LV = ir_var_at(c.vars, Lf.offset);
+        if (Lf.idx || !(Lf.size == 1 || Lf.size == D) || !LV || LV->size != Lf.size || !ir_positive_support(*LV))
+            return fail("ir: likelihood %d term %d: " B200_IR_SPEC_LS, l, t);
+        S.ls_ref = Lf.offset;
+        S.ls_size = Lf.size;
+    }
+    std::vector<double>& xt = c.reals.emplace_back((size_t)N * M);
+    for (long long i = 0; i < N; ++i)
+        for (int k = 0; k < M; ++k) {
+            const double v = T.coef[i * M + k];
+            if (!std::isfinite(v)) return fail("ir: likelihood %d term %d: " B200_IR_SPEC_PHI " (at row %lld, column %d)", l, t, i, k);
+            xt[(size_t)k * N + i] = v;
+        }
+    // log C_D of S = C_D prod_d l_d e^{h(Q)}, and h's nu and c (include/b200nuts.h)
+    const double hD = 0.5 * D, LOG_2PI = LOG_2 + LOG_PI;
+    if (cov == B200_IR_COV_EXPQUAD) {
+        S.log_c = hD * LOG_2PI;
+    } else {
+        const bool m52 = cov == B200_IR_COV_MATERN52;
+        const double nu = m52 ? 2.5 : 1.5;  // the Matern order; c = 2 nu, nu' = (D + 2 nu) / 2
+        S.c = 2.0 * nu;
+        S.nu = hD + nu;
+        S.log_c = D * LOG_2 + hD * LOG_PI + std::lgamma(S.nu) + nu * std::log(S.c) - std::log(m52 ? 0.75 : 0.5) - 0.5 * LOG_PI;
+    }
+    const int rows = (3 * M + 3) & ~3;
+    S.b_row = ((c.n + 3) & ~3) + c.simplex_rows + c.spec_rows;
+    S.gb_row = S.b_row + M;
+    S.s_row = S.gb_row + M;
+    c.spec_rows += rows;
+    IrSpecD& SD = c.specs.emplace_back(S);
+    if (Lf.size == 0) c.add(&SD.ls, ls, (size_t)D);
+    c.add(&SD.omega, omega, (size_t)M * D);
+    TD.n_factors = 3;
+    TD.n_cols = M;
+    TD.f[0] = IrFactorD{S.b_row, M, nullptr, nullptr, nullptr};
+    TD.f[1] = IrFactorD{S.gb_row, M, nullptr, nullptr, nullptr};
+    c.add(&TD.coef, T.coef, (size_t)N * M);
+    c.add(&TD.xt, xt.data(), xt.size());
+    c.has_design = true;
+    return 0;
+}
+
 // terms[t0 .. t1) of a likelihood: the predictor's, or those of the logit of a zero-inflated / hurdle psi
 static int ir_terms(IrPass& c, const b200_ir_lik& L, int l, int t0, int t1) {
     const long long N = L.N;
@@ -853,6 +946,10 @@ static int ir_terms(IrPass& c, const b200_ir_lik& L, int l, int t0, int t1) {
         if (T.n_factors < 0 || T.n_factors > 3) return fail("ir: likelihood %d term %d: 0..3 variable factors", l, t);
         IrTermD& TD = c.terms.emplace_back();
         TD.n_factors = T.n_factors;
+        if (T.n_cols != 0 && T.n_factors == 3) {  // a spectral term
+            if (ir_spectral(c, T, N, l, t, TD)) return -1;
+            continue;
+        }
         if (T.n_cols != 0) {  // design term: coef is X [N][n_cols]; the same checks and words as ModelIR.validate()
             const int K = T.n_cols;
             if (T.n_factors != 1) return fail("ir: likelihood %d term %d: a design term has exactly one factor", l, t);
@@ -1108,19 +1205,30 @@ static int prepare_ir(b200_model* m, const b200_model_desc* d) {
         if (ir_ar1(c, R->ar1[k], k, ars[k])) return -1;
     // the description is accepted: upload its data, then the tables that point into it
     if (use_current_device(m) || sg.commit() || sg.finish()) return -1;
-    const std::vector<IrTermD> terms(c.terms.begin(), c.terms.end());
+    // one allocation: the spectral terms' IrSpecD table, their count, then the terms (csrc/ir_model.cuh: ir_specs)
+    const long long n_spec = (long long)c.specs.size();
+    const size_t head = n_spec * sizeof(IrSpecD) + sizeof n_spec;
+    std::vector<unsigned char> tab(head + c.terms.size() * sizeof(IrTermD));
+    size_t at = 0;
+    for (const IrSpecD& S : c.specs) { std::memcpy(tab.data() + at, &S, sizeof S); at += sizeof S; }
+    std::memcpy(tab.data() + at, &n_spec, sizeof n_spec);
+    at += sizeof n_spec;
+    for (const IrTermD& T : c.terms) { std::memcpy(tab.data() + at, &T, sizeof T); at += sizeof T; }
+    const unsigned char* tab_d = nullptr;
     IrModel::Params& P = m->ir;
     P.n_vars = R->n_vars; P.n_priors = (int)priors.size(); P.n_liks = (int)m->ir_liks.size(); P.n_ar1 = (int)ars.size(); P.n = c.n;
-    if (upload(m, c.vars, &P.vars) || upload(m, priors, &P.priors) || upload(m, m->ir_liks, &P.liks) || upload(m, terms, &P.terms) ||
+    if (upload(m, c.vars, &P.vars) || upload(m, priors, &P.priors) || upload(m, m->ir_liks, &P.liks) || upload(m, tab, &tab_d) ||
         upload(m, ars, &P.ar1))
         return -1;
-    P.n_pad = ((c.n + 3) & ~3) + c.simplex_rows;  // x, then the simplex variables' rows
+    P.terms = reinterpret_cast<const IrTermD*>(tab_d + head);
+    P.n_pad = ((c.n + 3) & ~3) + c.simplex_rows + c.spec_rows;  // x, then the simplex variables' and spectral terms' rows
     // likelihoods are evaluated one after another: they share the row
     const long long row2 = std::max(std::max(c.ord_obs, c.zeta_obs), c.mix_obs);
     P.ord_row = row2 ? (int)(P.n_pad + ((c.max_obs + 3) & ~3LL)) : 0;  // after r, before the design partials
     P.stride = P.n_pad + ((c.max_obs + 3) & ~3LL) + ((row2 + 3) & ~3LL) + (c.has_design ? kIrPartDoubles : 0);
     m->ir_extended = std::any_of(c.vars.begin(), c.vars.end(), [](const IrVarD& V) { return ir_extended_transforms(V.transform); }) ||
-                     std::any_of(m->ir_liks.begin(), m->ir_liks.end(), [](const IrLikD& L) { return ir_extended_liks(L.dist); });
+                     std::any_of(m->ir_liks.begin(), m->ir_liks.end(), [](const IrLikD& L) { return ir_extended_liks(L.dist); }) ||
+                     !c.specs.empty() || c.has_inversegamma;
     return 0;
 }
 

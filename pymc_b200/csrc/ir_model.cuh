@@ -61,6 +61,30 @@ struct IrFactorD { int offset, size; const int* idx; const int* rowptr; const in
 struct IrTermD { const double* coef; int n_factors, n_cols; IrFactorD f[3]; const double* xt; };
 constexpr int kIrPartDoubles = 256;  // per-team slice partials of a design term's gradient, at the end of the team scratch
 
+// A spectral term (include/b200nuts.h) runs as a design term whose coefficients are b_k = s_k z_k: its device IrTermD has
+// n_factors == 3, f[0].offset = the b row and f[1].offset = the g_b row, both in the team slice.  ir_spectral_forward fills
+// the b row before any likelihood, so ir_eta and ir_design_row read it as they read a variable; term_grad writes
+// g_b = Phi^T r into the g_b row, and ir_spectral_grad takes it back to z, a and l.  One IrSpecD per spectral term, in
+// the table in front of the terms (ir_spec_count, ir_specs).
+//   log s_k = log a + (log C_D + sum_d log l_d + h(Q_k)) / 2,  Q_k = sum_d l_d^2 omega_kd^2,
+//   h = -Q / 2 (EXPQUAD: nu == 0) or -nu log(c + Q) (Matern: nu = (D + 5) / 2, c = 5 or nu = (D + 3) / 2, c = 3),
+// so s_k underflows to 0 instead of forming 0 * inf where the density is far below the double range.
+struct IrSpecD {
+    int z, b_row, gb_row, s_row;  // z's offset in x; the rows b = s z, g_b and s of the team slice
+    int M, D, a_ref, ls_ref;      // a_ref: the amplitude's offset in x, or -1 for the constant a
+    int ls_size, pad0, pad1, pad2;  // 1 or D: the lengthscale variable at ls_ref; 0: the constants ls[D]
+    double a, log_c, nu, c;
+    const double* ls;
+    const double* omega;  // [M][D]
+};
+static_assert(sizeof(IrSpecD) % alignof(IrTermD) == 0, "the IrSpecD table sits in front of the terms");
+// The terms' allocation is [IrSpecD x n_spec][long long n_spec][IrTermD ...] with IrModel::Params::terms at the first term:
+// IrModel and its kernels never look in front of it, so models without spectral terms keep every table and kernel they had.
+__host__ __device__ __forceinline__ int ir_spec_count(const IrTermD* terms) { return (int)reinterpret_cast<const long long*>(terms)[-1]; }
+__host__ __device__ __forceinline__ const IrSpecD* ir_specs(const IrTermD* terms, int n_spec) {
+    return reinterpret_cast<const IrSpecD*>(reinterpret_cast<const long long*>(terms) - 1) - n_spec;
+}
+
 // sum_k X[i][k] b[k], k ascending
 __device__ __forceinline__ double ir_design_row(const IrTermD& Tm, const double* b, int i, int N) {
     const double* xt = Tm.xt + i;
@@ -656,6 +680,96 @@ __device__ __noinline__ void ir_simplex_chain(const IrVarD* Vp, const double* x,
     for (int j = 0; j < K - 1; ++j) g[o + j] = (G[j] - exp(lw[j]) * S) - last;
 }
 
+// The InverseGamma prior (continuous.py:2631-2640): c0 - (alpha + 1) log x - beta / x per element, c0 = alpha log beta -
+// lgamma(alpha), with d / dx = -(alpha + 1) / x + beta / x^2.  Team-strided over the elements; returns this thread's part.
+__device__ __noinline__ double ir_inversegamma(const IrPriorD* Fp, const double* x, double* g, int tid, int TS) {
+    const int o = Fp->offset, n = Fp->size;
+    const double a1 = Fp->p[0].value + 1.0, b = Fp->p[1].value, c0 = Fp->c0;
+    double lp = 0.0;
+    for (int j = tid; j < n; j += TS) {
+        const double xv = x[o + j], ix = 1.0 / xv;
+        lp += c0 - a1 * log(xv) - b * ix;
+        g[o + j] += ix * (b * ix - a1);
+    }
+    return lp;
+}
+
+// h'(Q) of a spectral term's log density (see IrSpecD)
+__device__ __forceinline__ double ir_spectral_dh(const IrSpecD& S, double Q) { return S.nu == 0.0 ? -0.5 : -S.nu / (S.c + Q); }
+
+// Q_k = sum_d (l_d omega_kd)^2, d ascending
+__device__ __forceinline__ double ir_spectral_q(const IrSpecD& S, const double* ls, int ls_step, int k) {
+    double Q = 0.0;
+    for (int d = 0; d < S.D; ++d) {
+        const double t = ls[d * ls_step] * S.omega[(long long)k * S.D + d];
+        Q = fma(t, t, Q);
+    }
+    return Q;
+}
+
+// the lengthscales of S as this evaluation sees them, with the step between them (0: one isotropic variable)
+__device__ __forceinline__ const double* ir_spectral_ls(const IrSpecD& S, const double* x, int& step) {
+    step = S.ls_size == 1 ? 0 : 1;
+    return S.ls_size ? x + S.ls_ref : S.ls;
+}
+
+// Every spectral term's rows for this evaluation: s_k, b_k = s_k z_k, and g_b_k = 0.  Team-strided over k; the caller
+// synchronises the team before the rows are read.
+__device__ __noinline__ void ir_spectral_forward(const IrSpecD* Sp, int n_spec, double* x, int tid, int TS) {
+    for (int j = 0; j < n_spec; ++j) {
+        const IrSpecD& S = Sp[j];
+        int step;
+        const double* ls = ir_spectral_ls(S, x, step);
+        double base = S.log_c;
+        for (int d = 0; d < S.D; ++d) base += log(ls[d * step]);
+        base = fma(0.5, base, log(S.a_ref >= 0 ? x[S.a_ref] : S.a));
+        for (int k = tid; k < S.M; k += TS) {
+            const double Q = ir_spectral_q(S, ls, step, k);
+            const double h = S.nu == 0.0 ? -0.5 * Q : -S.nu * log(S.c + Q);
+            const double sk = exp(fma(0.5, h, base));
+            x[S.s_row + k] = sk;
+            x[S.b_row + k] = sk * x[S.z + k];
+            x[S.gb_row + k] = 0.0;
+        }
+    }
+}
+
+// The chain rule from g_b (complete in the g_b rows) to z, a and l: with w_k = z_k s_k g_b_k,
+//   d/dz_k = s_k g_b_k,  d/da = sum_k w_k / a,  d/dl_d = sum_k w_k / (2 l_d) + l_d sum_k w_k omega_kd^2 h'(Q_k)
+// (an isotropic l takes the sum over d).  Each sum is a team reduction in a fixed order; a k whose s_k underflowed adds
+// nothing.
+template <int W>
+__device__ __noinline__ void ir_spectral_grad(const IrSpecD* Sp, int n_spec, const double* x, double* g, int tid, double* red) {
+    constexpr int TS = 32 * W;
+    for (int j = 0; j < n_spec; ++j) {
+        const IrSpecD& S = Sp[j];
+        double sw = 0.0;
+        for (int k = tid; k < S.M; k += TS) {
+            const double sg = x[S.s_row + k] * x[S.gb_row + k];
+            g[S.z + k] += sg;
+            sw = fma(x[S.z + k], sg, sw);
+        }
+        if (S.a_ref < 0 && S.ls_size == 0) continue;  // uniform branch: constant hyperparameters
+        const double tw = team_sum<W>(sw, tid, red);
+        if (tid == 0 && S.a_ref >= 0) g[S.a_ref] += tw / x[S.a_ref];
+        if (S.ls_size == 0) continue;
+        int step;
+        const double* ls = ir_spectral_ls(S, x, step);
+        for (int d = 0; d < S.D; ++d) {
+            double sd = 0.0;
+            for (int k = tid; k < S.M; k += TS) {
+                const double w = x[S.z + k] * x[S.s_row + k] * x[S.gb_row + k];
+                if (w == 0.0) continue;
+                const double om = S.omega[(long long)k * S.D + d];
+                sd = fma(w * om * om, ir_spectral_dh(S, ir_spectral_q(S, ls, step, k)), sd);
+            }
+            const double td = team_sum<W>(sd, tid, red);
+            const double l = ls[d * step];
+            if (tid == 0) g[S.ls_ref + d * step] += fma(l, td, tw / (2.0 * l));
+        }
+    }
+}
+
 // ---- finite mixtures (mixture.py:469-494): log p(y_i) = lse_k(l_ik), l_ik = log w_k + log f_k(y_i), over K = L.nu
 // components, with the weights, component and (Normal) sigma blocks at terms[term0 + n_terms ..] (include/b200nuts.h).
 // f_k is Normal(eta + mu_k, sigma_k) or Poisson(lam_k e^eta), less the constants -log(2 pi) / 2 and -lgamma(y + 1) (in c0:
@@ -842,14 +956,18 @@ struct IrModel {
     // The gradient of every (term, factor) of the block terms[term0 .. term0 + n_terms) of length N, given r_i = d logp /
     // d (the block's sum)_i: d sum_i / d x_f = coef * (other factors).  A likelihood's predictor runs it with its r row,
     // the logit of a zero-inflated / hurdle psi with its zeta row.  The caller has synchronised the team after writing r.
-    template <int W>
+    template <int W, bool EXTENDED = false>
     __device__ __forceinline__ static void term_grad(const Params& P, int term0, int n_terms, const double* r, int N,
                                                      double* x, double* g_s, int tid, double* red) {
         constexpr int TS = 32 * W;
         for (int t = 0; t < n_terms; ++t) {
             const IrTermD& Tm = P.terms[term0 + t];
             if (Tm.n_cols) {  // uniform branch: the residuals r are complete after the caller's barrier
-                ir_design_grad<W>(Tm, r, N, g_s + Tm.f[0].offset, x + P.stride - kIrPartDoubles, tid);
+                double* gt = g_s + Tm.f[0].offset;
+                if constexpr (EXTENDED) {
+                    if (Tm.n_factors == 3) gt = x + Tm.f[1].offset;  // a spectral term: Phi^T r into its g_b row
+                }
+                ir_design_grad<W>(Tm, r, N, gt, x + P.stride - kIrPartDoubles, tid);
                 team_sync<W>();
                 continue;
             }
@@ -927,6 +1045,11 @@ struct IrModel {
                     team_sync<W>();
                     continue;
                 }
+                if (F.dist == B200_IR_P_INVERSEGAMMA) {  // uniform branch: out of line
+                    lp += ir_inversegamma(P.priors + k, x, g_s, tid, TS);
+                    team_sync<W>();
+                    continue;
+                }
             }
             const double a0 = par(F.p[0], x), a1 = par(F.p[1], x), a2 = par(F.p[2], x);
             double s[3] = {0.0, 0.0, 0.0};  // sums for the parameter gradients
@@ -994,6 +1117,14 @@ struct IrModel {
                 }
             }
             team_sync<W>();
+        }
+
+        if constexpr (EXTENDED) {
+            const int n_spec = ir_spec_count(P.terms);
+            if (n_spec) {  // uniform branch: the spectral terms' rows, before any likelihood reads them
+                ir_spectral_forward(ir_specs(P.terms, n_spec), n_spec, x, tid, TS);
+                team_sync<W>();
+            }
         }
 
         // ---- 2b. likelihoods: eta_i = sum_t coef_t[i] prod_f x_f[idx_f[i]] ----------------------------------------------
@@ -1070,7 +1201,7 @@ struct IrModel {
                 if (zi) {  // uniform branch: the psi block's gradient
                     const IrTermD* pt = P.terms + L.term0 + L.n_terms;
                     if (L.nu > 0.0) {  // the terms of logit(psi), fed the zeta row
-                        term_grad<W>(P, L.term0 + L.n_terms, (int)L.nu, x + P.ord_row, N, x, g_s, tid, red);
+                        term_grad<W, true>(P, L.term0 + L.n_terms, (int)L.nu, x + P.ord_row, N, x, g_s, tid, red);
                     } else if (pt->n_factors) {  // a psi variable: one team reduction
                         const double tot = team_sum<W>(s_psi, tid, red);
                         if (tid == 0) g_s[pt->f[0].offset] += tot;
@@ -1084,7 +1215,14 @@ struct IrModel {
                 team_sync<W>();
             }
             // gradient of every (term, factor) of the predictor: d eta_i / d x_f = coef * (other factors)
-            term_grad<W>(P, L.term0, L.n_terms, r, N, x, g_s, tid, red);
+            term_grad<W, EXTENDED>(P, L.term0, L.n_terms, r, N, x, g_s, tid, red);
+        }
+        if constexpr (EXTENDED) {
+            const int n_spec = ir_spec_count(P.terms);
+            if (n_spec) {  // uniform branch: the spectral terms' g_b rows back to z, a and l
+                ir_spectral_grad<W>(ir_specs(P.terms, n_spec), n_spec, x, g_s, tid, red);
+                team_sync<W>();
+            }
         }
 
         // ---- 2c. AR(1): h_0 ~ Normal(0, init_sigma), h_t - phi h_{t-1} ~ Normal(0, sigma)  (timeseries.py:646-676) ------
@@ -1228,6 +1366,13 @@ __global__ void __launch_bounds__(256) ir_pointwise_kernel(const IrModel::Params
             for (int j = lane; j < V.size; j += 32) x[V.offset + j] = ir_backward(V, q[V.offset + j], lj);
         }
         __syncwarp();
+        if constexpr (EXTENDED) {
+            const int n_spec = ir_spec_count(P.terms);
+            if (n_spec) {
+                ir_spectral_forward(ir_specs(P.terms, n_spec), n_spec, x, lane, 32);
+                __syncwarp();
+            }
+        }
         const double sg_s = ir_slot(L, x), la = log(sg_s);  // la: log alpha, read only by the families with a dispersion
         for (int i = lane; i < N; i += 32) {
             const double eta = ir_eta(P.terms, L.term0, L.n_terms, x, i, N);

@@ -30,7 +30,11 @@ pymc/model/fgraph.py:76-81, :139) -- and pattern-matches them onto the closed fa
                      finite mixtures: pm.NormalMixture(w, mu, sigma) and pm.Mixture(w, pm.Poisson.dist(lam, shape=K)), the
                      Mixture of ONE batched component, with w a free pm.Dirichlet or a constant K-vector, mu optionally
                      linear_predictor[:, None] + mu and lam optionally pm.math.exp(linear_predictor)[:, None] * lam
-    free RV      ->  pm.Dirichlet with a constant a -> the dirichlet prior on a simplex variable
+                 Gaussian processes: phi @ (beta * sqrt_psd), what pm.gp.HSGP.prior (non-centred) and prior_linearized
+                     build, with psd cov.py's ExpQuad / Matern52 / Matern32 density, optionally times eta**2 (eta a scalar
+                     free RV) or a constant, ls constants or a scalar or vector free RV -> an ir.Spectral term
+    free RV      ->  pm.Dirichlet with a constant a -> the dirichlet prior on a simplex variable; pm.InverseGamma with
+                     constant alpha, beta
     transform    ->  None, log, interval, Ordered() / Ordered(positive=True) -> "ordered" / "ordered_positive", and
                      SimplexTransform -> "simplex"
 
@@ -55,9 +59,28 @@ _PRIOR_BY_OP = {  # RV op class name (lower-cased, "rv" stripped) -> (ir dist, p
     "gamma": ("gamma", (0, 1)),           # (alpha, scale): beta = 1 / scale
     "beta": ("beta", (0, 1)),
     "lognormal": ("lognormal", (0, 1)),
+    "invgamma": ("inversegamma", (0, 1)),  # pm.InverseGamma's InvGammaRV: (alpha, beta) = (shape, scale), continuous.py:2593-2640
     "flat": ("flat", ()),
     "halfflat": ("flat", ()),
 }
+
+
+class _SpectralCoef:
+    """The coefficient slot of an HSGP term in ``terms_of``: Phi with its ``ir.Spectral``.  Such a term may only be added
+    to a predictor; scaling or negating it raises."""
+
+    def __init__(self, Phi, spectral):
+        self.Phi, self.spectral = Phi, spectral
+
+    def _refuse(self, *args):
+        raise NotImplementedError("linear predictor: an HSGP term phi @ (beta * sqrt_psd) may only be added, not scaled, "
+                                  "negated or multiplied")
+
+    __array__ = __float__ = __neg__ = __mul__ = __rmul__ = __truediv__ = _refuse
+
+
+HSGP_FORM = ("pm.gp.HSGP(m, c, cov_func=eta**2 * pm.gp.cov.ExpQuad | Matern52 | Matern32(D, ls)).prior (non-centred), "
+             "or phi @ (beta * sqrt_psd) from prior_linearized")
 
 
 def _op_name(rv) -> str:
@@ -211,7 +234,13 @@ def from_pymc(model) -> _ir.ModelIR:
             if A is not None and b in name_of and A.ndim == 2:
                 return [(np.ascontiguousarray(A[:, k], dtype=np.float64), [(use(b), np.full(N, k, dtype=np.int32))])
                         for k in range(A.shape[1])]
-            raise NotImplementedError("linear predictor: dot() is supported as constant_matrix @ vector_variable")
+            found = hsgp_of(b, A) if A is not None and A.ndim == 2 else None
+            if found is not None and isinstance(found[1], np.ndarray):  # constant sqrt_psd: the design term Phi diag(s)
+                return [(np.ascontiguousarray(A * found[1][None, :], dtype=np.float64), [(use(found[0]), None)])]
+            if found is not None:
+                return [(_SpectralCoef(np.ascontiguousarray(A, dtype=np.float64), found[1]), [(use(found[0]), None)])]
+            raise NotImplementedError("linear predictor: dot() is supported as constant_matrix @ vector_variable or "
+                                      f"an HSGP term ({HSGP_FORM})")
         son = scalar_op_name(node)
         if son == "add":
             return [t for inp in node.inputs for t in terms_of(inp, N)]
@@ -244,9 +273,178 @@ def from_pymc(model) -> _ir.ModelIR:
     def make_terms(x, N):
         out = []
         for c, f in terms_of(x, N):
+            if isinstance(c, _SpectralCoef):
+                out.append(_ir.Term(list(f), c.Phi, spectral=c.spectral))
+                continue
             coef = None if (np.ndim(c) == 0 and float(c) == 1.0) else (np.asarray(c, dtype=np.float64) if np.ndim(c) else float(c))
             out.append(_ir.Term(list(f), coef))
         return out
+
+    # ---- HSGP: phi @ (beta * sqrt(psd)) with psd as cov.py's power_spectral_density builds it --------------------------
+    def unshuffle(x):
+        while x.owner is not None and isinstance(x.owner.op, DimShuffle):
+            x = x.owner.inputs[0]
+        return x
+
+    def elem_inputs(x, want):
+        """inputs of the Elemwise `want` that x is, under any DimShuffle layers, or None"""
+        x = unshuffle(x)
+        if x.owner is not None and scalar_op_name(x.owner) == want:
+            return list(x.owner.inputs)
+        return None
+
+    def mul_leaves(x):
+        """the factors of a product, by the graph's structure (constant factors are not folded together)"""
+        x = unshuffle(x)
+        if x.owner is not None and scalar_op_name(x.owner) == "mul":
+            return [leaf for inp in x.owner.inputs for leaf in mul_leaves(inp)]
+        return [x]
+
+    def is_dot(x):
+        x = unshuffle(x)
+        return x.owner is not None and isinstance(x.owner.op, Dot)
+
+    def omega_ls_of(d):
+        """(omega [M][D], ls, the ls graph) of dot(square(omega), square(ls)), ls = ones(D) * ls as the covariance writes it"""
+        d = unshuffle(d)
+        a, b = (unshuffle(v) for v in d.owner.inputs)
+        om = _const_value(a.owner.inputs[0]) if a.owner is not None and scalar_op_name(a.owner) == "sqr" else None
+        if om is None:
+            om2 = _const_value(a)
+            om = None if om2 is None else np.sqrt(om2)
+        if om is None or b.owner is None or scalar_op_name(b.owner) != "sqr":
+            return None
+        om = np.asarray(om, dtype=np.float64).reshape(len(om), -1)
+        lsx = unshuffle(b.owner.inputs[0])
+        c = _const_value(lsx)
+        leaves = mul_leaves(lsx)
+        if c is None and all(_const_value(leaf) is not None for leaf in leaves):  # ones(D) * ls, each factor constant
+            c = np.prod([np.broadcast_to(_const_value(leaf), (om.shape[1],)) for leaf in leaves], axis=0)
+        if c is not None:  # constant lengthscales: the D values
+            return om, np.broadcast_to(np.asarray(c, dtype=np.float64).reshape(-1), (om.shape[1],)).copy(), lsx
+        for leaf in leaves:
+            if _const_value(leaf) is not None:
+                continue  # the ones(D) the covariance multiplies ls by
+            if leaf.owner is not None and scalar_op_name(leaf.owner) in ("truediv", "true_div", "reciprocal"):
+                raise NotImplementedError("HSGP: a covariance given ls_inv is outside the closed set (give ls)")
+            if leaf in name_of:
+                if size_of[name_of[leaf]] not in (1, om.shape[1]):
+                    raise NotImplementedError(f"HSGP: ls must be a scalar or one per input dimension ({HSGP_FORM})")
+                return om, _ir.Ref(use(leaf)), lsx
+            raise NotImplementedError(f"HSGP: ls must be constants, a scalar or a vector free RV ({HSGP_FORM})")
+        return None
+
+    def density_of(node, son):
+        """(cov, omega, ls, ls graph) when the psd factor `node` is exp(-0.5 dot(...)) (ExpQuad) or
+        power(c + dot(...), -(D + c) / 2) with c = 5 or 3 (Matern 5/2, 3/2), matched by structure; else None"""
+        if son == "exp":
+            ins = elem_inputs(node.inputs[0], "mul") or []
+            dots = [v for v in ins if is_dot(v)]
+            rest = [_const_value(v) for v in ins if not is_dot(v)]
+            if len(dots) != 1 or len(rest) != 1 or rest[0] is None or rest[0].size != 1 or float(rest[0]) != -0.5:
+                return None
+            got = omega_ls_of(dots[0])
+            return None if got is None else ("expquad",) + got
+        if son == "pow":
+            ins = elem_inputs(node.inputs[0], "add") or []
+            dots = [v for v in ins if is_dot(v)]
+            cs = [_const_value(v) for v in ins if not is_dot(v)]
+            e = _const_value(node.inputs[1])
+            if len(dots) != 1 or len(cs) != 1 or cs[0] is None or cs[0].size != 1 or e is None:
+                return None
+            got = omega_ls_of(dots[0])
+            if got is None:
+                return None
+            c0, D = float(cs[0]), got[0].shape[1]
+            cov = {5.0: "matern52", 3.0: "matern32"}.get(c0)
+            if cov is None or float(e) != -(D + c0) / 2.0:
+                raise NotImplementedError(f"HSGP: only the Matern 5/2 and 3/2 densities are in the closed set ({HSGP_FORM})")
+            return (cov,) + got
+        return None
+
+    def spectral_of(psd, M):
+        """ir.Spectral of sqrt_psd's argument psd (under psd[i:] when drop_first), else raise.  The factors are matched by
+        the graph's structure before any constant is folded, so constant lengthscales keep their frequencies."""
+        x, drop = unshuffle(psd), False
+        if x.owner is not None and isinstance(x.owner.op, Subtensor) and not isinstance(x.owner.op, (AdvancedSubtensor, AdvancedSubtensor1)):
+            x, drop = unshuffle(x.owner.inputs[0]), True
+        if x.owner is not None and scalar_op_name(x.owner) == "add":
+            raise NotImplementedError(f"HSGP: sums of kernels inside one term are outside the closed set (write one HSGP "
+                                      f"per kernel and add them; {HSGP_FORM})")
+        const, amp, found, prods = 1.0, None, [], []
+        for leaf in mul_leaves(x):
+            node = leaf.owner
+            son = scalar_op_name(node) if node is not None else ""
+            if node is not None and type(node.op).__name__.lower() == "prod":
+                prods.append(unshuffle(node.inputs[0]))  # prod(ls): checked against the density's ls below
+                continue
+            got = density_of(node, son) if son in ("exp", "pow") else None
+            if got is not None:
+                found.append(got)
+                continue
+            c = _const_value(leaf)
+            if c is not None:
+                if c.size != 1:
+                    raise NotImplementedError(f"HSGP: psd must be a scalar times the covariance's density ({HSGP_FORM})")
+                const *= float(c.reshape(()))
+                continue
+            if leaf in name_of:
+                raise NotImplementedError(f"HSGP: eta * cov with a random eta is outside the closed set (write eta**2 * cov; "
+                                          f"{HSGP_FORM})")
+            if son in ("sqr", "pow") and unshuffle(node.inputs[0]) in name_of:
+                e = _const_value(node.inputs[1]) if son == "pow" else np.array(2.0)
+                if e is None or float(e) != 2.0 or size_of[name_of[unshuffle(node.inputs[0])]] != 1:
+                    raise NotImplementedError(f"HSGP: the amplitude must be eta**2 with eta a scalar free RV ({HSGP_FORM})")
+                if amp is not None:
+                    raise NotImplementedError(f"HSGP: products of kernels are outside the closed set ({HSGP_FORM})")
+                amp = _ir.Ref(use(unshuffle(node.inputs[0])))
+                continue
+            if son == "exp":
+                raise NotImplementedError(f"HSGP: exp(...) is not ExpQuad's density ({HSGP_FORM})")
+            if son == "pow":
+                raise NotImplementedError(f"HSGP: a power that is not a Matern density ({HSGP_FORM})")
+            what = type(node.op).__name__ if node is not None else str(leaf)
+            if son in ("ive", "iv", "i0", "i1", "besseli") or "bessel" in what.lower():
+                raise NotImplementedError(f"HSGP: HSGPPeriodic is outside the closed set ({HSGP_FORM})")
+            raise NotImplementedError(f"HSGP: {what} in the power spectral density is outside the closed set ({HSGP_FORM})")
+        if len(found) != 1:
+            raise NotImplementedError(("HSGP: products of kernels are outside the closed set" if found else
+                                       "HSGP: no ExpQuad / Matern density in sqrt_psd") + f" ({HSGP_FORM})")
+        cov, om, ls, lsx = found[0]
+        if len(prods) != 1 or prods[0] is not lsx:
+            raise NotImplementedError(f"HSGP: the density must hold prod(ls) of the ls in its exponent once "
+                                      f"({HSGP_FORM})")
+        if drop:
+            om = om[1:]
+        if om.shape[0] != M:
+            raise NotImplementedError(f"HSGP: phi has {M} columns but psd {om.shape[0]} frequencies ({HSGP_FORM})")
+        scale2 = const / np.exp(_ir.spectral_log_const(cov, om.shape[1])[0])
+        if amp is not None and abs(scale2 - 1.0) > 1e-12:
+            raise NotImplementedError(f"HSGP: eta**2 times a further constant is outside the closed set ({HSGP_FORM})")
+        return _ir.Spectral(cov, om, ls, amp if amp is not None else float(np.sqrt(scale2)))
+
+    def hsgp_of(b, Phi):
+        """(z, ir.Spectral) of b = z * sqrt(psd) (either order), z a free RV of Phi's width, or (z, s) with s the M
+        constants of an already folded sqrt_psd; else None"""
+        ins = elem_inputs(b, "mul")
+        if ins is None or len(ins) != 2:
+            return None
+        for z, sq in (ins, ins[::-1]):
+            z = unshuffle(z)
+            if z not in name_of or size_of[name_of[z]] != Phi.shape[1]:
+                continue
+            root = elem_inputs(sq, "sqrt")
+            if root is not None:
+                return z, spectral_of(root[0], Phi.shape[1])
+            s = _const_value(sq)
+            if s is not None and s.shape == (Phi.shape[1],):
+                return z, np.asarray(s, dtype=np.float64)
+        return None
+        for z, sq in (ins, ins[::-1]):
+            z, root = unshuffle(z), inputs_of(sq, "sqrt")
+            if z in name_of and size_of[name_of[z]] == Phi.shape[1] and root is not None:
+                return z, spectral_of(root[0], Phi.shape[1])
+        return None
 
     priors, ar1 = [], []
     for rv in free:
@@ -292,6 +490,11 @@ def from_pymc(model) -> _ir.ModelIR:
             c = _const_value(ps[i]) if i == scale else None
             if c is not None and c.size > 1:  # one constant scale per element
                 return np.ravel(np.broadcast_to(c, np.shape(ip[by_rv[rv].name]))).astype(np.float64)
+            sq = unshuffle(ps[i])
+            if i == scale and c is None and sq.owner is not None and scalar_op_name(sq.owner) == "sqrt":
+                raise NotImplementedError(f"{rv.name}: the centred HSGP parametrisation (a Normal prior whose sigma is "
+                                          "sqrt_psd, a vector of random scales) is outside the closed set: use "
+                                          "parametrization='noncentered'")
             return param(ps[i], what)
 
         args = [prior_arg(i) for i in idx]
@@ -850,11 +1053,7 @@ def from_pymc(model) -> _ir.ModelIR:
         expr = dv
         if expr.owner is not None and _is_copy(expr.owner):
             expr = expr.owner.inputs[0]  # pm.Deterministic wraps its expression in a named copy
-        terms = []
-        for c, f in terms_of(expr, size):
-            coef = None if (np.ndim(c) == 0 and float(c) == 1.0) else (np.asarray(c, dtype=np.float64) if np.ndim(c) else float(c))
-            terms.append(_ir.Term(list(f), coef))
-        dets.append(_ir.Deterministic(dv.name, size, terms))
+        dets.append(_ir.Deterministic(dv.name, size, make_terms(expr, size)))
     out = _ir.ModelIR(vars_, priors, liks, ar1, name=getattr(model, "name", "") or "pymc_model", deterministics=dets)
     out.validate()
     return out

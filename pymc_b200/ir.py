@@ -51,6 +51,7 @@ PRIOR_DISTS = {
     "beta": (9, 2),          # (alpha, beta) constants                                  continuous.py:1250-1256
     "lognormal": (10, 2),    # (mu, sigma)                                              continuous.py:1807-1814
     "dirichlet": (11, 1),    # (a): K constants > 0 or one broadcast; on a simplex only  multivariate.py:557-585
+    "inversegamma": (12, 2), # (alpha, beta) constants                                  continuous.py:2631-2640
 }
 # likelihoods: name -> id
 LIK_DISTS = {
@@ -169,9 +170,21 @@ BB_TRIALS = "trials must be finite integers >= 0"
 BETA_SLOTS = ("beta_logit and beta_binomial_logit take phi, and no sigma, alpha, cutpoints, psi, weights, components or "
               "lower / upper")
 BETA_TRIALS = "trials belong to beta_binomial_logit (a Beta observes proportions, not counts)"
+# Spectral terms: a Hilbert-space approximate GP (pm.gp.HSGP, non-centred, hsgp_approx.py:453-473) as a design term whose
+# column weights depend on hyperparameters, f = Phi (z * s(theta)) with s_k = amplitude sqrt(S(omega_k; ls)) and S the
+# power spectral density of ``cov`` (cov.py:574-583, :690-710, :743-761).  Lowered as the ABI's spectral term
+# (include/b200nuts.h), or as a plain design term when ls and amplitude are constants.
+COV_FUNCS = {"expquad": 1, "matern52": 2, "matern32": 3}
+# the rules of spectral terms (csrc/b200nuts.cu: prepare_ir, same words)
+SPEC_PHI = "a spectral term's Phi must be finite with shape (N, M), M the size of its variable"
+SPEC_Z = "a spectral term's variable must be one whole variable with no index and no transform"
+SPEC_OMEGA = "omega must have shape (M, D), D >= 1, with finite entries >= 0"
+SPEC_COV = "cov must be expquad, matern52 or matern32"
+SPEC_LS = "ls must be a finite constant > 0, D of them, or a variable of size 1 or D with positive support"
+SPEC_AMP = "amplitude must be a finite constant > 0 or a scalar variable with positive support"
 # The support rule.  The device evaluates a density's formula wherever it is asked to, so every variable must be kept
 # inside its prior's support by its transform, and every scale parameter must be positive:
-POSITIVE_PRIORS = ("halfnormal", "halfcauchy", "exponential", "gamma", "lognormal")  # a log transform, or interval lo >= 0
+POSITIVE_PRIORS = ("halfnormal", "halfcauchy", "exponential", "gamma", "lognormal", "inversegamma")  # a log transform, or interval lo >= 0
 SCALE_PARAMS = {"normal": {1: "sigma"}, "lognormal": {1: "sigma"}, "halfnormal": {0: "sigma"}, "cauchy": {1: "beta"},
                 "halfcauchy": {0: "beta"}, "exponential": {0: "lam"}, "studentt": {2: "sigma"}}
 POSITIVE_SUPPORT = "a scalar variable with positive support (a log transform, or an interval with lo >= 0)"
@@ -202,6 +215,73 @@ def simplex_backward(z: np.ndarray) -> np.ndarray:
     ze = np.concatenate([z, -np.sum(z, axis=-1, keepdims=True)], axis=-1)
     e = np.exp(ze - np.max(ze, axis=-1, keepdims=True))
     return e / np.sum(e, axis=-1, keepdims=True)
+
+
+def spectral_log_const(cov: str, D: int) -> tuple[float, float, float]:
+    """(log C_D, nu, c) of S = C_D prod_d l_d exp(h(Q)) with h = -Q / 2 (expquad, nu = 0) or -nu log(c + Q) (Matern)."""
+    from scipy.special import gammaln
+
+    if cov == "expquad":
+        return 0.5 * D * np.log(2.0 * np.pi), 0.0, 0.0
+    order, den = (2.5, 0.75) if cov == "matern52" else (1.5, 0.5)
+    nu, c = 0.5 * D + order, 2.0 * order
+    return D * np.log(2.0) + 0.5 * D * np.log(np.pi) + gammaln(nu) + order * np.log(c) - np.log(den * np.sqrt(np.pi)), nu, c
+
+
+def spectral_log_scale(cov: str, omega, ls, amplitude) -> np.ndarray:
+    """log s_k = log amplitude + (log C_D + sum_d log l_d + h(Q_k)) / 2 with Q_k = sum_d l_d^2 omega_kd^2, as [..., M] for
+    ls [..., D] and amplitude [...] (leading axes: draws)."""
+    omega = np.asarray(omega, dtype=np.float64)
+    ls = np.asarray(ls, dtype=np.float64)
+    log_c, nu, c = spectral_log_const(cov, omega.shape[1])
+    Q = np.einsum("...d,kd->...k", ls * ls, omega * omega)
+    h = -0.5 * Q if cov == "expquad" else -nu * np.log(c + Q)
+    base = np.log(np.asarray(amplitude, dtype=np.float64)) + 0.5 * (log_c + np.sum(np.log(ls), axis=-1))
+    return base[..., None] + 0.5 * h
+
+
+def hsgp_basis(X, m, c=None, L=None, drop_first: bool = False):
+    """(Phi [N][M], omega [M][D], centre [D], L [D]) of the Hilbert-space approximation with m[d] basis functions per
+    dimension, by the method of pm.gp.HSGP.prior_linearized: the inputs are centred at (max + min) / 2; the half-width L_d
+    is c (max - min) / 2 unless L is given; the eigenvalues of the Laplacian on [-L, L]^D are lambda_jd = (pi j_d / (2
+    L_d))^2 for j_d = 1..m[d], combined over the dimensions in np.meshgrid's order; omega = sqrt(lambda) and phi_j(x) =
+    prod_d L_d^(-1/2) sin(sqrt(lambda_jd) (x_d + L_d)).  ``drop_first`` drops the first basis function."""
+    X = np.asarray(X, dtype=np.float64)
+    X = X[:, None] if X.ndim == 1 else X
+    D = X.shape[1]
+    m = [int(m)] * D if np.ndim(m) == 0 else [int(v) for v in m]
+    centre = 0.5 * (X.max(axis=0) + X.min(axis=0))
+    Xs = X - centre
+    if L is None:
+        if c is None:
+            raise ValueError("hsgp_basis needs c or L")
+        L = np.asarray(c, dtype=np.float64) * 0.5 * (X.max(axis=0) - X.min(axis=0))
+    L = np.broadcast_to(np.asarray(L, dtype=np.float64), (D,)).copy()
+    grid = np.meshgrid(*[np.arange(1, 1 + md) for md in m])
+    J = np.stack([g.ravel() for g in grid], axis=1).astype(np.float64)  # [M][D]
+    omega = np.pi * J / (2.0 * L)
+    Phi = np.ones((X.shape[0], J.shape[0]))
+    for d in range(D):
+        Phi *= np.sin(omega[:, d][None, :] * (Xs[:, d][:, None] + L[d])) / np.sqrt(L[d])
+    i = int(bool(drop_first))
+    return Phi[:, i:], omega[i:], centre, L
+
+
+def spectral_weights(ir, t, x: dict) -> np.ndarray:
+    """s(theta) [..., M] of spectral term t at the constrained values ``x`` (rv name -> draws, as ``constrain`` returns)."""
+    sp = t.spectral
+    D = np.shape(sp.omega)[1]
+    if isinstance(sp.ls, Ref):
+        v = ir.var(sp.ls.var)
+        ls = np.asarray(x[v.rv_name], dtype=np.float64)
+        ls = ls[..., None] if v.size == 1 else ls  # an isotropic lengthscale (or D = 1)
+    else:
+        ls = np.asarray(sp.ls, dtype=np.float64).reshape(-1)
+    amp = np.asarray(x[ir.var(sp.amplitude.var).rv_name] if isinstance(sp.amplitude, Ref) else sp.amplitude,
+                     dtype=np.float64)
+    lead = np.broadcast_shapes(ls.shape[:-1], amp.shape)
+    ls = np.broadcast_to(ls, lead + (D,))
+    return np.exp(spectral_log_scale(sp.cov, sp.omega, ls, np.broadcast_to(amp, lead)))
 
 
 def is_design(t) -> bool:
@@ -242,15 +322,32 @@ class Prior:
 
 
 @dataclass
+class Spectral:
+    """The spectral description of an HSGP term: s_k = amplitude * sqrt(S(omega_k; ls)) with S the power spectral density
+    of ``cov`` ("expquad", "matern52" or "matern32") at the frequencies omega [M][D] (``hsgp_basis``).  ``ls`` is a constant
+    > 0, D constants or a Ref to a variable of size 1 (isotropic) or D (ARD) with positive support; ``amplitude`` (PyMC's
+    eta of ``eta**2 * cov``) is a constant > 0 or a Ref to a scalar with positive support."""
+
+    cov: str
+    omega: np.ndarray
+    ls: float | np.ndarray | Ref = 1.0
+    amplitude: float | Ref = 1.0
+
+
+@dataclass
 class Term:
     """coef[i] * prod_f x_f[idx_f[i]].  A factor's idx is None for a scalar variable (broadcast) or for a vector variable of
     the likelihood's own length (elementwise).
 
     A design term has a 2-D coef X of shape [N][K] and exactly one factor, a variable of size K with no index:
-    it adds sum_k X[i, k] * x[k], i.e. ``pm.math.dot(X, beta)``, evaluated on the device as one team-parallel term."""
+    it adds sum_k X[i, k] * x[k], i.e. ``pm.math.dot(X, beta)``, evaluated on the device as one team-parallel term.
+
+    A spectral term is a design term with a ``spectral`` description: coef is the HSGP basis Phi [N][M], its factor the
+    coefficients z (size M, no transform), and it adds sum_k Phi[i, k] s_k(theta) z_k, ``phi @ (beta * sqrt_psd)``."""
 
     factors: list  # [(var_name, idx or None), ...]
     coef: np.ndarray | float | None = None
+    spectral: Spectral | None = None
 
 
 @dataclass
@@ -408,7 +505,7 @@ class ModelIR:
                 if isinstance(a, Ref):
                     if self.var(a.var).size != 1:
                         raise ValueError(f"prior on {p.var}: parameter {a.var} must be a scalar variable")
-                    if p.dist in ("uniform", "gamma", "beta") or (p.dist == "studentt" and k == 0):
+                    if p.dist in ("uniform", "gamma", "beta", "inversegamma") or (p.dist == "studentt" and k == 0):
                         raise ValueError(f"prior {p.dist} on {p.var}: parameter {k} must be a constant")
                 if k == scale and not isinstance(a, Ref) and np.ndim(a) == 1:  # one scale per element
                     s = np.asarray(a, dtype=np.float64)
@@ -604,6 +701,9 @@ class ModelIR:
     def _check_terms(self, terms, N: int, where: str, length: str) -> None:
         """Terms of a predictor of length N (a likelihood's observations, or the elements of a prior's variable)."""
         for t in terms:
+            if t.spectral is not None:
+                self._check_spectral(t, N, where)
+                continue
             if is_design(t):
                 self._check_design(t, N, where)
                 continue
@@ -635,6 +735,41 @@ class ModelIR:
         if not np.all(np.isfinite(X)):
             raise ValueError(f"{where}: X must be finite")
 
+    def _check_spectral(self, t, N: int, where: str) -> None:
+        """A spectral term: Phi [N][M] finite on one whole variable z of size M with no index and no transform, a known cov,
+        omega [M][D], ls and amplitude (the checks prepare_ir makes, in the same words)."""
+        sp = t.spectral
+        if len(t.factors) != 1:
+            raise ValueError(f"{where}: {SPEC_Z}")
+        vn, idx = t.factors[0]
+        v = self.var(vn)
+        if idx is not None or v.transform is not None:
+            raise ValueError(f"{where}: {SPEC_Z}")
+        Phi = np.asarray(t.coef, dtype=np.float64)
+        if Phi.shape != (N, v.size) or not np.all(np.isfinite(Phi)):
+            raise ValueError(f"{where}: {SPEC_PHI}")
+        if sp.cov not in COV_FUNCS:
+            raise ValueError(f"{where}: {SPEC_COV}")
+        om = np.asarray(sp.omega, dtype=np.float64)
+        if om.ndim != 2 or om.shape[0] != v.size or not 1 <= om.shape[1] <= 4096 or not (
+                np.all(np.isfinite(om)) and np.all(om >= 0)):
+            raise ValueError(f"{where}: {SPEC_OMEGA}")
+        D = om.shape[1]
+
+        def ok(a, sizes, shapes):  # a Ref to a variable of one of the sizes with positive support, or constants > 0
+            if isinstance(a, Ref):
+                w = self.var(a.var)
+                return w.size in sizes and _positive_support(w)
+            if isinstance(a, Linear):
+                return False
+            c = np.asarray(a, dtype=np.float64)
+            return c.shape in shapes and bool(np.all(np.isfinite(c)) and np.all(c > 0))
+
+        if not ok(sp.amplitude, (1,), ((),)):
+            raise ValueError(f"{where}: {SPEC_AMP}")
+        if not ok(sp.ls, (1, D), ((), (D,))):
+            raise ValueError(f"{where}: {SPEC_LS}")
+
     def _check_scale(self, a, what: str) -> None:
         """A scale slot (a prior's sigma / beta / lam, a likelihood's sigma, an AR(1) sigma, a dispersion alpha): a finite
         constant > 0, or a Ref to a scalar variable whose transform keeps it positive."""
@@ -659,6 +794,8 @@ class ModelIR:
             raise ValueError(f"prior studentt on {v.name}: StudentT nu must be a positive constant")
         if p.dist in ("gamma", "beta") and not all(np.isfinite(float(a)) and float(a) > 0 for a in p.params):
             raise ValueError(f"prior {p.dist} on {v.name}: {p.dist.capitalize()} needs constant alpha, beta > 0")
+        if p.dist == "inversegamma" and not all(np.isfinite(float(a)) and float(a) > 0 for a in p.params):
+            raise ValueError(f"prior inversegamma on {v.name}: InverseGamma needs constant alpha, beta > 0")
         if p.dist == "beta" and not (lo is not None and lo >= 0.0 and hi <= 1.0):
             raise ValueError(f"prior beta on {v.name}: the variable needs an interval inside [0, 1]")
         if p.dist == "uniform":
@@ -864,6 +1001,14 @@ class ModelIR:
             lead = None
             total = 0.0
             for t in d.terms:
+                if t.spectral is not None:  # Phi @ (z * s(theta))
+                    v = self.var(t.factors[0][0])
+                    z = np.asarray(posterior[v.rv_name], dtype=np.float64)
+                    z = z[..., None] if v.size == 1 else z
+                    b = z * spectral_weights(self, t, posterior)
+                    lead = b.shape[:-1]
+                    total = total + b @ np.asarray(t.coef, dtype=np.float64).T
+                    continue
                 if is_design(t):  # X @ x
                     v = self.var(t.factors[0][0])
                     x = np.asarray(posterior[v.rv_name])
@@ -893,8 +1038,10 @@ class ModelIR:
         out = {}
         for L in self.likelihoods:
             for k, t in enumerate(L.terms):
-                if t.coef is not None and np.ndim(t.coef) in (1, 2):  # 2: a design term's X
+                if t.coef is not None and np.ndim(t.coef) in (1, 2):  # 2: a design term's X, a spectral term's Phi
                     out[f"{L.name}_coef{k}"] = np.asarray(t.coef)
+                if t.spectral is not None:
+                    out[f"{L.name}_omega{k}"] = np.asarray(t.spectral.omega)
                 for vn, idx in t.factors:
                     if idx is not None:
                         out[f"{L.name}_{vn}_idx"] = np.asarray(idx)
@@ -909,6 +1056,8 @@ class ModelIR:
                 for k, t in enumerate(L.psi.terms):
                     if t.coef is not None and np.ndim(t.coef) in (1, 2):
                         out[f"{L.name}_psi_coef{k}"] = np.asarray(t.coef)
+                    if t.spectral is not None:
+                        out[f"{L.name}_psi_omega{k}"] = np.asarray(t.spectral.omega)
                     for vn, idx in t.factors:
                         if idx is not None:
                             out[f"{L.name}_psi_{vn}_idx"] = np.asarray(idx)
@@ -1383,6 +1532,70 @@ def beta_regression_ir(dist: str = "beta", phi: str = "var", n_obs: int = 400, n
                    likelihoods=[Likelihood(lik, y, terms, trials=trials, phi=par)])
 
 
+def hsgp_regression_ir(cov: str = "expquad", dims: int = 1, ls: str = "var", amplitude: str = "var", dist: str = "normal",
+                       n_obs: int = 300, m: int | None = None, c: float = 1.5, additive: bool = False, covariates: int = 0,
+                       seed: int = 83) -> ModelIR:
+    """A GP regression through the non-centred HSGP on simulated data, as ``pm.gp.HSGP(m, c, cov_func=eta**2 * cov).prior``
+    writes it: f = Phi (z * s(ell, eta)) with z ~ Normal(0, 1)^M, ell ~ InverseGamma(4, 4 ell_0) (ARD: one per input
+    dimension) and eta ~ HalfNormal(1), both under log transforms.  X is uniform on [0, 10]^dims and the data come from a
+    smooth known f.  ``ls`` / ``amplitude`` = "const" fixes them at the simulation's values (a plain design term).
+    ``additive``: a second HSGP term with its own shorter lengthscale and amplitude; ``covariates`` = F > 0: an intercept
+    b0 ~ Normal(0, 2) and a design term X_c beta_c.  ``dist``: "normal" (sigma ~ HalfNormal(1)), "poisson" (log link) or
+    "bernoulli" (logit link).  ``m`` basis functions per dimension (default 24 in 1-D, 12 per dimension in 2-D).  The GP's
+    values are recorded as the Deterministic ``f``."""
+    if cov not in COV_FUNCS:
+        raise ValueError(SPEC_COV)
+    if dist not in ("normal", "poisson", "bernoulli") or ls not in ("var", "const") or amplitude not in ("var", "const"):
+        raise ValueError("dist must be normal, poisson or bernoulli; ls and amplitude 'var' or 'const'")
+    m = m or (24 if dims == 1 else 12)
+    rng = np.random.default_rng(seed)
+    X = rng.uniform(0.0, 10.0, (n_obs, dims))
+    truth = np.sin(X[:, 0]) + (0.5 * np.cos(0.6 * X[:, 1]) if dims > 1 else 0.0)
+    vars_, priors, terms, gp_terms = [], [], [], []
+
+    def gp(tag, ell0, eta0, mm):
+        Phi, omega, _, _ = hsgp_basis(X, [mm] * dims, c=c)
+        M = Phi.shape[1]
+        z = f"{tag}_hsgp_coeffs"
+        vars_.append(Var(z, z, M))
+        priors.append(Prior("normal", z, (0.0, 1.0)))
+        lsv, av = np.full(dims, ell0) if dims > 1 else ell0, eta0
+        if ls == "var":
+            vars_.append(Var(f"ell_{tag}_log__", f"ell_{tag}", dims, "log", initial=np.log(ell0)))
+            priors.append(Prior("inversegamma", f"ell_{tag}_log__", (4.0, 4.0 * ell0)))
+            lsv = Ref(f"ell_{tag}_log__")
+        if amplitude == "var":
+            vars_.append(Var(f"eta_{tag}_log__", f"eta_{tag}", 1, "log", initial=np.log(eta0)))
+            priors.append(Prior("halfnormal", f"eta_{tag}_log__", (1.0,)))
+            av = Ref(f"eta_{tag}_log__")
+        t = Term([(z, None)], coef=Phi, spectral=Spectral(cov, omega, lsv, av))
+        terms.append(t)
+        gp_terms.append(t)
+
+    gp("f", 2.0, 1.0, m)
+    if additive:
+        truth = truth + 0.3 * np.sin(3.0 * X[:, 0])
+        gp("g", 0.4, 0.3, m)
+    eta = truth
+    if covariates:
+        Xc = rng.standard_normal((n_obs, covariates))
+        eta = eta + 0.3 + Xc @ rng.normal(0.0, 0.5, covariates)
+        vars_ += [Var("b0", "b0", 1), Var("beta", "beta", covariates)]
+        priors += [Prior("normal", "b0", (0.0, 2.0)), Prior("normal", "beta", (0.0, 1.0))]
+        terms += [Term([("b0", None)]), Term([("beta", None)], coef=Xc)]
+    if dist == "normal":
+        y = eta + rng.normal(0.0, 0.3, n_obs)
+        vars_.append(Var("sigma_log__", "sigma", 1, "log", initial=np.log(0.3)))
+        priors.append(Prior("halfnormal", "sigma_log__", (1.0,)))
+        lik = Likelihood("normal", y, terms, sigma=Ref("sigma_log__"))
+    elif dist == "poisson":
+        lik = Likelihood("poisson_log", rng.poisson(np.exp(0.5 + eta)).astype(np.float64), terms)
+    else:
+        lik = Likelihood("bernoulli_logit", (rng.random(n_obs) < 1.0 / (1.0 + np.exp(-2.0 * eta))).astype(np.float64), terms)
+    return ModelIR(name=f"hsgp_{cov}_{dims}d_{dist}", vars=vars_, priors=priors, likelihoods=[lik],
+                   deterministics=[Deterministic("f", n_obs, gp_terms)])
+
+
 # ------------------------------------------------------------------------------------------------------------------------
 # lowering: ModelIR -> flat arrays of the C ABI (include/b200nuts.h: b200_ir)
 # ------------------------------------------------------------------------------------------------------------------------
@@ -1418,6 +1631,9 @@ def _param(ir: ModelIR, a, off):
 def _lower_terms(ir: ModelIR, terms: list, N: int, off: dict) -> list:
     out = []
     for t in terms:
+        if t.spectral is not None:
+            out.append(_lower_spectral(ir, t, off))
+            continue
         if is_design(t):  # one ABI design term: coef = X row-major, n_cols = K
             v = ir.var(t.factors[0][0])
             out.append(dict(coef=np.ascontiguousarray(t.coef, dtype=np.float64), factors=[(off[v.name], v.size, None)],
@@ -1438,6 +1654,28 @@ def _lower_terms(ir: ModelIR, terms: list, N: int, off: dict) -> list:
             fs.append((off[v.name], v.size, None if idx is None else np.ascontiguousarray(idx, dtype=np.int32)))
         out.append(dict(coef=coef, factors=fs))
     return out
+
+
+def _lower_spectral(ir: ModelIR, t, off: dict) -> dict:
+    """A spectral term: with constant ls and amplitude, the design term X = Phi diag(s); else the ABI's spectral term,
+    coef = Phi followed by the block (cov, D, amplitude, ls_1 .. ls_D, omega), factors z, amplitude and ls, where a size
+    0 factor stands for the constants in the block (include/b200nuts.h)."""
+    sp = t.spectral
+    v = ir.var(t.factors[0][0])
+    Phi = np.asarray(t.coef, dtype=np.float64)
+    om = np.asarray(sp.omega, dtype=np.float64)
+    M, D = om.shape
+    if not isinstance(sp.ls, Ref) and not isinstance(sp.amplitude, Ref):
+        s = np.exp(spectral_log_scale(sp.cov, om, np.broadcast_to(np.asarray(sp.ls, dtype=np.float64).reshape(-1), (D,)),
+                                      float(sp.amplitude)))
+        return dict(coef=np.ascontiguousarray(Phi * s[None, :]), factors=[(off[v.name], M, None)], n_cols=M)
+    amp = (off[ir.var(sp.amplitude.var).name], 1, None) if isinstance(sp.amplitude, Ref) else (0, 0, None)
+    ls = (off[ir.var(sp.ls.var).name], ir.var(sp.ls.var).size, None) if isinstance(sp.ls, Ref) else (0, 0, None)
+    a_c = 0.0 if isinstance(sp.amplitude, Ref) else float(sp.amplitude)
+    ls_c = np.zeros(D) if isinstance(sp.ls, Ref) else np.broadcast_to(np.asarray(sp.ls, dtype=np.float64).reshape(-1), (D,))
+    blk = np.concatenate([[float(COV_FUNCS[sp.cov]), float(D), a_c], ls_c, om.ravel()])
+    return dict(coef=np.ascontiguousarray(np.concatenate([Phi.ravel(), blk])), factors=[(off[v.name], M, None), amp, ls],
+                n_cols=M)
 
 
 def _lower_slot(ir: ModelIR, par, off: dict) -> dict:
@@ -1605,6 +1843,8 @@ def specialise(ir: ModelIR, extended: bool = False):
     def const(p, k, want=None):
         return not isinstance(p.params[k], Ref) and (want is None or float(p.params[k]) == want)
 
+    if any(t.spectral is not None for L in ir.likelihoods for t in L.terms):
+        return None
     pri = {ir.var(p.var).name: p for p in ir.priors}
     if len(pri) != len(ir.priors) or len(ir.likelihoods) != 1 or ir.likelihoods[0].dist in ZI_LIKS + MIXTURE_LIKS + BETA_LIKS:
         return None
